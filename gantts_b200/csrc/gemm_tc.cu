@@ -5,13 +5,14 @@
 // into the same fp32 accumulator), which keeps ~2^-16 relative error per product -- fp32-grade parity at
 // 1.5x the cost of a single TF32 pass, where plain TF32/BF16 (2e-3) would miss the 1e-4 bar.
 //
-// One warp-specialised kernel per output tile (128 rows x BN columns), two operand layouts:
+// One persistent warp-specialised kernel, output tiles of 128 rows x BN columns, two operand layouts:
 //   MN = false : C[M][N] = A[M][K] * B[N][K]^T   both operands K-major   (layer forward, gx = gz W)
 //   MN = true  : C[N][K] = A[M][N]^T * B[M][K]   both operands MN-major  (gW = gz^T x, split over M)
-// warpgroup 0: one TMA producer thread; warpgroups 1-2: 64 output rows each, wgmma.m64n64k16 per 64 output columns.
-// smem ring of `num_stages` {A_hi, A_lo, B_hi, B_lo} tiles (SWIZZLE_128B), full/empty mbarriers per stage.  After the
-// reduction the accumulators go through a shared-memory tile (re-using the ring) so that each epilogue thread owns
-// 16 consecutive columns of one row: bias / LeakyReLU / dropout / sigmoid, 16-byte stores.
+// warpgroup 0: one TMA producer thread filling a smem ring of `num_stages` {A_hi, A_lo, B_hi, B_lo} tiles
+// (SWIZZLE_128B, full/empty mbarriers per stage) across all of the CTA's tiles; warpgroups 1-2: whole tiles in turn,
+// one wgmma.m64n{BN}k16 per product and 64-row block.  Each warpgroup stages its accumulators through its own
+// shared-memory tile so that each epilogue thread owns 16 consecutive columns of one row (bias / LeakyReLU / dropout /
+// sigmoid, 16-byte stores); that epilogue runs while the other warpgroup's MMAs keep the tensor cores busy.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -21,14 +22,19 @@
 
 namespace gantts {
 
-constexpr int TC_EPI_WARPS = 8;     // the two MMA warpgroups run the epilogue
-constexpr int TC_THREADS = 128 + 32 * TC_EPI_WARPS;   // warpgroup 0 TMA, warpgroups 1-2 MMA + epilogue
-constexpr int TC_BM = 128;          // output rows per tile (two warpgroups of m64)
-constexpr int TC_MAX_BN = 128;      // output columns per tile (64-column wgmma blocks)
+constexpr int TC_WG_WARPS = 4;      // warps of one MMA + epilogue warpgroup
+constexpr int TC_THREADS = 128 + 2 * 32 * TC_WG_WARPS;   // warpgroup 0 TMA, warpgroups 1-2 MMA + epilogue
+constexpr int TC_BM = 128;          // output rows per tile (one warpgroup: two wgmma m64 row blocks)
+constexpr int TC_WARP_PITCH = 20;   // floats per row of a warp's epilogue buffer (float4-aligned, conflict-free reads)
+constexpr int TC_WARP_BUF_FLOATS = 32 * TC_WARP_PITCH;   // one 32-row x 16-column chunk (>= the 2 KB fp32 scratch)
+constexpr int TC_MAX_BN = 128;      // output columns per tile
+constexpr int TC_KK_BK = 64;        // reduction elements per stage, K-major (one 128-byte swizzled row)
+constexpr int TC_MN_BK = 32;        // reduction rows per stage of the weight-gradient GEMM
 constexpr int TC_MAX_STAGES = 8;
+constexpr int TC_PRODUCER_REGS = 40;    // setmaxnreg: the TMA warpgroup gives registers to the MMA warpgroups
+constexpr int TC_CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
 constexpr uint32_t TC_SMEM_MAX = 227 * 1024;         // opt-in shared memory per block on sm_90
 constexpr uint32_t TC_BIAS_SMEM = 4096;              // staged bias vector (<= 1024 columns)
-constexpr uint32_t TC_F32_STAGE_SMEM = TC_EPI_WARPS * 2048;   // opt-in transpose scratch of the fp32 epilogue (2 KB per warp)
 constexpr uint32_t TC_ONES_SMEM = 1024;              // all-ones bf16 tile (MN-major bias gradient)
 
 // Epilogue flavours (template parameter of the kernel).
@@ -46,10 +52,9 @@ struct GemmParams {
   int num_stages;
   uint32_t stage_bytes, b_plane_bytes, tx_bytes;
   int64_t row0;         // global index of the first output row (dropout keys use global rows when a launch covers a row window)
-  int bk;               // reduction elements per smem stage
   uint32_t a_plane;     // bytes of one A plane tile in a stage
   uint32_t atom_bytes;  // MN-major: bytes of one 64-wide atom ([bk rows][128 B])
-  uint32_t ctile_pitch; // floats per row of the accumulator tile staged for the epilogue
+  uint32_t epi_off;     // byte offset (from the aligned smem base) of the 8 per-warp epilogue buffers
   uint32_t bar_off;     // byte offset (from the aligned smem base) of the mbarriers
   // EPI_F32 output
   float* C;
@@ -63,8 +68,8 @@ struct GemmParams {
   uint32_t* code;
   int64_t code_pitch;   // words per row
   uint32_t bias_off;    // byte offset (from the aligned smem base) of the staged bias vector, 0 = none
-  uint32_t f32_stage_off;   // EPI_F32 with an unaligned row stride: byte offset of the per-warp transpose scratch
-                            // (TC_EPI_WARPS x 2 KB), 0 = store straight from registers
+  int f32_stage;        // EPI_F32 with an unaligned row stride: write back through the warp's buffer as a transpose
+                        // scratch (epilogue_f32_staged), 0 = store straight from registers
   // MN-major only: column sums of A (= bias gradient) via an extra N=8 MMA against a tile of ones
   float* db;            // [num_z][rows_a] partial sums, or null
   uint32_t ones_off;    // byte offset of the all-ones bf16 tile from the aligned smem base
@@ -132,11 +137,14 @@ __device__ __forceinline__ void dropout16(float (&v)[16], uint64_t seed, uint32_
 // only issue 16 scalar stores per chunk and a warp store touches 32 rows = 32 sectors.  Here the warp's 32 x 16 tile
 // goes through a private 2 KB shared-memory scratch (float4 writes, XOR-swizzled: conflict-free) and is written back
 // with lanes 0-15 / 16-31 covering two whole 64-byte row segments per store instruction.  Same arithmetic, same
-// order.  Default on (GANTTS_B200_F32_STAGE=0 disables).
+// order.  Default on (GANTTS_B200_F32_STAGE=0 disables).  The warp's rows are row0 + (l % 16) + 64 (l / 16) for l < 32
+// (warp_row), the rows its wgmma fragments hold.
+__device__ __forceinline__ int64_t warp_row(int64_t row0, int l) { return row0 + (l & 15) + 64 * (l >> 4); }
+
 __device__ __forceinline__ void epilogue_f32_staged(const GemmParams& p, const uint32_t (&r)[16], int64_t row0,
                                                     int lane, int col, int z, const float* __restrict__ bias_s,
                                                     float* scr) {
-  const int64_t row = row0 + lane;
+  const int64_t row = warp_row(row0, lane);
   float v[16];
 #pragma unroll
   for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
@@ -166,7 +174,7 @@ __device__ __forceinline__ void epilogue_f32_staged(const GemmParams& p, const u
   float* cbase = p.C + (int64_t)z * p.c_zstride;
   const int j = lane & 15, hr = lane >> 4;
   const bool col_ok = col + j < p.cols_b;
-  float* q0 = cbase + (row0 + hr) * p.ldc + col + j;
+  float* q0 = cbase + col + j;
   // accumulate (the discriminator's input gradient added into its window of g_static): all loads of a half are issued
   // before its first store -- interleaved `*q = *q + val` serialises load -> store round trips per warp (the compiler
   // must assume the store aliases the next load)
@@ -175,14 +183,17 @@ __device__ __forceinline__ void epilogue_f32_staged(const GemmParams& p, const u
     float old[8];
     if (p.accumulate) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i)
-        old[i] = (col_ok && row0 + 2 * (8 * h + i) + hr < p.rows_a) ? __ldcg(q0 + (int64_t)(2 * (8 * h + i)) * p.ldc) : 0.f;
+      for (int i = 0; i < 8; ++i) {
+        const int64_t rw = warp_row(row0, 2 * (8 * h + i) + hr);
+        old[i] = (col_ok && rw < p.rows_a) ? __ldcg(q0 + rw * p.ldc) : 0.f;
+      }
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int rr = 2 * (8 * h + i) + hr;
       const float val = scr[rr * 16 + 4 * ((j >> 2) ^ ((rr >> 1) & 3)) + (j & 3)];
-      if (col_ok && row0 + rr < p.rows_a) q0[(int64_t)(2 * (8 * h + i)) * p.ldc] = p.accumulate ? old[i] + val : val;
+      const int64_t rw = warp_row(row0, rr);
+      if (col_ok && rw < p.rows_a) q0[rw * p.ldc] = p.accumulate ? old[i] + val : val;
     }
   }
   __syncwarp();
@@ -291,37 +302,102 @@ __device__ __forceinline__ uint32_t epilogue_chunk16(const GemmParams& p, const 
   return code;
 }
 
-// BN = output columns per tile (64 or 128): BN / 64 accumulator blocks of 32 fp32 registers per thread.
+// The reduction of one 128 x BN tile (two 64-row blocks) by one warpgroup: for each smem stage, BK/16 steps of
+// hi*hi, hi*lo, lo*hi (and, with DB, the two ones-tile MMAs of the bias gradient) into `acc`.  Stage s is released
+// once the wgmma group of stage s + 1 has been issued and stage s's group has completed (wait_group 1), so one stage's
+// MMAs are always in flight.  After the last stage is issued the other warpgroup is told (turn_other) that it may
+// start its next tile's MMAs.
+template <bool MN, int BN, bool DB>
+__device__ __forceinline__ void mma_tile(const GemmParams& p, float (&acc)[2][BN / 2], float (&accdb)[2][4],
+                                         uint32_t base, uint32_t full0, uint32_t empty0, uint32_t turn_other,
+                                         uint64_t d_ones, int nk, uint32_t& s, uint32_t& ph, int lane) {
+  constexpr int BK = MN ? TC_MN_BK : TC_KK_BK;
+  constexpr uint32_t kstep = MN ? 2048u : 32u;   // K = 16: 16 rows of 128 B (MN-major), 32 B inside the row (K-major)
+  const uint32_t a_half = MN ? p.atom_bytes : 8192u;  // rows 64-127 of A: the next MN atom / 64 rows of 128 B
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
+  uint32_t prev = 0;
+#pragma unroll 1
+  for (int kb = 0; kb < nk; ++kb) {
+    ptx::mbar_wait(full0 + 8 * s, ph);
+    const uint32_t sa_hi = base + s * p.stage_bytes, sa_lo = sa_hi + p.a_plane;
+    const uint32_t sb_hi = sa_lo + p.a_plane, sb_lo = sb_hi + p.b_plane_bytes;
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+      const uint64_t db_hi = ptx::make_smem_desc(sb_hi + k * kstep, p.atom_bytes, 1024u);
+      const uint64_t db_lo = ptx::make_smem_desc(sb_lo + k * kstep, p.atom_bytes, 1024u);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint64_t da_hi = ptx::make_smem_desc(sa_hi + h * a_half + k * kstep, p.atom_bytes, 1024u);
+        const uint64_t da_lo = ptx::make_smem_desc(sa_lo + h * a_half + k * kstep, p.atom_bytes, 1024u);
+        if constexpr (BN == 128) {
+          ptx::wgmma_m64n128k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_hi, db_hi);
+          ptx::wgmma_m64n128k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_hi, db_lo);
+          ptx::wgmma_m64n128k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_lo, db_hi);
+        } else {
+          ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_hi, db_hi);
+          ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_hi, db_lo);
+          ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_lo, db_hi);
+        }
+        if constexpr (DB) {
+          ptx::wgmma_m64n8k16<MN ? 1 : 0>(accdb[h], da_hi, d_ones);
+          ptx::wgmma_m64n8k16<MN ? 1 : 0>(accdb[h], da_lo, d_ones);
+        }
+      }
+    }
+    ptx::wgmma_commit();
+    if (kb > 0) {
+      ptx::wgmma_wait<1>();
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(empty0 + 8 * prev);   // the previous stage may be refilled
+    }
+    prev = s;
+    if (++s == (uint32_t)p.num_stages) { s = 0; ph ^= 1; }
+  }
+  __syncwarp();
+  if (lane == 0) ptx::mbar_arrive(turn_other);
+  ptx::wgmma_wait<0>();
+  ptx::fence_regs(acc[0]);
+  ptx::fence_regs(acc[1]);
+  ptx::fence_regs(accdb[0]);
+  ptx::fence_regs(accdb[1]);
+  __syncwarp();
+  if (lane == 0) ptx::mbar_arrive(empty0 + 8 * prev);
+}
+
+// Persistent kernel: CTA b walks the tiles b, b + gridDim.x, ... (numbering: z-slice of the reduction, then row tile,
+// then column tile, so the column tiles of one row tile are neighbours).  Warpgroup 0: one TMA producer thread runs
+// through the stage ring continuously across the CTA's tiles.  Warpgroups 1 and 2 take the CTA's tiles in turn (even,
+// odd), each with its own accumulators: a warpgroup runs its tile's epilogue while the other one's MMAs use the tensor
+// cores, and a pair of `turn` mbarriers keeps their MMA phases in tile order.
 template <bool MN, int EPI, int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                    const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
                    const GemmParams p) {
-  constexpr int NB = BN / 64;
+  constexpr int BK = MN ? TC_MN_BK : TC_KK_BK;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = ptx::smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* const gbase = smem_raw + (base - raw);
-  const uint32_t full0 = base + p.bar_off, empty0 = full0 + 8 * TC_MAX_STAGES;
-  const uint32_t ones_base = base + p.ones_off;
+  const uint32_t full0 = base + p.bar_off, empty0 = full0 + 8 * TC_MAX_STAGES, turn0 = empty0 + 8 * TC_MAX_STAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  // tile: z-slice of the reduction, then row tile, then column tile (column tiles of one row tile are neighbours)
   const int tiles_ab = p.num_a * p.num_b;
-  const int tile = (int)blockIdx.x;
-  const int z = tile / tiles_ab, rem = tile - z * tiles_ab;
-  const int ta = rem / p.num_b, tb = rem % p.num_b;
-  const int64_t r_beg = (int64_t)z * p.red_chunk;
-  const int64_t r_end = r_beg + p.red_chunk < p.red ? r_beg + p.red_chunk : p.red;
-  const int nk = (int)((r_end - r_beg + p.bk - 1) / p.bk);
-  const int a0 = ta * TC_BM, b0 = tb * BN;
-  const bool do_db = MN && p.db != nullptr && tb == 0;
+  const int tiles = tiles_ab * p.num_z;
+  auto k_blocks = [&](int z) {
+    const int64_t r_beg = (int64_t)z * p.red_chunk;
+    const int64_t r_end = r_beg + p.red_chunk < p.red ? r_beg + p.red_chunk : p.red;
+    return (int)((r_end - r_beg + BK - 1) / BK);
+  };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.num_stages; ++s) {
       ptx::mbar_init(full0 + 8 * s, 1);
-      ptx::mbar_init(empty0 + 8 * s, TC_EPI_WARPS);      // one arrive per MMA warp
+      ptx::mbar_init(empty0 + 8 * s, TC_WG_WARPS);      // one arrive per warp of the consuming warpgroup
     }
+    ptx::mbar_init(turn0, TC_WG_WARPS);
+    ptx::mbar_init(turn0 + 8, TC_WG_WARPS);
     ptx::fence_barrier_init();
     ptx::prefetch_tensormap(&tmAh);
     ptx::prefetch_tensormap(&tmAl);
@@ -339,7 +415,7 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
     for (int i = threadIdx.x; i < nb; i += TC_THREADS) bs[i] = i < p.cols_b ? p.bias[i] : 0.f;
     bias_s = bs;
   }
-  if (do_db) {
+  if (MN && p.db != nullptr) {
     // all-ones bf16 tile (any swizzle of a constant tile is the same tile)
     uint32_t* ones = reinterpret_cast<uint32_t*>(gbase + p.ones_off);
     for (int i = threadIdx.x; i < (int)(TC_ONES_SMEM / 4); i += TC_THREADS) ones[i] = 0x3F803F80u;
@@ -348,156 +424,143 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
   __syncthreads();
 
   if (warp < 4) {
+    ptx::setmaxnreg_dec<TC_PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       // ------------------------------------------------------------ TMA producer
       uint32_t s = 0, ph = 0;
-      for (int kb = 0; kb < nk; ++kb) {
-        const int64_t r0 = r_beg + (int64_t)kb * p.bk;
-        ptx::mbar_wait(empty0 + 8 * s, ph ^ 1);
-        const uint32_t fb = full0 + 8 * s;
-        ptx::mbar_expect_tx(fb, p.tx_bytes);
-        const uint32_t sa_hi = base + s * p.stage_bytes, sa_lo = sa_hi + p.a_plane;
-        const uint32_t sb_hi = sa_lo + p.a_plane, sb_lo = sb_hi + p.b_plane_bytes;
-        if (!MN) {
-          ptx::tma_load_2d(sa_hi, &tmAh, fb, (int32_t)r0, a0);
-          ptx::tma_load_2d(sb_hi, &tmBh, fb, (int32_t)r0, b0);
-          ptx::tma_load_2d(sa_lo, &tmAl, fb, (int32_t)r0, a0);
-          ptx::tma_load_2d(sb_lo, &tmBl, fb, (int32_t)r0, b0);
-        } else {
-          // 64-wide MN atoms, each [bk reduction rows][128 B]
-          for (int j = 0; j < TC_BM / 64; ++j) {
-            ptx::tma_load_2d(sa_hi + j * p.atom_bytes, &tmAh, fb, a0 + 64 * j, (int32_t)r0);
-            ptx::tma_load_2d(sa_lo + j * p.atom_bytes, &tmAl, fb, a0 + 64 * j, (int32_t)r0);
+      for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        const int z = t / tiles_ab, rem = t - z * tiles_ab;
+        const int a0 = (rem / p.num_b) * TC_BM, b0 = (rem % p.num_b) * BN;
+        const int64_t r_beg = (int64_t)z * p.red_chunk;
+        const int nk = k_blocks(z);
+        for (int kb = 0; kb < nk; ++kb) {
+          const int64_t r0 = r_beg + (int64_t)kb * BK;
+          ptx::mbar_wait(empty0 + 8 * s, ph ^ 1);
+          const uint32_t fb = full0 + 8 * s;
+          ptx::mbar_expect_tx(fb, p.tx_bytes);
+          const uint32_t sa_hi = base + s * p.stage_bytes, sa_lo = sa_hi + p.a_plane;
+          const uint32_t sb_hi = sa_lo + p.a_plane, sb_lo = sb_hi + p.b_plane_bytes;
+          if (!MN) {
+            ptx::tma_load_2d(sa_hi, &tmAh, fb, (int32_t)r0, a0);
+            ptx::tma_load_2d(sb_hi, &tmBh, fb, (int32_t)r0, b0);
+            ptx::tma_load_2d(sa_lo, &tmAl, fb, (int32_t)r0, a0);
+            ptx::tma_load_2d(sb_lo, &tmBl, fb, (int32_t)r0, b0);
+          } else {
+            // 64-wide MN atoms, each [BK reduction rows][128 B]
+            for (int j = 0; j < TC_BM / 64; ++j) {
+              ptx::tma_load_2d(sa_hi + j * p.atom_bytes, &tmAh, fb, a0 + 64 * j, (int32_t)r0);
+              ptx::tma_load_2d(sa_lo + j * p.atom_bytes, &tmAl, fb, a0 + 64 * j, (int32_t)r0);
+            }
+            for (int j = 0; j < BN / 64; ++j) {
+              ptx::tma_load_2d(sb_hi + j * p.atom_bytes, &tmBh, fb, b0 + 64 * j, (int32_t)r0);
+              ptx::tma_load_2d(sb_lo + j * p.atom_bytes, &tmBl, fb, b0 + 64 * j, (int32_t)r0);
+            }
           }
-          for (int j = 0; j < NB; ++j) {
-            ptx::tma_load_2d(sb_hi + j * p.atom_bytes, &tmBh, fb, b0 + 64 * j, (int32_t)r0);
-            ptx::tma_load_2d(sb_lo + j * p.atom_bytes, &tmBl, fb, b0 + 64 * j, (int32_t)r0);
-          }
+          if (++s == (uint32_t)p.num_stages) { s = 0; ph ^= 1; }
         }
-        if (++s == (uint32_t)p.num_stages) { s = 0; ph ^= 1; }
       }
     }
+    return;
   }
-  // ---------------------------------------------------------------- MMA warpgroups: rows [64 * mw, 64 * mw + 64)
-  const int mw = (warp >> 2) - 1;
-  float acc[NB][32];
-  float accdb[4] = {0.f, 0.f, 0.f, 0.f};
-  if (warp >= 4) {
-#pragma unroll
-    for (int n = 0; n < NB; ++n)
-#pragma unroll
-      for (int i = 0; i < 32; ++i) acc[n][i] = 0.f;
-    const uint64_t d_ones = ptx::make_smem_desc(ones_base, 0u, 1024u);
-    uint32_t s = 0, ph = 0;
-    for (int kb = 0; kb < nk; ++kb) {
-      ptx::mbar_wait(full0 + 8 * s, ph);
-      const uint32_t sa_hi = base + s * p.stage_bytes, sa_lo = sa_hi + p.a_plane;
-      const uint32_t sb_hi = sa_lo + p.a_plane, sb_lo = sb_hi + p.b_plane_bytes;
-      // K-major: this warpgroup's 64 A rows start 64 * 128 B into the plane, 64-row B blocks are 8 KB apart, K = 16
-      // advances 32 B inside the swizzled row.  MN-major: the warpgroup's A atom, B atoms atom_bytes apart, K = 16
-      // advances 16 rows of 128 B.
-      const uint32_t a_off = MN ? (uint32_t)mw * p.atom_bytes : (uint32_t)mw * 8192u;
-      const uint32_t b_blk = MN ? p.atom_bytes : 8192u;
-      const uint32_t kstep = MN ? 2048u : 32u;
-      ptx::wgmma_fence();
-#pragma unroll 1
-      for (int k = 0; k < p.bk / 16; ++k) {
-        const uint64_t da_hi = ptx::make_smem_desc(sa_hi + a_off + k * kstep, p.atom_bytes, 1024u);
-        const uint64_t da_lo = ptx::make_smem_desc(sa_lo + a_off + k * kstep, p.atom_bytes, 1024u);
-#pragma unroll
-        for (int n = 0; n < NB; ++n) {
-          const uint64_t db_hi = ptx::make_smem_desc(sb_hi + n * b_blk + k * kstep, p.atom_bytes, 1024u);
-          const uint64_t db_lo = ptx::make_smem_desc(sb_lo + n * b_blk + k * kstep, p.atom_bytes, 1024u);
-          ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc[n], da_hi, db_hi);
-          ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc[n], da_hi, db_lo);
-          ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc[n], da_lo, db_hi);
-        }
-        if (do_db) {
-          ptx::wgmma_m64n8k16<MN ? 1 : 0>(accdb, da_hi, d_ones);
-          ptx::wgmma_m64n8k16<MN ? 1 : 0>(accdb, da_lo, d_ones);
-        }
-      }
-      ptx::wgmma_commit();
-      ptx::wgmma_wait<0>();
-#pragma unroll
-      for (int n = 0; n < NB; ++n) ptx::fence_regs(acc[n]);
-      ptx::fence_regs(accdb);
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(empty0 + 8 * s);     // the stage may be refilled
-      if (++s == (uint32_t)p.num_stages) { s = 0; ph ^= 1; }
+
+  // ---------------------------------------------------------------- MMA + epilogue warpgroups
+  ptx::setmaxnreg_inc<TC_CONSUMER_REGS>();
+  const int wg = (warp >> 2) - 1;                        // takes the CTA's tiles i with i % 2 == wg
+  const int q = warp & 3;
+  const uint32_t turn_mine = turn0 + 8 * wg, turn_other = turn0 + 8 * (wg ^ 1);
+  float* const wbuf = reinterpret_cast<float*>(gbase + p.epi_off) + (warp - 4) * TC_WARP_BUF_FLOATS;
+  const uint64_t d_ones = ptx::make_smem_desc(base + p.ones_off, 0u, 1024u);
+  uint32_t s = 0, ph = 0;
+  int i = 0;
+  for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++i) {
+    const int z = t / tiles_ab, rem = t - z * tiles_ab;
+    const int nk = k_blocks(z);
+    if ((i & 1) != wg) {                                 // the other warpgroup's tile: skip its stages
+      const uint32_t adv = s + (uint32_t)nk;
+      ph ^= (adv / (uint32_t)p.num_stages) & 1u;
+      s = adv % (uint32_t)p.num_stages;
+      continue;
     }
+    const int ta = rem / p.num_b, tb = rem % p.num_b;
+    const int a0 = ta * TC_BM, b0 = tb * BN;
+    // warpgroup 0 goes first; afterwards each waits for the other to have issued its previous tile
+    ptx::mbar_wait(turn_mine, ((uint32_t)(i >> 1) & 1u) ^ (wg == 0 ? 1u : 0u));
+    float acc[2][BN / 2];
+    float accdb[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+    const bool do_db = MN && p.db != nullptr && tb == 0;
+    if (do_db)
+      mma_tile<MN, BN, MN>(p, acc, accdb, base, full0, empty0, turn_other, d_ones, nk, s, ph, lane);
+    else
+      mma_tile<MN, BN, false>(p, acc, accdb, base, full0, empty0, turn_other, d_ones, nk, s, ph, lane);
     if (do_db && (lane & 3) == 0) {
       // m64n8 layout: lane holds rows lane/4 and lane/4 + 8 of its warp's 16, columns 0-1 (all columns are equal)
-      const int64_t r = (int64_t)a0 + 64 * mw + 16 * (warp & 3) + (lane >> 2);
-      if (r < p.rows_a) p.db[(int64_t)z * p.rows_a + r] = accdb[0];
-      if (r + 8 < p.rows_a) p.db[(int64_t)z * p.rows_a + r + 8] = accdb[2];
-    }
-  }
-  __syncthreads();                      // every MMA has read its stage: the ring becomes the accumulator tile
-  float* const ctile = reinterpret_cast<float*>(gbase);
-  const int cp = (int)p.ctile_pitch;
-  if (warp >= 4) {
-    // m64nN layout: register 4j + 2h + e of block n is row 16 * (warp % 4) + lane / 4 + 8h, column 64n + 8j + 2 (lane % 4) + e
-    const int r = 64 * mw + 16 * (warp & 3) + (lane >> 2);
 #pragma unroll
-    for (int n = 0; n < NB; ++n)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int c = 64 * n + 8 * j + 2 * (lane & 3);
-        *reinterpret_cast<float2*>(ctile + r * cp + c) = make_float2(acc[n][4 * j], acc[n][4 * j + 1]);
-        *reinterpret_cast<float2*>(ctile + (r + 8) * cp + c) = make_float2(acc[n][4 * j + 2], acc[n][4 * j + 3]);
+      for (int h = 0; h < 2; ++h) {
+        const int64_t r = (int64_t)a0 + 64 * h + 16 * q + (lane >> 2);
+        if (r < p.rows_a) p.db[(int64_t)z * p.rows_a + r] = accdb[h][0];
+        if (r + 8 < p.rows_a) p.db[(int64_t)z * p.rows_a + r + 8] = accdb[h][2];
       }
-  }
-  __syncthreads();
-  if (warp < 4) return;
-
-  // -------------------------------------------------------------- epilogue: warp e takes rows 32 (e % 4) .. +31 and
-  // half e / 4 of the tile's columns; lane = row, 16 consecutive columns per chunk
-  const int e = warp - 4;
-  const int q = e & 3;
-  const int cw = BN / 2;                               // columns per warp (multiple of 16)
-  const int cbeg = (e >> 2) * cw, cend = cbeg + cw;
-  const int rl = q * 32 + lane;
-  const int64_t row = (int64_t)a0 + rl;
-  const int col0 = b0;
-  const bool row_ok = row < p.rows_a;
-  float* stage_scr = (EPI == EPI_F32 && p.f32_stage_off)
-                         ? reinterpret_cast<float*>(gbase + p.f32_stage_off) + e * 512
-                         : nullptr;
-  uint32_t codes[4] = {0u, 0u, 0u, 0u};
-  if (EPI == EPI_PLANES_BWD && row_ok) {
-    const uint32_t* cpp = p.code + row * p.code_pitch + ((col0 + cbeg) >> 4);
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-      if (cbeg + 16 * i < cend && col0 + cbeg + 16 * i < p.cols_b) codes[i] = __ldg(cpp + i);
-  }
-  uint32_t code_out[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-  for (int k = 0; k < cw / 16; ++k) {
-    const int c = cbeg + 16 * k;
-    uint32_t rr[16];
-    const float4* src = reinterpret_cast<const float4*>(ctile + rl * cp + c);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float4 f = src[i];
-      rr[4 * i] = __float_as_uint(f.x); rr[4 * i + 1] = __float_as_uint(f.y);
-      rr[4 * i + 2] = __float_as_uint(f.z); rr[4 * i + 3] = __float_as_uint(f.w);
     }
-    if (EPI == EPI_F32 && stage_scr != nullptr) {      // whole warp takes part; rows beyond rows_a masked at the store
-      if (col0 + c < p.cols_b) epilogue_f32_staged(p, rr, row - lane, lane, col0 + c, z, bias_s, stage_scr);
-    } else if (row_ok && col0 + c < p.cols_b) {
-      code_out[k] = epilogue_chunk16<EPI>(p, rr, row, col0 + c, z, bias_s, codes[k]);
-    }
-  }
-  if (EPI == EPI_PLANES_FWD && p.code != nullptr && row_ok) {
-    uint32_t* cpp = p.code + row * p.code_pitch + ((col0 + cbeg) >> 4);
-    if (cw == 64 && (p.code_pitch & 3) == 0) {
-      // whole 16-byte group inside the (4-word padded) row: one vector store
-      *reinterpret_cast<uint4*>(cpp) = make_uint4(code_out[0], code_out[1], code_out[2], code_out[3]);
-    } else {
+    // ------------------------------------------------------------ epilogue.  Warp q holds rows 16q .. 16q + 15 of
+    // both 64-row blocks; per 16-column chunk its fragments go through the warp's own shared-memory buffer
+    // [32][TC_WARP_PITCH] (lane l = row warp_row(a0 + 16q, l)) so that each lane owns 16 consecutive columns of one row.
+    const int64_t row0 = (int64_t)a0 + 16 * q;
+    const int64_t row = warp_row(row0, lane);
+    const bool row_ok = row < p.rows_a;
+    uint32_t codes[BN / 16];
+    uint32_t code_out[BN / 16];
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
-        if (cbeg + 16 * i < cend && col0 + cbeg + 16 * i < p.cols_b) cpp[i] = code_out[i];
+    for (int k = 0; k < BN / 16; ++k) {
+      codes[k] = code_out[k] = 0u;
+      if (EPI == EPI_PLANES_BWD && row_ok && b0 + 16 * k < p.cols_b)
+        codes[k] = __ldg(p.code + row * p.code_pitch + ((b0 + 16 * k) >> 4));
+    }
+#pragma unroll
+    for (int k = 0; k < BN / 16; ++k) {
+      __syncwarp();                                      // the previous chunk has been read out of the buffer
+      // m64nN layout: register 4j + 2g + e is row 16q + lane / 4 + 8g, column 8j + 2 (lane % 4) + e
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj) {
+          const int j = 2 * k + jj;
+          float* w = wbuf + (16 * h + (lane >> 2)) * TC_WARP_PITCH + 8 * jj + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(w) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+          *reinterpret_cast<float2*>(w + 8 * TC_WARP_PITCH) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+        }
+      __syncwarp();
+      uint32_t rr[16];
+      const float4* src = reinterpret_cast<const float4*>(wbuf + lane * TC_WARP_PITCH);
+#pragma unroll
+      for (int m = 0; m < 4; ++m) {
+        const float4 f = src[m];
+        rr[4 * m] = __float_as_uint(f.x); rr[4 * m + 1] = __float_as_uint(f.y);
+        rr[4 * m + 2] = __float_as_uint(f.z); rr[4 * m + 3] = __float_as_uint(f.w);
+      }
+      const int col = b0 + 16 * k;
+      if (EPI == EPI_F32 && p.f32_stage) {             // whole warp takes part; rows beyond rows_a masked at the store
+        __syncwarp();                                    // the buffer becomes the transpose scratch
+        if (col < p.cols_b) epilogue_f32_staged(p, rr, row0, lane, col, z, bias_s, wbuf);
+      } else if (row_ok && col < p.cols_b) {
+        code_out[k] = epilogue_chunk16<EPI>(p, rr, row, col, z, bias_s, codes[k]);
+      }
+    }
+    if (EPI == EPI_PLANES_FWD && p.code != nullptr && row_ok) {
+      uint32_t* cpp = p.code + row * p.code_pitch + (b0 >> 4);
+      bool vec = false;
+      if constexpr (BN == 128) {
+        vec = (p.code_pitch & 3) == 0;
+        if (vec) {
+          // whole 16-byte groups inside the (4-word padded) row: vector stores
+          reinterpret_cast<uint4*>(cpp)[0] = make_uint4(code_out[0], code_out[1], code_out[2], code_out[3]);
+          reinterpret_cast<uint4*>(cpp)[1] = make_uint4(code_out[4], code_out[5], code_out[6], code_out[7]);
+        }
+      }
+      if (!vec) {
+#pragma unroll
+        for (int k = 0; k < BN / 16; ++k)
+          if (b0 + 16 * k < p.cols_b) cpp[k] = code_out[k];
+      }
     }
   }
 }
@@ -697,23 +760,18 @@ static int use_pdl() {
   return v;
 }
 
-// Shared-memory plan of one launch (offsets from the 1024-aligned base): as many stages as fit, the ring re-used after
-// the reduction for the accumulator tile [TC_BM][bn + 8] (the padding spreads the fragment stores over all banks) and
-// the fp32 transpose scratch; then the ones tile, the bias vector and the mbarriers.  Returns the dynamic smem bytes.
+// Shared-memory plan of one launch (offsets from the 1024-aligned base): as many ring stages as fit next to the 8
+// per-warp epilogue buffers (20 KB), the ones tile, the bias vector and the mbarriers.  Returns the dynamic smem bytes.
 static size_t plan_smem(GemmParams& p, const EpiArgs& e) {
-  const uint32_t fixed = 1024 + TC_ONES_SMEM + TC_BIAS_SMEM + 256;
+  p.f32_stage = (use_f32_stage() && e.epi == EPI_F32 && !p.vec_ok && p.C) ? 1 : 0;
+  const uint32_t epi = 2 * TC_WG_WARPS * TC_WARP_BUF_FLOATS * 4;
+  const uint32_t fixed = 1024 + epi + TC_ONES_SMEM + TC_BIAS_SMEM + 256;
   p.num_stages = (int)((TC_SMEM_MAX - fixed) / p.stage_bytes);
   if (p.num_stages > TC_MAX_STAGES) p.num_stages = TC_MAX_STAGES;
-  p.ctile_pitch = (uint32_t)p.bn + 8;
-  const uint32_t ctile = (uint32_t)TC_BM * p.ctile_pitch * 4;
-  const bool stage_f32 = use_f32_stage() && e.epi == EPI_F32 && !p.vec_ok && p.C;
-  p.f32_stage_off = stage_f32 ? ctile : 0u;
-  uint32_t ring = (uint32_t)p.num_stages * p.stage_bytes;
-  const uint32_t epi = ctile + (stage_f32 ? TC_F32_STAGE_SMEM : 0u);
-  if (ring < epi) ring = (epi + 1023) / 1024 * 1024;
-  p.ones_off = ring;
-  p.bias_off = (e.bias && (size_t)p.num_b * p.bn * sizeof(float) <= TC_BIAS_SMEM) ? ring + TC_ONES_SMEM : 0u;
-  p.bar_off = ring + TC_ONES_SMEM + TC_BIAS_SMEM;
+  p.epi_off = (uint32_t)p.num_stages * p.stage_bytes;
+  p.ones_off = p.epi_off + epi;
+  p.bias_off = (e.bias && (size_t)p.num_b * p.bn * sizeof(float) <= TC_BIAS_SMEM) ? p.ones_off + TC_ONES_SMEM : 0u;
+  p.bar_off = p.ones_off + TC_ONES_SMEM + TC_BIAS_SMEM;
   return (size_t)p.bar_off + 256 + 1024;
 }
 
@@ -722,6 +780,11 @@ static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const C
                          const CUtensorMap& mBl, const GemmParams& p, size_t smem, cudaStream_t st) {
   if (smem > TC_SMEM_MAX) {
     set_error("gemm: shared-memory plan of %zu bytes exceeds %u", smem, TC_SMEM_MAX);
+    return GANTTS_E_UNSUPPORTED;
+  }
+  if (p.num_stages < 2) {
+    // a stage is released only after the next one has been issued: one stage would never be refilled
+    set_error("gemm: shared-memory plan leaves %d ring stage(s), the mainloop needs 2", p.num_stages);
     return GANTTS_E_UNSUPPORTED;
   }
   // the opt-in is per device (and context): remember it per device ordinal, not per process
@@ -733,9 +796,10 @@ static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const C
     if (dev >= 0 && dev < 64) attr[dev] = true;
   }
   const int tiles = p.num_a * p.num_b * p.num_z;
+  const int grid = tiles < num_sms() ? tiles : num_sms();
   prof_begin(MN ? PROF_GEMM_MN : PROF_GEMM_KK, 2.0 * (double)p.rows_a * p.cols_b * (double)p.red, st);
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)tiles);
+  cfg.gridDim = dim3((unsigned)grid);
   cfg.blockDim = dim3(TC_THREADS);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
@@ -768,9 +832,8 @@ static int launch_gemm_kk_one(const Planes& A, const Planes& B, const EpiArgs& e
     set_error("gemm_kk: reduction extents differ (%lld vs %lld)", (long long)A.cols, (long long)B.cols);
     return GANTTS_E_BADARG;
   }
-  p.bk = 64;                                               // one 128-byte swizzled row of K per stage
   p.a_plane = TC_BM * 128u;
-  p.red_chunk = (p.red + p.bk - 1) / p.bk * p.bk;
+  p.red_chunk = (p.red + TC_KK_BK - 1) / TC_KK_BK * TC_KK_BK;
   p.bn = pick_bn(p.cols_b, bn_cap);
   p.num_a = (int)((p.rows_a + TC_BM - 1) / TC_BM);
   p.num_b = (p.cols_b + p.bn - 1) / p.bn;
@@ -796,7 +859,7 @@ static int launch_gemm_kk_one(const Planes& A, const Planes& B, const EpiArgs& e
   return GANTTS_E_BADARG;
 }
 
-// Tail balancing, OPT-IN (GANTTS_B200_TAIL=1).  One CTA per SM runs a tile at a time, so a launch takes whole waves
+// Tail balancing, OPT-IN (GANTTS_B200_TAIL=1).  Each SM works through whole tiles, so a launch takes whole rounds
 // of tiles.  The rows of an incomplete last wave are cut off and given to a SECOND launch with narrower column tiles
 // (BN/2) so that they spread over more SMs.  The extra launch's fill and drain usually cost more than the part of a
 // wave it saves, so it stays off.
@@ -847,7 +910,6 @@ static int launch_gemm_kk(const Planes& A, const Planes& B, const EpiArgs& e, cu
 
 // C[n][k] (+)= sum_m A[m][n] * B[m][k]  (MN-major planes A [red][rows_a], B [red][cols_b]);
 // split over the reduction, partials in `partial`, reduced deterministically into C (ld = cols_b).
-constexpr int TC_MN_BK = 32;        // reduction rows per stage of the weight-gradient GEMM
 static size_t mn_partial_bytes(int64_t red, int rows_a, int cols_b, int* splits_out, int64_t* chunk_out) {
   int bn = pick_bn(cols_b);
   int tiles = ((rows_a + TC_BM - 1) / TC_BM) * ((cols_b + bn - 1) / bn);
@@ -970,8 +1032,7 @@ static int launch_gemm_mn(const Planes& A, const Planes& B, float* C, float* gb,
   p.bn = pick_bn(p.cols_b);
   p.num_a = (int)((p.rows_a + TC_BM - 1) / TC_BM);
   p.num_b = (p.cols_b + p.bn - 1) / p.bn;
-  p.bk = TC_MN_BK;
-  p.atom_bytes = (uint32_t)p.bk * 128;                      // [bk reduction rows][128 B of 64 MN elements]
+  p.atom_bytes = (uint32_t)TC_MN_BK * 128;                  // [bk reduction rows][128 B of 64 MN elements]
   p.a_plane = (TC_BM / 64) * p.atom_bytes;
   p.b_plane_bytes = (uint32_t)(p.bn / 64) * p.atom_bytes;
   p.stage_bytes = 2 * p.a_plane + 2 * p.b_plane_bytes;
@@ -989,10 +1050,10 @@ static int launch_gemm_mn(const Planes& A, const Planes& B, float* C, float* gb,
   const size_t smem = plan_smem(p, e);
   CUtensorMap mAh, mAl, mBh, mBl;
   int rc;
-  if ((rc = make_map(&mAh, A.hi, A.rows, A.cols, A.pitch, p.bk))) return rc;
-  if ((rc = make_map(&mAl, A.lo, A.rows, A.cols, A.pitch, p.bk))) return rc;
-  if ((rc = make_map(&mBh, B.hi, B.rows, B.cols, B.pitch, p.bk))) return rc;
-  if ((rc = make_map(&mBl, B.lo, B.rows, B.cols, B.pitch, p.bk))) return rc;
+  if ((rc = make_map(&mAh, A.hi, A.rows, A.cols, A.pitch, TC_MN_BK))) return rc;
+  if ((rc = make_map(&mAl, A.lo, A.rows, A.cols, A.pitch, TC_MN_BK))) return rc;
+  if ((rc = make_map(&mBh, B.hi, B.rows, B.cols, B.pitch, TC_MN_BK))) return rc;
+  if ((rc = make_map(&mBl, B.lo, B.rows, B.cols, B.pitch, TC_MN_BK))) return rc;
   if ((rc = launch_bn<true, EPI_F32>(mAh, mAl, mBh, mBl, p, smem, st))) return rc;
   if (!direct) {
     if (defer && defer->n + 2 <= REDUCE_MAX_JOBS) {

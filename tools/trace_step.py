@@ -1,0 +1,122 @@
+"""Per-launch view of one fused GAN step under torch.profiler (CUDA activities).
+
+    python tools/trace_step.py [--workload cfg2] [--warmup 10] [--steps 3] [--out FILE.md]
+
+Runs `--warmup` fused steps, then `--steps` more under the profiler with a synchronise after each, and splits the
+kernel list into steps (every step launches the same kernels).  Writes the launch list of the middle step in launch
+order with each kernel's duration.  The tensor-core GEMM launches are labelled with their shapes (the per-kind launch
+order in tools/per_launch.py) and get their executed TFLOP/s (3 x 2MNK for the bf16x3 split) and share of the step.
+Tracing adds host overhead between launches, so the step span here is not a bench value; compare kernel times and
+shares, and take step times from bench.py.
+"""
+import argparse
+import os
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+import bench  # noqa: E402
+from per_launch import KK, MN  # noqa: E402
+
+
+def short(name):
+    n = name.replace("gantts::", "").replace("void ", "")
+    cut = n.find("(")
+    return n[:cut] if cut > 0 else n
+
+
+def label_gemms(kernels, scale):
+    """kernels: [(name, us)] of one step -> [(name, us, label, executed flops or None)]."""
+    kk = list(KK)
+    mn = list(MN)
+    out = []
+    for name, us in kernels:
+        n = short(name)
+        label, flops = "", None
+        if n.startswith("gemm_bf16x3_kernel<"):
+            is_mn = n.startswith("gemm_bf16x3_kernel<true") or n.startswith("gemm_bf16x3_kernel<1")
+            queue = mn if is_mn else kk
+            if queue:
+                ent = queue.pop(0)
+                label, rows, N, K = ent[0], ent[1] * scale, ent[2], ent[3]
+                flops = 3.0 * 2.0 * rows * N * K
+                label = "%s [%d x %d x %d]" % (label, rows, N, K)
+            else:
+                label = "(unlabelled GEMM)"
+        out.append((n, us, label, flops))
+    return out, len(kk) + len(mn)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", default="cfg2", choices=[k for k, v in bench.WORKLOADS.items() if v["kind"] == "mlp"])
+    ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=3)
+    ap.add_argument("--out", default=None, help="markdown file for the launch list (default: stdout only)")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("trace_step.py: no CUDA device")
+    import __graft_entry__
+    __graft_entry__.build()
+    from gantts_b200 import fused, step as gstep
+    from torch.profiler import ProfilerActivity, profile
+
+    dev = torch.device("cuda", 0)
+    w = bench.WORKLOADS[args.workload]
+    torch.manual_seed(1234)
+    mg, md = bench.build_models(w, dev)
+    hpd = w["hp"]
+    hp = gstep.HParams(windows=bench.WINDOWS, stream_sizes=hpd["stream_sizes"],
+                       has_dynamic_features=hpd["has_dynamic_features"], adversarial_streams=hpd["adversarial_streams"],
+                       mask_nth_mgc_for_adv_loss=hpd["mask_nth_mgc_for_adv_loss"],
+                       discriminator_linguistic_condition=False)
+    fs = fused.FusedGanStep(mg, md, hp, w["B"], w["T"], w_d=1.0, mse_w=0.0, mge_w=1.0)
+    lengths = torch.full((w["B"],), w["T"], dtype=torch.int64, device=dev)
+    batches = [(x.to(dev), y.to(dev)) for x, y in bench.make_batches(w, 1234, bench.NUM_BATCHES, pinned=False)]
+    frames = w["B"] * w["T"]
+    for i in range(args.warmup):
+        fs.step(*batches[i % len(batches)], lengths, frames=frames)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for i in range(args.steps):
+            fs.step(*batches[i % len(batches)], lengths, frames=frames)
+            torch.cuda.synchronize()
+    evs = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
+           and not e.name.startswith(("Memcpy", "Memset", "[memory]"))]
+    evs.sort(key=lambda e: e.time_range.start)
+    if not evs or len(evs) % args.steps:
+        raise SystemExit("trace_step.py: %d kernels over %d steps do not split into equal steps" % (len(evs), args.steps))
+    per = len(evs) // args.steps
+    mid = evs[per * (args.steps // 2): per * (args.steps // 2 + 1)]
+    kernels = [(e.name, e.time_range.end - e.time_range.start) for e in mid]
+    span = mid[-1].time_range.end - mid[0].time_range.start
+    rows, unmatched = label_gemms(kernels, w["B"] * w["T"] // 32000)
+    tot = sum(us for _, us, _, _ in rows)
+    gemm_us = sum(us for _, us, _, f in rows if f is not None)
+    gemm_fl = sum(f for _, _, _, f in rows if f is not None)
+    lines = ["# Launch list of one fused %s step (torch.profiler, CUDA activities; step %d of %d after %d warm-up)"
+             % (args.workload, args.steps // 2 + 1, args.steps, args.warmup), "",
+             "Device: %s.  %d launches, %.1f us of kernel time, %.1f us from first start to last end (traced: host "
+             "overhead between launches is not a bench value)." % (torch.cuda.get_device_name(0), per, tot, span), "",
+             "| # | kernel | GEMM | us | executed TFLOP/s | share of kernel time |", "|---|---|---|---|---|---|"]
+    for i, (n, us, label, fl) in enumerate(rows):
+        tf = "%.0f" % (fl / (us * 1e-6) / 1e12) if fl and us else ""
+        lines.append("| %d | `%s` | %s | %.1f | %s | %.3f |" % (i, n[:60], label, us, tf, us / tot if tot else 0.0))
+    lines += ["", "GEMM launches: %d, %.1f us = %.3f of kernel time, %.0f TFLOP/s executed (bf16x3 = 3 x 2MNK)."
+              % (sum(1 for r in rows if r[3] is not None), gemm_us, gemm_us / tot if tot else 0.0,
+                 gemm_fl / (gemm_us * 1e-6) / 1e12 if gemm_us else 0.0)]
+    if unmatched:
+        lines.append("%d GEMM labels unused: the launch structure differs from tools/per_launch.py." % unmatched)
+    text = "\n".join(lines) + "\n"
+    print(text)
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        with open(args.out, "w") as f:
+            f.write(text)
+
+
+if __name__ == "__main__":
+    main()
