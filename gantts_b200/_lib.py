@@ -63,6 +63,13 @@ class MlpT(ctypes.Structure):
 MAX_COLS = 256
 
 
+class HighwayT(ctypes.Structure):
+    _fields_ = [("static_dim", ctypes.c_int),
+                ("W", ctypes.c_void_p), ("b", ctypes.c_void_p),
+                ("sumW", ctypes.c_void_p), ("sumb", ctypes.c_void_p),
+                ("sqW", ctypes.c_void_p), ("sqb", ctypes.c_void_p)]
+
+
 class GanStepT(ctypes.Structure):
     _fields_ = [("B", ctypes.c_int), ("T", ctypes.c_int),
                 ("g", MlpT), ("d", MlpT),
@@ -81,7 +88,8 @@ class GanStepT(ctypes.Structure):
                 ("optimizer", ctypes.c_int), ("beta1", ctypes.c_float), ("beta2", ctypes.c_float),
                 ("opt_step", ctypes.c_int64),
                 ("g_sqW", ctypes.c_void_p * MAX_LAYERS), ("g_sqb", ctypes.c_void_p * MAX_LAYERS),
-                ("d_sqW", ctypes.c_void_p * MAX_LAYERS), ("d_sqb", ctypes.c_void_p * MAX_LAYERS)]
+                ("d_sqW", ctypes.c_void_p * MAX_LAYERS), ("d_sqb", ctypes.c_void_p * MAX_LAYERS),
+                ("highway", HighwayT)]
 
 
 OPT_ADAGRAD, OPT_ADAM = 0, 1

@@ -318,13 +318,15 @@ static inline int blocks_1d(int64_t work, int per_block) {
   return (int)b;
 }
 
+constexpr int MAX_PARAMS = 2 * GANTTS_MAX_LAYERS + 2;     // + the highway gate's weight and bias
+
 struct ParamList {
   int n;
-  float* p[2 * GANTTS_MAX_LAYERS];
-  float* g[2 * GANTTS_MAX_LAYERS];
-  float* s[2 * GANTTS_MAX_LAYERS];
-  float* s2[2 * GANTTS_MAX_LAYERS];                     // Adam: exp_avg_sq (null for Adagrad)
-  int64_t sizes[2 * GANTTS_MAX_LAYERS];
+  float* p[MAX_PARAMS];
+  float* g[MAX_PARAMS];
+  float* s[MAX_PARAMS];
+  float* s2[MAX_PARAMS];                                // Adam: exp_avg_sq (null for Adagrad)
+  int64_t sizes[MAX_PARAMS];
   float* gW[GANTTS_MAX_LAYERS];
   float* gb[GANTTS_MAX_LAYERS];
   int64_t total;
@@ -352,6 +354,12 @@ struct StepLayout {
   size_t mlp_ws_bytes;
   RedWs* red;             // [R_COUNT] deferred loss partials
   float* opt_partial;     // [OPT_MAX_BLOCKS] sum-of-squares partials of the model being stepped
+  // highway generator only (zero bytes otherwise, so the plain MLP layout is unchanged)
+  float* hw_tx;           // [M][S] gate sigmoid(x_s W_T^T + b_T)
+  float* hw_gx;           // [M][S] MLPG output Gx
+  char* hw_w;             // planes of W_T [S][S]
+  char* hw_dz;            // planes of dz [M][S]
+  float* hw_partial;      // split-K partials of dW_T / db_T
   size_t total;
 };
 
@@ -359,6 +367,12 @@ static int64_t mlp_param_count(const gantts_mlp_t& m) {
   int64_t n = 0;
   for (int l = 0; l < m.num_layers; ++l) n += (int64_t)m.dims[l + 1] * m.dims[l] + m.dims[l + 1];
   return n;
+}
+
+// elements of the highway gate's parameters, which lead the generator's flat gradient buffer
+static int64_t gate_param_count(const gantts_gan_step_t* c) {
+  const int64_t S = c->highway.static_dim;
+  return S * S + S;
 }
 
 static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
@@ -375,7 +389,7 @@ static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
   L->y_static = (float*)take((size_t)M * c->n_static * sizeof(float));
   L->g_static = (float*)take((size_t)M * c->n_static * sizeof(float));
   L->g_yhat = (float*)take((size_t)M * c->g.dims[c->g.num_layers] * sizeof(float));
-  L->g_grads = (float*)take(mlp_param_count(c->g) * sizeof(float));
+  L->g_grads = (float*)take((gate_param_count(c) + mlp_param_count(c->g)) * sizeof(float));
   L->d_grads = (float*)take(mlp_param_count(c->d) * sizeof(float));
   L->g_tape_bytes = gantts_mlp_tape_bytes(&c->g, M);
   L->g_tape = take(L->g_tape_bytes);
@@ -386,13 +400,19 @@ static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
   L->mlp_ws = take(L->mlp_ws_bytes);
   L->red = (RedWs*)take(R_COUNT * sizeof(RedWs));
   L->opt_partial = (float*)take(OPT_MAX_BLOCKS * sizeof(float));
+  const int S = c->highway.static_dim;
+  const bool hw = S > 0;
+  L->hw_tx = (float*)take(hw ? (size_t)M * S * sizeof(float) : 0);
+  L->hw_gx = (float*)take(hw ? (size_t)M * S * sizeof(float) : 0);
+  L->hw_w = take(hw ? 2 * plane_bytes(S, S) : 0);
+  L->hw_dz = take(hw ? 2 * plane_bytes(M, S) : 0);
+  L->hw_partial = (float*)take(hw ? mn_partial_bytes(M, S, S, nullptr, nullptr) : 0);
   L->total = (size_t)(cur - base) + 256;
 }
 
+// appends the layers of m; `flat` is where their gradients start in the model's flat buffer
 static void param_list(const gantts_mlp_t& m, float* const* sumW, float* const* sumb, float* const* sqW, float* const* sqb,
                        float* flat, ParamList* pl) {
-  pl->n = 0;
-  pl->total = 0;
   float* cur = flat;
   for (int l = 0; l < m.num_layers; ++l) {
     const int64_t nw = (int64_t)m.dims[l + 1] * m.dims[l], nb = m.dims[l + 1];
@@ -411,7 +431,30 @@ static void param_list(const gantts_mlp_t& m, float* const* sumW, float* const* 
     pl->sizes[pl->n++] = nb;
     cur += nb;
   }
-  pl->total = cur - flat;
+  pl->total += cur - flat;
+}
+
+// generator parameters in model.parameters() order: [T.weight, T.bias] of a highway generator, then the MLP layers
+static void g_param_list(const gantts_gan_step_t* c, float* flat, ParamList* pl) {
+  pl->n = 0;
+  pl->total = 0;
+  const gantts_highway_t& h = c->highway;
+  if (h.static_dim > 0) {
+    const int64_t S = h.static_dim;
+    const int64_t sizes[2] = {S * S, S};
+    float* const ps[2] = {const_cast<float*>(h.W), const_cast<float*>(h.b)};
+    float* const ss[2] = {h.sumW, h.sumb};
+    float* const qs[2] = {h.sqW, h.sqb};
+    for (int i = 0; i < 2; ++i) {
+      pl->p[pl->n] = ps[i];
+      pl->g[pl->n] = flat + pl->total;
+      pl->s[pl->n] = ss[i];
+      pl->s2[pl->n] = qs[i];
+      pl->sizes[pl->n++] = sizes[i];
+      pl->total += sizes[i];
+    }
+  }
+  param_list(c->g, c->g_sumW, c->g_sumb, c->g_sqW, c->g_sqb, flat + pl->total, pl);
 }
 
 static inline int bce_blocks(int64_t rows) { return grid_for(rows, RED_THREADS); }
@@ -483,7 +526,63 @@ static int check_step(const gantts_gan_step_t* c) {
   }
   GANTTS_CHECK_ARG(c->g.last_act == GANTTS_ACT_NONE, "gan_step: generator must have a linear output");
   GANTTS_CHECK_ARG(c->mlpg_table, "gan_step: null MLPG table");
+  const gantts_highway_t& h = c->highway;
+  GANTTS_CHECK_ARG(h.static_dim >= 0, "gan_step: negative highway static_dim");
+  if (h.static_dim > 0) {
+    // the arithmetic of In2OutHighwayNet (models.py:54-69): x_s and y_hat_static are the same S columns, and the
+    // generator's output is the S static columns of one dynamic stream followed by their delta windows
+    const int S = h.static_dim, nw = c->windows.n, Lg = c->g.num_layers;
+    const gantts_streams_t& st = c->streams;
+    GANTTS_CHECK_ARG(st.n == 1 && st.dyn[0] && st.in_start[0] == 0 && st.out_start[0] == 0 && st.sd[0] == S,
+                     "gan_step: a highway generator needs exactly one dynamic stream with in_start = out_start = 0 and "
+                     "sd = static_dim = %d (got %d stream(s), first sd %d)", S, st.n, st.sd[0]);
+    GANTTS_CHECK_ARG(c->n_static == S, "gan_step: highway static_dim %d != n_static %d", S, c->n_static);
+    GANTTS_CHECK_ARG(c->g.dims[0] >= S, "gan_step: highway generator input width %d < static_dim %d", c->g.dims[0], S);
+    GANTTS_CHECK_ARG(c->g.dims[Lg] == nw * S, "gan_step: highway generator output width %d != %d windows x static_dim %d",
+                     c->g.dims[Lg], nw, S);
+    GANTTS_CHECK_ARG(h.W && h.b, "gan_step: null highway gate weight/bias");
+    GANTTS_CHECK_ARG((reinterpret_cast<uintptr_t>(h.b) & 15) == 0, "gan_step: highway gate bias must be 16-byte aligned");
+    GANTTS_CHECK_ARG(h.sumW && h.sumb, "gan_step: null highway gate optimiser state");
+    if (c->optimizer == GANTTS_OPT_ADAM)
+      GANTTS_CHECK_ARG(h.sqW && h.sqb, "gan_step: Adam needs exp_avg_sq for the highway gate");
+  }
   return GANTTS_OK;
+}
+
+// Tx = sigmoid(x_s W_T^T + b_T): the generator's input planes on its tape (written by its forward) with the first S
+// columns as the operand, so x is not converted twice.
+static int highway_gate_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, int64_t M,
+                            cudaStream_t st) {
+  const int S = c->highway.static_dim;
+  Planes xs;
+  int rc = mlp_tape_input_planes(&g, M, L.g_tape, L.g_tape_bytes, &xs);
+  if (rc) return rc;
+  xs.cols = S;
+  char* cur = L.hw_w;
+  const Planes w = carve_planes(cur, S, S);
+  if ((rc = launch_split(c->highway.W, S, S, S, w, 0, st))) return rc;
+  EpiArgs e;
+  e.epi = EPI_F32;
+  e.C = L.hw_tx;
+  e.ldc = S;
+  e.bias = c->highway.b;
+  e.act = GANTTS_ACT_SIGMOID;
+  return launch_gemm_kk(xs, w, e, st);
+}
+
+// dW_T = dz^T x_s and db_T = colsum(dz) (ones-tile MMA) into the first S * S + S entries of the generator's buffer
+static int highway_gate_bwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, int64_t M,
+                            cudaStream_t st) {
+  const int S = c->highway.static_dim;
+  Planes xs;
+  int rc = mlp_tape_input_planes(&g, M, L.g_tape, L.g_tape_bytes, &xs);
+  if (rc) return rc;
+  xs.cols = S;
+  char* cur = L.hw_dz;
+  const Planes dz = carve_planes(cur, M, S);
+  ReduceList rl;
+  if ((rc = launch_gemm_mn(dz, xs, L.g_grads, L.g_grads + (int64_t)S * S, 0, L.hw_partial, st, &rl))) return rc;
+  return flush_reduce(rl, 0, st);
 }
 
 }  // namespace gantts
@@ -507,7 +606,7 @@ extern "C" int gantts_gan_step_grad_buffer(const gantts_gan_step_t* c, void* wor
   StepLayout L;
   layout(c, reinterpret_cast<char*>(al256(reinterpret_cast<uintptr_t>(workspace))), &L);
   *ptr = which == 0 ? L.g_grads : L.d_grads;
-  *count = mlp_param_count(which == 0 ? c->g : c->d);
+  *count = which == 0 ? gate_param_count(c) + mlp_param_count(c->g) : mlp_param_count(c->d);
   return GANTTS_OK;
 }
 
@@ -536,8 +635,26 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
   const int cond_w = (has_d && c->d_conditioned) ? d_in : 0;
   const int nA = dD - cond_w;
   ParamList pg, pd;
-  param_list(c->g, c->g_sumW, c->g_sumb, c->g_sqW, c->g_sqb, L.g_grads, &pg);
+  g_param_list(c, L.g_grads, &pg);
+  pd.n = 0;
+  pd.total = 0;
   if (has_d) param_list(c->d, c->d_sumW, c->d_sumb, c->d_sqW, c->d_sqb, L.d_grads, &pd);
+  // In2OutHighwayNet: gate + combine around the MLPG (x_s = the first S columns of x)
+  const bool hw = c->highway.static_dim > 0;
+  HighwayArgs hwa{};
+  if (hw) {
+    char* cur = L.hw_dz;
+    const Planes dz = carve_planes(cur, M, nS);
+    hwa.x = x;
+    hwa.x_rs = d_in;
+    hwa.tx = L.hw_tx;
+    hwa.gx = L.hw_gx;
+    hwa.dz_hi = dz.hi;
+    hwa.dz_lo = dz.lo;
+    hwa.dz_pitch = dz.pitch;
+    hwa.S = nS;
+  }
+  const HighwayArgs* hwp = hw ? &hwa : nullptr;
   ColList static_cols, adv_cols;
   static_cols.n = c->n_static_cols;
   for (int i = 0; i < c->n_static_cols; ++i) static_cols.c[i] = c->static_cols[i];
@@ -571,8 +688,9 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
       GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(y_static)");
     }
     if ((rc = gantts_mlp_fwd(&g, x, d_in, M, y_hat, d_out, L.g_tape, L.g_tape_bytes, stream))) return rc;
-    if ((rc = gantts_mlpg_fwd(y_hat, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
-                              c->mlpg_table, &c->streams, &c->windows, c->B, c->T, stream)))
+    if (hw && (rc = highway_gate_fwd(c, g, L, M, st))) return rc;
+    if ((rc = mlpg_fwd_impl(y_hat, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
+                            c->mlpg_table, &c->streams, &c->windows, c->B, c->T, stream, hwp)))
       return rc;
     if (has_d) {
       gather_cols_list_kernel<<<blocks_1d(M * nA, 1024), 256, 0, st>>>(L.y_static, nS, L.d_in + cond_w, dD, adv_cols,
@@ -622,8 +740,9 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
     }
     // ---- apply_generator (train.py:336-355): G forward + MLPG
     if ((rc = gantts_mlp_fwd(&g, x, d_in, M, y_hat, d_out, L.g_tape, L.g_tape_bytes, stream))) return rc;
-    if ((rc = gantts_mlpg_fwd(y_hat, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
-                              c->mlpg_table, &c->streams, &c->windows, c->B, c->T, stream)))
+    if (hw && (rc = highway_gate_fwd(c, g, L, M, st))) return rc;
+    if ((rc = mlpg_fwd_impl(y_hat, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
+                            c->mlpg_table, &c->streams, &c->windows, c->B, c->T, stream, hwp)))
       return rc;
     // MGE loss (train.py:291) and its gradient in one pass; the gradient INITIALISES g_static, the two discriminator
     // passes then accumulate their input gradients on top of it
@@ -725,14 +844,16 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
       Planes gp;
       if ((rc = mlp_bwd_gy_planes(&g, M, L.mlp_ws, L.mlp_ws_bytes, &gp))) return rc;
       rc = mlpg_bwd_planes(L.g_static, (int64_t)c->T * nS, nS, gp.hi, gp.lo, gp.pitch, c->mlpg_table, &c->streams,
-                           &c->windows, c->B, c->T, stream);
+                           &c->windows, c->B, c->T, stream, hwp);
       if (rc == GANTTS_OK) direct = true;
       else if (rc != GANTTS_E_UNSUPPORTED) return rc;
     }
+    // (highway: the adjoint solves with Tx * g_static and leaves dz for the gate's weight gradient)
     if (!direct &&
-        (rc = gantts_mlpg_bwd(L.g_static, (int64_t)c->T * nS, nS, L.g_yhat, (int64_t)c->T * d_out, d_out, c->mlpg_table,
-                              &c->streams, &c->windows, c->B, c->T, c->mse_w != 0.f ? 1 : 0, stream)))
+        (rc = mlpg_bwd_impl(L.g_static, (int64_t)c->T * nS, nS, L.g_yhat, (int64_t)c->T * d_out, d_out, c->mlpg_table,
+                            &c->streams, &c->windows, c->B, c->T, c->mse_w != 0.f ? 1 : 0, stream, hwp)))
       return rc;
+    if (hw && (rc = highway_gate_bwd(c, g, L, M, st))) return rc;
     if ((rc = mlp_bwd_impl(&g, direct ? nullptr : L.g_yhat, d_out, nullptr, 0, M, L.g_tape, L.g_tape_bytes, nullptr, 0, 0,
                            pg.gW, pg.gb, 0, L.mlp_ws, L.mlp_ws_bytes, stream, -1, direct)))
       return rc;

@@ -986,7 +986,9 @@ __global__ void __launch_bounds__(32 * MR_WARPS) multi_reduce_kernel(ReduceList 
         t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
       }
       float* out = rl.out[j];
-      if (vec) {
+      // the flat gradient buffers need not be 16-byte aligned per tensor (a highway generator's gate shifts the
+      // stack's gradients by S * S + S floats): vector stores only where the output allows them
+      if (vec && (reinterpret_cast<uintptr_t>(out) & 15) == 0) {
         float4* o = reinterpret_cast<float4*>(out + e);
         if (accumulate) { const float4 c = *o; t.x += c.x; t.y += c.y; t.z += c.z; t.w += c.w; }
         *o = t;

@@ -272,6 +272,57 @@ constexpr int SOLVE_WARPS = 4;         // the warps of a block work on the SAME 
 constexpr int SOLVE_ZROWS = SC + 4 + 2 * SW;                        // strip rows per warp (backward: [t0-2, t1+2) + warm-up)
 constexpr int SOLVE_SMEM_FLOATS = SOLVE_ZROWS * 8 + SOLVE_WARPS * SOLVE_ZROWS * 32;   // Cholesky rows of the chunk + 4 strips
 
+// In2OutHighwayNet's combine around the MLPG of the fused step (gantts_highway_t): one dynamic stream whose output column
+// c is static column c, rows r = b * T + t.  Forward: y_hat_static = x_s + Tx * Gx, Gx kept for the backward.  Backward:
+// the adjoint solves with Tx * g, and dz = g * Gx * Tx * (1 - Tx) leaves as the bf16 hi/lo planes of the gate's
+// weight-gradient GEMM.  Separate roundings (no FMA contraction) as in the reference's eager arithmetic.
+struct HighwayArgs {
+  const float* x;                      // generator input; x_s = its first S columns
+  int64_t x_rs;
+  const float* tx;                     // [B*T][S] gate
+  float* gx;                           // [B*T][S] MLPG output
+  __nv_bfloat16 *dz_hi, *dz_lo;        // [B*T][dz_pitch]
+  int64_t dz_pitch;
+  int S;
+};
+
+__device__ __forceinline__ float highway_out(const HighwayArgs& hw, int64_t r, int c, float gxv) {
+  return __fadd_rn(hw.x[r * hw.x_rs + c], __fmul_rn(hw.tx[r * hw.S + c], gxv));
+}
+
+__device__ __forceinline__ void highway_dz(const HighwayArgs& hw, int64_t r, int c, float g) {
+  const int64_t i = r * hw.S + c;
+  const float t = hw.tx[i];
+  const float v = __fmul_rn(__fmul_rn(__fmul_rn(g, hw.gx[i]), __fsub_rn(1.f, t)), t);
+  const __nv_bfloat16 h = __float2bfloat16_rn(v);
+  hw.dz_hi[r * hw.dz_pitch + c] = h;
+  hw.dz_lo[r * hw.dz_pitch + c] = __float2bfloat16_rn(v - __bfloat162float(h));
+}
+
+// FIR family: the combine and the backward's preparation as plain elementwise passes around the unchanged kernels.
+__global__ void highway_combine_kernel(HighwayArgs hw, float* __restrict__ out, int64_t rows) {
+  pdl_entry();
+  const int64_t n = rows * hw.S;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / hw.S;
+    const int c = (int)(i - r * hw.S);
+    out[i] = highway_out(hw, r, c, hw.gx[i]);
+  }
+}
+
+// dz from g, then g *= Tx in place (the adjoint that follows sees dL/dGx)
+__global__ void highway_bwd_prep_kernel(HighwayArgs hw, float* __restrict__ g, int64_t rows) {
+  pdl_entry();
+  const int64_t n = rows * hw.S;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / hw.S;
+    const int c = (int)(i - r * hw.S);
+    const float gv = g[i];
+    highway_dz(hw, r, c, gv);
+    g[i] = __fmul_rn(gv, hw.tx[i]);
+  }
+}
+
 struct SolveTaps {
   float c[GANTTS_MAX_WINDOWS][5];      // coefficient of mu_w[t - k] in b_t, k = -2..2 at index k + 2 (0 where absent)
   int nw;
@@ -321,11 +372,12 @@ __device__ __forceinline__ void strip_forward(float* zs, const float4* cf, int l
   }
 }
 
-template <bool STD3>
+// HW: highway combine at the output store (HighwayArgs): out = x_s + Tx * y, y itself goes to hw.gx.
+template <bool STD3, bool HW>
 __global__ void __launch_bounds__(32 * SOLVE_WARPS, 4)
 mlpg_solve_fwd_kernel(const float* __restrict__ in, int64_t in_bs, int in_ts, float* __restrict__ out, int64_t out_bs,
                       int out_ts, const float* __restrict__ table, gantts_streams_t st, SolveTaps taps, int B, int T,
-                      int ncols, int ncg, int bpc) {
+                      int ncols, int ncg, int bpc, HighwayArgs hw) {
   pdl_entry();
   extern __shared__ __align__(16) float smem[];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -443,18 +495,27 @@ mlpg_solve_fwd_kernel(const float* __restrict__ in, int64_t in_bs, int in_ts, fl
     if (!dyn) y = zt;
     y2 = y1;
     y1 = y;
-    if (valid) *outp = y;
+    if (HW) {
+      if (valid) {
+        const int64_t r = (int64_t)it.b * T + s + i;
+        hw.gx[r * hw.S + oc] = y;
+        *outp = highway_out(hw, r, oc, y);
+      }
+    } else if (valid) {
+      *outp = y;
+    }
     outp -= out_ts;
   }
 }
 
 // Adjoint: z = P^-1 g (same two sweeps on the upstream gradient), gi_w[t] = sum_k coef_w[k+l] z_{t+k}.
-template <bool STD3>
+// HW: highway backward (HighwayArgs): the strip is loaded as Tx * g, and the chunk's own frames [t0, t1) emit dz.
+template <bool STD3, bool HW>
 __global__ void __launch_bounds__(32 * SOLVE_WARPS, 4)
 mlpg_solve_bwd_kernel(const float* __restrict__ go, int64_t go_bs, int go_ts, float* __restrict__ gi, int64_t gi_bs,
                       int gi_ts, const float* __restrict__ table, gantts_streams_t st, SolveTaps taps, int B, int T, int ncols,
                       int ncg, int bpc, int accumulate, __nv_bfloat16* __restrict__ phi, __nv_bfloat16* __restrict__ plo,
-                      int ppitch) {
+                      int ppitch, HighwayArgs hw) {
   pdl_entry();
   extern __shared__ __align__(16) float smem[];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -476,7 +537,23 @@ mlpg_solve_bwd_kernel(const float* __restrict__ go, int64_t go_bs, int go_ts, fl
   const bool valid = ci.in_col >= 0 && oc < ncols;
   const bool dyn = valid && ci.dyn;
   // (1) the strip of the upstream gradient
-  {
+  if (HW) {
+    const float* gop = go + (int64_t)it.b * go_bs + (valid ? oc : 0) + (int64_t)s * go_ts;
+    const int64_t r0 = (int64_t)it.b * T + s;
+    const float* txp = hw.tx + r0 * hw.S + (valid ? oc : 0);
+#pragma unroll 8
+    for (int i = 0; i < n; ++i) {
+      float gv = 0.f;
+      if (valid) {
+        gv = __ldg(gop);
+        if (s + i >= t0 && s + i < t1) highway_dz(hw, r0 + i, oc, gv);
+        gv = __fmul_rn(gv, __ldg(txp));
+      }
+      zs[i * 32 + lane] = gv;
+      gop += go_ts;
+      txp += hw.S;
+    }
+  } else {
     const float* gop = go + (int64_t)it.b * go_bs + (valid ? oc : 0) + (int64_t)s * go_ts;
 #pragma unroll 8
     for (int i = 0; i < n; ++i) {
@@ -740,31 +817,71 @@ extern "C" int gantts_mlpg_table(const gantts_windows_t* win, int T, float* tabl
   return GANTTS_OK;
 }
 
+namespace gantts {
+static int check_highway(const HighwayArgs* hw, int ncols, int64_t bs, int64_t ts, int T) {
+  if (!hw) return GANTTS_OK;
+  GANTTS_CHECK_ARG(hw->x && hw->tx && hw->gx && hw->dz_hi && hw->dz_lo && hw->S == ncols && ts == hw->S &&
+                       bs == (int64_t)T * hw->S,
+                   "mlpg: highway combine needs contiguous [B][T][S] static features, S = %d", ncols);
+  return GANTTS_OK;
+}
+
+static inline int elementwise_blocks(int64_t n) {
+  int64_t b = (n + 255) / 256;
+  if (b > 132 * 8) b = 132 * 8;
+  return (int)(b < 1 ? 1 : b);
+}
+
+// hw != null: the In2OutHighwayNet combine, `out` receives y_hat_static and hw->gx the MLPG output.
+static int mlpg_fwd_impl(const float* in, int64_t in_bs, int64_t in_ts, float* out, int64_t out_bs, int64_t out_ts,
+                         const float* table_dev, const gantts_streams_t* st, const gantts_windows_t* win, int B, int T,
+                         void* stream, const HighwayArgs* hw);
+}  // namespace gantts
+
 extern "C" int gantts_mlpg_fwd(const float* in, int64_t in_bs, int64_t in_ts, float* out,
                                int64_t out_bs, int64_t out_ts, const float* table_dev,
                                const gantts_streams_t* st, const gantts_windows_t* win, int B, int T,
                                void* stream) {
+  return mlpg_fwd_impl(in, in_bs, in_ts, out, out_bs, out_ts, table_dev, st, win, B, T, stream, nullptr);
+}
+
+static int gantts::mlpg_fwd_impl(const float* in, int64_t in_bs, int64_t in_ts, float* out, int64_t out_bs,
+                                 int64_t out_ts, const float* table_dev, const gantts_streams_t* st,
+                                 const gantts_windows_t* win, int B, int T, void* stream, const HighwayArgs* hw) {
   int ncols = 0;
   int rc = check_layout(st, win, &ncols);
   if (rc) return rc;
   GANTTS_CHECK_ARG(in && out && table_dev && B >= 1 && T >= 1, "mlpg_fwd: bad arguments");
+  if ((rc = check_highway(hw, ncols, out_bs, out_ts, T))) return rc;
   {
     SolveTaps tp;
     if (solve_taps(win, &tp, 1) && fits_i32((int64_t)T * in_ts) && fits_i32((int64_t)T * out_ts)) {
       const SolveGrid g = solve_grid(B, T, ncols);
-      auto fn = tp.std3 ? mlpg_solve_fwd_kernel<true> : mlpg_solve_fwd_kernel<false>;
+      auto fn = hw ? (tp.std3 ? mlpg_solve_fwd_kernel<true, true> : mlpg_solve_fwd_kernel<false, true>)
+                   : (tp.std3 ? mlpg_solve_fwd_kernel<true, false> : mlpg_solve_fwd_kernel<false, false>);
       GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
       // 50 KB per block: the full shared-memory carve-out lets 4 blocks (16 warps) share an SM
       GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
       int in_cols = 0;
       for (int s = 0; s < st->n; ++s) in_cols += st->sd[s] * (st->dyn[s] ? win->n : 1);
       prof_begin(PROF_MLPG_FWD, 4.0 * (double)B * T * (in_cols + ncols), as_stream(stream));
+      HighwayArgs none{};
       GANTTS_PDL_LAUNCH((fn), g.blocks, 32 * SOLVE_WARPS, g.smem, as_stream(stream), in, in_bs, (int)in_ts, out, out_bs, (int)out_ts, table_dev, *st,
-                                                                  tp, B, T, ncols, g.ncg, g.bpc);
+                                                                  tp, B, T, ncols, g.ncg, g.bpc, hw ? *hw : none);
       prof_end(as_stream(stream));
       GANTTS_LAUNCH_CHECK("mlpg_solve_fwd_kernel");
       return GANTTS_OK;
     }
+  }
+  if (hw) {
+    // FIR family: MLPG into Gx, then the combine as one elementwise pass
+    if ((rc = mlpg_fwd_impl(in, in_bs, in_ts, hw->gx, (int64_t)T * hw->S, hw->S, table_dev, st, win, B, T, stream,
+                            nullptr)))
+      return rc;
+    const int64_t rows = (int64_t)B * T;
+    GANTTS_PDL_LAUNCH((highway_combine_kernel), elementwise_blocks(rows * hw->S), 256, 0, as_stream(stream), *hw, out, rows);
+    GANTTS_LAUNCH_CHECK("highway_combine_kernel");
+    return GANTTS_OK;
   }
   const size_t smem = ((TT + 2 * K_HALF) * TC + TT * GROW) * sizeof(float);
   static bool attr_done_dev[64] = {};
@@ -794,54 +911,78 @@ extern "C" int gantts_mlpg_fwd(const float* in, int64_t in_bs, int64_t in_ts, fl
 // MLPG backward whose result leaves as bf16 hi/lo operand planes [B*T][pitch] (fused step: the gradient w.r.t. y_hat
 // is consumed by the generator's backward GEMMs only).  Returns GANTTS_E_UNSUPPORTED when the substitution kernel does
 // not apply (the caller then takes the fp32 route).
+// hw != null (both functions): the In2OutHighwayNet backward, go = dL/dy_hat_static; dz goes to hw's planes.
 namespace gantts {
 static int mlpg_bwd_planes(const float* go, int64_t go_bs, int64_t go_ts, __nv_bfloat16* phi, __nv_bfloat16* plo,
                            int64_t ppitch, const float* table_dev, const gantts_streams_t* st, const gantts_windows_t* win,
-                           int B, int T, void* stream) {
+                           int B, int T, void* stream, const HighwayArgs* hw = nullptr) {
   int ncols = 0;
   int rc = check_layout(st, win, &ncols);
   if (rc) return rc;
+  if ((rc = check_highway(hw, ncols, go_bs, go_ts, T))) return rc;
   SolveTaps tp;
   if (!solve_taps(win, &tp, 2) || !fits_i32((int64_t)T * go_ts) || !fits_i32((int64_t)B * T * ppitch)) return GANTTS_E_UNSUPPORTED;
   const SolveGrid g = solve_grid(B, T, ncols);
-  auto fn = tp.std3 ? mlpg_solve_bwd_kernel<true> : mlpg_solve_bwd_kernel<false>;
+  auto fn = hw ? (tp.std3 ? mlpg_solve_bwd_kernel<true, true> : mlpg_solve_bwd_kernel<false, true>)
+               : (tp.std3 ? mlpg_solve_bwd_kernel<true, false> : mlpg_solve_bwd_kernel<false, false>);
   GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
   GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
   int in_cols = 0;
   for (int s = 0; s < st->n; ++s) in_cols += st->sd[s] * (st->dyn[s] ? win->n : 1);
   prof_begin(PROF_MLPG_BWD, 4.0 * (double)B * T * (in_cols + ncols), as_stream(stream));
+  HighwayArgs none{};
   GANTTS_PDL_LAUNCH((fn), g.blocks, 32 * SOLVE_WARPS, g.smem, as_stream(stream), go, go_bs, (int)go_ts, nullptr, 0, 0, table_dev, *st, tp, B, T, ncols,
-                                                              g.ncg, g.bpc, 0, phi, plo, (int)ppitch);
+                                                              g.ncg, g.bpc, 0, phi, plo, (int)ppitch, hw ? *hw : none);
   prof_end(as_stream(stream));
   GANTTS_LAUNCH_CHECK("mlpg_solve_bwd_kernel(planes)");
   return GANTTS_OK;
 }
+
+// With hw and the FIR family, go is scaled by Tx in place before the unchanged adjoint runs on it.
+static int mlpg_bwd_impl(const float* go, int64_t go_bs, int64_t go_ts, float* gi, int64_t gi_bs, int64_t gi_ts,
+                         const float* table_dev, const gantts_streams_t* st, const gantts_windows_t* win, int B, int T,
+                         int accumulate, void* stream, const HighwayArgs* hw);
 }  // namespace gantts
 
 extern "C" int gantts_mlpg_bwd(const float* go, int64_t go_bs, int64_t go_ts, float* gi,
                                int64_t gi_bs, int64_t gi_ts, const float* table_dev,
                                const gantts_streams_t* st, const gantts_windows_t* win, int B, int T,
                                int accumulate, void* stream) {
+  return mlpg_bwd_impl(go, go_bs, go_ts, gi, gi_bs, gi_ts, table_dev, st, win, B, T, accumulate, stream, nullptr);
+}
+
+static int gantts::mlpg_bwd_impl(const float* go, int64_t go_bs, int64_t go_ts, float* gi, int64_t gi_bs, int64_t gi_ts,
+                                 const float* table_dev, const gantts_streams_t* st, const gantts_windows_t* win, int B,
+                                 int T, int accumulate, void* stream, const HighwayArgs* hw) {
   int ncols = 0;
   int rc = check_layout(st, win, &ncols);
   if (rc) return rc;
   GANTTS_CHECK_ARG(go && gi && table_dev && B >= 1 && T >= 1, "mlpg_bwd: bad arguments");
+  if ((rc = check_highway(hw, ncols, go_bs, go_ts, T))) return rc;
   {
     SolveTaps tp;
     if (solve_taps(win, &tp, 2) && fits_i32((int64_t)T * go_ts) && fits_i32((int64_t)T * gi_ts)) {
       const SolveGrid g = solve_grid(B, T, ncols);
-      auto fn = tp.std3 ? mlpg_solve_bwd_kernel<true> : mlpg_solve_bwd_kernel<false>;
+      auto fn = hw ? (tp.std3 ? mlpg_solve_bwd_kernel<true, true> : mlpg_solve_bwd_kernel<false, true>)
+                   : (tp.std3 ? mlpg_solve_bwd_kernel<true, false> : mlpg_solve_bwd_kernel<false, false>);
       GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
       GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
       int in_cols = 0;
       for (int s = 0; s < st->n; ++s) in_cols += st->sd[s] * (st->dyn[s] ? win->n : 1);
       prof_begin(PROF_MLPG_BWD, 4.0 * (double)B * T * (in_cols + ncols), as_stream(stream));
+      HighwayArgs none{};
       GANTTS_PDL_LAUNCH((fn), g.blocks, 32 * SOLVE_WARPS, g.smem, as_stream(stream), go, go_bs, (int)go_ts, gi, gi_bs, (int)gi_ts, table_dev, *st, tp, B, T,
-                                                                  ncols, g.ncg, g.bpc, accumulate, nullptr, nullptr, 0);
+                                                                  ncols, g.ncg, g.bpc, accumulate, nullptr, nullptr, 0, hw ? *hw : none);
       prof_end(as_stream(stream));
       GANTTS_LAUNCH_CHECK("mlpg_solve_bwd_kernel");
       return GANTTS_OK;
     }
+  }
+  if (hw) {
+    const int64_t rows = (int64_t)B * T;
+    GANTTS_PDL_LAUNCH((highway_bwd_prep_kernel), elementwise_blocks(rows * hw->S), 256, 0, as_stream(stream), *hw,
+                      const_cast<float*>(go), rows);
+    GANTTS_LAUNCH_CHECK("highway_bwd_prep_kernel");
   }
   const size_t smem = (GIN_ROWS * TC + 72 * GROW + 72 * TC) * sizeof(float);
   static bool attr_done_dev[64] = {};

@@ -1,7 +1,8 @@
-"""Fused GAN step: ONE C call (gantts_gan_step) per mini-batch for an MLP generator + MLP
+"""Fused GAN step: ONE C call (gantts_gan_step) per mini-batch for an MLP or In2OutHighwayNet generator + MLP
 discriminator -- the whole of reference train.py:528-580 enqueued on the current stream without a
 single host synchronisation (SURVEY.md 8f row 3).  Not drop-in for train.py (which owns its step
-functions); offered next to the compatible modular path (gantts_b200.step.GanTrainer).
+functions); offered next to the compatible modular path (gantts_b200.step.GanTrainer), which also runs
+the recurrent generators.
 
 Data parallel: utterance shards, the two flat gradient buffers are SUM all-reduced (NCCL via
 torch.distributed on the same stream) between the phases of the step; losses are normalised by the
@@ -13,6 +14,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from . import models
 from . import multistream
 from . import ops
 from . import parallel
@@ -21,8 +23,17 @@ LOSS_NAMES = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mse", "loss_mge", "l
               "real_correct", "fake_correct", "frames", "d_grad_norm", "g_grad_norm")
 
 
-def _fill_mlp(desc, model, p, last_act):
-    layers = list(model.layers) + [model.last_linear]
+def _generator_parts(model_g):
+    """(highway gate Linear or None, [hidden layers..., last_linear]) of a generator the fused step runs."""
+    if isinstance(model_g, models.In2OutHighwayNet):
+        return model_g.T, list(model_g.H) + [model_g.last_linear]
+    if hasattr(model_g, "layers") and hasattr(model_g, "last_linear"):
+        return None, list(model_g.layers) + [model_g.last_linear]
+    raise RuntimeError("FusedGanStep: generator %s is not supported (MLP and In2OutHighwayNet are); train it with "
+                       "gantts_b200.step.GanTrainer" % type(model_g).__name__)
+
+
+def _fill_mlp(desc, layers, p, last_act):
     if len(layers) > _lib.MAX_LAYERS:
         raise RuntimeError("gantts_b200: at most %d layers" % _lib.MAX_LAYERS)
     desc.num_layers = len(layers)
@@ -61,20 +72,41 @@ class FusedGanStep(object):
         parallel.broadcast_parameters(model_d, group=process_group)
         c = _lib.GanStepT()
         c.B, c.T = self.B, self.T
-        self._g_layers = _fill_mlp(c.g, model_g, model_g.dropout_p, _lib.ACT_NONE)
-        self._d_layers = _fill_mlp(c.d, model_d, model_d.dropout_p, _lib.ACT_SIGMOID)
-        if model_g.last_sigmoid or not model_d.last_sigmoid:
+        self._gate, g_layers = _generator_parts(model_g)
+        self._g_layers = _fill_mlp(c.g, g_layers, model_g.dropout_p, _lib.ACT_NONE)
+        self._d_layers = _fill_mlp(c.d, list(model_d.layers) + [model_d.last_linear], model_d.dropout_p,
+                                   _lib.ACT_SIGMOID)
+        if getattr(model_g, "last_sigmoid", False) or not model_d.last_sigmoid:
             raise RuntimeError("FusedGanStep: generator must be linear-output, discriminator sigmoid-output")
+        # the generator's modules with parameters, in model_g.parameters() order (the gate first)
+        self._g_mods = ([self._gate] if self._gate is not None else []) + self._g_layers
         self._sums, self._sqs = [], []      # Adagrad: state_sum | Adam: exp_avg, exp_avg_sq (model.parameters() order)
+
+        def new_state(l):
+            a, b = torch.zeros_like(l.weight), torch.zeros_like(l.bias)
+            self._sums += [a, b]
+            a2 = b2 = None
+            if optimizer == "Adam":
+                a2, b2 = torch.zeros_like(l.weight), torch.zeros_like(l.bias)
+                self._sqs += [a2, b2]
+            return a, b, a2, b2
+        if self._gate is not None:
+            gt, h = self._gate, c.highway
+            ops.require_cuda(gt.weight, gt.bias)
+            if not (gt.weight.is_contiguous() and gt.bias.is_contiguous()):
+                raise RuntimeError("gantts_b200: parameters must be contiguous")
+            h.static_dim = int(model_g.static_dim)
+            h.W, h.b = gt.weight.data_ptr(), gt.bias.data_ptr()
+            a, b, a2, b2 = new_state(gt)
+            h.sumW, h.sumb = a.data_ptr(), b.data_ptr()
+            if a2 is not None:
+                h.sqW, h.sqb = a2.data_ptr(), b2.data_ptr()
         for layers, sw, sb, qw, qb in ((self._g_layers, c.g_sumW, c.g_sumb, c.g_sqW, c.g_sqb),
                                        (self._d_layers, c.d_sumW, c.d_sumb, c.d_sqW, c.d_sqb)):
             for i, l in enumerate(layers):
-                a, b = torch.zeros_like(l.weight), torch.zeros_like(l.bias)
-                self._sums += [a, b]
+                a, b, a2, b2 = new_state(l)
                 sw[i], sb[i] = a.data_ptr(), b.data_ptr()
-                if optimizer == "Adam":
-                    a2, b2 = torch.zeros_like(l.weight), torch.zeros_like(l.bias)
-                    self._sqs += [a2, b2]
+                if a2 is not None:
                     qw[i], qb[i] = a2.data_ptr(), b2.data_ptr()
         nw = len(hp.windows)
         entries, n_static = multistream.mlpg_stream_entries(hp.stream_sizes, hp.has_dynamic_features,
@@ -156,6 +188,8 @@ class FusedGanStep(object):
         for desc, layers in ((self.cfg.g, self._g_layers), (self.cfg.d, self._d_layers)):
             for i, l in enumerate(layers):      # parameters may have been re-allocated (load_state_dict keeps them)
                 desc.W[i], desc.b[i] = l.weight.data_ptr(), l.bias.data_ptr()
+        if self._gate is not None:
+            self.cfg.highway.W, self.cfg.highway.b = self._gate.weight.data_ptr(), self._gate.bias.data_ptr()
         if train is None:
             if self.g.training != self.d.training:
                 raise RuntimeError("FusedGanStep: generator and discriminator disagree on train()/eval()")
@@ -219,13 +253,13 @@ class FusedGanStep(object):
                                   "differentiable": False, "fused": None, "params": list(range(n))}]}
 
     def state_dict(self):
-        ng, n = 2 * len(self._g_layers), len(self._sums)
+        ng, n = 2 * len(self._g_mods), len(self._sums)
         return {"optimizer_g": self._opt_state(0, ng, float(self.cfg.lr_g), float(self.cfg.wd_g)),
                 "optimizer_d": self._opt_state(ng, n, float(self.cfg.lr_d), float(self.cfg.wd_d)),
                 "step": self._step, "seed": self._seed}
 
     def load_state_dict(self, sd):
-        ng, n = 2 * len(self._g_layers), len(self._sums)
+        ng, n = 2 * len(self._g_mods), len(self._sums)
         for key, lo, hi in (("optimizer_g", 0, ng), ("optimizer_d", ng, n)):
             st = sd[key]["state"]
             for i in range(hi - lo):

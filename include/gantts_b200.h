@@ -304,7 +304,25 @@ int gantts_sru_bwd(const float* u, const float* x, const float* bias, const floa
  * step derive it on the device from lengths_dev (single-process use).
  * losses_dev[12] = loss_d, loss_fake_d, loss_real_d, loss_mse, loss_mge, loss_adv, loss_g,
  *                  real_correct, fake_correct, local frames, d_grad_norm, g_grad_norm.
+ *
+ * In2OutHighwayNet generator (reference gantts/models.py:21-69, hparams.py `vc`): highway.static_dim = S > 0.  Then g is
+ * the network's H stack + last_linear and the step computes, with x_s = x[:, :, :S] and h = g(x) (= y_hat),
+ *   Tx = sigmoid(x_s T.weight^T + T.bias),   Gx = MLPG(h),   y_hat_static = x_s + Tx * Gx,
+ * and in the backward, from g = dL/dy_hat_static:  dGx = Tx * g (into the MLPG adjoint and the stack's backward),
+ * dz = g * Gx * Tx * (1 - Tx),  dT.weight = dz^T x_s,  dT.bias = sum over rows of dz (no gradient w.r.t. x).
+ * Accepted layout: exactly one stream, dynamic, in_start = out_start = 0, sd = S; n_static = S; g.dims[0] >= S;
+ * g.dims[L] = windows.n * S; non-null W, b and optimiser state.  The gate is part of the generator everywhere: its two
+ * tensors come FIRST in the flat gradient buffer (model.parameters() order: T.weight, T.bias, then g's layers), in the
+ * clip norm and in the optimiser step.  The eval phase runs the same forward and leaves the gate and its state untouched.
  */
+typedef struct {
+  int static_dim;                          /* 0 = plain MLP generator; S > 0 = In2OutHighwayNet with S static columns */
+  const float* W;                          /* T.weight [S][S] (nn.Linear layout), updated in place */
+  const float* b;                          /* T.bias [S], 16-byte aligned, updated in place */
+  float *sumW, *sumb;                      /* Adagrad state_sum | Adam exp_avg */
+  float *sqW, *sqb;                        /* Adam exp_avg_sq (unused by Adagrad) */
+} gantts_highway_t;
+
 typedef struct {
   int B, T;
   gantts_mlp_t g;                          /* generator: dims[0] = linguistic width, dims[L] = acoustic width */
@@ -336,6 +354,7 @@ typedef struct {
   float* g_sqb[GANTTS_MAX_LAYERS];
   float* d_sqW[GANTTS_MAX_LAYERS];
   float* d_sqb[GANTTS_MAX_LAYERS];
+  gantts_highway_t highway;                /* static_dim = 0: plain MLP generator (all fields above keep their offsets) */
 } gantts_gan_step_t;
 #define GANTTS_OPT_ADAGRAD 0
 #define GANTTS_OPT_ADAM 1
