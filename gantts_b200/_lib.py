@@ -70,6 +70,19 @@ class HighwayT(ctypes.Structure):
                 ("sqW", ctypes.c_void_p), ("sqb", ctypes.c_void_p)]
 
 
+MAX_SRU_LAYERS = 8
+
+
+class SruStackT(ctypes.Structure):
+    _fields_ = [("num_layers", ctypes.c_int),
+                ("in_dim", ctypes.c_int), ("hidden", ctypes.c_int), ("bidirectional", ctypes.c_int),
+                ("act", ctypes.c_int),
+                ("dropout", ctypes.c_float), ("rnn_dropout", ctypes.c_float),
+                ("W", ctypes.c_void_p * MAX_SRU_LAYERS), ("b", ctypes.c_void_p * MAX_SRU_LAYERS),
+                ("sumW", ctypes.c_void_p * MAX_SRU_LAYERS), ("sumb", ctypes.c_void_p * MAX_SRU_LAYERS),
+                ("sqW", ctypes.c_void_p * MAX_SRU_LAYERS), ("sqb", ctypes.c_void_p * MAX_SRU_LAYERS)]
+
+
 class GanStepT(ctypes.Structure):
     _fields_ = [("B", ctypes.c_int), ("T", ctypes.c_int),
                 ("g", MlpT), ("d", MlpT),
@@ -89,7 +102,8 @@ class GanStepT(ctypes.Structure):
                 ("opt_step", ctypes.c_int64),
                 ("g_sqW", ctypes.c_void_p * MAX_LAYERS), ("g_sqb", ctypes.c_void_p * MAX_LAYERS),
                 ("d_sqW", ctypes.c_void_p * MAX_LAYERS), ("d_sqb", ctypes.c_void_p * MAX_LAYERS),
-                ("highway", HighwayT)]
+                ("highway", HighwayT),
+                ("sru", SruStackT)]
 
 
 OPT_ADAGRAD, OPT_ADAM = 0, 1
@@ -153,6 +167,7 @@ SIGNATURES = {
     "gantts_clip_adam_step": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _f, _f, _f, _f, _f, _f, _i64, _vp]),
     "gantts_gan_step_seed": (_u64, [_u64, _i]),
     "gantts_mlp_layer_seed": (_u64, [_u64, _i]),
+    "gantts_sru_mask_seed": (_u64, [_u64, _i, _i]),
 }
 
 STEP_D, STEP_G, STEP_FINISH, STEP_EVAL = 1, 2, 4, 8

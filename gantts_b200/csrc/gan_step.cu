@@ -318,7 +318,8 @@ static inline int blocks_1d(int64_t work, int per_block) {
   return (int)b;
 }
 
-constexpr int MAX_PARAMS = 2 * GANTTS_MAX_LAYERS + 2;     // + the highway gate's weight and bias
+// + the highway gate's weight and bias, or the SRU stack's weights and biases (the two are mutually exclusive)
+constexpr int MAX_PARAMS = 2 * GANTTS_MAX_LAYERS + 2 * GANTTS_MAX_SRU_LAYERS;
 
 struct ParamList {
   int n;
@@ -329,6 +330,8 @@ struct ParamList {
   int64_t sizes[MAX_PARAMS];
   float* gW[GANTTS_MAX_LAYERS];
   float* gb[GANTTS_MAX_LAYERS];
+  float* sgW[GANTTS_MAX_SRU_LAYERS];                    // SRU stack: gradient of W[l] / b[l] in the flat buffer
+  float* sgb[GANTTS_MAX_SRU_LAYERS];
   int64_t total;
 };
 
@@ -360,8 +363,26 @@ struct StepLayout {
   char* hw_w;             // planes of W_T [S][S]
   char* hw_dz;            // planes of dz [M][S]
   float* hw_partial;      // split-K partials of dW_T / db_T
+  // SRU generator only (zero bytes otherwise, so the MLP and highway layouts are unchanged); per layer l:
+  char* sru_in[GANTTS_MAX_SRU_LAYERS];    // planes of the masked GEMM input [M][n_in] (layer l > 0: written by scan l-1)
+  float* sru_u[GANTTS_MAX_SRU_LAYERS];    // U = planes(x * mask_x) W  [M][ncols * k]
+  float* sru_c[GANTTS_MAX_SRU_LAYERS];    // cell states [M][ncols]
+  float* sru_h[GANTTS_MAX_SRU_LAYERS];    // fp32 h [M][ncols] below the top layer (the next layer's highway input)
+  char* sru_w[GANTTS_MAX_SRU_LAYERS];     // planes of W [n_in][ncols * k], then of W^T [ncols * k][n_in]
+  float* sru_partial[GANTTS_MAX_SRU_LAYERS];   // split-K partials of dW
+  char* sru_du;           // planes of dU [M][ncols * k] (one layer at a time)
+  float* sru_dx;          // [M][ncols] dL/dh of the top layer, then dX = dU W of each layer for the one below
+  float* sru_dxp;         // [M][ncols] highway gradient (k = 3) for the layer below
+  float* sru_bpart;       // [B][2 * ncols] bias-gradient partials
   size_t total;
 };
+
+static inline int sru_ncols(const gantts_sru_stack_t& s) { return s.hidden * (s.bidirectional ? 2 : 1); }
+static inline int sru_nin(const gantts_sru_stack_t& s, int l) { return l == 0 ? s.in_dim : sru_ncols(s); }
+static inline int sru_k(const gantts_sru_stack_t& s, int l) { return sru_nin(s, l) != sru_ncols(s) ? 4 : 3; }
+
+// width of x: the SRU stack's input, else the generator MLP's
+static inline int gen_in_width(const gantts_gan_step_t* c) { return c->sru.num_layers > 0 ? c->sru.in_dim : c->g.dims[0]; }
 
 static int64_t mlp_param_count(const gantts_mlp_t& m) {
   int64_t n = 0;
@@ -373,6 +394,18 @@ static int64_t mlp_param_count(const gantts_mlp_t& m) {
 static int64_t gate_param_count(const gantts_gan_step_t* c) {
   const int64_t S = c->highway.static_dim;
   return S * S + S;
+}
+
+// elements of the SRU stack's parameters, which lead the generator's flat gradient buffer
+static int64_t sru_param_count(const gantts_gan_step_t* c) {
+  const gantts_sru_stack_t& s = c->sru;
+  int64_t n = 0;
+  for (int l = 0; l < s.num_layers; ++l) n += (int64_t)sru_nin(s, l) * sru_ncols(s) * sru_k(s, l) + 2 * sru_ncols(s);
+  return n;
+}
+
+static int64_t g_param_count(const gantts_gan_step_t* c) {
+  return gate_param_count(c) + sru_param_count(c) + mlp_param_count(c->g);
 }
 
 static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
@@ -389,7 +422,7 @@ static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
   L->y_static = (float*)take((size_t)M * c->n_static * sizeof(float));
   L->g_static = (float*)take((size_t)M * c->n_static * sizeof(float));
   L->g_yhat = (float*)take((size_t)M * c->g.dims[c->g.num_layers] * sizeof(float));
-  L->g_grads = (float*)take((gate_param_count(c) + mlp_param_count(c->g)) * sizeof(float));
+  L->g_grads = (float*)take(g_param_count(c) * sizeof(float));
   L->d_grads = (float*)take(mlp_param_count(c->d) * sizeof(float));
   L->g_tape_bytes = gantts_mlp_tape_bytes(&c->g, M);
   L->g_tape = take(L->g_tape_bytes);
@@ -407,6 +440,26 @@ static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
   L->hw_w = take(hw ? 2 * plane_bytes(S, S) : 0);
   L->hw_dz = take(hw ? 2 * plane_bytes(M, S) : 0);
   L->hw_partial = (float*)take(hw ? mn_partial_bytes(M, S, S, nullptr, nullptr) : 0);
+  const gantts_sru_stack_t& s = c->sru;
+  const int nl = s.num_layers, nc = nl > 0 ? sru_ncols(s) : 0;
+  int maxku = 0;
+  for (int l = 0; l < GANTTS_MAX_SRU_LAYERS; ++l) {
+    L->sru_in[l] = L->sru_w[l] = nullptr;
+    L->sru_u[l] = L->sru_c[l] = L->sru_h[l] = L->sru_partial[l] = nullptr;
+    if (l >= nl) continue;
+    const int ni = sru_nin(s, l), ku = nc * sru_k(s, l);
+    maxku = ku > maxku ? ku : maxku;
+    L->sru_in[l] = take(2 * plane_bytes(M, ni));
+    L->sru_u[l] = (float*)take((size_t)M * ku * sizeof(float));
+    L->sru_c[l] = (float*)take((size_t)M * nc * sizeof(float));
+    if (l < nl - 1) L->sru_h[l] = (float*)take((size_t)M * nc * sizeof(float));
+    L->sru_w[l] = take(2 * plane_bytes(ni, ku) + 2 * plane_bytes(ku, ni));
+    L->sru_partial[l] = (float*)take(mn_partial_bytes(M, ni, ku, nullptr, nullptr));
+  }
+  L->sru_du = take(nl > 0 ? 2 * plane_bytes(M, maxku) : 0);
+  L->sru_dx = (float*)take((size_t)M * nc * sizeof(float));
+  L->sru_dxp = (float*)take((size_t)M * nc * sizeof(float));
+  L->sru_bpart = (float*)take((size_t)c->B * 2 * nc * sizeof(float));
   L->total = (size_t)(cur - base) + 256;
 }
 
@@ -434,11 +487,29 @@ static void param_list(const gantts_mlp_t& m, float* const* sumW, float* const* 
   pl->total += cur - flat;
 }
 
-// generator parameters in model.parameters() order: [T.weight, T.bias] of a highway generator, then the MLP layers
+// generator parameters in model.parameters() order: [T.weight, T.bias] of a highway generator, or [W, b] of every layer
+// of an SRU stack, then the MLP layers
 static void g_param_list(const gantts_gan_step_t* c, float* flat, ParamList* pl) {
   pl->n = 0;
   pl->total = 0;
   const gantts_highway_t& h = c->highway;
+  const gantts_sru_stack_t& s = c->sru;
+  for (int l = 0; l < s.num_layers; ++l) {
+    const int64_t sizes[2] = {(int64_t)sru_nin(s, l) * sru_ncols(s) * sru_k(s, l), 2 * (int64_t)sru_ncols(s)};
+    float* const ps[2] = {const_cast<float*>(s.W[l]), const_cast<float*>(s.b[l])};
+    float* const ss[2] = {s.sumW[l], s.sumb[l]};
+    float* const qs[2] = {s.sqW[l], s.sqb[l]};
+    pl->sgW[l] = flat + pl->total;
+    pl->sgb[l] = flat + pl->total + sizes[0];
+    for (int i = 0; i < 2; ++i) {
+      pl->p[pl->n] = ps[i];
+      pl->g[pl->n] = flat + pl->total;
+      pl->s[pl->n] = ss[i];
+      pl->s2[pl->n] = qs[i];
+      pl->sizes[pl->n++] = sizes[i];
+      pl->total += sizes[i];
+    }
+  }
   if (h.static_dim > 0) {
     const int64_t S = h.static_dim;
     const int64_t sizes[2] = {S * S, S};
@@ -515,9 +586,31 @@ static int check_step(const gantts_gan_step_t* c) {
   GANTTS_CHECK_ARG(c->g.num_layers >= 1 && c->g.num_layers <= GANTTS_MAX_LAYERS, "gan_step: bad generator");
   GANTTS_CHECK_ARG(c->n_static >= 1 && c->n_static <= GANTTS_MAX_COLS, "gan_step: bad n_static");
   GANTTS_CHECK_ARG(c->n_static_cols == c->n_static, "gan_step: static column list must have n_static entries");
+  const gantts_sru_stack_t& s = c->sru;
+  GANTTS_CHECK_ARG(s.num_layers >= 0 && s.num_layers <= GANTTS_MAX_SRU_LAYERS, "gan_step: SRU layer count %d not in [0, %d]",
+                   s.num_layers, GANTTS_MAX_SRU_LAYERS);
+  if (s.num_layers > 0) {
+    // SRURNN (models.py:144-167): the SRU stack, then hidden2out as a one-layer MLP
+    GANTTS_CHECK_ARG(c->highway.static_dim == 0, "gan_step: the SRU stack and the highway gate are mutually exclusive");
+    GANTTS_CHECK_ARG(s.in_dim >= 1 && s.hidden >= 1 && (s.bidirectional == 0 || s.bidirectional == 1),
+                     "gan_step: bad SRU shape (in_dim %d, hidden %d, bidirectional %d)", s.in_dim, s.hidden, s.bidirectional);
+    GANTTS_CHECK_ARG(s.act >= 0 && s.act <= 2, "gan_step: SRU activation %d not in 0..2", s.act);
+    GANTTS_CHECK_ARG(s.dropout >= 0.f && s.dropout < 1.f && s.rnn_dropout >= 0.f && s.rnn_dropout < 1.f,
+                     "gan_step: SRU dropout / rnn_dropout out of [0, 1)");
+    const int nc = sru_ncols(s);
+    GANTTS_CHECK_ARG(c->g.num_layers == 1 && c->g.dims[0] == nc,
+                     "gan_step: with an SRU stack g is hidden2out alone: 1 layer of input width %d (got %d layer(s), input "
+                     "width %d)", nc, c->g.num_layers, c->g.dims[0]);
+    for (int l = 0; l < s.num_layers; ++l) {
+      GANTTS_CHECK_ARG(s.W[l] && s.b[l], "gan_step: null SRU weight/bias of layer %d", l);
+      GANTTS_CHECK_ARG(s.sumW[l] && s.sumb[l], "gan_step: null SRU optimiser state of layer %d", l);
+      if (c->optimizer == GANTTS_OPT_ADAM)
+        GANTTS_CHECK_ARG(s.sqW[l] && s.sqb[l], "gan_step: Adam needs exp_avg_sq for SRU layer %d", l);
+    }
+  }
   if (c->w_d > 0.f) {
     GANTTS_CHECK_ARG(c->d.num_layers >= 1 && c->d.num_layers <= GANTTS_MAX_LAYERS, "gan_step: bad discriminator");
-    const int cond_w = c->d_conditioned ? c->g.dims[0] : 0;
+    const int cond_w = c->d_conditioned ? gen_in_width(c) : 0;
     GANTTS_CHECK_ARG(c->n_adv >= 1 && c->n_adv <= GANTTS_MAX_COLS && c->d.dims[0] == cond_w + c->n_adv,
                      "gan_step: discriminator input width %d != %d conditioning + %d adversarial columns",
                      c->d.dims[0], cond_w, c->n_adv);
@@ -585,11 +678,163 @@ static int highway_gate_bwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, c
   return flush_reduce(rl, 0, st);
 }
 
+// SRU layer l's workspace: planes of its masked input, and of W [n_in][ncols k] then W^T [ncols k][n_in]
+static Planes sru_in_planes(const gantts_gan_step_t* c, const StepLayout& L, int l, int64_t M) {
+  char* cur = L.sru_in[l];
+  return carve_planes(cur, M, sru_nin(c->sru, l));
+}
+static void sru_w_planes(const gantts_gan_step_t* c, const StepLayout& L, int l, Planes* w, Planes* wt) {
+  const int ni = sru_nin(c->sru, l), ku = sru_ncols(c->sru) * sru_k(c->sru, l);
+  char* cur = L.sru_w[l];
+  *w = carve_planes(cur, ni, ku);
+  *wt = carve_planes(cur, ku, ni);
+}
+
+// SRU stack forward (rnn.SRUCell per layer): the last layer's h goes unmasked into hidden2out's tape input planes, so
+// the caller runs hidden2out with mlp_fwd_impl(..., input_ready = true).  train = false: no masks.
+static int sru_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, const float* x, int64_t M,
+                         uint64_t seed, bool train, cudaStream_t st) {
+  const gantts_sru_stack_t& s = c->sru;
+  const int nl = s.num_layers, nc = sru_ncols(s);
+  const float p_h = train ? s.dropout : 0.f, p_x = train ? s.rnn_dropout : 0.f;
+  int rc;
+  {
+    // every layer's weight -> planes as stored (operand of dX = dU W^T) and transposed (operand of U = x W), one launch
+    WeightSplitList wl;
+    wl.n = nl;
+    wl.off[0] = 0;
+    for (int l = 0; l < nl; ++l) {
+      Planes w, wt;
+      sru_w_planes(c, L, l, &w, &wt);
+      wl.W[l] = s.W[l];
+      wl.N[l] = (int)w.rows;
+      wl.K[l] = (int)w.cols;
+      wl.hi[l] = w.hi;
+      wl.lo[l] = w.lo;
+      wl.pitch[l] = w.pitch;
+      wl.thi[l] = wt.hi;
+      wl.tlo[l] = wt.lo;
+      wl.tpitch[l] = wt.pitch;
+      wl.off[l + 1] = wl.off[l] + (int64_t)((w.rows + 31) / 32) * ((w.cols + 31) / 32);
+    }
+    int nb = (int)(wl.off[nl] < num_sms() * 8 ? wl.off[nl] : num_sms() * 8);
+    GANTTS_PDL_LAUNCH((split_weights_kernel), nb < 1 ? 1 : nb, 256, 0, st, wl);
+    GANTTS_LAUNCH_CHECK("split_weights_kernel(sru)");
+  }
+  const Planes in0 = sru_in_planes(c, L, 0, M);
+  if (p_x > 0.f) {
+    GANTTS_PDL_LAUNCH((sru_mask_split_kernel), blocks_1d(M * s.in_dim, 1024), 256, 0, st, x, (int64_t)s.in_dim, M, s.in_dim,
+                      c->T, sru_mask(gantts_sru_mask_seed(seed, 0, 0), p_x), in0.hi, in0.lo, in0.pitch);
+    GANTTS_LAUNCH_CHECK("sru_mask_split_kernel");
+  } else if ((rc = launch_split(x, s.in_dim, M, s.in_dim, in0, 0, st))) {
+    return rc;
+  }
+  Planes top;
+  if ((rc = mlp_tape_input_planes(&g, M, L.g_tape, L.g_tape_bytes, &top))) return rc;
+  for (int l = 0; l < nl; ++l) {
+    const int k = sru_k(s, l);
+    const bool last = l == nl - 1;
+    Planes w, wt;
+    sru_w_planes(c, L, l, &w, &wt);
+    EpiArgs e;
+    e.epi = EPI_F32;
+    e.C = L.sru_u[l];
+    e.ldc = (int64_t)nc * k;
+    if ((rc = launch_gemm_kk(sru_in_planes(c, L, l, M), wt, e, st))) return rc;
+    const Planes out = last ? top : sru_in_planes(c, L, l + 1, M);
+    SruStepFwd p{};
+    p.u = L.sru_u[l];
+    p.xh = k == 3 ? (l == 0 ? x : L.sru_h[l - 1]) : nullptr;
+    p.xh_rs = l == 0 ? s.in_dim : nc;
+    p.bias = s.b[l];
+    p.c = L.sru_c[l];
+    p.h = L.sru_h[l];
+    p.hi = out.hi;
+    p.lo = out.lo;
+    p.pitch = out.pitch;
+    p.mh = sru_mask(gantts_sru_mask_seed(seed, l, 1), last ? 0.f : p_h);      // SRU(): no output dropout on the last layer
+    p.mx = sru_mask(gantts_sru_mask_seed(seed, l + 1, 0), last ? 0.f : p_x);
+    p.B = c->B;
+    p.T = c->T;
+    p.d = s.hidden;
+    p.bidir = s.bidirectional;
+    p.act = s.act;
+    if ((rc = launch_sru_step_fwd(p, k, st))) return rc;
+  }
+  return GANTTS_OK;
+}
+
+// SRU stack backward from dL/dh of the top layer in L.sru_dx (hidden2out's input gradient), top layer first:
+//   scan backward -> dU planes, highway gradient dx' (k = 3), bias partials -> bias gradient (fixed order over B)
+//   dW = (x * mask_x)^T dU  (MN-major, lands in the [n_in][ncols k] parameter layout)
+//   dX = dU W^T             (K-major on W as stored; not for layer 0)
+// The layer below's dh = mask_x * dX + dx' is formed on load by its scan backward.
+static int sru_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const ParamList& pg, const float* x, int64_t M,
+                         uint64_t seed, cudaStream_t st) {
+  const gantts_sru_stack_t& s = c->sru;
+  const int nl = s.num_layers, nc = sru_ncols(s);
+  int rc;
+  ReduceList rl;
+  for (int l = nl - 1; l >= 0; --l) {
+    const int k = sru_k(s, l);
+    const bool top = l == nl - 1;
+    char* cur = L.sru_du;
+    const Planes du = carve_planes(cur, M, (int64_t)nc * k);
+    SruStepBwd p{};
+    p.u = L.sru_u[l];
+    p.xh = k == 3 ? (l == 0 ? x : L.sru_h[l - 1]) : nullptr;
+    p.xh_rs = l == 0 ? s.in_dim : nc;
+    p.bias = s.b[l];
+    p.c = L.sru_c[l];
+    p.dx = L.sru_dx;
+    p.dxp_in = top ? nullptr : L.sru_dxp;
+    p.mxu = sru_mask(gantts_sru_mask_seed(seed, l + 1, 0), top ? 0.f : s.rnn_dropout);
+    p.mh = sru_mask(gantts_sru_mask_seed(seed, l, 1), top ? 0.f : s.dropout);
+    p.du_hi = du.hi;
+    p.du_lo = du.lo;
+    p.du_pitch = du.pitch;
+    p.dxp_out = (k == 3 && l > 0) ? L.sru_dxp : nullptr;
+    p.dbias_part = L.sru_bpart;
+    p.B = c->B;
+    p.T = c->T;
+    p.d = s.hidden;
+    p.bidir = s.bidirectional;
+    p.act = s.act;
+    if ((rc = launch_sru_step_bwd(p, k, st))) return rc;
+    GANTTS_PDL_LAUNCH((sru_bias_reduce_kernel), (2 * nc + 255) / 256, 256, 0, st, L.sru_bpart, c->B, 2 * nc, pg.sgb[l]);
+    GANTTS_LAUNCH_CHECK("sru_bias_reduce_kernel");
+    if ((rc = launch_gemm_mn(sru_in_planes(c, L, l, M), du, pg.sgW[l], nullptr, 0, L.sru_partial[l], st, &rl))) return rc;
+    if (l > 0) {
+      Planes w, wt;
+      sru_w_planes(c, L, l, &w, &wt);
+      EpiArgs e;
+      e.epi = EPI_F32;
+      e.C = L.sru_dx;
+      e.ldc = nc;
+      if ((rc = launch_gemm_kk(du, w, e, st))) return rc;
+    }
+  }
+  return flush_reduce(rl, 0, st);
+}
+
+// Generator forward into y_hat: the MLP from x, or the SRU stack and then hidden2out on the planes it left in the tape.
+static int generator_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, const float* x, int x_rs,
+                         int64_t M, float* y_hat, int d_out, uint64_t seed, bool train, cudaStream_t st) {
+  if (c->sru.num_layers == 0) return gantts_mlp_fwd(&g, x, x_rs, M, y_hat, d_out, L.g_tape, L.g_tape_bytes, st);
+  int rc = sru_stack_fwd(c, g, L, x, M, seed, train, st);
+  if (rc) return rc;
+  return mlp_fwd_impl(&g, nullptr, 0, M, y_hat, d_out, L.g_tape, L.g_tape_bytes, st, true);
+}
+
 }  // namespace gantts
 
 using namespace gantts;
 
 extern "C" uint64_t gantts_gan_step_seed(uint64_t seed, int which) { return seed * 4 + (uint64_t)which; }
+
+extern "C" uint64_t gantts_sru_mask_seed(uint64_t seed, int layer, int which) {
+  return gantts_mlp_layer_seed(gantts_gan_step_seed(seed, 3), 2 * layer + which);
+}
 
 extern "C" size_t gantts_gan_step_workspace_bytes(const gantts_gan_step_t* c) {
   if (check_step(c)) return 0;
@@ -606,7 +851,7 @@ extern "C" int gantts_gan_step_grad_buffer(const gantts_gan_step_t* c, void* wor
   StepLayout L;
   layout(c, reinterpret_cast<char*>(al256(reinterpret_cast<uintptr_t>(workspace))), &L);
   *ptr = which == 0 ? L.g_grads : L.d_grads;
-  *count = which == 0 ? gate_param_count(c) + mlp_param_count(c->g) : mlp_param_count(c->d);
+  *count = which == 0 ? g_param_count(c) : mlp_param_count(c->d);
   return GANTTS_OK;
 }
 
@@ -626,7 +871,8 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
   StepLayout L;
   layout(c, reinterpret_cast<char*>(al256(reinterpret_cast<uintptr_t>(workspace))), &L);
   const int64_t M = (int64_t)c->B * c->T;
-  const int Lg = c->g.num_layers, d_in = c->g.dims[0], d_out = c->g.dims[Lg];
+  // d_in: the width (and row stride) of x -- the SRU stack's input width when there is one
+  const int Lg = c->g.num_layers, d_in = gen_in_width(c), d_out = c->g.dims[Lg];
   const int dD = c->d.dims[0], nS = c->n_static;
   const bool has_d = c->w_d > 0.f;
   const bool has_adv = has_d && c->adv_w > 0.f;
@@ -687,7 +933,7 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
       gather_cols_list_kernel<<<blocks_1d(M * nS, 1024), 256, 0, st>>>(y, d_out, L.y_static, nS, static_cols, M);
       GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(y_static)");
     }
-    if ((rc = gantts_mlp_fwd(&g, x, d_in, M, y_hat, d_out, L.g_tape, L.g_tape_bytes, stream))) return rc;
+    if ((rc = generator_fwd(c, g, L, x, d_in, M, y_hat, d_out, seed, false, st))) return rc;
     if (hw && (rc = highway_gate_fwd(c, g, L, M, st))) return rc;
     if ((rc = mlpg_fwd_impl(y_hat, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
                             c->mlpg_table, &c->streams, &c->windows, c->B, c->T, stream, hwp)))
@@ -739,7 +985,7 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
       GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(y_static)");
     }
     // ---- apply_generator (train.py:336-355): G forward + MLPG
-    if ((rc = gantts_mlp_fwd(&g, x, d_in, M, y_hat, d_out, L.g_tape, L.g_tape_bytes, stream))) return rc;
+    if ((rc = generator_fwd(c, g, L, x, d_in, M, y_hat, d_out, seed, true, st))) return rc;
     if (hw && (rc = highway_gate_fwd(c, g, L, M, st))) return rc;
     if ((rc = mlpg_fwd_impl(y_hat, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
                             c->mlpg_table, &c->streams, &c->windows, c->B, c->T, stream, hwp)))
@@ -854,9 +1100,13 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
                             &c->streams, &c->windows, c->B, c->T, c->mse_w != 0.f ? 1 : 0, stream, hwp)))
       return rc;
     if (hw && (rc = highway_gate_bwd(c, g, L, M, st))) return rc;
-    if ((rc = mlp_bwd_impl(&g, direct ? nullptr : L.g_yhat, d_out, nullptr, 0, M, L.g_tape, L.g_tape_bytes, nullptr, 0, 0,
-                           pg.gW, pg.gb, 0, L.mlp_ws, L.mlp_ws_bytes, stream, -1, direct)))
+    // (SRU stack: hidden2out's input gradient is dL/dh of the top SRU layer)
+    const bool sru = c->sru.num_layers > 0;
+    if ((rc = mlp_bwd_impl(&g, direct ? nullptr : L.g_yhat, d_out, nullptr, 0, M, L.g_tape, L.g_tape_bytes,
+                           sru ? L.sru_dx : nullptr, sru ? sru_ncols(c->sru) : 0, 0, pg.gW, pg.gb, 0, L.mlp_ws, L.mlp_ws_bytes,
+                           stream, -1, direct)))
       return rc;
+    if (sru && (rc = sru_stack_bwd(c, L, pg, x, M, seed, st))) return rc;
   }
   if (phases & 4) {
     NvtxRange r4("gantts_gan_step/phase4: G step, losses");

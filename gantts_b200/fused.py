@@ -1,8 +1,8 @@
-"""Fused GAN step: ONE C call (gantts_gan_step) per mini-batch for an MLP or In2OutHighwayNet generator + MLP
+"""Fused GAN step: ONE C call (gantts_gan_step) per mini-batch for an MLP, In2OutHighwayNet or SRURNN generator + MLP
 discriminator -- the whole of reference train.py:528-580 enqueued on the current stream without a
 single host synchronisation (SURVEY.md 8f row 3).  Not drop-in for train.py (which owns its step
 functions); offered next to the compatible modular path (gantts_b200.step.GanTrainer), which also runs
-the recurrent generators.
+the LSTM generators.
 
 Data parallel: utterance shards, the two flat gradient buffers are SUM all-reduced (NCCL via
 torch.distributed on the same stream) between the phases of the step; losses are normalised by the
@@ -24,13 +24,36 @@ LOSS_NAMES = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mse", "loss_mge", "l
 
 
 def _generator_parts(model_g):
-    """(highway gate Linear or None, [hidden layers..., last_linear]) of a generator the fused step runs."""
+    """(highway gate Linear or None, [SRUCell...] (empty unless SRURNN), [MLP layers..., last layer]) of a generator the
+    fused step runs."""
     if isinstance(model_g, models.In2OutHighwayNet):
-        return model_g.T, list(model_g.H) + [model_g.last_linear]
+        return model_g.T, [], list(model_g.H) + [model_g.last_linear]
+    if isinstance(model_g, models.SRURNN):
+        return None, list(model_g.gru.rnn_lst), [model_g.hidden2out]
     if hasattr(model_g, "layers") and hasattr(model_g, "last_linear"):
-        return None, list(model_g.layers) + [model_g.last_linear]
-    raise RuntimeError("FusedGanStep: generator %s is not supported (MLP and In2OutHighwayNet are); train it with "
+        return None, [], list(model_g.layers) + [model_g.last_linear]
+    raise RuntimeError("FusedGanStep: generator %s is not supported (MLP, In2OutHighwayNet and SRURNN are); train it with "
                        "gantts_b200.step.GanTrainer" % type(model_g).__name__)
+
+
+def _fill_sru(desc, cells):
+    """The shape block of gantts_sru_stack_t from an SRU stack (rnn.SRU.rnn_lst); pointers are set by the caller."""
+    if len(cells) > _lib.MAX_SRU_LAYERS:
+        raise RuntimeError("gantts_b200: at most %d SRU layers" % _lib.MAX_SRU_LAYERS)
+    c0 = cells[0]
+    ncols = c0.n_out * (2 if c0.bidirectional else 1)
+    for i, cell in enumerate(cells):
+        same = (cell.n_out, cell.bidirectional, cell.activation_type, cell.rnn_dropout) == \
+               (c0.n_out, c0.bidirectional, c0.activation_type, c0.rnn_dropout)
+        # rnn.SRU: layer i > 0 reads the ncols outputs of the one below; every layer but the last has the stack's
+        # output dropout
+        if not same or (i > 0 and cell.n_in != ncols) or (i + 1 < len(cells) and cell.dropout != c0.dropout):
+            raise RuntimeError("FusedGanStep: the SRU layers must form one rnn.SRU stack")
+    desc.num_layers = len(cells)
+    desc.in_dim, desc.hidden, desc.bidirectional = int(c0.n_in), int(c0.n_out), int(bool(c0.bidirectional))
+    desc.act = int(c0.activation_type)
+    desc.dropout = float(c0.dropout) if len(cells) > 1 else 0.0
+    desc.rnn_dropout = float(c0.rnn_dropout)
 
 
 def _fill_mlp(desc, layers, p, last_act):
@@ -72,14 +95,14 @@ class FusedGanStep(object):
         parallel.broadcast_parameters(model_d, group=process_group)
         c = _lib.GanStepT()
         c.B, c.T = self.B, self.T
-        self._gate, g_layers = _generator_parts(model_g)
-        self._g_layers = _fill_mlp(c.g, g_layers, model_g.dropout_p, _lib.ACT_NONE)
+        self._gate, self._sru, g_layers = _generator_parts(model_g)
+        self._g_layers = _fill_mlp(c.g, g_layers, getattr(model_g, "dropout_p", 0.0), _lib.ACT_NONE)
         self._d_layers = _fill_mlp(c.d, list(model_d.layers) + [model_d.last_linear], model_d.dropout_p,
                                    _lib.ACT_SIGMOID)
         if getattr(model_g, "last_sigmoid", False) or not model_d.last_sigmoid:
             raise RuntimeError("FusedGanStep: generator must be linear-output, discriminator sigmoid-output")
-        # the generator's modules with parameters, in model_g.parameters() order (the gate first)
-        self._g_mods = ([self._gate] if self._gate is not None else []) + self._g_layers
+        # the generator's modules with parameters, in model_g.parameters() order (the gate or the SRU layers first)
+        self._g_mods = ([self._gate] if self._gate is not None else []) + self._sru + self._g_layers
         self._sums, self._sqs = [], []      # Adagrad: state_sum | Adam: exp_avg, exp_avg_sq (model.parameters() order)
 
         def new_state(l):
@@ -101,6 +124,18 @@ class FusedGanStep(object):
             h.sumW, h.sumb = a.data_ptr(), b.data_ptr()
             if a2 is not None:
                 h.sqW, h.sqb = a2.data_ptr(), b2.data_ptr()
+        if self._sru:
+            su = c.sru
+            _fill_sru(su, self._sru)
+            for i, cell in enumerate(self._sru):
+                ops.require_cuda(cell.weight, cell.bias)
+                if not (cell.weight.is_contiguous() and cell.bias.is_contiguous()):
+                    raise RuntimeError("gantts_b200: parameters must be contiguous")
+                su.W[i], su.b[i] = cell.weight.data_ptr(), cell.bias.data_ptr()
+                a, b, a2, b2 = new_state(cell)
+                su.sumW[i], su.sumb[i] = a.data_ptr(), b.data_ptr()
+                if a2 is not None:
+                    su.sqW[i], su.sqb[i] = a2.data_ptr(), b2.data_ptr()
         for layers, sw, sb, qw, qb in ((self._g_layers, c.g_sumW, c.g_sumb, c.g_sqW, c.g_sqb),
                                        (self._d_layers, c.d_sumW, c.d_sumb, c.d_sqW, c.d_sqb)):
             for i, l in enumerate(layers):
@@ -190,6 +225,8 @@ class FusedGanStep(object):
                 desc.W[i], desc.b[i] = l.weight.data_ptr(), l.bias.data_ptr()
         if self._gate is not None:
             self.cfg.highway.W, self.cfg.highway.b = self._gate.weight.data_ptr(), self._gate.bias.data_ptr()
+        for i, cell in enumerate(self._sru):
+            self.cfg.sru.W[i], self.cfg.sru.b[i] = cell.weight.data_ptr(), cell.bias.data_ptr()
         if train is None:
             if self.g.training != self.d.training:
                 raise RuntimeError("FusedGanStep: generator and discriminator disagree on train()/eval()")

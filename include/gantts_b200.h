@@ -323,6 +323,31 @@ typedef struct {
   float *sqW, *sqb;                        /* Adam exp_avg_sq (unused by Adagrad) */
 } gantts_highway_t;
 
+/* SRURNN generator (reference gantts/models.py:144-167, hparams.py `tts_acoustic` / `tts_duration`): num_layers > 0.
+ * Then g is hidden2out alone (g.num_layers == 1, g.dims[0] = ncols = hidden * (bidirectional ? 2 : 1)) and the step
+ * runs the SRU stack of gantts_sru_fwd in front of it.  Layer l has n_in = in_dim (l = 0) or ncols, k = 4 when
+ * n_in != ncols else 3, weight W[l] [n_in][ncols * k] and bias b[l] [2 * ncols] = forget | reset (the SRUCell layout).
+ * In training, layer l multiplies its GEMM input (only: the highway term keeps the unmasked input) by the variational
+ * mask gantts_dropout(ones[B][n_in], rnn_dropout, gantts_sru_mask_seed(seed, l, 0)) and, for every layer but the last,
+ * g(c_t) by gantts_dropout(ones[B][ncols], dropout, gantts_sru_mask_seed(seed, l, 1)); both are shared over time.
+ * The reverse direction starts at the padded frame T - 1: the generator ignores `lengths` like the reference's SRURNN.
+ * The stack's tensors come FIRST in model.parameters() order (gru.rnn_lst.0.weight, .0.bias, ..., then hidden2out)
+ * in the flat gradient buffer, the clip norm, and the optimiser step.  A conditioned D has d.dims[0] = in_dim + n_adv.
+ * Mutually exclusive with the highway block. */
+#define GANTTS_MAX_SRU_LAYERS 8
+typedef struct {
+  int num_layers;                          /* 0 = no SRU stack (all other generators) */
+  int in_dim, hidden, bidirectional;
+  int act;                                 /* 0 identity, 1 tanh, 2 relu */
+  float dropout, rnn_dropout;              /* each in [0, 1) */
+  const float* W[GANTTS_MAX_SRU_LAYERS];   /* [n_in][ncols * k], updated in place */
+  const float* b[GANTTS_MAX_SRU_LAYERS];   /* [2 * ncols], updated in place */
+  float* sumW[GANTTS_MAX_SRU_LAYERS];      /* Adagrad state_sum | Adam exp_avg */
+  float* sumb[GANTTS_MAX_SRU_LAYERS];
+  float* sqW[GANTTS_MAX_SRU_LAYERS];       /* Adam exp_avg_sq (unused by Adagrad) */
+  float* sqb[GANTTS_MAX_SRU_LAYERS];
+} gantts_sru_stack_t;
+
 typedef struct {
   int B, T;
   gantts_mlp_t g;                          /* generator: dims[0] = linguistic width, dims[L] = acoustic width */
@@ -355,6 +380,7 @@ typedef struct {
   float* d_sqW[GANTTS_MAX_LAYERS];
   float* d_sqb[GANTTS_MAX_LAYERS];
   gantts_highway_t highway;                /* static_dim = 0: plain MLP generator (all fields above keep their offsets) */
+  gantts_sru_stack_t sru;                  /* num_layers = 0: no SRU stack (all fields above keep their offsets) */
 } gantts_gan_step_t;
 #define GANTTS_OPT_ADAGRAD 0
 #define GANTTS_OPT_ADAM 1
@@ -375,6 +401,10 @@ typedef struct {
  * run with seed s draws its mask as gantts_dropout(ones[rows][dims[l+1]], p, gantts_mlp_layer_seed(s, l)). */
 uint64_t gantts_gan_step_seed(uint64_t seed, int which);
 uint64_t gantts_mlp_layer_seed(uint64_t seed, int layer);
+/* Seed of SRU layer `layer`'s masks in a step called with `seed`: which = 0 the variational input mask [B][n_in],
+ * 1 the output mask [B][ncols].  A stream of its own (gantts_mlp_layer_seed(gantts_gan_step_seed(seed, 3), 2 layer +
+ * which)), apart from the three MLP forwards above. */
+uint64_t gantts_sru_mask_seed(uint64_t seed, int layer, int which);
 
 size_t gantts_gan_step_workspace_bytes(const gantts_gan_step_t* cfg);
 /* Flat gradient buffer inside `workspace` (which: 0 = generator, 1 = discriminator). */

@@ -1,0 +1,482 @@
+"""The fused GAN step (gantts_gan_step / FusedGanStep) with the SRURNN generator of hparams `tts_acoustic` and
+`tts_duration` (reference gantts/models.py:144-167): the SRU stack's GEMMs and scans, its backward and its optimiser
+step inside the one-call step.
+
+The checker is the CPU restatement of the SRU recurrence in oracle/gantts_port.py (sru_layer_forward) composed into an
+SRURNN below; SRU parity with the upstream `cuda_functional` package stays unpinned (it is not vendored).  Train-mode
+parity injects the step's own masks: every SRU mask is gantts_dropout(ones, p, gantts_sru_mask_seed(seed, layer, which)),
+the discriminator's masks come from gantts_gan_step_seed as in test_gpu_fused_highway.py.  Tolerances: losses, outputs
+and gradient norms 2e-4 relative; post-step weights median |delta| < 5e-6 and max <= 0.0201 (a first Adagrad / Adam
+step moves a weight by lr * sign(g)).  The configuration-rule test is host-only (no mark).
+"""
+import ctypes
+
+import numpy as np
+import pytest
+import torch
+
+from conftest import WINDOWS, TTS_HP, rel_err
+from oracle import gantts_port as gp
+from oracle import nnmnkwii_port as nnp
+
+ACOUSTIC_HP = dict(TTS_HP, discriminator_linguistic_condition=True)
+DURATION_HP = dict(stream_sizes=[5], has_dynamic_features=[False], adversarial_streams=[True],
+                   mask_nth_mgc_for_adv_loss=0, num_windows=1, discriminator_linguistic_condition=True)
+LOSS_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mge", "loss_mse", "loss_adv", "loss_g")
+TOL = 2e-4
+
+
+@pytest.fixture(scope="module")
+def dev():
+    import __graft_entry__
+    __graft_entry__.build()
+    return torch.device("cuda:0")
+
+
+def npy(t):
+    return t.detach().cpu().numpy()
+
+
+def step_hp(ohp):
+    from gantts_b200 import step as gstep
+    return gstep.HParams(windows=WINDOWS[:ohp["num_windows"]], stream_sizes=ohp["stream_sizes"],
+                         has_dynamic_features=ohp["has_dynamic_features"],
+                         adversarial_streams=ohp["adversarial_streams"],
+                         mask_nth_mgc_for_adv_loss=ohp["mask_nth_mgc_for_adv_loss"],
+                         discriminator_linguistic_condition=ohp["discriminator_linguistic_condition"])
+
+
+def ragged_lengths(B, T, seed):
+    rng = np.random.RandomState(seed)
+    return sorted([T] + [int(v) for v in rng.randint(T // 2, T, B - 1)], reverse=True)
+
+
+def make_batch(B, T, d_in, d_out, lens, seed):
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(B, T, d_in, generator=g)
+    y = torch.randn(B, T, d_out, generator=g)
+    for b, n in enumerate(lens):
+        x[b, n:] = 0
+        y[b, n:] = 0
+    return x, y
+
+
+def sd_numpy(m):
+    return {k: v.detach().cpu().numpy() for k, v in m.state_dict().items()}
+
+
+def sru_models(seed, in_dim, out_dim, layers, hidden, bidir, relu, p, rnn_p, d_hidden, d_layers, d_p, n_adv):
+    import gantts_b200
+    torch.manual_seed(seed)
+    mg = gantts_b200.models.SRURNN(in_dim=in_dim, out_dim=out_dim, num_hidden=layers, hidden_dim=hidden,
+                                   bidirectional=bidir, dropout=p, use_relu=int(relu), rnn_dropout=rnn_p)
+    for cell in mg.gru.rnn_lst:                        # non-zero forget / reset biases
+        cell.bias.data.uniform_(-0.5, 0.5)
+    md = gantts_b200.models.MLP(in_dim + n_adv, 1, d_layers, d_hidden, dropout=d_p, last_sigmoid=True)
+    return mg, md
+
+
+class SruOracle(object):
+    """CPU SRURNN for gp.gan_step built from the model's state_dict (gru.rnn_lst.{i}.weight / .bias, hidden2out.*):
+    gp.sru_layer_forward per layer with injected masks, then hidden2out.  ``named`` / ``params()`` follow
+    model_g.parameters() order; ``sums`` is the Adagrad state."""
+
+    def __init__(self, sd, bidirectional, act):
+        t = lambda k: torch.as_tensor(np.asarray(sd[k])).clone().float().requires_grad_(True)
+        n = len([k for k in sd if k.startswith("gru.rnn_lst.") and k.endswith(".weight")])
+        self.named = {}
+        for i in range(n):
+            for s in ("weight", "bias"):
+                self.named["gru.rnn_lst.%d.%s" % (i, s)] = t("gru.rnn_lst.%d.%s" % (i, s))
+        self.named["hidden2out.weight"], self.named["hidden2out.bias"] = t("hidden2out.weight"), t("hidden2out.bias")
+        self.n, self.bidir, self.act = n, bidirectional, act
+        self.sums = [torch.zeros_like(p) for p in self.params()]
+
+    def params(self):
+        return list(self.named.values())
+
+    def forward(self, x, R, hp, masks=None):
+        """(y_hat, y_hat_static); masks = [(mask_x [B][n_in], mask_h [B][ncols] or None)] per layer, or None."""
+        dirs = 2 if self.bidir else 1
+        h = x
+        for i in range(self.n):
+            W, b = self.named["gru.rnn_lst.%d.weight" % i], self.named["gru.rnn_lst.%d.bias" % i]
+            nc = b.numel() // 2
+            bport = torch.stack([b[:nc].view(dirs, nc // dirs), b[nc:].view(dirs, nc // dirs)], 1).reshape(-1)
+            mx, mh = masks[i] if masks is not None else (None, None)
+            h = gp.sru_layer_forward(h.transpose(0, 1), W, bport, bidirectional=self.bidir, use_tanh=self.act == 1,
+                                     use_relu=self.act == 2, mask_x=mx, mask_h=mh).transpose(0, 1)
+        y_hat = torch.nn.functional.linear(h, self.named["hidden2out.weight"], self.named["hidden2out.bias"])
+        return gp.apply_generator(y_hat, x, R, hp)
+
+
+def sru_masks(fs, mg, B, dev):
+    """The SRU masks the last training step of `fs` drew."""
+    from gantts_b200 import ops, _lib
+    lib = _lib.load()
+    cells = list(mg.gru.rnn_lst)
+    out = []
+    for i, cell in enumerate(cells):
+        nc = cell.n_out * (2 if cell.bidirectional else 1)
+        mx = ops.dropout_mask(B, cell.n_in, cell.rnn_dropout, lib.gantts_sru_mask_seed(fs.last_seed, i, 0), dev).cpu()
+        mh = ops.dropout_mask(B, nc, cell.dropout, lib.gantts_sru_mask_seed(fs.last_seed, i, 1), dev).cpu() \
+            if i + 1 < len(cells) else None
+        out.append((mx, mh))
+    return out
+
+
+def d_masks(fs, M, d_hidden, p, dev):
+    from gantts_b200 import ops, _lib
+    lib = _lib.load()
+    s = fs.last_seed
+    stacked = ops.mlp_dropout_masks(2 * M, d_hidden, p, lib.gantts_gan_step_seed(s, 1), dev)
+    return {"real": [m[:M].cpu() for m in stacked], "fake": [m[M:].cpu() for m in stacked],
+            "adv": [m.cpu() for m in ops.mlp_dropout_masks(M, d_hidden, p, lib.gantts_gan_step_seed(s, 2), dev)]}
+
+
+def adv_loss_with(md, x, ys_ref, lens, ohp, adv_masks):
+    """loss_adv of the oracle's y_hat_static through the PRODUCT's updated discriminator.  The adversarial forward runs
+    after the discriminator's first Adagrad / Adam step, which moves every weight by about lr * sign(g): a weight whose
+    gradient is within rounding of zero lands 2 lr apart in the two implementations, and at the conditioned D's 483
+    inputs those few weights move loss_adv by a few 1e-4.  With the product's D on both sides the comparison isolates
+    the generator's output and the loss arithmetic."""
+    ps = list(md.parameters())
+    layers = [(w.detach().cpu(), b.detach().cpu()) for w, b in zip(ps[0::2], ps[1::2])]
+    fake_in = gp.get_selected_static_stream(ys_ref, ohp)
+    if ohp["discriminator_linguistic_condition"]:
+        fake_in = torch.cat((x, fake_in), -1)
+    mask = gp.sequence_mask(lens, x.size(1)).unsqueeze(-1)
+    D = gp.mlp_forward(fake_in, layers, last_sigmoid=True, masks=adv_masks)
+    return float(gp.bce_real(D, mask, mask.sum().item()))
+
+
+def loss_errors(got, ref, keys):
+    return {k: abs(float(got[k]) - ref[k]) / max(abs(ref[k]), 1e-12) for k in keys}
+
+
+def check_weights(params, ref_params, tag):
+    for i, (q, r) in enumerate(zip(params, ref_params)):
+        d = np.abs(npy(q) - r.detach().numpy())
+        assert np.median(d) < 5e-6 and d.max() <= 0.0201, (tag, i, np.median(d), d.max())
+
+
+def resync(mg, md, fs, gen, d_layers, d_sum):
+    """Start the oracle's next step from the product's weights and Adagrad state."""
+    with torch.no_grad():
+        for r, q in zip(gen.params(), mg.parameters()):
+            r.copy_(q.detach().cpu())
+        for r, q in zip([t for pair in d_layers for t in pair], md.parameters()):
+            r.copy_(q.detach().cpu())
+        ng = len(gen.params())
+        for r, s in zip(gen.sums + d_sum, fs._sums[:ng] + fs._sums[ng:]):
+            r.copy_(s.cpu())
+
+
+def run_vs_oracle(dev, mg, md, ohp, B, T, steps, mse_w, p_d, d_hidden, seed, tag, with_outputs=True):
+    from gantts_b200 import fused
+    in_dim = mg.gru.rnn_lst[0].n_in
+    out_dim = mg.hidden2out.weight.shape[0]
+    relu = mg.gru.rnn_lst[0].activation_type
+    gen = SruOracle(sd_numpy(mg), mg.gru.rnn_lst[0].bidirectional, relu)
+    d_layers = gp.discriminator_layers(sd_numpy(md))
+    d_sum = [torch.zeros_like(t) for pair in d_layers for t in pair]
+    mg.to(dev).train(), md.to(dev).train()
+    fs = fused.FusedGanStep(mg, md, step_hp(ohp), B, T, w_d=1.0, mse_w=mse_w, mge_w=1.0, weight_decay=0.0, seed=seed)
+    R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, T))
+    for it in range(steps):
+        lens = ragged_lengths(B, T, seed + 10 * it)
+        x, y = make_batch(B, T, in_dim, out_dim, lens, seed + 10 * it + 1)
+        fs.step(x.to(dev), y.to(dev), torch.LongTensor(lens).to(dev), frames=sum(lens))
+        got = fs.loss_dict()
+        gm, dm = sru_masks(fs, mg, B, dev), d_masks(fs, B * T, [d_hidden] * (len(d_layers) - 1), p_d, dev)
+        ref, yh_ref, ys_ref = gp.gan_step(lambda: gen.forward(x, R, ohp, gm), gen.params(), gen.sums, d_layers, d_sum,
+                                          x, y, lens, R, ohp, w_d=1.0, mse_w=mse_w, mge_w=1.0, adv_w=1.0, dropout_d=p_d,
+                                          training=True, weight_decay=0.0, d_masks=dm)
+        ref = dict(ref, loss_adv=adv_loss_with(md, x, ys_ref, lens, ohp, dm["adv"]))
+        errs = loss_errors(got, ref, LOSS_KEYS + ("d_grad_norm", "g_grad_norm"))
+        if with_outputs:
+            errs["y_hat"] = rel_err(npy(fs.y_hat), yh_ref.numpy())
+            errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), ys_ref.numpy())
+        assert max(errs.values()) < TOL, (tag, it, errs)
+        assert abs(got["real_correct"] - ref["real_correct"]) <= 3 and abs(got["fake_correct"] - ref["fake_correct"]) <= 3
+        check_weights(list(mg.parameters()), gen.params(), "%s step %d" % (tag, it))
+        resync(mg, md, fs, gen, d_layers, d_sum)
+    return fs
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("mse_w", [0.0, 1.0])
+@pytest.mark.parametrize("k0", [4, 3])
+@pytest.mark.parametrize("relu", [True, False])
+@pytest.mark.parametrize("bidir", [True, False])
+def test_fused_sru_toy_vs_oracle(dev, bidir, relu, k0, mse_w):
+    """A small SRURNN (3 layers, 16 hidden units per direction; layer 0 with k = 4 or, when in_dim = ncols, k = 3) on the
+    tts_acoustic stream layout with a conditioned D, dropout 0.2 / rnn_dropout 0.2 in G and 0.5 in D, two training steps
+    against the oracle.  mse_w = 0 takes the MLPG adjoint that writes the operand planes directly, 1 the fp32 one."""
+    nc = 16 * (2 if bidir else 1)
+    in_dim = nc if k0 == 3 else 20
+    mg, md = sru_models(100 + 8 * bidir + 4 * relu + k0, in_dim, 187, 3, 16, bidir, relu, 0.2, 0.2, 32, 3, 0.5, 58)
+    assert mg.gru.rnn_lst[0].k == k0
+    run_vs_oracle(dev, mg, md, ACOUSTIC_HP, 3, 40, 2, mse_w, 0.5, 32, 200 + k0, "toy")
+
+
+@pytest.mark.gpu
+def test_fused_sru_tts_acoustic_full_width(dev):
+    """hparams tts_acoustic: SRURNN 425 -> 6 x 512 bidirectional ReLU -> 187, dropout 0.2, rnn_dropout 0.2; D 483 ->
+    256 x 3 -> 1 conditioned on x, dropout 0.5; Adagrad.  B = 4 x T = 200 ragged, train mode, one step against the
+    oracle: the losses, y_hat, y_hat_static, both gradient norms and every updated generator weight."""
+    mg, md = sru_models(7, 425, 187, 6, 512, True, True, 0.2, 0.2, 256, 3, 0.5, 58)
+    run_vs_oracle(dev, mg, md, ACOUSTIC_HP, 4, 200, 1, 0.0, 0.5, 256, 300, "tts_acoustic")
+
+
+@pytest.mark.gpu
+def test_fused_sru_tts_duration_adam_and_resume(dev):
+    """hparams tts_duration: SRURNN 416 -> 6 x 512 bidirectional ReLU -> 5 (one static stream), D 421 -> 256 x 3 -> 1
+    conditioned, Adam lr 1e-3 betas (0.5, 0.9).  Three steps against the oracle's Adam, each starting from the product's
+    weights and moments; then a step resumed from state_dict() is bit-identical to the uninterrupted one."""
+    from gantts_b200 import fused
+    B, T, p, pd = 4, 128, 0.2, 0.5
+    okw = dict(lr=1e-3, betas=(0.5, 0.9), weight_decay=0.0, eps=1e-8)
+
+    def build():
+        return sru_models(11, 416, 5, 6, 512, True, True, p, p, 256, 3, pd, 5)
+    mg, md = build()
+    gen = SruOracle(sd_numpy(mg), True, 2)
+    d_layers = gp.discriminator_layers(sd_numpy(md))
+    d_params = [t for pair in d_layers for t in pair]
+    g_opt, d_opt = gp.AdamStepper(gen.params(), **okw), gp.AdamStepper(d_params, **okw)
+    mg.to(dev).train(), md.to(dev).train()
+    hp = step_hp(DURATION_HP)
+    fs = fused.FusedGanStep(mg, md, hp, B, T, w_d=1.0, mse_w=1.0, mge_w=0.0, seed=12, optimizer="Adam",
+                            optimizer_params=okw)
+    for it in range(3):
+        lens = ragged_lengths(B, T, 40 + it)
+        x, y = make_batch(B, T, 416, 5, lens, 50 + it)
+        fs.step(x.to(dev), y.to(dev), torch.LongTensor(lens).to(dev), frames=sum(lens))
+        got = fs.loss_dict()
+        gm, dm = sru_masks(fs, mg, B, dev), d_masks(fs, B * T, [256] * 3, pd, dev)
+        ref, yh_ref, ys_ref = gp.gan_step(lambda: gen.forward(x, None, DURATION_HP, gm), gen.params(), None, d_layers,
+                                          None, x, y, lens, None, DURATION_HP, w_d=1.0, mse_w=1.0, mge_w=0.0, adv_w=1.0,
+                                          dropout_d=pd, training=True, d_masks=dm, d_opt=d_opt, g_opt=g_opt)
+        ref = dict(ref, loss_adv=adv_loss_with(md, x, ys_ref, lens, DURATION_HP, dm["adv"]))
+        errs = loss_errors(got, ref, ("loss_d", "loss_mse", "loss_adv", "loss_g", "d_grad_norm", "g_grad_norm"))
+        errs["y_hat"] = rel_err(npy(fs.y_hat), yh_ref.numpy())
+        errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), ys_ref.numpy())
+        assert max(errs.values()) < TOL, (it, errs)
+        sd = fs.state_dict()
+        for mod, params, key, st in ((mg, gen.params(), "optimizer_g", g_opt), (md, d_params, "optimizer_d", d_opt)):
+            check_weights(list(mod.parameters()), params, "tts_duration %s step %d" % (key, it))
+            with torch.no_grad():
+                for i, (q, r) in enumerate(zip(mod.parameters(), params)):
+                    r.copy_(q.detach().cpu())
+                    st.m[i].copy_(sd[key]["state"][i]["exp_avg"].cpu())
+                    st.v[i].copy_(sd[key]["state"][i]["exp_avg_sq"].cpu())
+    snap = [q.detach().clone() for q in list(mg.parameters()) + list(md.parameters())]
+    sd = fs.state_dict()
+    lens = ragged_lengths(B, T, 60)
+    x, y = make_batch(B, T, 416, 5, lens, 61)
+    xd, yd, ld = x.to(dev), y.to(dev), torch.LongTensor(lens).to(dev)
+    fs.step(xd, yd, ld)
+    want = fs.loss_dict()
+    after = [q.detach().clone() for q in list(mg.parameters()) + list(md.parameters())]
+    g2, d2 = build()
+    g2.to(dev).train(), d2.to(dev).train()
+    with torch.no_grad():
+        for q, v in zip(list(g2.parameters()) + list(d2.parameters()), snap):
+            q.copy_(v)
+    fs2 = fused.FusedGanStep(g2, d2, hp, B, T, w_d=1.0, mse_w=1.0, mge_w=0.0, seed=999, optimizer="Adam",
+                             optimizer_params=okw)
+    fs2.load_state_dict(sd)
+    fs2.step(xd, yd, ld)
+    assert fs2.loss_dict() == want
+    for q, v in zip(list(g2.parameters()) + list(d2.parameters()), after):
+        assert torch.equal(q.detach(), v)
+
+
+@pytest.mark.gpu
+def test_fused_sru_matches_gan_trainer(dev):
+    """tts_acoustic widths with every dropout 0: two training steps of FusedGanStep and of the modular GanTrainer from
+    the same weights agree on the losses, y_hat, y_hat_static and the updated weights; so do their eval phases on the
+    same weights (the fused step's, copied over: a first Adagrad step moves a weight whose gradient is near zero by
+    +-lr on either side, which alone moves the outputs by more than the tolerance)."""
+    from gantts_b200 import fused, step as gstep
+    B, T = 4, 200
+    hp = step_hp(ACOUSTIC_HP)
+    mk = lambda: sru_models(21, 425, 187, 6, 512, True, True, 0.0, 0.0, 256, 3, 0.0, 58)
+    (mg, md), (tg, td) = mk(), mk()
+    for m in (mg, md, tg, td):
+        m.to(dev).train()
+    fs = fused.FusedGanStep(mg, md, hp, B, T, w_d=1.0, mse_w=0.5, mge_w=1.0, weight_decay=0.0, seed=22)
+    tr = gstep.GanTrainer(tg, td, hp, w_d=1.0, mse_w=0.5, mge_w=1.0, weight_decay=0.0)
+    R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, T)).to(dev)
+    for it in range(3):
+        train = it < 2
+        if not train:
+            with torch.no_grad():
+                for a, b in zip(list(mg.parameters()) + list(md.parameters()),
+                                list(tg.parameters()) + list(td.parameters())):
+                    b.copy_(a)
+            for m in (mg, md, tg, td):
+                m.eval()
+        lens = ragged_lengths(B, T, 23 + it)
+        x, y = make_batch(B, T, 425, 187, lens, 24 + it)
+        xd, yd = x.to(dev), y.to(dev)
+        fs.step(xd, yd, torch.LongTensor(lens).to(dev))
+        got = fs.loss_dict()
+        out, yh, ys = tr.step(xd, yd, lens, R, train=train)
+        errs = loss_errors(got, {k: float(out[k]) for k in LOSS_KEYS}, LOSS_KEYS)
+        errs["y_hat"] = rel_err(npy(fs.y_hat), npy(yh))
+        errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), npy(ys))
+        assert max(errs.values()) < TOL, (it, errs)
+        for i, (a, b) in enumerate(zip(list(mg.parameters()) + list(md.parameters()),
+                                       list(tg.parameters()) + list(td.parameters()))):
+            d = np.abs(npy(a) - npy(b))
+            assert np.median(d) < 5e-6 and d.max() <= 0.0201, (it, i, np.median(d), d.max())
+
+
+@pytest.mark.gpu
+def test_fused_sru_invariants(dev):
+    """An eval-phase call leaves every parameter and all optimiser state bit-unchanged; phases 1, 2 and 4 called one by
+    one give exactly what one call gives, and grad_buffer(0) holds every generator parameter in model_g.parameters()
+    order; state_dict()'s generator part loads into torch.optim.Adagrad(model_g.parameters())."""
+    from gantts_b200 import fused
+    B, T = 3, 60
+    hp = step_hp(ACOUSTIC_HP)
+    lens = ragged_lengths(B, T, 31)
+    x, y = make_batch(B, T, 30, 187, lens, 32)
+    xd, yd, ld = x.to(dev), y.to(dev), torch.LongTensor(lens).to(dev)
+    runs = []
+    for split in (False, True):
+        mg, md = sru_models(33, 30, 187, 3, 24, True, True, 0.2, 0.2, 32, 3, 0.5, 58)
+        mg.to(dev).train(), md.to(dev).train()
+        fs = fused.FusedGanStep(mg, md, hp, B, T, mse_w=0.5, weight_decay=0.0, seed=34)
+        if split:
+            fs.cfg.adv_w, fs._step, fs.cfg.opt_step = 1.0, 1, 1
+            for ph in (1, 2, 4):
+                fs._call(ph, xd, yd, ld, 0.0, fs._seed)
+        else:
+            fs.step(xd, yd, ld)
+            assert fs.last_seed == fs._seed
+        gb = fs.grad_buffer(0)
+        params = list(mg.parameters())
+        assert gb.numel() == sum(q.numel() for q in params)
+        off = 0
+        for q, s in zip(params, fs._sums):                 # weight decay 0: Adagrad's first state_sum = g^2
+            n = q.numel()
+            assert torch.equal((gb[off:off + n] * gb[off:off + n]).view_as(q), s)
+            off += n
+        runs.append([fs.losses.clone(), fs.y_hat.clone(), fs.y_hat_static.clone(), gb.clone(), fs.grad_buffer(1).clone()]
+                    + [q.detach().clone() for q in list(mg.parameters()) + list(md.parameters())]
+                    + [s.clone() for s in fs._sums])
+    for a, b in zip(*runs):
+        assert torch.equal(a, b)
+    # eval phase: nothing changes
+    wsnap = [q.detach().clone() for q in list(mg.parameters()) + list(md.parameters())]
+    ssnap = [s.clone() for s in fs._sums]
+    mg.eval(), md.eval()
+    fs.step(xd, yd, ld)
+    assert fs.loss_dict()["g_grad_norm"] == 0.0
+    for a, b in zip(wsnap, list(mg.parameters()) + list(md.parameters())):
+        assert torch.equal(a, b.detach())
+    for a, b in zip(ssnap, fs._sums):
+        assert torch.equal(a, b)
+    sd = fs.state_dict()
+    opt = torch.optim.Adagrad(mg.parameters(), lr=0.01, weight_decay=0.0)
+    opt.load_state_dict(sd["optimizer_g"])
+    first = mg.gru.rnn_lst[0].weight
+    assert torch.equal(opt.state[first]["sum"], fs._sums[0])
+    assert len(sd["optimizer_g"]["state"]) == len(list(mg.parameters()))
+
+
+@pytest.mark.gpu
+def test_fused_sru_rejects_sigmoid_output(dev):
+    """An SRURNN with last_sigmoid=True is refused like any sigmoid-output generator."""
+    import gantts_b200
+    from gantts_b200 import fused
+    mg = gantts_b200.models.SRURNN(in_dim=20, out_dim=187, num_hidden=2, hidden_dim=8, last_sigmoid=True).to(dev)
+    md = gantts_b200.models.MLP(58, 1, 2, 16, dropout=0.0, last_sigmoid=True).to(dev)
+    with pytest.raises(RuntimeError, match="linear-output"):
+        fused.FusedGanStep(mg, md, step_hp(TTS_HP), 2, 10)
+
+
+def _sru_step_config():
+    """A valid SRURNN configuration of gantts_gan_step_t on the tts_acoustic layout with a conditioned D (host pointers
+    are placeholders: only the configuration check and the workspace layout run)."""
+    from gantts_b200 import _lib, multistream, step as gstep
+    fake, in_dim, hidden, nl = 1 << 20, 40, 16, 3
+    c = _lib.GanStepT()
+    c.B, c.T = 2, 16
+    c.g.num_layers = 1
+    c.g.dims[0], c.g.dims[1] = 2 * hidden, 187
+    c.d.num_layers = 2
+    for i, v in enumerate((in_dim + 58, 32, 1)):
+        c.d.dims[i] = v
+    for m in (c.g, c.d):
+        for i in range(m.num_layers):
+            m.W[i] = m.b[i] = fake
+    c.g_sumW[0] = c.g_sumb[0] = fake
+    c.g.last_act, c.d.last_act = _lib.ACT_NONE, _lib.ACT_SIGMOID
+    hp = gstep.TTS_ACOUSTIC
+    entries, n_static = multistream.mlpg_stream_entries(hp.stream_sizes, hp.has_dynamic_features, [True] * 4, 3)
+    c.streams = _lib.make_streams(entries)
+    c.windows = _lib.make_windows(WINDOWS)
+    c.mlpg_table = fake
+    c.n_static = c.n_static_cols = n_static
+    for i in range(n_static):
+        c.static_cols[i] = i
+    c.n_adv = 58
+    for i in range(58):
+        c.adv_cols[i] = 2 + i
+    c.d_conditioned = 1
+    c.w_d, c.mge_w, c.adv_w, c.max_norm, c.lr_g, c.lr_d, c.eps = 1.0, 1.0, 1.0, 1.0, 0.01, 0.01, 1e-10
+    c.optimizer = _lib.OPT_ADAGRAD
+    s = c.sru
+    s.num_layers, s.in_dim, s.hidden, s.bidirectional, s.act = nl, in_dim, hidden, 1, 2
+    s.dropout, s.rnn_dropout = 0.2, 0.2
+    for i in range(nl):
+        s.W[i] = s.b[i] = s.sumW[i] = s.sumb[i] = fake
+    return c
+
+
+def test_sru_step_config_rules():
+    """gantts_gan_step_workspace_bytes (host-only) accepts the SRURNN layout, lays out no SRU workspace without a stack,
+    and rejects, with a message naming the rule, every SRU configuration the step does not implement."""
+    import __graft_entry__
+    __graft_entry__.build()
+    from gantts_b200 import _lib
+    lib = _lib.load()
+    ws = lambda c: lib.gantts_gan_step_workspace_bytes(ctypes.byref(c))
+    err = lambda: lib.gantts_last_error_string().decode()
+    assert lib.gantts_version() == 103
+    c = _sru_step_config()
+    assert ws(c) > 0, err()
+    with_sru = ws(c)
+    c.sru.num_layers = 0                                # the same config without a stack: D then sees g.dims[0] columns
+    c.d.dims[0] = 32 + 58
+    assert 0 < ws(c) < with_sru, err()
+
+    def rejected(mutate, needle):
+        c = _sru_step_config()
+        mutate(c)
+        assert ws(c) == 0 and needle in err(), (needle, err())
+    rejected(lambda c: setattr(c.highway, "static_dim", 59), "mutually exclusive")
+    rejected(lambda c: setattr(c.sru, "num_layers", _lib.MAX_SRU_LAYERS + 1), "SRU layer count")
+    rejected(lambda c: setattr(c.sru, "num_layers", -1), "SRU layer count")
+    rejected(lambda c: setattr(c.sru, "act", 3), "activation")
+    rejected(lambda c: setattr(c.sru, "dropout", 1.0), "dropout")
+    rejected(lambda c: setattr(c.sru, "rnn_dropout", -0.1), "dropout")
+    rejected(lambda c: c.g.dims.__setitem__(0, 31), "hidden2out")
+    rejected(lambda c: setattr(c.g, "num_layers", 2), "hidden2out")
+    rejected(lambda c: c.sru.W.__setitem__(2, None), "null SRU weight")
+    rejected(lambda c: c.sru.b.__setitem__(0, None), "null SRU weight")
+    rejected(lambda c: c.sru.sumb.__setitem__(1, None), "optimiser state")
+
+    def adam(c):                                         # exp_avg_sq for every SRU layer but the last
+        c.optimizer, c.beta1, c.beta2 = _lib.OPT_ADAM, 0.5, 0.9
+        for i in range(c.sru.num_layers - 1):
+            c.sru.sqW[i] = c.sru.sqb[i] = 1 << 20
+    rejected(adam, "exp_avg_sq for SRU layer 2")
+    rejected(lambda c: c.d.dims.__setitem__(0, 32 + 58), "discriminator input width")
+    # the seeds of the SRU masks are a stream of their own
+    seeds = {lib.gantts_sru_mask_seed(5, l, w) for l in range(8) for w in range(2)}
+    assert len(seeds) == 16 and not seeds & {lib.gantts_gan_step_seed(5, w) for w in range(3)}
