@@ -83,6 +83,19 @@ class SruStackT(ctypes.Structure):
                 ("sqW", ctypes.c_void_p * MAX_SRU_LAYERS), ("sqb", ctypes.c_void_p * MAX_SRU_LAYERS)]
 
 
+MAX_LSTM_LAYERS = 3
+_LstmPtrs = (ctypes.c_void_p * 2) * MAX_LSTM_LAYERS       # [layer][direction]
+
+
+class LstmStackT(ctypes.Structure):
+    _fields_ = [("num_layers", ctypes.c_int),
+                ("in_dim", ctypes.c_int), ("hidden", ctypes.c_int), ("bidirectional", ctypes.c_int),
+                ("dropout", ctypes.c_float),
+                ("W_ih", _LstmPtrs), ("W_hh", _LstmPtrs), ("b_ih", _LstmPtrs), ("b_hh", _LstmPtrs),
+                ("sumW_ih", _LstmPtrs), ("sumW_hh", _LstmPtrs), ("sumb_ih", _LstmPtrs), ("sumb_hh", _LstmPtrs),
+                ("sqW_ih", _LstmPtrs), ("sqW_hh", _LstmPtrs), ("sqb_ih", _LstmPtrs), ("sqb_hh", _LstmPtrs)]
+
+
 class GanStepT(ctypes.Structure):
     _fields_ = [("B", ctypes.c_int), ("T", ctypes.c_int),
                 ("g", MlpT), ("d", MlpT),
@@ -103,7 +116,8 @@ class GanStepT(ctypes.Structure):
                 ("g_sqW", ctypes.c_void_p * MAX_LAYERS), ("g_sqb", ctypes.c_void_p * MAX_LAYERS),
                 ("d_sqW", ctypes.c_void_p * MAX_LAYERS), ("d_sqb", ctypes.c_void_p * MAX_LAYERS),
                 ("highway", HighwayT),
-                ("sru", SruStackT)]
+                ("sru", SruStackT),
+                ("lstm", LstmStackT)]
 
 
 OPT_ADAGRAD, OPT_ADAM = 0, 1
@@ -168,6 +182,7 @@ SIGNATURES = {
     "gantts_gan_step_seed": (_u64, [_u64, _i]),
     "gantts_mlp_layer_seed": (_u64, [_u64, _i]),
     "gantts_sru_mask_seed": (_u64, [_u64, _i, _i]),
+    "gantts_lstm_mask_seed": (_u64, [_u64, _i]),
 }
 
 STEP_D, STEP_G, STEP_FINISH, STEP_EVAL = 1, 2, 4, 8

@@ -318,8 +318,11 @@ static inline int blocks_1d(int64_t work, int per_block) {
   return (int)b;
 }
 
-// + the highway gate's weight and bias, or the SRU stack's weights and biases (the two are mutually exclusive)
+// + the highway gate's weight and bias, or the SRU stack's weights and biases (the two are mutually exclusive); an
+// LSTM generator (gate, 8 tensors per layer, hidden2out) fits in the same count and in one TensorList of the clip kernels
 constexpr int MAX_PARAMS = 2 * GANTTS_MAX_LAYERS + 2 * GANTTS_MAX_SRU_LAYERS;
+static_assert(2 + 8 * GANTTS_MAX_LSTM_LAYERS + 2 <= MAX_PARAMS && 2 + 8 * GANTTS_MAX_LSTM_LAYERS + 2 <= OPT_MAX_TENSORS,
+              "the LSTM generator's tensors must fit one TensorList");
 
 struct ParamList {
   int n;
@@ -332,6 +335,10 @@ struct ParamList {
   float* gb[GANTTS_MAX_LAYERS];
   float* sgW[GANTTS_MAX_SRU_LAYERS];                    // SRU stack: gradient of W[l] / b[l] in the flat buffer
   float* sgb[GANTTS_MAX_SRU_LAYERS];
+  float* lgW_ih[GANTTS_MAX_LSTM_LAYERS][2];             // LSTM stack: gradients of layer l, direction d in the flat buffer
+  float* lgW_hh[GANTTS_MAX_LSTM_LAYERS][2];
+  float* lgb_ih[GANTTS_MAX_LSTM_LAYERS][2];
+  float* lgb_hh[GANTTS_MAX_LSTM_LAYERS][2];
   int64_t total;
 };
 
@@ -374,15 +381,33 @@ struct StepLayout {
   float* sru_dx;          // [M][ncols] dL/dh of the top layer, then dX = dU W of each layer for the one below
   float* sru_dxp;         // [M][ncols] highway gradient (k = 3) for the layer below
   float* sru_bpart;       // [B][2 * ncols] bias-gradient partials
+  // LSTM generator only (zero bytes otherwise, so every other layout is unchanged); per layer l:
+  char* lstm_in[GANTTS_MAX_LSTM_LAYERS];      // planes of the GEMM input [M][n_in]: x (l = 0), else h_{l-1} * mask_{l-1}
+  char* lstm_w[GANTTS_MAX_LSTM_LAYERS];       // planes of W_ih of both directions [ndir 4H][n_in], then [n_in][ndir 4H]
+  float* lstm_bias[GANTTS_MAX_LSTM_LAYERS];   // b_ih + b_hh [ndir 4H]
+  float* lstm_h[GANTTS_MAX_LSTM_LAYERS];      // h [M][ndir H]
+  float* lstm_gates[GANTTS_MAX_LSTM_LAYERS];  // [ndir][M][4H]
+  float* lstm_cells[GANTTS_MAX_LSTM_LAYERS];  // [ndir][M][H]
+  float* lstm_xproj;      // [M][ndir 4H] xproj of one layer; in the backward, dgates of one layer
+  float* lstm_out;        // [M][d_out] hidden2out's output, the MLPG's input
+  float* lstm_dh;         // [M][ndir H] dL/dh of the top layer, then mask * dX of each layer for the one below
+  char* lstm_dg;          // planes of dgates [M][ndir 4H]
+  char* lstm_hp;          // planes of hprev [M][H]
+  float* lstm_part[2][2]; // split-K partials per direction: [d][0] dW_ih | db_ih, [d][1] dW_hh (one layer at a time)
+  unsigned int* lstm_bar; // grid-barrier counters of the recurrence
   size_t total;
 };
 
 static inline int sru_ncols(const gantts_sru_stack_t& s) { return s.hidden * (s.bidirectional ? 2 : 1); }
 static inline int sru_nin(const gantts_sru_stack_t& s, int l) { return l == 0 ? s.in_dim : sru_ncols(s); }
 static inline int sru_k(const gantts_sru_stack_t& s, int l) { return sru_nin(s, l) != sru_ncols(s) ? 4 : 3; }
+static inline int lstm_ndir(const gantts_lstm_stack_t& s) { return s.bidirectional ? 2 : 1; }
+static inline int lstm_nin(const gantts_lstm_stack_t& s, int l) { return l == 0 ? s.in_dim : lstm_ndir(s) * s.hidden; }
 
-// width of x: the SRU stack's input, else the generator MLP's
-static inline int gen_in_width(const gantts_gan_step_t* c) { return c->sru.num_layers > 0 ? c->sru.in_dim : c->g.dims[0]; }
+// width of x: the SRU or LSTM stack's input, else the generator MLP's
+static inline int gen_in_width(const gantts_gan_step_t* c) {
+  return c->sru.num_layers > 0 ? c->sru.in_dim : (c->lstm.num_layers > 0 ? c->lstm.in_dim : c->g.dims[0]);
+}
 
 static int64_t mlp_param_count(const gantts_mlp_t& m) {
   int64_t n = 0;
@@ -404,8 +429,17 @@ static int64_t sru_param_count(const gantts_gan_step_t* c) {
   return n;
 }
 
+// elements of the LSTM stack's parameters, which follow the gate in the generator's flat gradient buffer
+static int64_t lstm_param_count(const gantts_gan_step_t* c) {
+  const gantts_lstm_stack_t& s = c->lstm;
+  const int64_t G4 = 4 * (int64_t)s.hidden;
+  int64_t n = 0;
+  for (int l = 0; l < s.num_layers; ++l) n += lstm_ndir(s) * (G4 * lstm_nin(s, l) + G4 * s.hidden + 2 * G4);
+  return n;
+}
+
 static int64_t g_param_count(const gantts_gan_step_t* c) {
-  return gate_param_count(c) + sru_param_count(c) + mlp_param_count(c->g);
+  return gate_param_count(c) + sru_param_count(c) + lstm_param_count(c) + mlp_param_count(c->g);
 }
 
 static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
@@ -460,6 +494,35 @@ static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
   L->sru_dx = (float*)take((size_t)M * nc * sizeof(float));
   L->sru_dxp = (float*)take((size_t)M * nc * sizeof(float));
   L->sru_bpart = (float*)take((size_t)c->B * 2 * nc * sizeof(float));
+  const gantts_lstm_stack_t& ls = c->lstm;
+  const int lnl = ls.num_layers, H = lnl > 0 ? ls.hidden : 0, nd = lstm_ndir(ls), n4 = nd * 4 * H;
+  size_t part_ih = 0, part_hh = 0;
+  for (int l = 0; l < GANTTS_MAX_LSTM_LAYERS; ++l) {
+    L->lstm_in[l] = L->lstm_w[l] = nullptr;
+    L->lstm_bias[l] = L->lstm_h[l] = L->lstm_gates[l] = L->lstm_cells[l] = nullptr;
+    if (l >= lnl) continue;
+    const int ni = lstm_nin(ls, l);
+    L->lstm_in[l] = take(2 * plane_bytes(M, ni));
+    L->lstm_w[l] = take(2 * plane_bytes(n4, ni) + 2 * plane_bytes(ni, n4));
+    L->lstm_bias[l] = (float*)take((size_t)n4 * sizeof(float));
+    L->lstm_h[l] = (float*)take((size_t)M * nd * H * sizeof(float));
+    L->lstm_gates[l] = (float*)take((size_t)M * n4 * sizeof(float));
+    L->lstm_cells[l] = (float*)take((size_t)M * nd * H * sizeof(float));
+    const size_t pi = mn_partial_bytes(M, 4 * H, ni, nullptr, nullptr), ph = mn_partial_bytes(M, 4 * H, H, nullptr, nullptr);
+    part_ih = pi > part_ih ? pi : part_ih;
+    part_hh = ph > part_hh ? ph : part_hh;
+  }
+  const bool lstm = lnl > 0;
+  L->lstm_xproj = (float*)take((size_t)M * n4 * sizeof(float));
+  L->lstm_out = (float*)take(lstm ? (size_t)M * c->g.dims[c->g.num_layers] * sizeof(float) : 0);
+  L->lstm_dh = (float*)take((size_t)M * nd * H * sizeof(float));
+  L->lstm_dg = take(lstm ? 2 * plane_bytes(M, n4) : 0);
+  L->lstm_hp = take(lstm ? 2 * plane_bytes(M, H) : 0);
+  for (int d = 0; d < 2; ++d) {
+    L->lstm_part[d][0] = (float*)take(d < nd ? part_ih : 0);
+    L->lstm_part[d][1] = (float*)take(d < nd ? part_hh : 0);
+  }
+  L->lstm_bar = (unsigned int*)take(lstm ? 256 : 0);
   L->total = (size_t)(cur - base) + 256;
 }
 
@@ -488,7 +551,7 @@ static void param_list(const gantts_mlp_t& m, float* const* sumW, float* const* 
 }
 
 // generator parameters in model.parameters() order: [T.weight, T.bias] of a highway generator, or [W, b] of every layer
-// of an SRU stack, then the MLP layers
+// of an SRU stack; then [W_ih, W_hh, b_ih, b_hh] of every layer and direction of an LSTM stack; then the MLP layers
 static void g_param_list(const gantts_gan_step_t* c, float* flat, ParamList* pl) {
   pl->n = 0;
   pl->total = 0;
@@ -525,6 +588,26 @@ static void g_param_list(const gantts_gan_step_t* c, float* flat, ParamList* pl)
       pl->total += sizes[i];
     }
   }
+  const gantts_lstm_stack_t& ls = c->lstm;
+  for (int l = 0; l < ls.num_layers; ++l)
+    for (int d = 0; d < lstm_ndir(ls); ++d) {
+      const int64_t G4 = 4 * (int64_t)ls.hidden;
+      const int64_t sizes[4] = {G4 * lstm_nin(ls, l), G4 * ls.hidden, G4, G4};
+      float* const ps[4] = {const_cast<float*>(ls.W_ih[l][d]), const_cast<float*>(ls.W_hh[l][d]),
+                            const_cast<float*>(ls.b_ih[l][d]), const_cast<float*>(ls.b_hh[l][d])};
+      float* const ss[4] = {ls.sumW_ih[l][d], ls.sumW_hh[l][d], ls.sumb_ih[l][d], ls.sumb_hh[l][d]};
+      float* const qs[4] = {ls.sqW_ih[l][d], ls.sqW_hh[l][d], ls.sqb_ih[l][d], ls.sqb_hh[l][d]};
+      float** const gs[4] = {&pl->lgW_ih[l][d], &pl->lgW_hh[l][d], &pl->lgb_ih[l][d], &pl->lgb_hh[l][d]};
+      for (int i = 0; i < 4; ++i) {
+        *gs[i] = flat + pl->total;
+        pl->p[pl->n] = ps[i];
+        pl->g[pl->n] = flat + pl->total;
+        pl->s[pl->n] = ss[i];
+        pl->s2[pl->n] = qs[i];
+        pl->sizes[pl->n++] = sizes[i];
+        pl->total += sizes[i];
+      }
+    }
   param_list(c->g, c->g_sumW, c->g_sumb, c->g_sqW, c->g_sqb, flat + pl->total, pl);
 }
 
@@ -586,6 +669,41 @@ static int check_step(const gantts_gan_step_t* c) {
   GANTTS_CHECK_ARG(c->g.num_layers >= 1 && c->g.num_layers <= GANTTS_MAX_LAYERS, "gan_step: bad generator");
   GANTTS_CHECK_ARG(c->n_static >= 1 && c->n_static <= GANTTS_MAX_COLS, "gan_step: bad n_static");
   GANTTS_CHECK_ARG(c->n_static_cols == c->n_static, "gan_step: static column list must have n_static entries");
+  const gantts_lstm_stack_t& ls = c->lstm;
+  GANTTS_CHECK_ARG(ls.num_layers >= 0 && ls.num_layers <= GANTTS_MAX_LSTM_LAYERS,
+                   "gan_step: LSTM layer count %d not in [0, %d] (train larger stacks with GanTrainer)", ls.num_layers,
+                   GANTTS_MAX_LSTM_LAYERS);
+  if (ls.num_layers > 0) {
+    // In2OutRNNHighwayNet (models.py:72-118): the gate, the LSTM stack, then hidden2out as a one-layer MLP
+    GANTTS_CHECK_ARG(c->highway.static_dim > 0,
+                     "gan_step: an LSTM stack runs only with the highway gate (In2OutRNNHighwayNet); LSTMRNN and GRURNN "
+                     "train with GanTrainer");
+    GANTTS_CHECK_ARG(c->sru.num_layers == 0, "gan_step: the LSTM stack and the SRU stack are mutually exclusive");
+    GANTTS_CHECK_ARG(ls.in_dim >= 1 && (ls.bidirectional == 0 || ls.bidirectional == 1),
+                     "gan_step: bad LSTM shape (in_dim %d, bidirectional %d)", ls.in_dim, ls.bidirectional);
+    GANTTS_CHECK_ARG(ls.hidden >= 4 && ls.hidden % 4 == 0, "gan_step: LSTM hidden size %d is not a positive multiple of 4",
+                     ls.hidden);
+    GANTTS_CHECK_ARG(c->B <= LSTM_MAX_B, "gan_step: an LSTM stack runs at most LSTM_MAX_B = %d sequences (B = %d)",
+                     LSTM_MAX_B, c->B);
+    GANTTS_CHECK_ARG(ls.dropout >= 0.f && ls.dropout < 1.f, "gan_step: LSTM dropout out of [0, 1)");
+    const int nh = lstm_ndir(ls) * ls.hidden;
+    GANTTS_CHECK_ARG(c->g.num_layers == 1 && c->g.dims[0] == nh,
+                     "gan_step: with an LSTM stack g is hidden2out alone: 1 layer of input width %d (got %d layer(s), "
+                     "input width %d)", nh, c->g.num_layers, c->g.dims[0]);
+    GANTTS_CHECK_ARG(ls.in_dim == c->g.dims[1],
+                     "gan_step: LSTM in_dim %d != hidden2out output width %d (the model returns its input as y_hat)",
+                     ls.in_dim, c->g.dims[1]);
+    for (int l = 0; l < ls.num_layers; ++l)
+      for (int d = 0; d < lstm_ndir(ls); ++d) {
+        GANTTS_CHECK_ARG(ls.W_ih[l][d] && ls.W_hh[l][d] && ls.b_ih[l][d] && ls.b_hh[l][d],
+                         "gan_step: null LSTM weight/bias of layer %d direction %d", l, d);
+        GANTTS_CHECK_ARG(ls.sumW_ih[l][d] && ls.sumW_hh[l][d] && ls.sumb_ih[l][d] && ls.sumb_hh[l][d],
+                         "gan_step: null LSTM optimiser state of layer %d direction %d", l, d);
+        if (c->optimizer == GANTTS_OPT_ADAM)
+          GANTTS_CHECK_ARG(ls.sqW_ih[l][d] && ls.sqW_hh[l][d] && ls.sqb_ih[l][d] && ls.sqb_hh[l][d],
+                           "gan_step: Adam needs exp_avg_sq for LSTM layer %d direction %d", l, d);
+      }
+  }
   const gantts_sru_stack_t& s = c->sru;
   GANTTS_CHECK_ARG(s.num_layers >= 0 && s.num_layers <= GANTTS_MAX_SRU_LAYERS, "gan_step: SRU layer count %d not in [0, %d]",
                    s.num_layers, GANTTS_MAX_SRU_LAYERS);
@@ -630,7 +748,8 @@ static int check_step(const gantts_gan_step_t* c) {
                      "gan_step: a highway generator needs exactly one dynamic stream with in_start = out_start = 0 and "
                      "sd = static_dim = %d (got %d stream(s), first sd %d)", S, st.n, st.sd[0]);
     GANTTS_CHECK_ARG(c->n_static == S, "gan_step: highway static_dim %d != n_static %d", S, c->n_static);
-    GANTTS_CHECK_ARG(c->g.dims[0] >= S, "gan_step: highway generator input width %d < static_dim %d", c->g.dims[0], S);
+    GANTTS_CHECK_ARG(gen_in_width(c) >= S, "gan_step: highway generator input width %d < static_dim %d", gen_in_width(c),
+                     S);
     GANTTS_CHECK_ARG(c->g.dims[Lg] == nw * S, "gan_step: highway generator output width %d != %d windows x static_dim %d",
                      c->g.dims[Lg], nw, S);
     GANTTS_CHECK_ARG(h.W && h.b, "gan_step: null highway gate weight/bias");
@@ -642,15 +761,39 @@ static int check_step(const gantts_gan_step_t* c) {
   return GANTTS_OK;
 }
 
-// Tx = sigmoid(x_s W_T^T + b_T): the generator's input planes on its tape (written by its forward) with the first S
-// columns as the operand, so x is not converted twice.
+// LSTM layer l's workspace: planes of its GEMM input, and of W_ih of both directions [ndir 4H][n_in] then transposed
+static Planes lstm_in_planes(const gantts_gan_step_t* c, const StepLayout& L, int l, int64_t M) {
+  char* cur = L.lstm_in[l];
+  return carve_planes(cur, M, lstm_nin(c->lstm, l));
+}
+static void lstm_w_planes(const gantts_gan_step_t* c, const StepLayout& L, int l, Planes* w, Planes* wt) {
+  const int ni = lstm_nin(c->lstm, l), n4 = lstm_ndir(c->lstm) * 4 * c->lstm.hidden;
+  char* cur = L.lstm_w[l];
+  *w = carve_planes(cur, n4, ni);
+  *wt = carve_planes(cur, ni, n4);
+}
+
+// x_s: the first S columns of x's operand planes -- the generator MLP's tape input, or the LSTM stack's layer-0 input
+// (written by the generator's forward), so x is not converted twice.
+static int gate_input_planes(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, int64_t M,
+                             Planes* xs) {
+  if (c->lstm.num_layers > 0) {
+    *xs = lstm_in_planes(c, L, 0, M);
+  } else {
+    int rc = mlp_tape_input_planes(&g, M, L.g_tape, L.g_tape_bytes, xs);
+    if (rc) return rc;
+  }
+  xs->cols = c->highway.static_dim;
+  return GANTTS_OK;
+}
+
+// Tx = sigmoid(x_s W_T^T + b_T)
 static int highway_gate_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, int64_t M,
                             cudaStream_t st) {
   const int S = c->highway.static_dim;
   Planes xs;
-  int rc = mlp_tape_input_planes(&g, M, L.g_tape, L.g_tape_bytes, &xs);
+  int rc = gate_input_planes(c, g, L, M, &xs);
   if (rc) return rc;
-  xs.cols = S;
   char* cur = L.hw_w;
   const Planes w = carve_planes(cur, S, S);
   if ((rc = launch_split(c->highway.W, S, S, S, w, 0, st))) return rc;
@@ -668,9 +811,8 @@ static int highway_gate_bwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, c
                             cudaStream_t st) {
   const int S = c->highway.static_dim;
   Planes xs;
-  int rc = mlp_tape_input_planes(&g, M, L.g_tape, L.g_tape_bytes, &xs);
+  int rc = gate_input_planes(c, g, L, M, &xs);
   if (rc) return rc;
-  xs.cols = S;
   char* cur = L.hw_dz;
   const Planes dz = carve_planes(cur, M, S);
   ReduceList rl;
@@ -817,12 +959,165 @@ static int sru_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const 
   return flush_reduce(rl, 0, st);
 }
 
-// Generator forward into y_hat: the MLP from x, or the SRU stack and then hidden2out on the planes it left in the tape.
+static LstmParams lstm_layer_params(const gantts_gan_step_t* c, const StepLayout& L, int l, const int64_t* lengths) {
+  const gantts_lstm_stack_t& s = c->lstm;
+  LstmParams p{};
+  p.W_hh = s.W_hh[l][0];
+  if (s.bidirectional)      // the two directions' tensors are 4-byte aligned: their distance is a whole number of floats
+    p.W_hh_dir = ((int64_t)reinterpret_cast<uintptr_t>(s.W_hh[l][1]) - (int64_t)reinterpret_cast<uintptr_t>(s.W_hh[l][0])) /
+                 (int64_t)sizeof(float);
+  p.lengths = lengths;
+  p.h_out = L.lstm_h[l];
+  p.gates = L.lstm_gates[l];
+  p.cells = L.lstm_cells[l];
+  p.bar = L.lstm_bar;
+  p.B = c->B;
+  p.T = c->T;
+  p.H = s.hidden;
+  p.ndir = lstm_ndir(s);
+  return p;
+}
+
+// LSTM stack forward (nn.LSTM on packed sequences, per-element dropout between layers): per layer one xproj GEMM over
+// both directions, the cooperative recurrence, and one kernel that writes the next GEMM's operand planes of h * mask --
+// on the top layer the unmasked h into hidden2out's tape input planes, so the caller runs hidden2out with
+// mlp_fwd_impl(..., input_ready = true).  train = false: no masks.
+static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, const float* x,
+                          const int64_t* lengths, int64_t M, uint64_t seed, bool train, cudaStream_t st) {
+  const gantts_lstm_stack_t& s = c->lstm;
+  const int nl = s.num_layers, H = s.hidden, nd = lstm_ndir(s), G4 = 4 * H, nh = nd * H;
+  const float p_drop = train ? s.dropout : 0.f;
+  int rc;
+  {
+    // every W_ih -> planes as stored (rows d * 4H.. of the direction-stacked operand of xproj) and transposed (columns
+    // d * 4H.. of the operand of dX = dgates W_ih), one launch; and b_ih + b_hh of every layer and direction, one launch
+    WeightSplitList wl;
+    LstmBiasList bl;
+    wl.n = bl.n = nl * nd;
+    wl.off[0] = 0;
+    bl.len = G4;
+    for (int l = 0; l < nl; ++l) {
+      Planes w, wt;
+      lstm_w_planes(c, L, l, &w, &wt);
+      for (int d = 0; d < nd; ++d) {
+        const int i = l * nd + d;
+        wl.W[i] = s.W_ih[l][d];
+        wl.N[i] = G4;
+        wl.K[i] = lstm_nin(s, l);
+        wl.hi[i] = w.hi + (int64_t)d * G4 * w.pitch;
+        wl.lo[i] = w.lo + (int64_t)d * G4 * w.pitch;
+        wl.pitch[i] = w.pitch;
+        wl.thi[i] = wt.hi + (int64_t)d * G4;
+        wl.tlo[i] = wt.lo + (int64_t)d * G4;
+        wl.tpitch[i] = wt.pitch;
+        wl.off[i + 1] = wl.off[i] + (int64_t)((G4 + 31) / 32) * ((wl.K[i] + 31) / 32);
+        bl.a[i] = s.b_ih[l][d];
+        bl.b[i] = s.b_hh[l][d];
+        bl.out[i] = L.lstm_bias[l] + (int64_t)d * G4;
+      }
+    }
+    const int nb = (int)(wl.off[wl.n] < num_sms() * 8 ? wl.off[wl.n] : num_sms() * 8);
+    GANTTS_PDL_LAUNCH((split_weights_kernel), nb < 1 ? 1 : nb, 256, 0, st, wl);
+    GANTTS_LAUNCH_CHECK("split_weights_kernel(lstm)");
+    GANTTS_PDL_LAUNCH((lstm_bias_sum_kernel), (bl.n * G4 + 255) / 256, 256, 0, st, bl);
+    GANTTS_LAUNCH_CHECK("lstm_bias_sum_kernel");
+  }
+  if ((rc = launch_split(x, s.in_dim, M, s.in_dim, lstm_in_planes(c, L, 0, M), 0, st))) return rc;
+  Planes top;
+  if ((rc = mlp_tape_input_planes(&g, M, L.g_tape, L.g_tape_bytes, &top))) return rc;
+  for (int l = 0; l < nl; ++l) {
+    const bool last = l == nl - 1;
+    Planes w, wt;
+    lstm_w_planes(c, L, l, &w, &wt);
+    EpiArgs e;
+    e.epi = EPI_F32;
+    e.C = L.lstm_xproj;
+    e.ldc = (int64_t)nd * G4;
+    e.bias = L.lstm_bias[l];
+    if ((rc = launch_gemm_kk(lstm_in_planes(c, L, l, M), w, e, st))) return rc;
+    LstmParams p = lstm_layer_params(c, L, l, lengths);
+    p.xproj = L.lstm_xproj;
+    if ((rc = lstm_run(false, p, st))) return rc;
+    const Planes out = last ? top : lstm_in_planes(c, L, l + 1, M);
+    const float pl = last ? 0.f : p_drop;             // nn.LSTM: no dropout on the last layer's output
+    GANTTS_PDL_LAUNCH((lstm_planes_kernel), blocks_1d(M * nh, 1024), 256, 0, st, L.lstm_h[l], M, nh,
+                      gantts_lstm_mask_seed(seed, l), pl > 0.f ? (uint32_t)(pl * 65536.f + 0.5f) : 0u,
+                      pl > 0.f ? 1.f / (1.f - pl) : 1.f, out.hi, out.lo, out.pitch);
+    GANTTS_LAUNCH_CHECK("lstm_planes_kernel");
+  }
+  return GANTTS_OK;
+}
+
+// LSTM stack backward from dL/dh of the top layer in L.lstm_dh (hidden2out's input gradient), top layer first:
+//   recurrence backward -> dgates (fp32, in the xproj buffer) -> dgates planes
+//   per direction: dW_ih and db_ih = dgates_d^T in (MN-major, ones-tile bias), dW_hh = dgates_d^T hprev_d (MN-major)
+//   dX = dgates W_ih, times the mask of the layer below in the GEMM epilogue (not for layer 0)
+//   db_hh = db_ih (b_ih and b_hh enter xproj as one sum)
+// Each layer's split-K reductions go through one flush_reduce.
+static int lstm_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const ParamList& pg, const int64_t* lengths,
+                          int64_t M, uint64_t seed, cudaStream_t st) {
+  const gantts_lstm_stack_t& s = c->lstm;
+  const int nl = s.num_layers, H = s.hidden, nd = lstm_ndir(s), G4 = 4 * H, nh = nd * H;
+  int rc;
+  char* cur = L.lstm_dg;
+  const Planes dg = carve_planes(cur, M, (int64_t)nd * G4);
+  cur = L.lstm_hp;
+  const Planes hp = carve_planes(cur, M, H);
+  ReduceList rl;
+  for (int l = nl - 1; l >= 0; --l) {
+    LstmParams p = lstm_layer_params(c, L, l, lengths);
+    p.dh_out = L.lstm_dh;
+    p.dxproj = L.lstm_xproj;
+    if ((rc = lstm_run(true, p, st))) return rc;
+    if ((rc = launch_split(L.lstm_xproj, (int64_t)nd * G4, M, nd * G4, dg, 0, st))) return rc;
+    const Planes in = lstm_in_planes(c, L, l, M);
+    for (int d = 0; d < nd; ++d) {
+      Planes dgd = dg;
+      dgd.hi += (int64_t)d * G4;
+      dgd.lo += (int64_t)d * G4;
+      dgd.cols = G4;
+      if ((rc = launch_gemm_mn(dgd, in, pg.lgW_ih[l][d], pg.lgb_ih[l][d], 0, L.lstm_part[d][0], st, &rl))) return rc;
+      GANTTS_PDL_LAUNCH((lstm_hprev_planes_kernel), blocks_1d(M * H, 1024), 256, 0, st, L.lstm_h[l], lengths, c->B, c->T, H, nd,
+                        d, hp.hi, hp.lo, hp.pitch);
+      GANTTS_LAUNCH_CHECK("lstm_hprev_planes_kernel");
+      if ((rc = launch_gemm_mn(dgd, hp, pg.lgW_hh[l][d], nullptr, 0, L.lstm_part[d][1], st, &rl))) return rc;
+    }
+    if (l > 0) {
+      Planes w, wt;
+      lstm_w_planes(c, L, l, &w, &wt);
+      EpiArgs e;
+      e.epi = EPI_F32;
+      e.C = L.lstm_dh;
+      e.ldc = nh;
+      if (s.dropout > 0.f) {      // dh_{l-1} = mask_{l-1} * dX: LeakyReLU with slope 1 is the identity, then the mask
+        e.act = GANTTS_ACT_LEAKY_DROPOUT;
+        e.slope = 1.f;
+        e.p = s.dropout;
+        e.seed = gantts_lstm_mask_seed(seed, l - 1);
+      }
+      if ((rc = launch_gemm_kk(dg, wt, e, st))) return rc;
+    }
+    if ((rc = flush_reduce(rl, 0, st))) return rc;
+    for (int d = 0; d < nd; ++d)
+      GANTTS_CUDA(cudaMemcpyAsync(pg.lgb_hh[l][d], pg.lgb_ih[l][d], (size_t)G4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  }
+  return GANTTS_OK;
+}
+
+// Generator forward: the MLP from x into y_hat; or the SRU stack and then hidden2out on the planes it left in the tape,
+// into y_hat; or the LSTM stack and then hidden2out into L.lstm_out, with y_hat a copy of x (models.py:118).
 static int generator_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, const float* x, int x_rs,
-                         int64_t M, float* y_hat, int d_out, uint64_t seed, bool train, cudaStream_t st) {
+                         const int64_t* lengths, int64_t M, float* y_hat, int d_out, uint64_t seed, bool train,
+                         cudaStream_t st) {
+  int rc;
+  if (c->lstm.num_layers > 0) {
+    if ((rc = lstm_stack_fwd(c, g, L, x, lengths, M, seed, train, st))) return rc;
+    if ((rc = mlp_fwd_impl(&g, nullptr, 0, M, L.lstm_out, d_out, L.g_tape, L.g_tape_bytes, st, true))) return rc;
+    GANTTS_CUDA(cudaMemcpyAsync(y_hat, x, (size_t)M * x_rs * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return GANTTS_OK;
+  }
   if (c->sru.num_layers == 0) return gantts_mlp_fwd(&g, x, x_rs, M, y_hat, d_out, L.g_tape, L.g_tape_bytes, st);
-  int rc = sru_stack_fwd(c, g, L, x, M, seed, train, st);
-  if (rc) return rc;
+  if ((rc = sru_stack_fwd(c, g, L, x, M, seed, train, st))) return rc;
   return mlp_fwd_impl(&g, nullptr, 0, M, y_hat, d_out, L.g_tape, L.g_tape_bytes, st, true);
 }
 
@@ -834,6 +1129,11 @@ extern "C" uint64_t gantts_gan_step_seed(uint64_t seed, int which) { return seed
 
 extern "C" uint64_t gantts_sru_mask_seed(uint64_t seed, int layer, int which) {
   return gantts_mlp_layer_seed(gantts_gan_step_seed(seed, 3), 2 * layer + which);
+}
+
+// after every SRU index 2 * layer + which < 2 * GANTTS_MAX_SRU_LAYERS of the same stream
+extern "C" uint64_t gantts_lstm_mask_seed(uint64_t seed, int layer) {
+  return gantts_mlp_layer_seed(gantts_gan_step_seed(seed, 3), 2 * GANTTS_MAX_SRU_LAYERS + layer);
 }
 
 extern "C" size_t gantts_gan_step_workspace_bytes(const gantts_gan_step_t* c) {
@@ -918,6 +1218,10 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
   }
   gantts_mlp_t g = c->g, d = c->d;
   g.seed = gantts_gan_step_seed(seed, 0);
+  // In2OutRNNHighwayNet: hidden2out's output feeds the MLPG, y_hat is x, and loss_mse sends no gradient into G
+  const bool lstm = c->lstm.num_layers > 0;
+  const float* gen_out = lstm ? L.lstm_out : y_hat;
+  const bool mse_grad = c->mse_w != 0.f && !lstm;
 
   RedCounts cnt{};
   if (phases & GANTTS_STEP_EVAL) {
@@ -933,9 +1237,9 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
       gather_cols_list_kernel<<<blocks_1d(M * nS, 1024), 256, 0, st>>>(y, d_out, L.y_static, nS, static_cols, M);
       GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(y_static)");
     }
-    if ((rc = generator_fwd(c, g, L, x, d_in, M, y_hat, d_out, seed, false, st))) return rc;
+    if ((rc = generator_fwd(c, g, L, x, d_in, lengths_dev, M, y_hat, d_out, seed, false, st))) return rc;
     if (hw && (rc = highway_gate_fwd(c, g, L, M, st))) return rc;
-    if ((rc = mlpg_fwd_impl(y_hat, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
+    if ((rc = mlpg_fwd_impl(gen_out, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
                             c->mlpg_table, &c->streams, &c->windows, c->B, c->T, stream, hwp)))
       return rc;
     if (has_d) {
@@ -985,9 +1289,9 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
       GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(y_static)");
     }
     // ---- apply_generator (train.py:336-355): G forward + MLPG
-    if ((rc = generator_fwd(c, g, L, x, d_in, M, y_hat, d_out, seed, true, st))) return rc;
+    if ((rc = generator_fwd(c, g, L, x, d_in, lengths_dev, M, y_hat, d_out, seed, true, st))) return rc;
     if (hw && (rc = highway_gate_fwd(c, g, L, M, st))) return rc;
-    if ((rc = mlpg_fwd_impl(y_hat, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
+    if ((rc = mlpg_fwd_impl(gen_out, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
                             c->mlpg_table, &c->streams, &c->windows, c->B, c->T, stream, hwp)))
       return rc;
     // MGE loss (train.py:291) and its gradient in one pass; the gradient INITIALISES g_static, the two discriminator
@@ -1080,13 +1384,13 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
     }
     // ---- loss_g.backward(): MSE term (train.py:294) + MLPG backward + generator backward on the summed gradient.
     // With mse_w != 0 the MSE pass stores its gradient into g_yhat and the MLPG backward accumulates on top of it.
-    if ((rc = launch_sse(y_hat, d_out, y, d_out, L.mask, M, d_out, L.scal + S_MSE_SCALE, c->mse_w != 0.f ? L.g_yhat : nullptr,
+    if ((rc = launch_sse(y_hat, d_out, y, d_out, L.mask, M, d_out, L.scal + S_MSE_SCALE, mse_grad ? L.g_yhat : nullptr,
                          d_out, &L.red[R_MSE], st)))
       return rc;
-    // mse_w == 0 (the CLI default, train.py:15): nothing else adds to dL/dy_hat, so the MLPG backward writes the
-    // operand planes of the generator's backward GEMMs directly (no fp32 matrix, no conversion pass)
+    // no MSE gradient (mse_w == 0, the CLI default, train.py:15; or y_hat = x): nothing else adds to dL/dy_hat, so the
+    // MLPG backward writes the operand planes of the generator's backward GEMMs directly (no fp32 matrix, no conversion)
     bool direct = false;
-    if (c->mse_w == 0.f) {
+    if (!mse_grad) {
       Planes gp;
       if ((rc = mlp_bwd_gy_planes(&g, M, L.mlp_ws, L.mlp_ws_bytes, &gp))) return rc;
       rc = mlpg_bwd_planes(L.g_static, (int64_t)c->T * nS, nS, gp.hi, gp.lo, gp.pitch, c->mlpg_table, &c->streams,
@@ -1097,16 +1401,18 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
     // (highway: the adjoint solves with Tx * g_static and leaves dz for the gate's weight gradient)
     if (!direct &&
         (rc = mlpg_bwd_impl(L.g_static, (int64_t)c->T * nS, nS, L.g_yhat, (int64_t)c->T * d_out, d_out, c->mlpg_table,
-                            &c->streams, &c->windows, c->B, c->T, c->mse_w != 0.f ? 1 : 0, stream, hwp)))
+                            &c->streams, &c->windows, c->B, c->T, mse_grad ? 1 : 0, stream, hwp)))
       return rc;
     if (hw && (rc = highway_gate_bwd(c, g, L, M, st))) return rc;
-    // (SRU stack: hidden2out's input gradient is dL/dh of the top SRU layer)
+    // (SRU or LSTM stack: hidden2out's input gradient is dL/dh of the stack's top layer)
     const bool sru = c->sru.num_layers > 0;
-    if ((rc = mlp_bwd_impl(&g, direct ? nullptr : L.g_yhat, d_out, nullptr, 0, M, L.g_tape, L.g_tape_bytes,
-                           sru ? L.sru_dx : nullptr, sru ? sru_ncols(c->sru) : 0, 0, pg.gW, pg.gb, 0, L.mlp_ws, L.mlp_ws_bytes,
-                           stream, -1, direct)))
+    float* gx = sru ? L.sru_dx : (lstm ? L.lstm_dh : nullptr);
+    const int gx_rs = sru ? sru_ncols(c->sru) : (lstm ? lstm_ndir(c->lstm) * c->lstm.hidden : 0);
+    if ((rc = mlp_bwd_impl(&g, direct ? nullptr : L.g_yhat, d_out, nullptr, 0, M, L.g_tape, L.g_tape_bytes, gx, gx_rs, 0,
+                           pg.gW, pg.gb, 0, L.mlp_ws, L.mlp_ws_bytes, stream, -1, direct)))
       return rc;
     if (sru && (rc = sru_stack_bwd(c, L, pg, x, M, seed, st))) return rc;
+    if (lstm && (rc = lstm_stack_bwd(c, L, pg, lengths_dev, M, seed, st))) return rc;
   }
   if (phases & 4) {
     NvtxRange r4("gantts_gan_step/phase4: G step, losses");

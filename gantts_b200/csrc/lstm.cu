@@ -22,7 +22,8 @@ constexpr int LSTM_MAX_B = 128;
 
 struct LstmParams {
   const float* xproj;    // [B][T][ndir*4H]
-  const float* W_hh;     // [ndir][4H][H]
+  const float* W_hh;     // [4H][H] of direction 0; direction d's starts at W_hh + d * W_hh_dir (nn.LSTM keeps the
+  int64_t W_hh_dir;      // directions as separate tensors: a stride, not a copy)
   const int64_t* lengths;
   float* h_out;          // [B][T][ndir*H]
   float* gates;          // [ndir][B][T][4H]
@@ -71,7 +72,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_fwd_kernel(const LstmPar
   const int dir = blockIdx.x / p.slices, sl = blockIdx.x % p.slices, u0 = sl * HS;
   const int tid = threadIdx.x;
   const int ldx = p.ndir * 4 * H, ldh = p.ndir * H;
-  const float* Wd = p.W_hh + (int64_t)dir * 4 * H * H;
+  const float* Wd = p.W_hh + (int64_t)dir * p.W_hh_dir;
   for (int i = tid; i < R * H; i += LSTM_THREADS) {
     const int r = i / H, k = i - r * H;
     const int g = r / HS, u = r - g * HS;
@@ -164,7 +165,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_bwd_kernel(const LstmPar
   const int dir = blockIdx.x / p.slices, sl = blockIdx.x % p.slices, u0 = sl * HS;
   const int tid = threadIdx.x;
   const int ldx = p.ndir * 4 * H, ldh = p.ndir * H;
-  const float* Wd = p.W_hh + (int64_t)dir * 4 * H * H;
+  const float* Wd = p.W_hh + (int64_t)dir * p.W_hh_dir;
   for (int i = tid; i < HS * G4; i += LSTM_THREADS) {
     const int row = i / HS, k = i - row * HS;
     Wt[k * GP + row] = (u0 + k < H) ? Wd[(int64_t)row * H + u0 + k] : 0.f;
@@ -265,7 +266,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_fwd_reg_kernel(const Lst
   const int dir = blockIdx.x / p.slices, sl = blockIdx.x % p.slices, u0 = sl * HS;
   const int tid = threadIdx.x;
   const int ldx = p.ndir * 4 * H, ldh = p.ndir * H;
-  const float* Wd = p.W_hh + (int64_t)dir * 4 * H * H;
+  const float* Wd = p.W_hh + (int64_t)dir * p.W_hh_dir;
   const int r = tid % R, kq = tid / R;
   float w[KR];
   {
@@ -399,7 +400,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_bwd_reg_kernel(const Lst
   const int dir = blockIdx.x / p.slices, sl = blockIdx.x % p.slices, u0 = sl * HS;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int ldx = p.ndir * 4 * H, ldh = p.ndir * H;
-  const float* Wd = p.W_hh + (int64_t)dir * 4 * H * H;
+  const float* Wd = p.W_hh + (int64_t)dir * p.W_hh_dir;
   float w[RPT][HS];
 #pragma unroll
   for (int i = 0; i < RPT; ++i) {
@@ -620,6 +621,86 @@ static int lstm_launch_reg(bool bwd, LstmParams& p, cudaStream_t st) {
   return GANTTS_OK;
 }
 
+// One layer's recurrence (forward or backward) in one cooperative launch; p.slices is chosen here.  The barrier
+// counters at p.bar are zeroed on the stream before the launch.
+static int lstm_run(bool bwd, LstmParams& p, cudaStream_t st) {
+  const int hs = lstm_pick_hs(p.H, p.ndir, &p.slices);
+  if (hs == 8 && p.H <= 512 && lstm_use_reg()) return lstm_launch_reg(bwd, p, st);
+  if (hs == 8) return lstm_launch<8>(bwd, p, st);
+  if (hs == 16) return lstm_launch<16>(bwd, p, st);
+  set_error("lstm: hidden size %d x %d directions does not fit one wave of CTAs", p.H, p.ndir);
+  return GANTTS_E_UNSUPPORTED;
+}
+
+// ---------------------------------------------------------------------------- LSTM stack of the fused GAN step
+// The fused step (gan_step.cu) runs xproj = planes(in) W_ih^T + (b_ih + b_hh) as one bf16x3 GEMM per layer, the
+// recurrence above, and these element-wise kernels around them.  Planes are bf16 hi/lo operand planes of the GEMM engine.
+
+// Planes of h * mask, mask = gantts_dropout(ones[rows][cols], p, seed) (thresh 0 / scale 1: no mask): the next layer's
+// GEMM operand, or hidden2out's input on the top layer.  One warp per row, a lane converts pairs of columns.
+__global__ void lstm_planes_kernel(const float* __restrict__ h, int64_t rows, int cols, uint64_t seed, uint32_t thresh,
+                                   float scale, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo,
+                                   int64_t pitch) {
+  pdl_entry();
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t r = warp; r < rows; r += nwarps) {
+    const float* hr_in = h + r * cols;
+    uint32_t* hr = reinterpret_cast<uint32_t*>(hi + r * pitch);
+    uint32_t* lr = reinterpret_cast<uint32_t*>(lo + r * pitch);
+    for (int c = 2 * lane; c < cols; c += 64) {
+      const float m0 = dropout_keep(seed, (uint32_t)r, (uint32_t)cols, (uint32_t)c, thresh) ? scale : 0.f;
+      const float m1 = dropout_keep(seed, (uint32_t)r, (uint32_t)cols, (uint32_t)(c + 1), thresh) ? scale : 0.f;
+      const float a = hr_in[c] * m0, v = (c + 1 < cols) ? hr_in[c + 1] * m1 : 0.f;
+      const uint32_t hp = pack_bf16x2(a, v);
+      hr[c >> 1] = hp;
+      lr[c >> 1] = pack_bf16x2(a - __uint_as_float(hp << 16), v - __uint_as_float(hp & 0xffff0000u));
+    }
+  }
+}
+
+// Planes of hprev (the values of lstm_hprev_kernel for direction `dir`): the right operand of dW_hh = dgates^T hprev.
+__global__ void lstm_hprev_planes_kernel(const float* __restrict__ h, const int64_t* __restrict__ lengths, int B, int T,
+                                         int H, int ndir, int dir, __nv_bfloat16* __restrict__ hi,
+                                         __nv_bfloat16* __restrict__ lo, int64_t pitch) {
+  pdl_entry();
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t r = warp; r < (int64_t)B * T; r += nwarps) {
+    const int t = (int)(r % T), b = (int)(r / T);
+    const int64_t len = lengths[b];
+    const int tp = dir == 0 ? t - 1 : t + 1;
+    const bool ok = (int64_t)t < len && tp >= 0 && (int64_t)tp < len;
+    const float* src = h + ((int64_t)b * T + tp) * (ndir * H) + dir * H;
+    uint32_t* hr = reinterpret_cast<uint32_t*>(hi + r * pitch);
+    uint32_t* lr = reinterpret_cast<uint32_t*>(lo + r * pitch);
+    for (int c = 2 * lane; c < H; c += 64) {      // H is a multiple of 4
+      const float a = ok ? src[c] : 0.f, v = ok ? src[c + 1] : 0.f;
+      const uint32_t hp = pack_bf16x2(a, v);
+      hr[c >> 1] = hp;
+      lr[c >> 1] = pack_bf16x2(a - __uint_as_float(hp << 16), v - __uint_as_float(hp & 0xffff0000u));
+    }
+  }
+}
+
+// out[l][d * 4H + i] = b_ih[l][d][i] + b_hh[l][d][i] for every layer and direction (the xproj GEMM's bias), one launch.
+struct LstmBiasList {
+  int n, len;                             // n = layers * ndir vectors of len = 4H
+  const float* a[2 * GANTTS_MAX_LSTM_LAYERS];
+  const float* b[2 * GANTTS_MAX_LSTM_LAYERS];
+  float* out[2 * GANTTS_MAX_LSTM_LAYERS];
+};
+__global__ void lstm_bias_sum_kernel(LstmBiasList bl) {
+  pdl_entry();
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (int64_t)bl.n * bl.len;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    const int v = (int)(i / bl.len), e = (int)(i - (int64_t)v * bl.len);
+    bl.out[v][e] = bl.a[v][e] + bl.b[v][e];
+  }
+}
+
 }  // namespace gantts
 
 using namespace gantts;
@@ -634,15 +715,12 @@ extern "C" int gantts_lstm_layer_fwd(const float* xproj, const float* W_hh, cons
   GANTTS_CHECK_ARG(xproj && W_hh && lengths_dev && h_out && gates && cells, "lstm_fwd: null pointer");
   GANTTS_CHECK_ARG(workspace && workspace_bytes >= 256, "lstm_fwd: workspace too small");
   LstmParams p{};
-  p.xproj = xproj; p.W_hh = W_hh; p.lengths = lengths_dev; p.h_out = h_out; p.gates = gates; p.cells = cells;
+  p.xproj = xproj; p.lengths = lengths_dev; p.h_out = h_out; p.gates = gates; p.cells = cells;
+  p.W_hh = W_hh;
+  p.W_hh_dir = (int64_t)4 * H * H;
   p.bar = static_cast<unsigned int*>(workspace);
   p.B = B; p.T = T; p.H = H; p.ndir = ndir;
-  const int hs = lstm_pick_hs(H, ndir, &p.slices);
-  if (hs == 8 && H <= 512 && lstm_use_reg()) return lstm_launch_reg(false, p, as_stream(stream));
-  if (hs == 8) return lstm_launch<8>(false, p, as_stream(stream));
-  if (hs == 16) return lstm_launch<16>(false, p, as_stream(stream));
-  set_error("lstm: hidden size %d x %d directions does not fit one wave of CTAs", H, ndir);
-  return GANTTS_E_UNSUPPORTED;
+  return lstm_run(false, p, as_stream(stream));
 }
 
 extern "C" int gantts_lstm_layer_bwd(const float* dh_out, const float* W_hh, const int64_t* lengths_dev,
@@ -653,16 +731,13 @@ extern "C" int gantts_lstm_layer_bwd(const float* dh_out, const float* W_hh, con
   GANTTS_CHECK_ARG(dh_out && W_hh && lengths_dev && gates && cells && dxproj, "lstm_bwd: null pointer");
   GANTTS_CHECK_ARG(workspace && workspace_bytes >= 256, "lstm_bwd: workspace too small");
   LstmParams p{};
-  p.W_hh = W_hh; p.lengths = lengths_dev; p.gates = const_cast<float*>(gates); p.cells = const_cast<float*>(cells);
+  p.lengths = lengths_dev; p.gates = const_cast<float*>(gates); p.cells = const_cast<float*>(cells);
+  p.W_hh = W_hh;
+  p.W_hh_dir = (int64_t)4 * H * H;
   p.dh_out = dh_out; p.dxproj = dxproj;
   p.bar = static_cast<unsigned int*>(workspace);
   p.B = B; p.T = T; p.H = H; p.ndir = ndir;
-  const int hs = lstm_pick_hs(H, ndir, &p.slices);
-  if (hs == 8 && H <= 512 && lstm_use_reg()) return lstm_launch_reg(true, p, as_stream(stream));
-  if (hs == 8) return lstm_launch<8>(true, p, as_stream(stream));
-  if (hs == 16) return lstm_launch<16>(true, p, as_stream(stream));
-  set_error("lstm: hidden size %d x %d directions does not fit one wave of CTAs", H, ndir);
-  return GANTTS_E_UNSUPPORTED;
+  return lstm_run(true, p, as_stream(stream));
 }
 
 extern "C" int gantts_lstm_hprev(const float* h, const int64_t* lengths_dev, float* hprev, int B, int T, int H,

@@ -1,8 +1,8 @@
-"""Fused GAN step: ONE C call (gantts_gan_step) per mini-batch for an MLP, In2OutHighwayNet or SRURNN generator + MLP
-discriminator -- the whole of reference train.py:528-580 enqueued on the current stream without a
+"""Fused GAN step: ONE C call (gantts_gan_step) per mini-batch for an MLP, In2OutHighwayNet, In2OutRNNHighwayNet or
+SRURNN generator + MLP discriminator -- the whole of reference train.py:528-580 enqueued on the current stream without a
 single host synchronisation (SURVEY.md 8f row 3).  Not drop-in for train.py (which owns its step
 functions); offered next to the compatible modular path (gantts_b200.step.GanTrainer), which also runs
-the LSTM generators.
+the LSTMRNN / GRURNN generators.
 
 Data parallel: utterance shards, the two flat gradient buffers are SUM all-reduced (NCCL via
 torch.distributed on the same stream) between the phases of the step; losses are normalised by the
@@ -24,16 +24,44 @@ LOSS_NAMES = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mse", "loss_mge", "l
 
 
 def _generator_parts(model_g):
-    """(highway gate Linear or None, [SRUCell...] (empty unless SRURNN), [MLP layers..., last layer]) of a generator the
-    fused step runs."""
+    """(highway gate Linear or None, [SRUCell...] (empty unless SRURNN), nn.LSTM or None (In2OutRNNHighwayNet),
+    [MLP layers..., last layer]) of a generator the fused step runs."""
     if isinstance(model_g, models.In2OutHighwayNet):
-        return model_g.T, [], list(model_g.H) + [model_g.last_linear]
+        return model_g.T, [], None, list(model_g.H) + [model_g.last_linear]
+    if isinstance(model_g, models.In2OutRNNHighwayNet):
+        return model_g.T, [], _check_lstm(model_g.lstm), [model_g.hidden2out]
     if isinstance(model_g, models.SRURNN):
-        return None, list(model_g.gru.rnn_lst), [model_g.hidden2out]
+        return None, list(model_g.gru.rnn_lst), None, [model_g.hidden2out]
     if hasattr(model_g, "layers") and hasattr(model_g, "last_linear"):
-        return None, [], list(model_g.layers) + [model_g.last_linear]
-    raise RuntimeError("FusedGanStep: generator %s is not supported (MLP, In2OutHighwayNet and SRURNN are); train it with "
-                       "gantts_b200.step.GanTrainer" % type(model_g).__name__)
+        return None, [], None, list(model_g.layers) + [model_g.last_linear]
+    raise RuntimeError("FusedGanStep: generator %s is not supported (MLP, In2OutHighwayNet, In2OutRNNHighwayNet and SRURNN "
+                       "are); train it with gantts_b200.step.GanTrainer" % type(model_g).__name__)
+
+
+def _check_lstm(lstm):
+    """The nn.LSTM of an In2OutRNNHighwayNet, if the fused step implements it."""
+    why = None
+    if getattr(lstm, "proj_size", 0) > 0:
+        why = "proj_size > 0"
+    elif not lstm.bias:
+        why = "bias=False"
+    elif not lstm.batch_first:
+        why = "batch_first=False"
+    elif lstm.num_layers > _lib.MAX_LSTM_LAYERS:
+        why = "%d layers (at most %d)" % (lstm.num_layers, _lib.MAX_LSTM_LAYERS)
+    if why is not None:
+        raise RuntimeError("FusedGanStep: an nn.LSTM with %s is not supported; train it with gantts_b200.step.GanTrainer"
+                           % why)
+    return lstm
+
+
+def _lstm_tensors(lstm):
+    """[(layer, direction, [weight_ih, weight_hh, bias_ih, bias_hh])] of an nn.LSTM in its parameters() order."""
+    out = []
+    for k in range(lstm.num_layers):
+        for d, sfx in enumerate(["", "_reverse"][:2 if lstm.bidirectional else 1]):
+            out.append((k, d, [getattr(lstm, "%s_l%d%s" % (n, k, sfx)) for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")]))
+    return out
 
 
 def _fill_sru(desc, cells):
@@ -95,23 +123,25 @@ class FusedGanStep(object):
         parallel.broadcast_parameters(model_d, group=process_group)
         c = _lib.GanStepT()
         c.B, c.T = self.B, self.T
-        self._gate, self._sru, g_layers = _generator_parts(model_g)
+        self._gate, self._sru, self._lstm, g_layers = _generator_parts(model_g)
         self._g_layers = _fill_mlp(c.g, g_layers, getattr(model_g, "dropout_p", 0.0), _lib.ACT_NONE)
         self._d_layers = _fill_mlp(c.d, list(model_d.layers) + [model_d.last_linear], model_d.dropout_p,
                                    _lib.ACT_SIGMOID)
         if getattr(model_g, "last_sigmoid", False) or not model_d.last_sigmoid:
             raise RuntimeError("FusedGanStep: generator must be linear-output, discriminator sigmoid-output")
-        # the generator's modules with parameters, in model_g.parameters() order (the gate or the SRU layers first)
-        self._g_mods = ([self._gate] if self._gate is not None else []) + self._sru + self._g_layers
         self._sums, self._sqs = [], []      # Adagrad: state_sum | Adam: exp_avg, exp_avg_sq (model.parameters() order)
 
-        def new_state(l):
-            a, b = torch.zeros_like(l.weight), torch.zeros_like(l.bias)
-            self._sums += [a, b]
-            a2 = b2 = None
+        def new_state1(t):
+            a = torch.zeros_like(t)
+            self._sums.append(a)
+            a2 = None
             if optimizer == "Adam":
-                a2, b2 = torch.zeros_like(l.weight), torch.zeros_like(l.bias)
-                self._sqs += [a2, b2]
+                a2 = torch.zeros_like(t)
+                self._sqs.append(a2)
+            return a, a2
+
+        def new_state(l):
+            (a, a2), (b, b2) = new_state1(l.weight), new_state1(l.bias)
             return a, b, a2, b2
         if self._gate is not None:
             gt, h = self._gate, c.highway
@@ -136,6 +166,25 @@ class FusedGanStep(object):
                 su.sumW[i], su.sumb[i] = a.data_ptr(), b.data_ptr()
                 if a2 is not None:
                     su.sqW[i], su.sqb[i] = a2.data_ptr(), b2.data_ptr()
+        if self._lstm is not None:
+            ls, lm = c.lstm, self._lstm
+            ls.num_layers, ls.in_dim, ls.hidden = lm.num_layers, lm.input_size, lm.hidden_size
+            ls.bidirectional = int(bool(lm.bidirectional))
+            ls.dropout = float(lm.dropout) if lm.num_layers > 1 else 0.0
+            for k, d, ts in _lstm_tensors(lm):
+                ops.require_cuda(*ts)
+                if not all(t.is_contiguous() for t in ts):
+                    raise RuntimeError("gantts_b200: parameters must be contiguous")
+                for t, sums, sqs in zip(ts, (ls.sumW_ih, ls.sumW_hh, ls.sumb_ih, ls.sumb_hh),
+                                        (ls.sqW_ih, ls.sqW_hh, ls.sqb_ih, ls.sqb_hh)):
+                    a, a2 = new_state1(t)
+                    sums[k][d] = a.data_ptr()
+                    if a2 is not None:
+                        sqs[k][d] = a2.data_ptr()
+            self._set_lstm_pointers(c)
+        # number of generator tensors (the MLP layers' state is added below): their optimiser state comes first in
+        # self._sums / self._sqs
+        self._ng = len(self._sums) + 2 * len(self._g_layers)
         for layers, sw, sb, qw, qb in ((self._g_layers, c.g_sumW, c.g_sumb, c.g_sqW, c.g_sqb),
                                        (self._d_layers, c.d_sumW, c.d_sumb, c.d_sqW, c.d_sqb)):
             for i, l in enumerate(layers):
@@ -186,6 +235,12 @@ class FusedGanStep(object):
         self._step = 0
         self._grad_views = {}
 
+    def _set_lstm_pointers(self, cfg):
+        ls = cfg.lstm
+        for k, d, ts in _lstm_tensors(self._lstm):
+            for t, dst in zip(ts, (ls.W_ih, ls.W_hh, ls.b_ih, ls.b_hh)):
+                dst[k][d] = t.data_ptr()
+
     def grad_buffer(self, which):
         """Flat fp32 gradient buffer (0 = generator, 1 = discriminator) as a tensor view."""
         if which not in self._grad_views:
@@ -227,6 +282,8 @@ class FusedGanStep(object):
             self.cfg.highway.W, self.cfg.highway.b = self._gate.weight.data_ptr(), self._gate.bias.data_ptr()
         for i, cell in enumerate(self._sru):
             self.cfg.sru.W[i], self.cfg.sru.b[i] = cell.weight.data_ptr(), cell.bias.data_ptr()
+        if self._lstm is not None:
+            self._set_lstm_pointers(self.cfg)
         if train is None:
             if self.g.training != self.d.training:
                 raise RuntimeError("FusedGanStep: generator and discriminator disagree on train()/eval()")
@@ -290,13 +347,13 @@ class FusedGanStep(object):
                                   "differentiable": False, "fused": None, "params": list(range(n))}]}
 
     def state_dict(self):
-        ng, n = 2 * len(self._g_mods), len(self._sums)
+        ng, n = self._ng, len(self._sums)
         return {"optimizer_g": self._opt_state(0, ng, float(self.cfg.lr_g), float(self.cfg.wd_g)),
                 "optimizer_d": self._opt_state(ng, n, float(self.cfg.lr_d), float(self.cfg.wd_d)),
                 "step": self._step, "seed": self._seed}
 
     def load_state_dict(self, sd):
-        ng, n = 2 * len(self._g_mods), len(self._sums)
+        ng, n = self._ng, len(self._sums)
         for key, lo, hi in (("optimizer_g", 0, ng), ("optimizer_d", ng, n)):
             st = sd[key]["state"]
             for i in range(hi - lo):

@@ -348,6 +348,41 @@ typedef struct {
   float* sqb[GANTTS_MAX_SRU_LAYERS];
 } gantts_sru_stack_t;
 
+/* In2OutRNNHighwayNet generator (reference gantts/models.py:72-118, the RNN VC model of hparams.py): num_layers > 0,
+ * together with the highway block (static_dim = S).  Then g is hidden2out alone (g.num_layers == 1, g.dims[0] =
+ * ndir * hidden, g.dims[1] = in_dim) and the step computes, with x_s = x[:, :, :S],
+ *   h = nn.LSTM(in_dim, hidden, num_layers, bidirectional, dropout)(x) with the packed-sequence semantics of
+ *       gantts_lstm_layer_fwd (sequence b runs for t < lengths[b], outputs beyond are zero),
+ *   Tx = sigmoid(x_s T.weight^T + T.bias),   Gx = MLPG(hidden2out(h)),   y_hat_static = x_s + Tx * Gx,   y_hat = x.
+ * Like the reference the model returns its INPUT as y_hat (models.py:118), so loss_mse = MaskedMSE(x, y) is reported
+ * but sends no gradient into the generator.  In training the output of every layer but the last is multiplied by
+ * gantts_dropout(ones[B * T][ndir * hidden], dropout, gantts_lstm_mask_seed(seed, layer)) (nn.LSTM's per-element
+ * inter-layer dropout).  Layer l has n_in = in_dim (l = 0) or ndir * hidden and, per direction d (0 forward, 1 reverse),
+ * the torch.nn.LSTM tensors W_ih[l][d] [4H][n_in], W_hh[l][d] [4H][H], b_ih[l][d], b_hh[l][d] [4H] (gates i, f, g, o).
+ * In model.parameters() order the gate's two tensors come first, then per layer and direction W_ih, W_hh, b_ih, b_hh,
+ * then hidden2out, in the flat gradient buffer, the clip norm and the optimiser step; b_ih and b_hh get the same
+ * gradient and keep separate optimiser state.  B <= 128, hidden a multiple of 4.  LSTMRNN / GRURNN (an LSTM stack
+ * without the gate) and stacks of more than GANTTS_MAX_LSTM_LAYERS layers train with the modular path.  Mutually
+ * exclusive with the SRU block. */
+#define GANTTS_MAX_LSTM_LAYERS 3
+typedef struct {
+  int num_layers;                          /* 0 = no LSTM stack (all other generators) */
+  int in_dim, hidden, bidirectional;
+  float dropout;                           /* in [0, 1) */
+  const float* W_ih[GANTTS_MAX_LSTM_LAYERS][2];   /* updated in place, like every tensor below */
+  const float* W_hh[GANTTS_MAX_LSTM_LAYERS][2];
+  const float* b_ih[GANTTS_MAX_LSTM_LAYERS][2];
+  const float* b_hh[GANTTS_MAX_LSTM_LAYERS][2];
+  float* sumW_ih[GANTTS_MAX_LSTM_LAYERS][2];      /* Adagrad state_sum | Adam exp_avg */
+  float* sumW_hh[GANTTS_MAX_LSTM_LAYERS][2];
+  float* sumb_ih[GANTTS_MAX_LSTM_LAYERS][2];
+  float* sumb_hh[GANTTS_MAX_LSTM_LAYERS][2];
+  float* sqW_ih[GANTTS_MAX_LSTM_LAYERS][2];       /* Adam exp_avg_sq (unused by Adagrad) */
+  float* sqW_hh[GANTTS_MAX_LSTM_LAYERS][2];
+  float* sqb_ih[GANTTS_MAX_LSTM_LAYERS][2];
+  float* sqb_hh[GANTTS_MAX_LSTM_LAYERS][2];
+} gantts_lstm_stack_t;
+
 typedef struct {
   int B, T;
   gantts_mlp_t g;                          /* generator: dims[0] = linguistic width, dims[L] = acoustic width */
@@ -381,6 +416,7 @@ typedef struct {
   float* d_sqb[GANTTS_MAX_LAYERS];
   gantts_highway_t highway;                /* static_dim = 0: plain MLP generator (all fields above keep their offsets) */
   gantts_sru_stack_t sru;                  /* num_layers = 0: no SRU stack (all fields above keep their offsets) */
+  gantts_lstm_stack_t lstm;                /* num_layers = 0: no LSTM stack (all fields above keep their offsets) */
 } gantts_gan_step_t;
 #define GANTTS_OPT_ADAGRAD 0
 #define GANTTS_OPT_ADAM 1
@@ -405,6 +441,9 @@ uint64_t gantts_mlp_layer_seed(uint64_t seed, int layer);
  * 1 the output mask [B][ncols].  A stream of its own (gantts_mlp_layer_seed(gantts_gan_step_seed(seed, 3), 2 layer +
  * which)), apart from the three MLP forwards above. */
 uint64_t gantts_sru_mask_seed(uint64_t seed, int layer, int which);
+/* Seed of the inter-layer dropout mask on the output of LSTM layer `layer` in a step called with `seed`: a stream of its
+ * own, apart from the three MLP forwards and every SRU mask. */
+uint64_t gantts_lstm_mask_seed(uint64_t seed, int layer);
 
 size_t gantts_gan_step_workspace_bytes(const gantts_gan_step_t* cfg);
 /* Flat gradient buffer inside `workspace` (which: 0 = generator, 1 = discriminator). */

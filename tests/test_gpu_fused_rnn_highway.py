@@ -1,0 +1,564 @@
+"""The fused GAN step (gantts_gan_step / FusedGanStep) with the In2OutRNNHighwayNet generator (reference
+gantts/models.py:72-118; bench.py cfg3): the sigmoid gate on x_static, the packed-sequence LSTM stack, hidden2out and the
+highway combine around the MLPG, their backward and their optimiser step inside the one-call step.
+
+The checker composes one-layer CPU torch nn.LSTMs on packed sequences and injects the step's own inter-layer dropout masks
+between them (every mask is gantts_dropout(ones[B * T][ndir * H], p, gantts_lstm_mask_seed(seed, layer))); with all-ones
+masks it equals the oracle port's In2OutRNNHighwayNet.  The discriminator's masks come from gantts_gan_step_seed as in
+test_gpu_fused_highway.py.  Tolerances: losses, gradient norms and y_hat_static 2e-4 relative (the cfg3 bound of
+test_gpu_train_mode.py); y_hat is the input, bit for bit; post-step weights median |delta| < 5e-6 and max <= 0.0201 (a
+first Adagrad / Adam step moves a weight by lr * sign(g)).  The configuration-rule test is host-only (no mark).
+"""
+import ctypes
+import os
+
+import numpy as np
+import pytest
+import torch
+
+from conftest import WINDOWS, rel_err
+from oracle import gantts_port as gp
+from oracle import nnmnkwii_port as nnp
+
+LOSS_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mge", "loss_mse", "loss_adv", "loss_g")
+GOLD_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mse", "loss_mge", "loss_adv", "loss_g",
+             "real_correct", "fake_correct")
+TOL = 2e-4
+KINDS = ("weight_ih", "weight_hh", "bias_ih", "bias_hh")
+
+
+def vc_ohp(width, cond=False):
+    return dict(stream_sizes=[width], has_dynamic_features=[True], adversarial_streams=[True],
+                mask_nth_mgc_for_adv_loss=0, num_windows=3, discriminator_linguistic_condition=cond)
+
+
+@pytest.fixture(scope="module")
+def dev():
+    import __graft_entry__
+    __graft_entry__.build()
+    return torch.device("cuda:0")
+
+
+def npy(t):
+    return t.detach().cpu().numpy()
+
+
+def step_hp(ohp):
+    from gantts_b200 import step as gstep
+    return gstep.HParams(windows=WINDOWS, stream_sizes=ohp["stream_sizes"], has_dynamic_features=ohp["has_dynamic_features"],
+                         adversarial_streams=ohp["adversarial_streams"], mask_nth_mgc_for_adv_loss=0,
+                         discriminator_linguistic_condition=ohp["discriminator_linguistic_condition"])
+
+
+def ragged_lengths(B, T, seed):
+    rng = np.random.RandomState(seed)
+    return sorted([T] + [int(v) for v in rng.randint(T // 2, T, B - 1)], reverse=True)
+
+
+def make_batch(B, T, d_in, d_out, lens, seed):
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(B, T, d_in, generator=g)
+    y = torch.randn(B, T, d_out, generator=g)
+    for b, n in enumerate(lens):
+        x[b, n:] = 0
+        y[b, n:] = 0
+    return x, y
+
+
+def sd_numpy(m):
+    return {k: v.detach().cpu().numpy() for k, v in m.state_dict().items()}
+
+
+def rhw_models(seed, S, layers, hidden, bidir, p, d_hidden, d_layers, p_d, cond=False):
+    import gantts_b200
+    torch.manual_seed(seed)
+    mg = gantts_b200.models.In2OutRNNHighwayNet(in_dim=3 * S, out_dim=3 * S, static_dim=S, num_hidden=layers,
+                                                hidden_dim=hidden, bidirectional=bidir, dropout=p)
+    md = gantts_b200.models.MLP(S + (3 * S if cond else 0), 1, d_layers, d_hidden, dropout=p_d, last_sigmoid=True)
+    return mg, md
+
+
+class RnnHighwayOracle(object):
+    """CPU In2OutRNNHighwayNet for gp.gan_step: one single-layer torch nn.LSTM per layer on packed sequences, with the
+    inter-layer dropout multipliers injected between them.  ``named`` maps the model's state_dict keys to the leaf
+    tensors; ``sums`` is the Adagrad state in the same order."""
+
+    def __init__(self, sd, num_layers, hidden, bidir, static_dim):
+        t = lambda k: torch.as_tensor(np.asarray(sd[k])).clone().float().requires_grad_(True)
+        self.S, self.sfx = static_dim, ["", "_reverse"][:2 if bidir else 1]
+        self.named = {"T.weight": t("T.weight"), "T.bias": t("T.bias")}
+        self.layers = []
+        for k in range(num_layers):
+            n_in = np.asarray(sd["lstm.weight_ih_l%d" % k]).shape[1]
+            m = torch.nn.LSTM(n_in, hidden, 1, batch_first=True, bidirectional=bidir)
+            with torch.no_grad():
+                for s in self.sfx:
+                    for n in KINDS:
+                        getattr(m, "%s_l0%s" % (n, s)).copy_(torch.as_tensor(np.asarray(sd["lstm.%s_l%d%s" % (n, k, s)])))
+                        self.named["lstm.%s_l%d%s" % (n, k, s)] = getattr(m, "%s_l0%s" % (n, s))
+            self.layers.append(m)
+        self.named["hidden2out.weight"], self.named["hidden2out.bias"] = t("hidden2out.weight"), t("hidden2out.bias")
+        self.sums = [torch.zeros_like(q) for q in self.params()]
+
+    def params(self):
+        return list(self.named.values())
+
+    def forward(self, x, R, lengths, masks=None):
+        """(y_hat, y_hat_static) = (x, x_s + sigmoid(T x_s) * MLPG(hidden2out(LSTM(x)))); masks[k] multiplies the output
+        of layer k < num_layers - 1, or None."""
+        xs = x[:, :, :self.S]
+        Tx = torch.sigmoid(torch.nn.functional.linear(xs, self.named["T.weight"], self.named["T.bias"]))
+        h = x
+        for k, m in enumerate(self.layers):
+            packed = torch.nn.utils.rnn.pack_padded_sequence(h, [int(v) for v in lengths], batch_first=True)
+            out, _ = m(packed)
+            h, _ = torch.nn.utils.rnn.pad_packed_sequence(out, batch_first=True, total_length=x.size(1))
+            if masks is not None and k + 1 < len(self.layers):
+                h = h * masks[k].view_as(h)
+        out = torch.nn.functional.linear(h, self.named["hidden2out.weight"], self.named["hidden2out.bias"])
+        return x, xs + Tx * nnp.unit_variance_mlpg(R, out)
+
+
+def lstm_masks(fs, mg, B, T, dev):
+    """The inter-layer masks the last training step of `fs` drew."""
+    from gantts_b200 import ops, _lib
+    lib = _lib.load()
+    lm = mg.lstm
+    nh = lm.hidden_size * (2 if lm.bidirectional else 1)
+    return [ops.dropout_mask(B * T, nh, lm.dropout, lib.gantts_lstm_mask_seed(fs.last_seed, k), dev).cpu()
+            for k in range(lm.num_layers - 1)]
+
+
+def d_masks(fs, M, d_hidden, p, dev):
+    from gantts_b200 import ops, _lib
+    lib = _lib.load()
+    s = fs.last_seed
+    stacked = ops.mlp_dropout_masks(2 * M, d_hidden, p, lib.gantts_gan_step_seed(s, 1), dev)
+    return {"real": [m[:M].cpu() for m in stacked], "fake": [m[M:].cpu() for m in stacked],
+            "adv": [m.cpu() for m in ops.mlp_dropout_masks(M, d_hidden, p, lib.gantts_gan_step_seed(s, 2), dev)]}
+
+
+def adv_loss_with(md, x, ys_ref, lens, ohp, adv_masks):
+    """loss_adv of the oracle's y_hat_static through the PRODUCT's updated discriminator (see test_gpu_fused_sru.py:
+    after D's first optimiser step, weights with near-zero gradients land 2 lr apart in the two implementations)."""
+    ps = list(md.parameters())
+    layers = [(w.detach().cpu(), b.detach().cpu()) for w, b in zip(ps[0::2], ps[1::2])]
+    fake_in = gp.get_selected_static_stream(ys_ref, ohp)
+    if ohp["discriminator_linguistic_condition"]:
+        fake_in = torch.cat((x, fake_in), -1)
+    mask = gp.sequence_mask(lens, x.size(1)).unsqueeze(-1)
+    D = gp.mlp_forward(fake_in, layers, last_sigmoid=True, masks=adv_masks)
+    return float(gp.bce_real(D, mask, mask.sum().item()))
+
+
+def loss_errors(got, ref, keys):
+    return {k: abs(float(got[k]) - ref[k]) / max(abs(ref[k]), 1e-12) for k in keys}
+
+
+def check_weights(model, named, tag):
+    for k, v in model.state_dict().items():
+        d = np.abs(npy(v) - named[k].detach().numpy())
+        assert np.median(d) < 5e-6 and d.max() <= 0.0201, (tag, k, np.median(d), d.max())
+
+
+def run_vs_oracle(dev, mg, md, ohp, B, T, steps, mse_w, p_d, d_hidden, seed, tag, optimizer="Adagrad"):
+    """`steps` training steps of FusedGanStep, each against the oracle started from the product's weights and optimiser
+    state, with the step's own masks injected."""
+    from gantts_b200 import fused
+    lm = mg.lstm
+    S = mg.static_dim
+    gen = RnnHighwayOracle(sd_numpy(mg), lm.num_layers, lm.hidden_size, lm.bidirectional, S)
+    d_layers = gp.discriminator_layers(sd_numpy(md))
+    d_params = [t for pair in d_layers for t in pair]
+    d_sum = [torch.zeros_like(t) for t in d_params]
+    okw = dict(lr=1e-3, betas=(0.5, 0.9), weight_decay=0.0, eps=1e-8) if optimizer == "Adam" else None
+    g_opt = gp.AdamStepper(gen.params(), **okw) if okw else None
+    d_opt = gp.AdamStepper(d_params, **okw) if okw else None
+    mg.to(dev).train(), md.to(dev).train()
+    fs = fused.FusedGanStep(mg, md, step_hp(ohp), B, T, w_d=1.0, mse_w=mse_w, mge_w=1.0, weight_decay=0.0, seed=seed,
+                            optimizer=optimizer, optimizer_params=okw)
+    names = [n for n, _ in mg.named_parameters()]
+    R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, T))
+    in_dim = 3 * S
+    for it in range(steps):
+        lens = ragged_lengths(B, T, seed + 10 * it)
+        x, y = make_batch(B, T, in_dim, in_dim, lens, seed + 10 * it + 1)
+        xd = x.to(dev)
+        fs.step(xd, y.to(dev), torch.LongTensor(lens).to(dev), frames=sum(lens))
+        got = fs.loss_dict()
+        gm = lstm_masks(fs, mg, B, T, dev)
+        dm = d_masks(fs, B * T, [d_hidden] * (len(d_layers) - 1), p_d, dev)
+        ref, yh_ref, ys_ref = gp.gan_step(lambda: gen.forward(x, R, lens, gm), gen.params(), gen.sums, d_layers, d_sum,
+                                          x, y, lens, R, ohp, w_d=1.0, mse_w=mse_w, mge_w=1.0, adv_w=1.0, dropout_d=p_d,
+                                          training=True, weight_decay=0.0, d_masks=dm, d_opt=d_opt, g_opt=g_opt)
+        ref = dict(ref, loss_adv=adv_loss_with(md, x, ys_ref, lens, ohp, dm["adv"]))
+        errs = loss_errors(got, ref, LOSS_KEYS + ("d_grad_norm", "g_grad_norm"))
+        errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), ys_ref.numpy())
+        assert max(errs.values()) < TOL, (tag, it, errs)
+        assert torch.equal(fs.y_hat, xd)                                   # models.py:118: the input is y_hat
+        assert abs(got["real_correct"] - ref["real_correct"]) <= 3 and abs(got["fake_correct"] - ref["fake_correct"]) <= 3
+        check_weights(mg, gen.named, "%s step %d" % (tag, it))
+        # the next step starts from the product's weights and optimiser state
+        sd = fs.state_dict()
+        with torch.no_grad():
+            for i, n in enumerate(names):
+                gen.named[n].copy_(mg.state_dict()[n].cpu())
+            for r, q in zip(d_params, md.parameters()):
+                r.copy_(q.detach().cpu())
+            order = list(gen.named)
+            for key, params, keys, sums, opt in (("optimizer_g", None, names, gen.sums, g_opt),
+                                                 ("optimizer_d", d_params, None, d_sum, d_opt)):
+                st = sd[key]["state"]
+                for i in range(len(st)):
+                    j = order.index(keys[i]) if keys is not None else i      # oracle order of parameter i
+                    if opt is None:
+                        sums[j].copy_(st[i]["sum"].cpu())
+                    else:
+                        opt.m[j].copy_(st[i]["exp_avg"].cpu())
+                        opt.v[j].copy_(st[i]["exp_avg_sq"].cpu())
+    return fs
+
+
+@pytest.mark.gpu
+def test_fused_rnn_highway_golden(dev, golden_step_models):
+    """The `rhw_` vectors of the UNMODIFIED reference's train.py step functions (In2OutRNNHighwayNet 27 -> 27, S = 9,
+    2 x 12 bidirectional LSTM, D 9 -> 16 -> 16 -> 1, B = 3, T = 24, two mini-batches, ragged lengths, Adagrad wd 1e-7)
+    through FusedGanStep: every loss (the counts exactly), y_hat == x bit for bit, y_hat_static, and every post-step
+    generator and discriminator tensor."""
+    import gantts_b200
+    from gantts_b200 import fused
+    g = golden_step_models
+    sub = lambda pre: {k[len(pre):]: torch.from_numpy(g[k]) for k in g.files if k.startswith(pre)}
+    mg = gantts_b200.models.In2OutRNNHighwayNet(in_dim=27, out_dim=27, static_dim=9, num_hidden=2, hidden_dim=12,
+                                                bidirectional=True, dropout=0.0)
+    mg.load_state_dict(sub("rhw_g0_"))
+    md = gantts_b200.models.MLP(9, 1, 2, 16, dropout=0.0, last_sigmoid=True)
+    md.load_state_dict(sub("rhw_d0_"))
+    mg.to(dev).train(), md.to(dev).train()
+    w_d, mse_w, mge_w = [float(v) for v in g["rhw_cfg"]]
+    fs = fused.FusedGanStep(mg, md, step_hp(vc_ohp(27)), 3, 24, w_d=w_d, mse_w=mse_w, mge_w=mge_w, seed=5)
+    for it in range(2):
+        p = "rhw_it%d_" % it
+        lens = [int(v) for v in g[p + "lengths"]]
+        xd = torch.from_numpy(g[p + "x"]).to(dev)
+        fs.step(xd, torch.from_numpy(g[p + "y"]).to(dev), torch.LongTensor(lens).to(dev), adv_w=1.0 if w_d > 0 else 0.0)
+        got = fs.loss_dict()
+        for k, v in zip(GOLD_KEYS, g[p + "losses"]):
+            if np.isnan(v):
+                continue
+            if k.endswith("correct"):
+                assert got[k] == v, (it, k, got[k], v)
+            else:
+                assert abs(got[k] - v) <= 1e-4 * max(abs(v), 1e-3), (it, k, got[k], v)
+        assert torch.equal(fs.y_hat, xd)
+        assert np.array_equal(npy(fs.y_hat), g[p + "y_hat"])
+        assert rel_err(npy(fs.y_hat_static), g[p + "y_hat_static"]) < 1e-4
+        for pre, m in (("g_", mg), ("d_", md)):
+            for k, v in m.state_dict().items():
+                d = np.abs(npy(v) - g[p + pre + k])
+                assert np.median(d) < 5e-6 and d.max() <= 0.0201, (it, pre + k, np.median(d), d.max())
+
+
+@pytest.mark.gpu
+def test_fused_rnn_highway_cfg3_widths_train_mode(dev):
+    """cfg3 widths: In2OutRNNHighwayNet 177 -> 177 (S = 59, 3 x 512 bidirectional LSTM, LSTM dropout 0.5), D 59 -> 256 ->
+    256 -> 1 with dropout 0.5, B = 4 x T = 300 ragged (max length T), train mode, Adagrad: one step against the oracle
+    with the step's own masks -- the losses, both gradient norms, y_hat_static, and every post-step generator tensor
+    (weight_ih, weight_hh and both biases of every layer and direction).  With all-ones masks the oracle equals the
+    oracle port's In2OutRNNHighwayNet."""
+    B, T = 4, 300
+    mg, md = rhw_models(5, 59, 3, 512, True, 0.5, 256, 2, 0.5)
+    lens = ragged_lengths(B, T, 7)
+    x, _ = make_batch(B, T, 177, 177, lens, 8)
+    R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, T))
+    sd = sd_numpy(mg)
+    port = gp.GeneratorOracle("rnn_highway", sd, static_dim=59, num_hidden=3, hidden_dim=512, bidirectional=True)
+    mine = RnnHighwayOracle(sd, 3, 512, True, 59)
+    with torch.no_grad():
+        _, a = port.forward(x, R, lens, vc_ohp(177))
+        _, b = mine.forward(x, R, lens, None)
+    assert rel_err(b.numpy(), a.numpy()) < 1e-5
+    run_vs_oracle(dev, mg, md, vc_ohp(177), B, T, 1, 0.0, 0.5, 256, 300, "cfg3")
+
+
+TOY_CASES = [  # (bidirectional, layers, mse_w, conditioned D, optimizer)
+    (True, 1, 0.0, False, "Adagrad"),
+    (False, 2, 0.5, False, "Adagrad"),
+    (True, 3, 0.5, True, "Adagrad"),
+    (True, 2, 0.0, True, "Adam"),
+    (False, 3, 0.0, False, "Adam"),
+    (True, 3, 0.5, False, "Adam"),
+]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("bidir,layers,mse_w,cond,optimizer", TOY_CASES)
+def test_fused_rnn_highway_toy_vs_oracle(dev, bidir, layers, mse_w, cond, optimizer):
+    """Small stacks (S = 8: 24 -> 24, 12 hidden units per direction, LSTM dropout 0.3, D dropout 0.5), B = 3 x T = 40
+    ragged, two training steps against the oracle across uni/bi, 1-3 layers, mse_w 0 / 0.5, a conditioned D, Adagrad
+    and Adam."""
+    mg, md = rhw_models(40 + layers + 4 * bidir, 8, layers, 12, bidir, 0.3, 32, 2, 0.5, cond)
+    run_vs_oracle(dev, mg, md, vc_ohp(24, cond), 3, 40, 2, mse_w, 0.5, 32, 500 + layers, "toy", optimizer)
+
+
+@pytest.mark.gpu
+def test_fused_rnn_highway_matches_gan_trainer(dev):
+    """bench.py cfg3 shape (B = 16, T = 2000, ragged with max length T) with every dropout 0: two training steps of
+    FusedGanStep and of the modular GanTrainer agree on the losses, y_hat, y_hat_static and the updated weights; so do
+    their eval phases.  Each step starts both from the fused step's weights: a first Adagrad step moves a weight whose
+    gradient is near zero by +-lr on either side, and through 2000 recurrent steps that alone moves y_hat_static by
+    more than the tolerance (3e-3 measured; the losses still agree to 1e-5)."""
+    from gantts_b200 import fused, step as gstep
+    B, T = 16, 2000
+    hp = step_hp(vc_ohp(177))
+    mk = lambda: rhw_models(21, 59, 3, 512, True, 0.0, 256, 2, 0.0)
+    (mg, md), (tg, td) = mk(), mk()
+    for m in (mg, md, tg, td):
+        m.to(dev).train()
+    fs = fused.FusedGanStep(mg, md, hp, B, T, w_d=1.0, mse_w=0.0, mge_w=1.0, weight_decay=0.0, seed=22)
+    tr = gstep.GanTrainer(tg, td, hp, w_d=1.0, mse_w=0.0, mge_w=1.0, weight_decay=0.0)
+    R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, T)).to(dev)
+    for it in range(3):
+        train = it < 2
+        with torch.no_grad():
+            for a, b in zip(list(mg.parameters()) + list(md.parameters()), list(tg.parameters()) + list(td.parameters())):
+                b.copy_(a)
+        if not train:
+            for m in (mg, md, tg, td):
+                m.eval()
+        lens = ragged_lengths(B, T, 23 + it)
+        x, y = make_batch(B, T, 177, 177, lens, 24 + it)
+        xd, yd = x.to(dev), y.to(dev)
+        fs.step(xd, yd, torch.LongTensor(lens).to(dev))
+        got = fs.loss_dict()
+        out, yh, ys = tr.step(xd, yd, lens, R, train=train)
+        errs = loss_errors(got, {k: float(out[k]) for k in LOSS_KEYS}, LOSS_KEYS)
+        errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), npy(ys))
+        assert max(errs.values()) < TOL, (it, errs)
+        assert torch.equal(fs.y_hat, yh) and torch.equal(fs.y_hat, xd)
+        for i, (a, b) in enumerate(zip(list(mg.parameters()) + list(md.parameters()),
+                                       list(tg.parameters()) + list(td.parameters()))):
+            d = np.abs(npy(a) - npy(b))
+            assert np.median(d) < 5e-6 and d.max() <= 0.0201, (it, i, np.median(d), d.max())
+
+
+@pytest.mark.gpu
+def test_fused_rnn_highway_invariants(dev):
+    """Phases 1, 2 and 4 called one by one give exactly what one call gives, with grad_buffer(0) holding every generator
+    tensor in model_g.parameters() order; mse_w moves no generator weight (the model returns its input); an eval-phase
+    call leaves every parameter and all optimiser state bit-unchanged; state_dict()'s generator part loads into
+    torch.optim.Adagrad(model_g.parameters())."""
+    from gantts_b200 import fused
+    B, T = 3, 60
+    hp = step_hp(vc_ohp(24))
+    lens = ragged_lengths(B, T, 31)
+    x, y = make_batch(B, T, 24, 24, lens, 32)
+    xd, yd, ld = x.to(dev), y.to(dev), torch.LongTensor(lens).to(dev)
+    runs = []
+    for split, mse_w in ((False, 0.5), (True, 0.5), (False, 0.0)):
+        mg, md = rhw_models(33, 8, 3, 16, True, 0.3, 32, 2, 0.5)
+        mg.to(dev).train(), md.to(dev).train()
+        fs = fused.FusedGanStep(mg, md, hp, B, T, mse_w=mse_w, weight_decay=0.0, seed=34)
+        if split:
+            fs.cfg.adv_w, fs._step, fs.cfg.opt_step = 1.0, 1, 1
+            for ph in (1, 2, 4):
+                fs._call(ph, xd, yd, ld, 0.0, fs._seed)
+        else:
+            fs.step(xd, yd, ld)
+            assert fs.last_seed == fs._seed
+        gb = fs.grad_buffer(0)
+        params = list(mg.parameters())
+        assert gb.numel() == sum(q.numel() for q in params) and len(params) == 2 + 8 * 3 + 2
+        off = 0
+        for q, s in zip(params, fs._sums):                 # weight decay 0: Adagrad's first state_sum = g^2
+            n = q.numel()
+            assert torch.equal((gb[off:off + n] * gb[off:off + n]).view_as(q), s)
+            off += n
+        ng = len(params)
+        assert torch.equal(fs._sums[4], fs._sums[5])       # bias_ih_l0 and bias_hh_l0 get the same gradient
+        runs.append([fs.losses.clone(), fs.y_hat.clone(), fs.y_hat_static.clone(), gb.clone(), fs.grad_buffer(1).clone()]
+                    + [q.detach().clone() for q in list(mg.parameters()) + list(md.parameters())]
+                    + [s.clone() for s in fs._sums[:ng]])
+    for a, b in zip(runs[0], runs[1]):
+        assert torch.equal(a, b)
+    assert runs[2][0][6] != runs[0][0][6]                  # loss_g carries the MSE term ...
+    for a, b in zip(runs[0][3:], runs[2][3:]):             # ... which sends no gradient into G
+        assert torch.equal(a, b)
+    wsnap = [q.detach().clone() for q in list(mg.parameters()) + list(md.parameters())]
+    ssnap = [s.clone() for s in fs._sums]
+    mg.eval(), md.eval()
+    fs.step(xd, yd, ld)
+    assert fs.loss_dict()["g_grad_norm"] == 0.0 and torch.equal(fs.y_hat, xd)
+    for a, b in zip(wsnap, list(mg.parameters()) + list(md.parameters())):
+        assert torch.equal(a, b.detach())
+    for a, b in zip(ssnap, fs._sums):
+        assert torch.equal(a, b)
+    sd = fs.state_dict()
+    assert len(sd["optimizer_g"]["state"]) == ng and len(sd["optimizer_d"]["state"]) == len(list(md.parameters()))
+    opt = torch.optim.Adagrad(mg.parameters(), lr=0.01, weight_decay=0.0)
+    opt.load_state_dict(sd["optimizer_g"])
+    assert torch.equal(opt.state[mg.T.weight]["sum"], fs._sums[0])
+    assert torch.equal(opt.state[mg.lstm.weight_hh_l2_reverse]["sum"], fs._sums[2 + 8 * 2 + 4 + 1])
+    assert torch.equal(opt.state[mg.hidden2out.bias]["sum"], fs._sums[ng - 1])
+
+
+@pytest.mark.gpu
+def test_fused_rnn_highway_adam_resume(dev):
+    """Under Adam, a step resumed from state_dict() in a new FusedGanStep is bit-identical to the uninterrupted one."""
+    from gantts_b200 import fused
+    B, T = 3, 50
+    hp = step_hp(vc_ohp(24))
+    okw = dict(lr=1e-3, betas=(0.5, 0.9), weight_decay=0.0, eps=1e-8)
+    build = lambda: rhw_models(51, 8, 2, 16, True, 0.3, 32, 2, 0.5)
+    mg, md = build()
+    mg.to(dev).train(), md.to(dev).train()
+    fs = fused.FusedGanStep(mg, md, hp, B, T, seed=52, optimizer="Adam", optimizer_params=okw)
+    lens = ragged_lengths(B, T, 53)
+    x, y = make_batch(B, T, 24, 24, lens, 54)
+    xd, yd, ld = x.to(dev), y.to(dev), torch.LongTensor(lens).to(dev)
+    fs.step(xd, yd, ld)
+    snap = [q.detach().clone() for q in list(mg.parameters()) + list(md.parameters())]
+    sd = fs.state_dict()
+    fs.step(xd, yd, ld)
+    want = fs.loss_dict()
+    after = [q.detach().clone() for q in list(mg.parameters()) + list(md.parameters())]
+    g2, d2 = build()
+    g2.to(dev).train(), d2.to(dev).train()
+    with torch.no_grad():
+        for q, v in zip(list(g2.parameters()) + list(d2.parameters()), snap):
+            q.copy_(v)
+    fs2 = fused.FusedGanStep(g2, d2, hp, B, T, seed=999, optimizer="Adam", optimizer_params=okw)
+    fs2.load_state_dict(sd)
+    fs2.step(xd, yd, ld)
+    assert fs2.loss_dict() == want
+    for q, v in zip(list(g2.parameters()) + list(d2.parameters()), after):
+        assert torch.equal(q.detach(), v)
+
+
+@pytest.mark.gpu
+def test_fused_step_still_rejects_grurnn_and_unsupported_lstms(dev):
+    """GRURNN (an LSTM stack without the gate) is refused with a message that points to GanTrainer, and so is an
+    In2OutRNNHighwayNet whose nn.LSTM the fused step does not implement."""
+    import gantts_b200
+    from gantts_b200 import fused
+    hp = step_hp(vc_ohp(24))
+    md = gantts_b200.models.MLP(8, 1, 2, 16, dropout=0.0, last_sigmoid=True).to(dev)
+    mg = gantts_b200.models.GRURNN(in_dim=24, out_dim=24, num_hidden=1, hidden_dim=16).to(dev)
+    with pytest.raises(RuntimeError, match="GanTrainer"):
+        fused.FusedGanStep(mg, md, hp, 2, 10)
+    for kw in (dict(proj_size=4), dict(bias=False), dict(batch_first=False), dict(num_layers=4)):
+        mg, _ = rhw_models(1, 8, 2, 16, True, 0.0, 16, 2, 0.0)
+        a = dict(input_size=24, hidden_size=16, num_layers=2, batch_first=True, bidirectional=True)
+        a.update(kw)
+        mg.lstm = torch.nn.LSTM(**a)
+        mg.hidden2out = torch.nn.Linear((4 if "proj_size" in kw else 16) * 2, 24)
+        with pytest.raises(RuntimeError, match="GanTrainer"):
+            fused.FusedGanStep(mg.to(dev), md, hp, 2, 10)
+
+
+def _rhw_step_config():
+    """A valid In2OutRNNHighwayNet configuration of gantts_gan_step_t on the cfg3 layout (host pointers are
+    placeholders: only the configuration check and the workspace layout run)."""
+    from gantts_b200 import _lib
+    S, fake, H, nl = 59, 1 << 20, 16, 3
+    c = _lib.GanStepT()
+    c.B, c.T = 2, 16
+    c.g.num_layers = 1
+    c.g.dims[0], c.g.dims[1] = 2 * H, 3 * S
+    c.d.num_layers = 2
+    for i, v in enumerate((S, 32, 1)):
+        c.d.dims[i] = v
+    for m in (c.g, c.d):
+        for i in range(m.num_layers):
+            m.W[i] = m.b[i] = fake
+    c.g_sumW[0] = c.g_sumb[0] = fake
+    c.g.last_act, c.d.last_act = _lib.ACT_NONE, _lib.ACT_SIGMOID
+    c.streams = _lib.make_streams([(0, S, True, 0)])
+    c.windows = _lib.make_windows(WINDOWS)
+    c.mlpg_table = fake
+    c.n_static = c.n_static_cols = c.n_adv = S
+    for i in range(S):
+        c.static_cols[i] = c.adv_cols[i] = i
+    c.w_d, c.mge_w, c.adv_w, c.max_norm, c.lr_g, c.lr_d, c.eps = 1.0, 1.0, 1.0, 1.0, 0.01, 0.01, 1e-10
+    c.optimizer = _lib.OPT_ADAGRAD
+    h = c.highway
+    h.static_dim = S
+    h.W = h.b = h.sumW = h.sumb = fake
+    ls = c.lstm
+    ls.num_layers, ls.in_dim, ls.hidden, ls.bidirectional, ls.dropout = nl, 3 * S, H, 1, 0.5
+    for k in range(nl):
+        for d in range(2):
+            for f in ("W_ih", "W_hh", "b_ih", "b_hh", "sumW_ih", "sumW_hh", "sumb_ih", "sumb_hh"):
+                getattr(ls, f)[k][d] = fake
+    return c
+
+
+def test_rnn_highway_step_config_rules(tmp_path):
+    """gantts_gan_step_workspace_bytes (host-only) accepts the In2OutRNNHighwayNet layout and rejects, with a message
+    naming the rule, every LSTM configuration the step does not implement; the LSTM mask seeds are a stream of their
+    own; the ctypes mirror of the appended block matches the header."""
+    import subprocess
+    import __graft_entry__
+    __graft_entry__.build()
+    from gantts_b200 import _lib
+    lib = _lib.load()
+    ws = lambda c: lib.gantts_gan_step_workspace_bytes(ctypes.byref(c))
+    err = lambda: lib.gantts_last_error_string().decode()
+    c = _rhw_step_config()
+    assert ws(c) > 0, err()
+    with_lstm = ws(c)
+    c.lstm.num_layers = 0                         # the gate + a one-layer MLP on x: no LSTM workspace
+    c.g.dims[0] = 3 * 59
+    assert 0 < ws(c) < with_lstm, err()
+
+    def rejected(mutate, needle):
+        c = _rhw_step_config()
+        mutate(c)
+        assert ws(c) == 0 and needle in err(), (needle, err())
+    rejected(lambda c: setattr(c.highway, "static_dim", 0), "highway gate")
+    rejected(lambda c: setattr(c.sru, "num_layers", 1), "mutually exclusive")
+    rejected(lambda c: setattr(c.lstm, "num_layers", _lib.MAX_LSTM_LAYERS + 1), "LSTM layer count")
+    rejected(lambda c: setattr(c.lstm, "num_layers", -1), "LSTM layer count")
+    rejected(lambda c: setattr(c.lstm, "hidden", 18), "multiple of 4")
+    rejected(lambda c: setattr(c, "B", 129), "LSTM_MAX_B")
+    rejected(lambda c: setattr(c.lstm, "dropout", 1.0), "LSTM dropout")
+    rejected(lambda c: setattr(c.lstm, "dropout", -0.1), "LSTM dropout")
+    rejected(lambda c: c.g.dims.__setitem__(0, 16), "hidden2out")
+    rejected(lambda c: setattr(c.g, "num_layers", 2), "hidden2out")
+    rejected(lambda c: setattr(c.lstm, "in_dim", 3 * 59 - 1), "in_dim")
+
+    def narrow(c):                                # in_dim < S (with a matching hidden2out)
+        c.lstm.in_dim = c.g.dims[1] = 40
+    rejected(narrow, "static_dim")
+    rejected(lambda c: c.lstm.W_hh[2].__setitem__(1, None), "null LSTM weight")
+    rejected(lambda c: c.lstm.b_ih[0].__setitem__(0, None), "null LSTM weight")
+    rejected(lambda c: c.lstm.sumb_hh[1].__setitem__(0, None), "optimiser state")
+
+    def adam(c):                                  # exp_avg_sq for every tensor but layer 2's reverse W_hh
+        c.optimizer, c.beta1, c.beta2 = _lib.OPT_ADAM, 0.5, 0.9
+        c.highway.sqW = c.highway.sqb = c.g_sqW[0] = c.g_sqb[0] = 1 << 20
+        for k in range(3):
+            for d in range(2):
+                for f in ("sqW_ih", "sqW_hh", "sqb_ih", "sqb_hh"):
+                    getattr(c.lstm, f)[k][d] = 1 << 20
+        c.lstm.sqW_hh[2][1] = None
+    rejected(adam, "exp_avg_sq for LSTM layer 2 direction 1")
+    # the seeds of the LSTM masks are a stream of their own
+    for seed in (0, 5, 12345):
+        lstm_seeds = {lib.gantts_lstm_mask_seed(seed, l) for l in range(_lib.MAX_LSTM_LAYERS)}
+        others = {lib.gantts_gan_step_seed(seed, w) for w in range(4)}
+        others |= {lib.gantts_sru_mask_seed(seed, l, w) for l in range(_lib.MAX_SRU_LAYERS) for w in range(2)}
+        assert len(lstm_seeds) == _lib.MAX_LSTM_LAYERS and not lstm_seeds & others
+    # offsets of the appended block and inside it, against the C compiler's view of the header
+    fields = [("gantts_gan_step_t", "lstm", _lib.GanStepT.lstm.offset)]
+    for f in ("in_dim", "dropout", "W_ih", "b_hh", "sumW_ih", "sqb_hh"):
+        fields.append(("gantts_lstm_stack_t", f, getattr(_lib.LstmStackT, f).offset))
+    src = tmp_path / "layout.c"
+    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "gantts_b200.h"\nint main(void) {\n'
+                   '  printf("%zu %zu", sizeof(gantts_gan_step_t), sizeof(gantts_lstm_stack_t));\n' +
+                   "".join('  printf(" %%zu", offsetof(%s, %s));\n' % (s, f) for s, f, _ in fields) + "  return 0;\n}\n")
+    exe = tmp_path / "layout"
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    subprocess.run(["gcc", "-I", os.path.join(root, "include"), "-o", str(exe), str(src)], check=True)
+    got = [int(v) for v in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
+    assert got == [ctypes.sizeof(_lib.GanStepT), ctypes.sizeof(_lib.LstmStackT)] + [o for _, _, o in fields]
