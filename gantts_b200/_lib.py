@@ -64,10 +64,7 @@ MAX_COLS = 256
 
 
 class HighwayT(ctypes.Structure):
-    _fields_ = [("static_dim", ctypes.c_int),
-                ("W", ctypes.c_void_p), ("b", ctypes.c_void_p),
-                ("sumW", ctypes.c_void_p), ("sumb", ctypes.c_void_p),
-                ("sqW", ctypes.c_void_p), ("sqb", ctypes.c_void_p)]
+    _fields_ = [("static_dim", ctypes.c_int)]
 
 
 MAX_SRU_LAYERS = 8
@@ -77,30 +74,32 @@ class SruStackT(ctypes.Structure):
     _fields_ = [("num_layers", ctypes.c_int),
                 ("in_dim", ctypes.c_int), ("hidden", ctypes.c_int), ("bidirectional", ctypes.c_int),
                 ("act", ctypes.c_int),
-                ("dropout", ctypes.c_float), ("rnn_dropout", ctypes.c_float),
-                ("W", ctypes.c_void_p * MAX_SRU_LAYERS), ("b", ctypes.c_void_p * MAX_SRU_LAYERS),
-                ("sumW", ctypes.c_void_p * MAX_SRU_LAYERS), ("sumb", ctypes.c_void_p * MAX_SRU_LAYERS),
-                ("sqW", ctypes.c_void_p * MAX_SRU_LAYERS), ("sqb", ctypes.c_void_p * MAX_SRU_LAYERS)]
+                ("dropout", ctypes.c_float), ("rnn_dropout", ctypes.c_float)]
 
 
 MAX_LSTM_LAYERS = 3
-_LstmPtrs = (ctypes.c_void_p * 2) * MAX_LSTM_LAYERS       # [layer][direction]
 
 
 class LstmStackT(ctypes.Structure):
     _fields_ = [("num_layers", ctypes.c_int),
                 ("in_dim", ctypes.c_int), ("hidden", ctypes.c_int), ("bidirectional", ctypes.c_int),
-                ("dropout", ctypes.c_float),
-                ("W_ih", _LstmPtrs), ("W_hh", _LstmPtrs), ("b_ih", _LstmPtrs), ("b_hh", _LstmPtrs),
-                ("sumW_ih", _LstmPtrs), ("sumW_hh", _LstmPtrs), ("sumb_ih", _LstmPtrs), ("sumb_hh", _LstmPtrs),
-                ("sqW_ih", _LstmPtrs), ("sqW_hh", _LstmPtrs), ("sqb_ih", _LstmPtrs), ("sqb_hh", _LstmPtrs)]
+                ("dropout", ctypes.c_float)]
+
+
+MAX_STEP_TENSORS = 32
+
+
+class StepTensorsT(ctypes.Structure):
+    _fields_ = [("n", ctypes.c_int),
+                ("param", ctypes.c_void_p * MAX_STEP_TENSORS),
+                ("state", ctypes.c_void_p * MAX_STEP_TENSORS),
+                ("state2", ctypes.c_void_p * MAX_STEP_TENSORS)]
 
 
 class GanStepT(ctypes.Structure):
     _fields_ = [("B", ctypes.c_int), ("T", ctypes.c_int),
-                ("g", MlpT), ("d", MlpT),
-                ("g_sumW", ctypes.c_void_p * MAX_LAYERS), ("g_sumb", ctypes.c_void_p * MAX_LAYERS),
-                ("d_sumW", ctypes.c_void_p * MAX_LAYERS), ("d_sumb", ctypes.c_void_p * MAX_LAYERS),
+                ("g", MlpT), ("highway", HighwayT), ("sru", SruStackT), ("lstm", LstmStackT), ("d", MlpT),
+                ("g_tensors", StepTensorsT), ("d_tensors", StepTensorsT),
                 ("streams", StreamsT), ("windows", WindowsT),
                 ("mlpg_table", ctypes.c_void_p),
                 ("n_static", ctypes.c_int), ("n_static_cols", ctypes.c_int),
@@ -112,12 +111,7 @@ class GanStepT(ctypes.Structure):
                 ("w_d", ctypes.c_float), ("mse_w", ctypes.c_float), ("mge_w", ctypes.c_float),
                 ("adv_w", ctypes.c_float),
                 ("optimizer", ctypes.c_int), ("beta1", ctypes.c_float), ("beta2", ctypes.c_float),
-                ("opt_step", ctypes.c_int64),
-                ("g_sqW", ctypes.c_void_p * MAX_LAYERS), ("g_sqb", ctypes.c_void_p * MAX_LAYERS),
-                ("d_sqW", ctypes.c_void_p * MAX_LAYERS), ("d_sqb", ctypes.c_void_p * MAX_LAYERS),
-                ("highway", HighwayT),
-                ("sru", SruStackT),
-                ("lstm", LstmStackT)]
+                ("opt_step", ctypes.c_int64)]
 
 
 OPT_ADAGRAD, OPT_ADAM = 0, 1

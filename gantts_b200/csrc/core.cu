@@ -91,7 +91,7 @@ extern "C" int gantts_profile_collect(double* ms, double* work, long long* launc
   return GANTTS_OK;
 }
 
-extern "C" int gantts_version(void) { return 103; }
+extern "C" int gantts_version(void) { return 104; }
 
 extern "C" const char* gantts_last_error_string(void) { return gantts::g_err; }
 

@@ -201,12 +201,11 @@ sse_fwd_bwd_kernel(const float* __restrict__ a, int64_t a_rs, const float* __res
   }
 }
 
-// clip_grad_norm_ + Adagrad with the sum of squares taken from the per-block partials of sumsq_partial_kernel:
-// every block re-reduces the (<= 592) partials itself in the same fixed order, which removes the finish launch.
-__global__ void __launch_bounds__(OPT_THREADS)
-clip_adagrad_partials_kernel(TensorList tl, const float* __restrict__ partial, int npartial, float* __restrict__ sumsq_out,
-                             float max_norm, float lr, float wd, float eps) {
-  pdl_entry();
+// clip_grad_norm_'s coefficient min(1, max_norm / (norm + 1e-6)) with the sum of squares taken from the per-block partials
+// of sumsq_partial_kernel: every block re-reduces the (<= 592) partials itself in the same fixed order, which removes the
+// finish launch; block 0 stores the sum of squares.
+__device__ __forceinline__ float clip_coef(const float* __restrict__ partial, int npartial, float* __restrict__ sumsq_out,
+                                           float max_norm) {
   __shared__ float sm[32];
   __shared__ float total_s;
   float v[1] = {0.f};
@@ -218,8 +217,16 @@ clip_adagrad_partials_kernel(TensorList tl, const float* __restrict__ partial, i
   }
   __syncthreads();
   const float total_norm = sqrtf(total_s);
-  float coef = max_norm / (total_norm + 1e-6f);
-  coef = coef < 1.f ? coef : 1.f;
+  const float coef = max_norm / (total_norm + 1e-6f);
+  return coef < 1.f ? coef : 1.f;
+}
+
+// clip_grad_norm_ + Adagrad
+__global__ void __launch_bounds__(OPT_THREADS)
+clip_adagrad_partials_kernel(TensorList tl, const float* __restrict__ partial, int npartial, float* __restrict__ sumsq_out,
+                             float max_norm, float lr, float wd, float eps) {
+  pdl_entry();
+  const float coef = clip_coef(partial, npartial, sumsq_out, max_norm);
   const int64_t total = tl.off[tl.n];
   for (int64_t i = (int64_t)blockIdx.x * OPT_THREADS + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * OPT_THREADS) {
@@ -241,19 +248,7 @@ __global__ void __launch_bounds__(OPT_THREADS)
 clip_adam_partials_kernel(TensorList tl, const float* __restrict__ partial, int npartial, float* __restrict__ sumsq_out,
                           float max_norm, float b1, float b2, float wd, float eps, float step_size, float inv_sqrt_bc2) {
   pdl_entry();
-  __shared__ float sm[32];
-  __shared__ float total_s;
-  float v[1] = {0.f};
-  for (int i = threadIdx.x; i < npartial; i += OPT_THREADS) v[0] += partial[i];
-  block_sum<1>(v, sm);
-  if (threadIdx.x == 0) {
-    total_s = v[0];
-    if (blockIdx.x == 0) sumsq_out[0] = v[0];
-  }
-  __syncthreads();
-  const float total_norm = sqrtf(total_s);
-  float coef = max_norm / (total_norm + 1e-6f);
-  coef = coef < 1.f ? coef : 1.f;
+  const float coef = clip_coef(partial, npartial, sumsq_out, max_norm);
   const int64_t total = tl.off[tl.n];
   for (int64_t i = (int64_t)blockIdx.x * OPT_THREADS + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * OPT_THREADS) {
@@ -318,40 +313,95 @@ static inline int blocks_1d(int64_t work, int per_block) {
   return (int)b;
 }
 
-// + the highway gate's weight and bias, or the SRU stack's weights and biases (the two are mutually exclusive); an
-// LSTM generator (gate, 8 tensors per layer, hidden2out) fits in the same count and in one TensorList of the clip kernels
-constexpr int MAX_PARAMS = 2 * GANTTS_MAX_LAYERS + 2 * GANTTS_MAX_SRU_LAYERS;
-static_assert(2 + 8 * GANTTS_MAX_LSTM_LAYERS + 2 <= MAX_PARAMS && 2 + 8 * GANTTS_MAX_LSTM_LAYERS + 2 <= OPT_MAX_TENSORS,
-              "the LSTM generator's tensors must fit one TensorList");
+static_assert(GANTTS_MAX_STEP_TENSORS == OPT_MAX_TENSORS, "one model's tensor table is one TensorList of the clip kernels");
+static_assert(2 + 2 * GANTTS_MAX_LAYERS <= GANTTS_MAX_STEP_TENSORS && 2 * GANTTS_MAX_SRU_LAYERS + 2 <= GANTTS_MAX_STEP_TENSORS &&
+                  2 + 8 * GANTTS_MAX_LSTM_LAYERS + 2 <= GANTTS_MAX_STEP_TENSORS,
+              "every generator the step accepts fits one tensor table");
 
+struct Bound {
+  float* p;               // parameter (updated in place)
+  float* g;               // its gradient in the model's flat buffer
+};
+enum { WEIGHT = 0, BIAS = 1 };
+enum { W_IH = 0, W_HH = 1, B_IH = 2, B_HH = 3 };     // nn.LSTM's tensors of one layer and direction
+
+// One model's tensor table bound to its stages (g_param_list / d_param_list): the lists of the clip + optimiser kernels,
+// and the pointers each stage uses.  The MLP layers' parameters go into the step's local gantts_mlp_t.
 struct ParamList {
   int n;
-  float* p[MAX_PARAMS];
-  float* g[MAX_PARAMS];
-  float* s[MAX_PARAMS];
-  float* s2[MAX_PARAMS];                                // Adam: exp_avg_sq (null for Adagrad)
-  int64_t sizes[MAX_PARAMS];
-  float* gW[GANTTS_MAX_LAYERS];
-  float* gb[GANTTS_MAX_LAYERS];
-  float* sgW[GANTTS_MAX_SRU_LAYERS];                    // SRU stack: gradient of W[l] / b[l] in the flat buffer
-  float* sgb[GANTTS_MAX_SRU_LAYERS];
-  float* lgW_ih[GANTTS_MAX_LSTM_LAYERS][2];             // LSTM stack: gradients of layer l, direction d in the flat buffer
-  float* lgW_hh[GANTTS_MAX_LSTM_LAYERS][2];
-  float* lgb_ih[GANTTS_MAX_LSTM_LAYERS][2];
-  float* lgb_hh[GANTTS_MAX_LSTM_LAYERS][2];
+  float* p[GANTTS_MAX_STEP_TENSORS];
+  float* g[GANTTS_MAX_STEP_TENSORS];
+  float* s[GANTTS_MAX_STEP_TENSORS];
+  float* s2[GANTTS_MAX_STEP_TENSORS];                   // Adam: exp_avg_sq
+  int64_t sizes[GANTTS_MAX_STEP_TENSORS];
   int64_t total;
+  Bound gate[2];                                        // T.weight, T.bias
+  Bound sru[GANTTS_MAX_SRU_LAYERS][2];                  // weight, bias per SRU layer
+  Bound lstm[GANTTS_MAX_LSTM_LAYERS][2][4];             // [layer][direction] W_ih, W_hh, b_ih, b_hh
+  float* gW[GANTTS_MAX_LAYERS];                         // gradients of the MLP layers
+  float* gb[GANTTS_MAX_LAYERS];
 };
 
 static inline size_t al256(size_t v) { return (v + 255) / 256 * 256; }
 
+// The step's workspace, carved front to back; every buffer starts on a 256-byte boundary (base nullptr: sizes only).
+struct Arena {
+  char* cur;
+  char* take(size_t bytes) {
+    char* p = cur;
+    cur += al256(bytes);
+    return p;
+  }
+  float* f32(size_t n) { return reinterpret_cast<float*>(take(n * sizeof(float))); }
+};
+
+// highway generator (zero bytes otherwise)
+struct HighwayWs {
+  float* tx;              // [M][S] gate sigmoid(x_s W_T^T + b_T)
+  float* gx;              // [M][S] MLPG output Gx
+  char* w;                // planes of W_T [S][S]
+  char* dz;               // planes of dz [M][S]
+  float* partial;         // split-K partials of dW_T / db_T
+};
+
+// SRU generator (zero bytes otherwise); per layer l:
+struct SruWs {
+  char* in[GANTTS_MAX_SRU_LAYERS];       // planes of the masked GEMM input [M][n_in] (layer l > 0: written by scan l-1)
+  float* u[GANTTS_MAX_SRU_LAYERS];       // U = planes(x * mask_x) W  [M][ncols * k]
+  float* c[GANTTS_MAX_SRU_LAYERS];       // cell states [M][ncols]
+  float* h[GANTTS_MAX_SRU_LAYERS];       // fp32 h [M][ncols] below the top layer (the next layer's highway input)
+  char* w[GANTTS_MAX_SRU_LAYERS];        // planes of W [n_in][ncols * k], then of W^T [ncols * k][n_in]
+  float* partial[GANTTS_MAX_SRU_LAYERS]; // split-K partials of dW
+  char* du;               // planes of dU [M][ncols * k] (one layer at a time)
+  float* dx;              // [M][ncols] dL/dh of the top layer, then dX = dU W of each layer for the one below
+  float* dxp;             // [M][ncols] highway gradient (k = 3) for the layer below
+  float* bpart;           // [B][2 * ncols] bias-gradient partials
+};
+
+// LSTM generator (zero bytes otherwise); per layer l:
+struct LstmWs {
+  char* in[GANTTS_MAX_LSTM_LAYERS];      // planes of the GEMM input [M][n_in]: x (l = 0), else h_{l-1} * mask_{l-1}
+  char* w[GANTTS_MAX_LSTM_LAYERS];       // planes of W_ih of both directions [ndir 4H][n_in], then [n_in][ndir 4H]
+  float* bias[GANTTS_MAX_LSTM_LAYERS];   // b_ih + b_hh [ndir 4H]
+  float* h[GANTTS_MAX_LSTM_LAYERS];      // h [M][ndir H]
+  float* gates[GANTTS_MAX_LSTM_LAYERS];  // [ndir][M][4H]
+  float* cells[GANTTS_MAX_LSTM_LAYERS];  // [ndir][M][H]
+  float* xproj;           // [M][ndir 4H] xproj of one layer; in the backward, dgates of one layer
+  float* out;             // [M][d_out] hidden2out's output, the MLPG's input
+  float* dh;              // [M][ndir H] dL/dh of the top layer, then mask * dX of each layer for the one below
+  char* dg;               // planes of dgates [M][ndir 4H]
+  char* hp;               // planes of hprev [M][H]
+  float* part[2][2];      // split-K partials per direction: [d][0] dW_ih | db_ih, [d][1] dW_hh (one layer at a time)
+  unsigned int* bar;      // grid-barrier counters of the recurrence
+};
+
 struct StepLayout {
   float* scal;
   float* mask;            // [M]
-  float* d_in;            // [2M][dD]  rows 0..M-1 real, M..2M-1 fake
+  float* d_in;            // [2M][dD]  rows 0..M-1 real, M..2M-1 fake (conditioned discriminator)
   float* d_out;           // [2M]
   float* g_dout;          // [2M]
   float* g_din;           // [2M][dD]
-  float* y_static;        // [M][n_static]
   float* g_static;        // [M][n_static]
   float* g_yhat;          // [M][d_out]
   float* g_grads;         // flat generator gradients
@@ -364,37 +414,9 @@ struct StepLayout {
   size_t mlp_ws_bytes;
   RedWs* red;             // [R_COUNT] deferred loss partials
   float* opt_partial;     // [OPT_MAX_BLOCKS] sum-of-squares partials of the model being stepped
-  // highway generator only (zero bytes otherwise, so the plain MLP layout is unchanged)
-  float* hw_tx;           // [M][S] gate sigmoid(x_s W_T^T + b_T)
-  float* hw_gx;           // [M][S] MLPG output Gx
-  char* hw_w;             // planes of W_T [S][S]
-  char* hw_dz;            // planes of dz [M][S]
-  float* hw_partial;      // split-K partials of dW_T / db_T
-  // SRU generator only (zero bytes otherwise, so the MLP and highway layouts are unchanged); per layer l:
-  char* sru_in[GANTTS_MAX_SRU_LAYERS];    // planes of the masked GEMM input [M][n_in] (layer l > 0: written by scan l-1)
-  float* sru_u[GANTTS_MAX_SRU_LAYERS];    // U = planes(x * mask_x) W  [M][ncols * k]
-  float* sru_c[GANTTS_MAX_SRU_LAYERS];    // cell states [M][ncols]
-  float* sru_h[GANTTS_MAX_SRU_LAYERS];    // fp32 h [M][ncols] below the top layer (the next layer's highway input)
-  char* sru_w[GANTTS_MAX_SRU_LAYERS];     // planes of W [n_in][ncols * k], then of W^T [ncols * k][n_in]
-  float* sru_partial[GANTTS_MAX_SRU_LAYERS];   // split-K partials of dW
-  char* sru_du;           // planes of dU [M][ncols * k] (one layer at a time)
-  float* sru_dx;          // [M][ncols] dL/dh of the top layer, then dX = dU W of each layer for the one below
-  float* sru_dxp;         // [M][ncols] highway gradient (k = 3) for the layer below
-  float* sru_bpart;       // [B][2 * ncols] bias-gradient partials
-  // LSTM generator only (zero bytes otherwise, so every other layout is unchanged); per layer l:
-  char* lstm_in[GANTTS_MAX_LSTM_LAYERS];      // planes of the GEMM input [M][n_in]: x (l = 0), else h_{l-1} * mask_{l-1}
-  char* lstm_w[GANTTS_MAX_LSTM_LAYERS];       // planes of W_ih of both directions [ndir 4H][n_in], then [n_in][ndir 4H]
-  float* lstm_bias[GANTTS_MAX_LSTM_LAYERS];   // b_ih + b_hh [ndir 4H]
-  float* lstm_h[GANTTS_MAX_LSTM_LAYERS];      // h [M][ndir H]
-  float* lstm_gates[GANTTS_MAX_LSTM_LAYERS];  // [ndir][M][4H]
-  float* lstm_cells[GANTTS_MAX_LSTM_LAYERS];  // [ndir][M][H]
-  float* lstm_xproj;      // [M][ndir 4H] xproj of one layer; in the backward, dgates of one layer
-  float* lstm_out;        // [M][d_out] hidden2out's output, the MLPG's input
-  float* lstm_dh;         // [M][ndir H] dL/dh of the top layer, then mask * dX of each layer for the one below
-  char* lstm_dg;          // planes of dgates [M][ndir 4H]
-  char* lstm_hp;          // planes of hprev [M][H]
-  float* lstm_part[2][2]; // split-K partials per direction: [d][0] dW_ih | db_ih, [d][1] dW_hh (one layer at a time)
-  unsigned int* lstm_bar; // grid-barrier counters of the recurrence
+  HighwayWs hw;
+  SruWs sru;
+  LstmWs lstm;
   size_t total;
 };
 
@@ -409,206 +431,75 @@ static inline int gen_in_width(const gantts_gan_step_t* c) {
   return c->sru.num_layers > 0 ? c->sru.in_dim : (c->lstm.num_layers > 0 ? c->lstm.in_dim : c->g.dims[0]);
 }
 
+// tensor pl->n of table t: the next `size` elements of the model's flat gradient buffer (flat nullptr: counts only)
+static Bound take_tensor(const gantts_step_tensors_t& t, int64_t size, float* flat, ParamList* pl) {
+  const int i = pl->n++;
+  const Bound b{t.param[i], flat ? flat + pl->total : nullptr};
+  pl->p[i] = b.p;
+  pl->g[i] = b.g;
+  pl->s[i] = t.state[i];
+  pl->s2[i] = t.state2[i];
+  pl->sizes[i] = size;
+  pl->total += size;
+  return b;
+}
+
+// the layers of m in order [W, b] each: parameters into m->W / m->b, gradients into pl->gW / pl->gb
+static void bind_mlp(const gantts_step_tensors_t& t, gantts_mlp_t* m, float* flat, ParamList* pl) {
+  for (int l = 0; l < m->num_layers; ++l) {
+    const Bound w = take_tensor(t, (int64_t)m->dims[l + 1] * m->dims[l], flat, pl);
+    const Bound b = take_tensor(t, m->dims[l + 1], flat, pl);
+    m->W[l] = w.p;
+    m->b[l] = b.p;
+    pl->gW[l] = w.g;
+    pl->gb[l] = b.g;
+  }
+}
+
+// The generator's table bound from the shapes, in model.parameters() order: [weight, bias] of every SRU layer, or
+// [T.weight, T.bias] of the highway gate and then [W_ih, W_hh, b_ih, b_hh] of every LSTM layer and direction; then the
+// MLP layers (hidden2out alone after a stack).  pl->n is the tensor count the shapes give, pl->total the elements.
+static void g_param_list(const gantts_gan_step_t* c, gantts_mlp_t* g, float* flat, ParamList* pl) {
+  pl->n = 0;
+  pl->total = 0;
+  const gantts_step_tensors_t& t = c->g_tensors;
+  const gantts_sru_stack_t& s = c->sru;
+  for (int l = 0; l < s.num_layers; ++l) {
+    pl->sru[l][WEIGHT] = take_tensor(t, (int64_t)sru_nin(s, l) * sru_ncols(s) * sru_k(s, l), flat, pl);
+    pl->sru[l][BIAS] = take_tensor(t, 2 * (int64_t)sru_ncols(s), flat, pl);
+  }
+  const int64_t S = c->highway.static_dim;
+  if (S > 0) {
+    pl->gate[WEIGHT] = take_tensor(t, S * S, flat, pl);
+    pl->gate[BIAS] = take_tensor(t, S, flat, pl);
+  }
+  const gantts_lstm_stack_t& ls = c->lstm;
+  const int64_t G4 = 4 * (int64_t)ls.hidden;
+  for (int l = 0; l < ls.num_layers; ++l)
+    for (int d = 0; d < lstm_ndir(ls); ++d) {
+      const int64_t sizes[4] = {G4 * lstm_nin(ls, l), G4 * ls.hidden, G4, G4};
+      for (int i = 0; i < 4; ++i) pl->lstm[l][d][i] = take_tensor(t, sizes[i], flat, pl);
+    }
+  bind_mlp(t, g, flat, pl);
+}
+
+static void d_param_list(const gantts_gan_step_t* c, gantts_mlp_t* d, float* flat, ParamList* pl) {
+  pl->n = 0;
+  pl->total = 0;
+  bind_mlp(c->d_tensors, d, flat, pl);
+}
+
+static int64_t g_param_count(const gantts_gan_step_t* c) {
+  ParamList pl;
+  gantts_mlp_t g = c->g;
+  g_param_list(c, &g, nullptr, &pl);
+  return pl.total;
+}
+
 static int64_t mlp_param_count(const gantts_mlp_t& m) {
   int64_t n = 0;
   for (int l = 0; l < m.num_layers; ++l) n += (int64_t)m.dims[l + 1] * m.dims[l] + m.dims[l + 1];
   return n;
-}
-
-// elements of the highway gate's parameters, which lead the generator's flat gradient buffer
-static int64_t gate_param_count(const gantts_gan_step_t* c) {
-  const int64_t S = c->highway.static_dim;
-  return S * S + S;
-}
-
-// elements of the SRU stack's parameters, which lead the generator's flat gradient buffer
-static int64_t sru_param_count(const gantts_gan_step_t* c) {
-  const gantts_sru_stack_t& s = c->sru;
-  int64_t n = 0;
-  for (int l = 0; l < s.num_layers; ++l) n += (int64_t)sru_nin(s, l) * sru_ncols(s) * sru_k(s, l) + 2 * sru_ncols(s);
-  return n;
-}
-
-// elements of the LSTM stack's parameters, which follow the gate in the generator's flat gradient buffer
-static int64_t lstm_param_count(const gantts_gan_step_t* c) {
-  const gantts_lstm_stack_t& s = c->lstm;
-  const int64_t G4 = 4 * (int64_t)s.hidden;
-  int64_t n = 0;
-  for (int l = 0; l < s.num_layers; ++l) n += lstm_ndir(s) * (G4 * lstm_nin(s, l) + G4 * s.hidden + 2 * G4);
-  return n;
-}
-
-static int64_t g_param_count(const gantts_gan_step_t* c) {
-  return gate_param_count(c) + sru_param_count(c) + lstm_param_count(c) + mlp_param_count(c->g);
-}
-
-static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
-  const int64_t M = (int64_t)c->B * c->T;
-  const int dD = c->d.dims[0];
-  char* cur = base;
-  auto take = [&](size_t bytes) { char* p = cur; cur += al256(bytes); return p; };
-  L->scal = (float*)take(S_COUNT * sizeof(float));
-  L->mask = (float*)take(M * sizeof(float));
-  L->d_in = (float*)take((size_t)2 * M * dD * sizeof(float));
-  L->d_out = (float*)take((size_t)2 * M * sizeof(float));
-  L->g_dout = (float*)take((size_t)2 * M * sizeof(float));
-  L->g_din = (float*)take((size_t)2 * M * dD * sizeof(float));
-  L->y_static = (float*)take((size_t)M * c->n_static * sizeof(float));
-  L->g_static = (float*)take((size_t)M * c->n_static * sizeof(float));
-  L->g_yhat = (float*)take((size_t)M * c->g.dims[c->g.num_layers] * sizeof(float));
-  L->g_grads = (float*)take(g_param_count(c) * sizeof(float));
-  L->d_grads = (float*)take(mlp_param_count(c->d) * sizeof(float));
-  L->g_tape_bytes = gantts_mlp_tape_bytes(&c->g, M);
-  L->g_tape = take(L->g_tape_bytes);
-  L->d_tape_bytes = gantts_mlp_tape_bytes(&c->d, 2 * M);
-  L->d_tape = take(L->d_tape_bytes);
-  size_t a = gantts_mlp_workspace_bytes(&c->g, M), b = gantts_mlp_workspace_bytes(&c->d, 2 * M);
-  L->mlp_ws_bytes = a > b ? a : b;
-  L->mlp_ws = take(L->mlp_ws_bytes);
-  L->red = (RedWs*)take(R_COUNT * sizeof(RedWs));
-  L->opt_partial = (float*)take(OPT_MAX_BLOCKS * sizeof(float));
-  const int S = c->highway.static_dim;
-  const bool hw = S > 0;
-  L->hw_tx = (float*)take(hw ? (size_t)M * S * sizeof(float) : 0);
-  L->hw_gx = (float*)take(hw ? (size_t)M * S * sizeof(float) : 0);
-  L->hw_w = take(hw ? 2 * plane_bytes(S, S) : 0);
-  L->hw_dz = take(hw ? 2 * plane_bytes(M, S) : 0);
-  L->hw_partial = (float*)take(hw ? mn_partial_bytes(M, S, S, nullptr, nullptr) : 0);
-  const gantts_sru_stack_t& s = c->sru;
-  const int nl = s.num_layers, nc = nl > 0 ? sru_ncols(s) : 0;
-  int maxku = 0;
-  for (int l = 0; l < GANTTS_MAX_SRU_LAYERS; ++l) {
-    L->sru_in[l] = L->sru_w[l] = nullptr;
-    L->sru_u[l] = L->sru_c[l] = L->sru_h[l] = L->sru_partial[l] = nullptr;
-    if (l >= nl) continue;
-    const int ni = sru_nin(s, l), ku = nc * sru_k(s, l);
-    maxku = ku > maxku ? ku : maxku;
-    L->sru_in[l] = take(2 * plane_bytes(M, ni));
-    L->sru_u[l] = (float*)take((size_t)M * ku * sizeof(float));
-    L->sru_c[l] = (float*)take((size_t)M * nc * sizeof(float));
-    if (l < nl - 1) L->sru_h[l] = (float*)take((size_t)M * nc * sizeof(float));
-    L->sru_w[l] = take(2 * plane_bytes(ni, ku) + 2 * plane_bytes(ku, ni));
-    L->sru_partial[l] = (float*)take(mn_partial_bytes(M, ni, ku, nullptr, nullptr));
-  }
-  L->sru_du = take(nl > 0 ? 2 * plane_bytes(M, maxku) : 0);
-  L->sru_dx = (float*)take((size_t)M * nc * sizeof(float));
-  L->sru_dxp = (float*)take((size_t)M * nc * sizeof(float));
-  L->sru_bpart = (float*)take((size_t)c->B * 2 * nc * sizeof(float));
-  const gantts_lstm_stack_t& ls = c->lstm;
-  const int lnl = ls.num_layers, H = lnl > 0 ? ls.hidden : 0, nd = lstm_ndir(ls), n4 = nd * 4 * H;
-  size_t part_ih = 0, part_hh = 0;
-  for (int l = 0; l < GANTTS_MAX_LSTM_LAYERS; ++l) {
-    L->lstm_in[l] = L->lstm_w[l] = nullptr;
-    L->lstm_bias[l] = L->lstm_h[l] = L->lstm_gates[l] = L->lstm_cells[l] = nullptr;
-    if (l >= lnl) continue;
-    const int ni = lstm_nin(ls, l);
-    L->lstm_in[l] = take(2 * plane_bytes(M, ni));
-    L->lstm_w[l] = take(2 * plane_bytes(n4, ni) + 2 * plane_bytes(ni, n4));
-    L->lstm_bias[l] = (float*)take((size_t)n4 * sizeof(float));
-    L->lstm_h[l] = (float*)take((size_t)M * nd * H * sizeof(float));
-    L->lstm_gates[l] = (float*)take((size_t)M * n4 * sizeof(float));
-    L->lstm_cells[l] = (float*)take((size_t)M * nd * H * sizeof(float));
-    const size_t pi = mn_partial_bytes(M, 4 * H, ni, nullptr, nullptr), ph = mn_partial_bytes(M, 4 * H, H, nullptr, nullptr);
-    part_ih = pi > part_ih ? pi : part_ih;
-    part_hh = ph > part_hh ? ph : part_hh;
-  }
-  const bool lstm = lnl > 0;
-  L->lstm_xproj = (float*)take((size_t)M * n4 * sizeof(float));
-  L->lstm_out = (float*)take(lstm ? (size_t)M * c->g.dims[c->g.num_layers] * sizeof(float) : 0);
-  L->lstm_dh = (float*)take((size_t)M * nd * H * sizeof(float));
-  L->lstm_dg = take(lstm ? 2 * plane_bytes(M, n4) : 0);
-  L->lstm_hp = take(lstm ? 2 * plane_bytes(M, H) : 0);
-  for (int d = 0; d < 2; ++d) {
-    L->lstm_part[d][0] = (float*)take(d < nd ? part_ih : 0);
-    L->lstm_part[d][1] = (float*)take(d < nd ? part_hh : 0);
-  }
-  L->lstm_bar = (unsigned int*)take(lstm ? 256 : 0);
-  L->total = (size_t)(cur - base) + 256;
-}
-
-// appends the layers of m; `flat` is where their gradients start in the model's flat buffer
-static void param_list(const gantts_mlp_t& m, float* const* sumW, float* const* sumb, float* const* sqW, float* const* sqb,
-                       float* flat, ParamList* pl) {
-  float* cur = flat;
-  for (int l = 0; l < m.num_layers; ++l) {
-    const int64_t nw = (int64_t)m.dims[l + 1] * m.dims[l], nb = m.dims[l + 1];
-    pl->gW[l] = cur;
-    pl->p[pl->n] = const_cast<float*>(m.W[l]);
-    pl->g[pl->n] = cur;
-    pl->s[pl->n] = sumW[l];
-    pl->s2[pl->n] = sqW[l];
-    pl->sizes[pl->n++] = nw;
-    cur += nw;
-    pl->gb[l] = cur;
-    pl->p[pl->n] = const_cast<float*>(m.b[l]);
-    pl->g[pl->n] = cur;
-    pl->s[pl->n] = sumb[l];
-    pl->s2[pl->n] = sqb[l];
-    pl->sizes[pl->n++] = nb;
-    cur += nb;
-  }
-  pl->total += cur - flat;
-}
-
-// generator parameters in model.parameters() order: [T.weight, T.bias] of a highway generator, or [W, b] of every layer
-// of an SRU stack; then [W_ih, W_hh, b_ih, b_hh] of every layer and direction of an LSTM stack; then the MLP layers
-static void g_param_list(const gantts_gan_step_t* c, float* flat, ParamList* pl) {
-  pl->n = 0;
-  pl->total = 0;
-  const gantts_highway_t& h = c->highway;
-  const gantts_sru_stack_t& s = c->sru;
-  for (int l = 0; l < s.num_layers; ++l) {
-    const int64_t sizes[2] = {(int64_t)sru_nin(s, l) * sru_ncols(s) * sru_k(s, l), 2 * (int64_t)sru_ncols(s)};
-    float* const ps[2] = {const_cast<float*>(s.W[l]), const_cast<float*>(s.b[l])};
-    float* const ss[2] = {s.sumW[l], s.sumb[l]};
-    float* const qs[2] = {s.sqW[l], s.sqb[l]};
-    pl->sgW[l] = flat + pl->total;
-    pl->sgb[l] = flat + pl->total + sizes[0];
-    for (int i = 0; i < 2; ++i) {
-      pl->p[pl->n] = ps[i];
-      pl->g[pl->n] = flat + pl->total;
-      pl->s[pl->n] = ss[i];
-      pl->s2[pl->n] = qs[i];
-      pl->sizes[pl->n++] = sizes[i];
-      pl->total += sizes[i];
-    }
-  }
-  if (h.static_dim > 0) {
-    const int64_t S = h.static_dim;
-    const int64_t sizes[2] = {S * S, S};
-    float* const ps[2] = {const_cast<float*>(h.W), const_cast<float*>(h.b)};
-    float* const ss[2] = {h.sumW, h.sumb};
-    float* const qs[2] = {h.sqW, h.sqb};
-    for (int i = 0; i < 2; ++i) {
-      pl->p[pl->n] = ps[i];
-      pl->g[pl->n] = flat + pl->total;
-      pl->s[pl->n] = ss[i];
-      pl->s2[pl->n] = qs[i];
-      pl->sizes[pl->n++] = sizes[i];
-      pl->total += sizes[i];
-    }
-  }
-  const gantts_lstm_stack_t& ls = c->lstm;
-  for (int l = 0; l < ls.num_layers; ++l)
-    for (int d = 0; d < lstm_ndir(ls); ++d) {
-      const int64_t G4 = 4 * (int64_t)ls.hidden;
-      const int64_t sizes[4] = {G4 * lstm_nin(ls, l), G4 * ls.hidden, G4, G4};
-      float* const ps[4] = {const_cast<float*>(ls.W_ih[l][d]), const_cast<float*>(ls.W_hh[l][d]),
-                            const_cast<float*>(ls.b_ih[l][d]), const_cast<float*>(ls.b_hh[l][d])};
-      float* const ss[4] = {ls.sumW_ih[l][d], ls.sumW_hh[l][d], ls.sumb_ih[l][d], ls.sumb_hh[l][d]};
-      float* const qs[4] = {ls.sqW_ih[l][d], ls.sqW_hh[l][d], ls.sqb_ih[l][d], ls.sqb_hh[l][d]};
-      float** const gs[4] = {&pl->lgW_ih[l][d], &pl->lgW_hh[l][d], &pl->lgb_ih[l][d], &pl->lgb_hh[l][d]};
-      for (int i = 0; i < 4; ++i) {
-        *gs[i] = flat + pl->total;
-        pl->p[pl->n] = ps[i];
-        pl->g[pl->n] = flat + pl->total;
-        pl->s[pl->n] = ss[i];
-        pl->s2[pl->n] = qs[i];
-        pl->sizes[pl->n++] = sizes[i];
-        pl->total += sizes[i];
-      }
-    }
-  param_list(c->g, c->g_sumW, c->g_sumb, c->g_sqW, c->g_sqb, flat + pl->total, pl);
 }
 
 static inline int bce_blocks(int64_t rows) { return grid_for(rows, RED_THREADS); }
@@ -645,7 +536,6 @@ static int clip_opt_model(const gantts_gan_step_t* c, const ParamList& pl, float
   GANTTS_PDL_LAUNCH((sumsq_partial_kernel), nb, OPT_THREADS, 0, st, tl, partial);
   GANTTS_LAUNCH_CHECK("sumsq_partial_kernel");
   if (adam) {
-    for (int i = 0; i < pl.n; ++i) GANTTS_CHECK_ARG(pl.s[i] && pl.s2[i], "gan_step: Adam needs exp_avg and exp_avg_sq for every tensor");
     GANTTS_CHECK_ARG(c->opt_step >= 1, "gan_step: Adam needs opt_step >= 1 (the number of the step being taken)");
     const double t = (double)c->opt_step;
     const float step_size = (float)((double)lr / (1.0 - pow((double)c->beta1, t)));
@@ -656,6 +546,18 @@ static int clip_opt_model(const gantts_gan_step_t* c, const ParamList& pl, float
   } else {
     GANTTS_PDL_LAUNCH((clip_adagrad_partials_kernel), nb, OPT_THREADS, 0, st, tl, partial, nb, sumsq_out, c->max_norm, lr, wd, c->eps);
     GANTTS_LAUNCH_CHECK("clip_adagrad_partials_kernel");
+  }
+  return GANTTS_OK;
+}
+
+// a model's table: the tensor count its shapes give, every tensor and its optimiser state non-null
+static int check_table(const gantts_gan_step_t* c, const gantts_step_tensors_t& t, int want, const char* model) {
+  GANTTS_CHECK_ARG(t.n == want, "gan_step: the %s table has %d tensors, its shapes give %d", model, t.n, want);
+  for (int i = 0; i < t.n; ++i) {
+    GANTTS_CHECK_ARG(t.param[i], "gan_step: null %s tensor %d", model, i);
+    GANTTS_CHECK_ARG(t.state[i], "gan_step: null %s optimiser state of tensor %d", model, i);
+    if (c->optimizer == GANTTS_OPT_ADAM)
+      GANTTS_CHECK_ARG(t.state2[i], "gan_step: Adam needs exp_avg_sq for %s tensor %d", model, i);
   }
   return GANTTS_OK;
 }
@@ -693,16 +595,6 @@ static int check_step(const gantts_gan_step_t* c) {
     GANTTS_CHECK_ARG(ls.in_dim == c->g.dims[1],
                      "gan_step: LSTM in_dim %d != hidden2out output width %d (the model returns its input as y_hat)",
                      ls.in_dim, c->g.dims[1]);
-    for (int l = 0; l < ls.num_layers; ++l)
-      for (int d = 0; d < lstm_ndir(ls); ++d) {
-        GANTTS_CHECK_ARG(ls.W_ih[l][d] && ls.W_hh[l][d] && ls.b_ih[l][d] && ls.b_hh[l][d],
-                         "gan_step: null LSTM weight/bias of layer %d direction %d", l, d);
-        GANTTS_CHECK_ARG(ls.sumW_ih[l][d] && ls.sumW_hh[l][d] && ls.sumb_ih[l][d] && ls.sumb_hh[l][d],
-                         "gan_step: null LSTM optimiser state of layer %d direction %d", l, d);
-        if (c->optimizer == GANTTS_OPT_ADAM)
-          GANTTS_CHECK_ARG(ls.sqW_ih[l][d] && ls.sqW_hh[l][d] && ls.sqb_ih[l][d] && ls.sqb_hh[l][d],
-                           "gan_step: Adam needs exp_avg_sq for LSTM layer %d direction %d", l, d);
-      }
   }
   const gantts_sru_stack_t& s = c->sru;
   GANTTS_CHECK_ARG(s.num_layers >= 0 && s.num_layers <= GANTTS_MAX_SRU_LAYERS, "gan_step: SRU layer count %d not in [0, %d]",
@@ -719,12 +611,6 @@ static int check_step(const gantts_gan_step_t* c) {
     GANTTS_CHECK_ARG(c->g.num_layers == 1 && c->g.dims[0] == nc,
                      "gan_step: with an SRU stack g is hidden2out alone: 1 layer of input width %d (got %d layer(s), input "
                      "width %d)", nc, c->g.num_layers, c->g.dims[0]);
-    for (int l = 0; l < s.num_layers; ++l) {
-      GANTTS_CHECK_ARG(s.W[l] && s.b[l], "gan_step: null SRU weight/bias of layer %d", l);
-      GANTTS_CHECK_ARG(s.sumW[l] && s.sumb[l], "gan_step: null SRU optimiser state of layer %d", l);
-      if (c->optimizer == GANTTS_OPT_ADAM)
-        GANTTS_CHECK_ARG(s.sqW[l] && s.sqb[l], "gan_step: Adam needs exp_avg_sq for SRU layer %d", l);
-    }
   }
   if (c->w_d > 0.f) {
     GANTTS_CHECK_ARG(c->d.num_layers >= 1 && c->d.num_layers <= GANTTS_MAX_LAYERS, "gan_step: bad discriminator");
@@ -752,25 +638,68 @@ static int check_step(const gantts_gan_step_t* c) {
                      S);
     GANTTS_CHECK_ARG(c->g.dims[Lg] == nw * S, "gan_step: highway generator output width %d != %d windows x static_dim %d",
                      c->g.dims[Lg], nw, S);
-    GANTTS_CHECK_ARG(h.W && h.b, "gan_step: null highway gate weight/bias");
-    GANTTS_CHECK_ARG((reinterpret_cast<uintptr_t>(h.b) & 15) == 0, "gan_step: highway gate bias must be 16-byte aligned");
-    GANTTS_CHECK_ARG(h.sumW && h.sumb, "gan_step: null highway gate optimiser state");
-    if (c->optimizer == GANTTS_OPT_ADAM)
-      GANTTS_CHECK_ARG(h.sqW && h.sqb, "gan_step: Adam needs exp_avg_sq for the highway gate");
   }
-  return GANTTS_OK;
+  // the tensor tables, bound from the shapes checked above
+  ParamList pl;
+  gantts_mlp_t g = c->g;
+  g_param_list(c, &g, nullptr, &pl);
+  int rc = check_table(c, c->g_tensors, pl.n, "generator");
+  if (rc) return rc;
+  if (h.static_dim > 0)
+    GANTTS_CHECK_ARG((reinterpret_cast<uintptr_t>(pl.gate[BIAS].p) & 15) == 0,
+                     "gan_step: highway gate bias must be 16-byte aligned");
+  return c->w_d > 0.f ? check_table(c, c->d_tensors, 2 * c->d.num_layers, "discriminator") : GANTTS_OK;
+}
+
+static void layout_lstm(const gantts_gan_step_t* c, int64_t M, Arena& a, LstmWs* w) {
+  const gantts_lstm_stack_t& ls = c->lstm;
+  const int nl = ls.num_layers, H = nl > 0 ? ls.hidden : 0, nd = lstm_ndir(ls), n4 = nd * 4 * H;
+  const bool on = nl > 0;
+  size_t part_ih = 0, part_hh = 0;
+  for (int l = 0; l < nl; ++l) {
+    const int ni = lstm_nin(ls, l);
+    w->in[l] = a.take(2 * plane_bytes(M, ni));
+    w->w[l] = a.take(2 * plane_bytes(n4, ni) + 2 * plane_bytes(ni, n4));
+    w->bias[l] = a.f32((size_t)n4);
+    w->h[l] = a.f32((size_t)M * nd * H);
+    w->gates[l] = a.f32((size_t)M * n4);
+    w->cells[l] = a.f32((size_t)M * nd * H);
+    const size_t pi = mn_partial_bytes(M, 4 * H, ni, nullptr, nullptr), ph = mn_partial_bytes(M, 4 * H, H, nullptr, nullptr);
+    part_ih = pi > part_ih ? pi : part_ih;
+    part_hh = ph > part_hh ? ph : part_hh;
+  }
+  w->xproj = a.f32((size_t)M * n4);
+  w->out = a.f32(on ? (size_t)M * c->g.dims[c->g.num_layers] : 0);
+  w->dh = a.f32((size_t)M * nd * H);
+  w->dg = a.take(on ? 2 * plane_bytes(M, n4) : 0);
+  w->hp = a.take(on ? 2 * plane_bytes(M, H) : 0);
+  for (int d = 0; d < 2; ++d) {
+    w->part[d][0] = reinterpret_cast<float*>(a.take(d < nd ? part_ih : 0));
+    w->part[d][1] = reinterpret_cast<float*>(a.take(d < nd ? part_hh : 0));
+  }
+  w->bar = reinterpret_cast<unsigned int*>(a.take(on ? 256 : 0));
 }
 
 // LSTM layer l's workspace: planes of its GEMM input, and of W_ih of both directions [ndir 4H][n_in] then transposed
 static Planes lstm_in_planes(const gantts_gan_step_t* c, const StepLayout& L, int l, int64_t M) {
-  char* cur = L.lstm_in[l];
+  char* cur = L.lstm.in[l];
   return carve_planes(cur, M, lstm_nin(c->lstm, l));
 }
 static void lstm_w_planes(const gantts_gan_step_t* c, const StepLayout& L, int l, Planes* w, Planes* wt) {
   const int ni = lstm_nin(c->lstm, l), n4 = lstm_ndir(c->lstm) * 4 * c->lstm.hidden;
-  char* cur = L.lstm_w[l];
+  char* cur = L.lstm.w[l];
   *w = carve_planes(cur, n4, ni);
   *wt = carve_planes(cur, ni, n4);
+}
+
+static void layout_highway(const gantts_gan_step_t* c, int64_t M, Arena& a, HighwayWs* w) {
+  const int S = c->highway.static_dim;
+  const bool on = S > 0;
+  w->tx = a.f32(on ? (size_t)M * S : 0);
+  w->gx = a.f32(on ? (size_t)M * S : 0);
+  w->w = a.take(on ? 2 * plane_bytes(S, S) : 0);
+  w->dz = a.take(on ? 2 * plane_bytes(M, S) : 0);
+  w->partial = reinterpret_cast<float*>(a.take(on ? mn_partial_bytes(M, S, S, nullptr, nullptr) : 0));
 }
 
 // x_s: the first S columns of x's operand planes -- the generator MLP's tape input, or the LSTM stack's layer-0 input
@@ -788,54 +717,74 @@ static int gate_input_planes(const gantts_gan_step_t* c, const gantts_mlp_t& g, 
 }
 
 // Tx = sigmoid(x_s W_T^T + b_T)
-static int highway_gate_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, int64_t M,
-                            cudaStream_t st) {
+static int highway_gate_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const ParamList& pg, const StepLayout& L,
+                            int64_t M, cudaStream_t st) {
   const int S = c->highway.static_dim;
   Planes xs;
   int rc = gate_input_planes(c, g, L, M, &xs);
   if (rc) return rc;
-  char* cur = L.hw_w;
+  char* cur = L.hw.w;
   const Planes w = carve_planes(cur, S, S);
-  if ((rc = launch_split(c->highway.W, S, S, S, w, 0, st))) return rc;
+  if ((rc = launch_split(pg.gate[WEIGHT].p, S, S, S, w, 0, st))) return rc;
   EpiArgs e;
   e.epi = EPI_F32;
-  e.C = L.hw_tx;
+  e.C = L.hw.tx;
   e.ldc = S;
-  e.bias = c->highway.b;
+  e.bias = pg.gate[BIAS].p;
   e.act = GANTTS_ACT_SIGMOID;
   return launch_gemm_kk(xs, w, e, st);
 }
 
 // dW_T = dz^T x_s and db_T = colsum(dz) (ones-tile MMA) into the first S * S + S entries of the generator's buffer
-static int highway_gate_bwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, int64_t M,
-                            cudaStream_t st) {
+static int highway_gate_bwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const ParamList& pg, const StepLayout& L,
+                            int64_t M, cudaStream_t st) {
   const int S = c->highway.static_dim;
   Planes xs;
   int rc = gate_input_planes(c, g, L, M, &xs);
   if (rc) return rc;
-  char* cur = L.hw_dz;
+  char* cur = L.hw.dz;
   const Planes dz = carve_planes(cur, M, S);
   ReduceList rl;
-  if ((rc = launch_gemm_mn(dz, xs, L.g_grads, L.g_grads + (int64_t)S * S, 0, L.hw_partial, st, &rl))) return rc;
+  if ((rc = launch_gemm_mn(dz, xs, pg.gate[WEIGHT].g, pg.gate[BIAS].g, 0, L.hw.partial, st, &rl))) return rc;
   return flush_reduce(rl, 0, st);
+}
+
+static void layout_sru(const gantts_gan_step_t* c, int64_t M, Arena& a, SruWs* w) {
+  const gantts_sru_stack_t& s = c->sru;
+  const int nl = s.num_layers, nc = nl > 0 ? sru_ncols(s) : 0;
+  int maxku = 0;
+  for (int l = 0; l < nl; ++l) {
+    const int ni = sru_nin(s, l), ku = nc * sru_k(s, l);
+    maxku = ku > maxku ? ku : maxku;
+    w->in[l] = a.take(2 * plane_bytes(M, ni));
+    w->u[l] = a.f32((size_t)M * ku);
+    w->c[l] = a.f32((size_t)M * nc);
+    if (l < nl - 1) w->h[l] = a.f32((size_t)M * nc);
+    w->w[l] = a.take(2 * plane_bytes(ni, ku) + 2 * plane_bytes(ku, ni));
+    w->partial[l] = reinterpret_cast<float*>(a.take(mn_partial_bytes(M, ni, ku, nullptr, nullptr)));
+  }
+  w->du = a.take(nl > 0 ? 2 * plane_bytes(M, maxku) : 0);
+  w->dx = a.f32((size_t)M * nc);
+  w->dxp = a.f32((size_t)M * nc);
+  w->bpart = a.f32((size_t)c->B * 2 * nc);
 }
 
 // SRU layer l's workspace: planes of its masked input, and of W [n_in][ncols k] then W^T [ncols k][n_in]
 static Planes sru_in_planes(const gantts_gan_step_t* c, const StepLayout& L, int l, int64_t M) {
-  char* cur = L.sru_in[l];
+  char* cur = L.sru.in[l];
   return carve_planes(cur, M, sru_nin(c->sru, l));
 }
 static void sru_w_planes(const gantts_gan_step_t* c, const StepLayout& L, int l, Planes* w, Planes* wt) {
   const int ni = sru_nin(c->sru, l), ku = sru_ncols(c->sru) * sru_k(c->sru, l);
-  char* cur = L.sru_w[l];
+  char* cur = L.sru.w[l];
   *w = carve_planes(cur, ni, ku);
   *wt = carve_planes(cur, ku, ni);
 }
 
 // SRU stack forward (rnn.SRUCell per layer): the last layer's h goes unmasked into hidden2out's tape input planes, so
 // the caller runs hidden2out with mlp_fwd_impl(..., input_ready = true).  train = false: no masks.
-static int sru_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, const float* x, int64_t M,
-                         uint64_t seed, bool train, cudaStream_t st) {
+static int sru_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const ParamList& pg, const StepLayout& L,
+                         const float* x, int64_t M, uint64_t seed, bool train, cudaStream_t st) {
   const gantts_sru_stack_t& s = c->sru;
   const int nl = s.num_layers, nc = sru_ncols(s);
   const float p_h = train ? s.dropout : 0.f, p_x = train ? s.rnn_dropout : 0.f;
@@ -848,7 +797,7 @@ static int sru_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, cons
     for (int l = 0; l < nl; ++l) {
       Planes w, wt;
       sru_w_planes(c, L, l, &w, &wt);
-      wl.W[l] = s.W[l];
+      wl.W[l] = pg.sru[l][WEIGHT].p;
       wl.N[l] = (int)w.rows;
       wl.K[l] = (int)w.cols;
       wl.hi[l] = w.hi;
@@ -880,17 +829,17 @@ static int sru_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, cons
     sru_w_planes(c, L, l, &w, &wt);
     EpiArgs e;
     e.epi = EPI_F32;
-    e.C = L.sru_u[l];
+    e.C = L.sru.u[l];
     e.ldc = (int64_t)nc * k;
     if ((rc = launch_gemm_kk(sru_in_planes(c, L, l, M), wt, e, st))) return rc;
     const Planes out = last ? top : sru_in_planes(c, L, l + 1, M);
     SruStepFwd p{};
-    p.u = L.sru_u[l];
-    p.xh = k == 3 ? (l == 0 ? x : L.sru_h[l - 1]) : nullptr;
+    p.u = L.sru.u[l];
+    p.xh = k == 3 ? (l == 0 ? x : L.sru.h[l - 1]) : nullptr;
     p.xh_rs = l == 0 ? s.in_dim : nc;
-    p.bias = s.b[l];
-    p.c = L.sru_c[l];
-    p.h = L.sru_h[l];
+    p.bias = pg.sru[l][BIAS].p;
+    p.c = L.sru.c[l];
+    p.h = L.sru.h[l];
     p.hi = out.hi;
     p.lo = out.lo;
     p.pitch = out.pitch;
@@ -906,7 +855,7 @@ static int sru_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, cons
   return GANTTS_OK;
 }
 
-// SRU stack backward from dL/dh of the top layer in L.sru_dx (hidden2out's input gradient), top layer first:
+// SRU stack backward from dL/dh of the top layer in L.sru.dx (hidden2out's input gradient), top layer first:
 //   scan backward -> dU planes, highway gradient dx' (k = 3), bias partials -> bias gradient (fixed order over B)
 //   dW = (x * mask_x)^T dU  (MN-major, lands in the [n_in][ncols k] parameter layout)
 //   dX = dU W^T             (K-major on W as stored; not for layer 0)
@@ -920,38 +869,38 @@ static int sru_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const 
   for (int l = nl - 1; l >= 0; --l) {
     const int k = sru_k(s, l);
     const bool top = l == nl - 1;
-    char* cur = L.sru_du;
+    char* cur = L.sru.du;
     const Planes du = carve_planes(cur, M, (int64_t)nc * k);
     SruStepBwd p{};
-    p.u = L.sru_u[l];
-    p.xh = k == 3 ? (l == 0 ? x : L.sru_h[l - 1]) : nullptr;
+    p.u = L.sru.u[l];
+    p.xh = k == 3 ? (l == 0 ? x : L.sru.h[l - 1]) : nullptr;
     p.xh_rs = l == 0 ? s.in_dim : nc;
-    p.bias = s.b[l];
-    p.c = L.sru_c[l];
-    p.dx = L.sru_dx;
-    p.dxp_in = top ? nullptr : L.sru_dxp;
+    p.bias = pg.sru[l][BIAS].p;
+    p.c = L.sru.c[l];
+    p.dx = L.sru.dx;
+    p.dxp_in = top ? nullptr : L.sru.dxp;
     p.mxu = sru_mask(gantts_sru_mask_seed(seed, l + 1, 0), top ? 0.f : s.rnn_dropout);
     p.mh = sru_mask(gantts_sru_mask_seed(seed, l, 1), top ? 0.f : s.dropout);
     p.du_hi = du.hi;
     p.du_lo = du.lo;
     p.du_pitch = du.pitch;
-    p.dxp_out = (k == 3 && l > 0) ? L.sru_dxp : nullptr;
-    p.dbias_part = L.sru_bpart;
+    p.dxp_out = (k == 3 && l > 0) ? L.sru.dxp : nullptr;
+    p.dbias_part = L.sru.bpart;
     p.B = c->B;
     p.T = c->T;
     p.d = s.hidden;
     p.bidir = s.bidirectional;
     p.act = s.act;
     if ((rc = launch_sru_step_bwd(p, k, st))) return rc;
-    GANTTS_PDL_LAUNCH((sru_bias_reduce_kernel), (2 * nc + 255) / 256, 256, 0, st, L.sru_bpart, c->B, 2 * nc, pg.sgb[l]);
+    GANTTS_PDL_LAUNCH((sru_bias_reduce_kernel), (2 * nc + 255) / 256, 256, 0, st, L.sru.bpart, c->B, 2 * nc, pg.sru[l][BIAS].g);
     GANTTS_LAUNCH_CHECK("sru_bias_reduce_kernel");
-    if ((rc = launch_gemm_mn(sru_in_planes(c, L, l, M), du, pg.sgW[l], nullptr, 0, L.sru_partial[l], st, &rl))) return rc;
+    if ((rc = launch_gemm_mn(sru_in_planes(c, L, l, M), du, pg.sru[l][WEIGHT].g, nullptr, 0, L.sru.partial[l], st, &rl))) return rc;
     if (l > 0) {
       Planes w, wt;
       sru_w_planes(c, L, l, &w, &wt);
       EpiArgs e;
       e.epi = EPI_F32;
-      e.C = L.sru_dx;
+      e.C = L.sru.dx;
       e.ldc = nc;
       if ((rc = launch_gemm_kk(du, w, e, st))) return rc;
     }
@@ -959,18 +908,19 @@ static int sru_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const 
   return flush_reduce(rl, 0, st);
 }
 
-static LstmParams lstm_layer_params(const gantts_gan_step_t* c, const StepLayout& L, int l, const int64_t* lengths) {
+static LstmParams lstm_layer_params(const gantts_gan_step_t* c, const ParamList& pg, const StepLayout& L, int l,
+                                    const int64_t* lengths) {
   const gantts_lstm_stack_t& s = c->lstm;
   LstmParams p{};
-  p.W_hh = s.W_hh[l][0];
+  p.W_hh = pg.lstm[l][0][W_HH].p;
   if (s.bidirectional)      // the two directions' tensors are 4-byte aligned: their distance is a whole number of floats
-    p.W_hh_dir = ((int64_t)reinterpret_cast<uintptr_t>(s.W_hh[l][1]) - (int64_t)reinterpret_cast<uintptr_t>(s.W_hh[l][0])) /
+    p.W_hh_dir = ((int64_t)reinterpret_cast<uintptr_t>(pg.lstm[l][1][W_HH].p) - (int64_t)reinterpret_cast<uintptr_t>(pg.lstm[l][0][W_HH].p)) /
                  (int64_t)sizeof(float);
   p.lengths = lengths;
-  p.h_out = L.lstm_h[l];
-  p.gates = L.lstm_gates[l];
-  p.cells = L.lstm_cells[l];
-  p.bar = L.lstm_bar;
+  p.h_out = L.lstm.h[l];
+  p.gates = L.lstm.gates[l];
+  p.cells = L.lstm.cells[l];
+  p.bar = L.lstm.bar;
   p.B = c->B;
   p.T = c->T;
   p.H = s.hidden;
@@ -982,8 +932,8 @@ static LstmParams lstm_layer_params(const gantts_gan_step_t* c, const StepLayout
 // both directions, the cooperative recurrence, and one kernel that writes the next GEMM's operand planes of h * mask --
 // on the top layer the unmasked h into hidden2out's tape input planes, so the caller runs hidden2out with
 // mlp_fwd_impl(..., input_ready = true).  train = false: no masks.
-static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, const float* x,
-                          const int64_t* lengths, int64_t M, uint64_t seed, bool train, cudaStream_t st) {
+static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const ParamList& pg, const StepLayout& L,
+                          const float* x, const int64_t* lengths, int64_t M, uint64_t seed, bool train, cudaStream_t st) {
   const gantts_lstm_stack_t& s = c->lstm;
   const int nl = s.num_layers, H = s.hidden, nd = lstm_ndir(s), G4 = 4 * H, nh = nd * H;
   const float p_drop = train ? s.dropout : 0.f;
@@ -1001,7 +951,7 @@ static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, con
       lstm_w_planes(c, L, l, &w, &wt);
       for (int d = 0; d < nd; ++d) {
         const int i = l * nd + d;
-        wl.W[i] = s.W_ih[l][d];
+        wl.W[i] = pg.lstm[l][d][W_IH].p;
         wl.N[i] = G4;
         wl.K[i] = lstm_nin(s, l);
         wl.hi[i] = w.hi + (int64_t)d * G4 * w.pitch;
@@ -1011,9 +961,9 @@ static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, con
         wl.tlo[i] = wt.lo + (int64_t)d * G4;
         wl.tpitch[i] = wt.pitch;
         wl.off[i + 1] = wl.off[i] + (int64_t)((G4 + 31) / 32) * ((wl.K[i] + 31) / 32);
-        bl.a[i] = s.b_ih[l][d];
-        bl.b[i] = s.b_hh[l][d];
-        bl.out[i] = L.lstm_bias[l] + (int64_t)d * G4;
+        bl.a[i] = pg.lstm[l][d][B_IH].p;
+        bl.b[i] = pg.lstm[l][d][B_HH].p;
+        bl.out[i] = L.lstm.bias[l] + (int64_t)d * G4;
       }
     }
     const int nb = (int)(wl.off[wl.n] < num_sms() * 8 ? wl.off[wl.n] : num_sms() * 8);
@@ -1031,16 +981,16 @@ static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, con
     lstm_w_planes(c, L, l, &w, &wt);
     EpiArgs e;
     e.epi = EPI_F32;
-    e.C = L.lstm_xproj;
+    e.C = L.lstm.xproj;
     e.ldc = (int64_t)nd * G4;
-    e.bias = L.lstm_bias[l];
+    e.bias = L.lstm.bias[l];
     if ((rc = launch_gemm_kk(lstm_in_planes(c, L, l, M), w, e, st))) return rc;
-    LstmParams p = lstm_layer_params(c, L, l, lengths);
-    p.xproj = L.lstm_xproj;
+    LstmParams p = lstm_layer_params(c, pg, L, l, lengths);
+    p.xproj = L.lstm.xproj;
     if ((rc = lstm_run(false, p, st))) return rc;
     const Planes out = last ? top : lstm_in_planes(c, L, l + 1, M);
     const float pl = last ? 0.f : p_drop;             // nn.LSTM: no dropout on the last layer's output
-    GANTTS_PDL_LAUNCH((lstm_planes_kernel), blocks_1d(M * nh, 1024), 256, 0, st, L.lstm_h[l], M, nh,
+    GANTTS_PDL_LAUNCH((lstm_planes_kernel), blocks_1d(M * nh, 1024), 256, 0, st, L.lstm.h[l], M, nh,
                       gantts_lstm_mask_seed(seed, l), pl > 0.f ? (uint32_t)(pl * 65536.f + 0.5f) : 0u,
                       pl > 0.f ? 1.f / (1.f - pl) : 1.f, out.hi, out.lo, out.pitch);
     GANTTS_LAUNCH_CHECK("lstm_planes_kernel");
@@ -1048,7 +998,7 @@ static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, con
   return GANTTS_OK;
 }
 
-// LSTM stack backward from dL/dh of the top layer in L.lstm_dh (hidden2out's input gradient), top layer first:
+// LSTM stack backward from dL/dh of the top layer in L.lstm.dh (hidden2out's input gradient), top layer first:
 //   recurrence backward -> dgates (fp32, in the xproj buffer) -> dgates planes
 //   per direction: dW_ih and db_ih = dgates_d^T in (MN-major, ones-tile bias), dW_hh = dgates_d^T hprev_d (MN-major)
 //   dX = dgates W_ih, times the mask of the layer below in the GEMM epilogue (not for layer 0)
@@ -1059,35 +1009,35 @@ static int lstm_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const
   const gantts_lstm_stack_t& s = c->lstm;
   const int nl = s.num_layers, H = s.hidden, nd = lstm_ndir(s), G4 = 4 * H, nh = nd * H;
   int rc;
-  char* cur = L.lstm_dg;
+  char* cur = L.lstm.dg;
   const Planes dg = carve_planes(cur, M, (int64_t)nd * G4);
-  cur = L.lstm_hp;
+  cur = L.lstm.hp;
   const Planes hp = carve_planes(cur, M, H);
   ReduceList rl;
   for (int l = nl - 1; l >= 0; --l) {
-    LstmParams p = lstm_layer_params(c, L, l, lengths);
-    p.dh_out = L.lstm_dh;
-    p.dxproj = L.lstm_xproj;
+    LstmParams p = lstm_layer_params(c, pg, L, l, lengths);
+    p.dh_out = L.lstm.dh;
+    p.dxproj = L.lstm.xproj;
     if ((rc = lstm_run(true, p, st))) return rc;
-    if ((rc = launch_split(L.lstm_xproj, (int64_t)nd * G4, M, nd * G4, dg, 0, st))) return rc;
+    if ((rc = launch_split(L.lstm.xproj, (int64_t)nd * G4, M, nd * G4, dg, 0, st))) return rc;
     const Planes in = lstm_in_planes(c, L, l, M);
     for (int d = 0; d < nd; ++d) {
       Planes dgd = dg;
       dgd.hi += (int64_t)d * G4;
       dgd.lo += (int64_t)d * G4;
       dgd.cols = G4;
-      if ((rc = launch_gemm_mn(dgd, in, pg.lgW_ih[l][d], pg.lgb_ih[l][d], 0, L.lstm_part[d][0], st, &rl))) return rc;
-      GANTTS_PDL_LAUNCH((lstm_hprev_planes_kernel), blocks_1d(M * H, 1024), 256, 0, st, L.lstm_h[l], lengths, c->B, c->T, H, nd,
+      if ((rc = launch_gemm_mn(dgd, in, pg.lstm[l][d][W_IH].g, pg.lstm[l][d][B_IH].g, 0, L.lstm.part[d][0], st, &rl))) return rc;
+      GANTTS_PDL_LAUNCH((lstm_hprev_planes_kernel), blocks_1d(M * H, 1024), 256, 0, st, L.lstm.h[l], lengths, c->B, c->T, H, nd,
                         d, hp.hi, hp.lo, hp.pitch);
       GANTTS_LAUNCH_CHECK("lstm_hprev_planes_kernel");
-      if ((rc = launch_gemm_mn(dgd, hp, pg.lgW_hh[l][d], nullptr, 0, L.lstm_part[d][1], st, &rl))) return rc;
+      if ((rc = launch_gemm_mn(dgd, hp, pg.lstm[l][d][W_HH].g, nullptr, 0, L.lstm.part[d][1], st, &rl))) return rc;
     }
     if (l > 0) {
       Planes w, wt;
       lstm_w_planes(c, L, l, &w, &wt);
       EpiArgs e;
       e.epi = EPI_F32;
-      e.C = L.lstm_dh;
+      e.C = L.lstm.dh;
       e.ldc = nh;
       if (s.dropout > 0.f) {      // dh_{l-1} = mask_{l-1} * dX: LeakyReLU with slope 1 is the identity, then the mask
         e.act = GANTTS_ACT_LEAKY_DROPOUT;
@@ -1099,26 +1049,216 @@ static int lstm_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const
     }
     if ((rc = flush_reduce(rl, 0, st))) return rc;
     for (int d = 0; d < nd; ++d)
-      GANTTS_CUDA(cudaMemcpyAsync(pg.lgb_hh[l][d], pg.lgb_ih[l][d], (size_t)G4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      GANTTS_CUDA(cudaMemcpyAsync(pg.lstm[l][d][B_HH].g, pg.lstm[l][d][B_IH].g, (size_t)G4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
   }
   return GANTTS_OK;
 }
 
-// Generator forward: the MLP from x into y_hat; or the SRU stack and then hidden2out on the planes it left in the tape,
-// into y_hat; or the LSTM stack and then hidden2out into L.lstm_out, with y_hat a copy of x (models.py:118).
-static int generator_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, const float* x, int x_rs,
-                         const int64_t* lengths, int64_t M, float* y_hat, int d_out, uint64_t seed, bool train,
-                         cudaStream_t st) {
+static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
+  const int64_t M = (int64_t)c->B * c->T;
+  const int dD = c->d.dims[0];
+  *L = StepLayout{};      // the buffers of absent layers stay null
+  Arena a{base};
+  L->scal = a.f32(S_COUNT);
+  L->mask = a.f32((size_t)M);
+  L->d_in = a.f32((size_t)2 * M * dD);
+  L->d_out = a.f32((size_t)2 * M);
+  L->g_dout = a.f32((size_t)2 * M);
+  L->g_din = a.f32((size_t)2 * M * dD);
+  L->g_static = a.f32((size_t)M * c->n_static);
+  L->g_yhat = a.f32((size_t)M * c->g.dims[c->g.num_layers]);
+  L->g_grads = a.f32(g_param_count(c));
+  L->d_grads = a.f32(mlp_param_count(c->d));
+  L->g_tape_bytes = gantts_mlp_tape_bytes(&c->g, M);
+  L->g_tape = a.take(L->g_tape_bytes);
+  L->d_tape_bytes = gantts_mlp_tape_bytes(&c->d, 2 * M);
+  L->d_tape = a.take(L->d_tape_bytes);
+  const size_t gb = gantts_mlp_workspace_bytes(&c->g, M), db = gantts_mlp_workspace_bytes(&c->d, 2 * M);
+  L->mlp_ws_bytes = gb > db ? gb : db;
+  L->mlp_ws = a.take(L->mlp_ws_bytes);
+  L->red = reinterpret_cast<RedWs*>(a.take(R_COUNT * sizeof(RedWs)));
+  L->opt_partial = a.f32(OPT_MAX_BLOCKS);
+  layout_highway(c, M, a, &L->hw);
+  layout_sru(c, M, a, &L->sru);
+  layout_lstm(c, M, a, &L->lstm);
+  L->total = (size_t)(a.cur - base) + 256;
+}
+
+// Everything one gantts_gan_step call works with: the config, its workspace, the bound tables and the batch.
+struct Step {
+  const gantts_gan_step_t* c;
+  StepLayout L;
+  gantts_mlp_t g, d;      // local copies: parameters from the tables, per-forward dropout and seed
+  ParamList pg, pd;
+  const float *x, *y;
+  const int64_t* lengths;
+  float *y_hat, *y_hat_static;
+  int64_t M;
+  int d_in, d_out, dD, nS;  // d_in: the width (and row stride) of x -- the SRU or LSTM stack's input width when there is one
+  int cond_w, nA;           // conditioning columns of D's input (copies of x), adversarial columns
+  bool has_d, has_adv;
+  bool adv_window;          // the adversarial columns are one contiguous window of y_hat_static
+  HighwayArgs hwa;
+  ColList static_cols, adv_cols, real_cols;
+  uint64_t seed;
+  void* stream;
+  cudaStream_t st;
+  const HighwayArgs* hw() const { return c->highway.static_dim > 0 ? &hwa : nullptr; }
+};
+
+// batch prologue (train.py:528-535): sequence mask and loss scales
+static int step_prologue(const Step& s, float inv_frames, bool eval) {
+  const gantts_gan_step_t* c = s.c;
+  int rc = gantts_sequence_mask(s.lengths, s.L.mask, c->B, c->T, s.stream);
+  if (rc) return rc;
+  GANTTS_PDL_LAUNCH((set_scales_kernel), 1, 32, 0, s.st, s.L.scal, inv_frames, s.has_adv ? c->adv_w : 0.f, c->mge_w, c->mse_w,
+                    eval ? 1 : 0, s.lengths, c->B, c->T);
+  GANTTS_LAUNCH_CHECK("set_scales_kernel");
+  return GANTTS_OK;
+}
+
+// the loss scalars from every deferred partial the step wrote
+static int step_finalize(const Step& s, float* losses_dev) {
+  const gantts_gan_step_t* c = s.c;
+  RedCounts cnt{};
+  if (s.has_d) cnt.n[R_REAL] = cnt.n[R_FAKE] = bce_blocks(s.M);
+  if (s.has_adv) cnt.n[R_ADV] = bce_blocks(s.M);
+  cnt.n[R_MGE] = sse_blocks(s.M, s.nS);
+  cnt.n[R_MSE] = sse_blocks(s.M, s.d_out);
+  GANTTS_PDL_LAUNCH((finalize_losses_kernel), 1, RED_THREADS, 0, s.st, s.L.scal, losses_dev, s.L.red, cnt,
+                    s.has_adv ? c->adv_w : 0.f, c->mge_w, c->mse_w, s.has_d ? 1 : 0);
+  GANTTS_LAUNCH_CHECK("finalize_losses_kernel");
+  return GANTTS_OK;
+}
+
+// Generator forward (apply_generator, train.py:336-355) into y_hat and y_hat_static: the MLP from x; or the SRU stack and
+// then hidden2out on the planes it left in the tape; or the LSTM stack and then hidden2out into L.lstm.out, with y_hat a
+// copy of x (models.py:118).  Then the highway gate, and the MLPG (with the highway combine) on the generator's output.
+// train = false: no SRU / LSTM masks (the caller sets g.dropout_p).
+static int generator_fwd(Step& s, bool train) {
+  const gantts_gan_step_t* c = s.c;
+  const StepLayout& L = s.L;
+  const int64_t M = s.M;
+  const float* gen_out = s.y_hat;
   int rc;
   if (c->lstm.num_layers > 0) {
-    if ((rc = lstm_stack_fwd(c, g, L, x, lengths, M, seed, train, st))) return rc;
-    if ((rc = mlp_fwd_impl(&g, nullptr, 0, M, L.lstm_out, d_out, L.g_tape, L.g_tape_bytes, st, true))) return rc;
-    GANTTS_CUDA(cudaMemcpyAsync(y_hat, x, (size_t)M * x_rs * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    return GANTTS_OK;
+    if ((rc = lstm_stack_fwd(c, s.g, s.pg, L, s.x, s.lengths, M, s.seed, train, s.st))) return rc;
+    if ((rc = mlp_fwd_impl(&s.g, nullptr, 0, M, L.lstm.out, s.d_out, L.g_tape, L.g_tape_bytes, s.st, true))) return rc;
+    GANTTS_CUDA(cudaMemcpyAsync(s.y_hat, s.x, (size_t)M * s.d_in * sizeof(float), cudaMemcpyDeviceToDevice, s.st));
+    gen_out = L.lstm.out;
+  } else if (c->sru.num_layers > 0) {
+    if ((rc = sru_stack_fwd(c, s.g, s.pg, L, s.x, M, s.seed, train, s.st))) return rc;
+    if ((rc = mlp_fwd_impl(&s.g, nullptr, 0, M, s.y_hat, s.d_out, L.g_tape, L.g_tape_bytes, s.st, true))) return rc;
+  } else if ((rc = gantts_mlp_fwd(&s.g, s.x, s.d_in, M, s.y_hat, s.d_out, L.g_tape, L.g_tape_bytes, s.st))) {
+    return rc;
   }
-  if (c->sru.num_layers == 0) return gantts_mlp_fwd(&g, x, x_rs, M, y_hat, d_out, L.g_tape, L.g_tape_bytes, st);
-  if ((rc = sru_stack_fwd(c, g, L, x, M, seed, train, st))) return rc;
-  return mlp_fwd_impl(&g, nullptr, 0, M, y_hat, d_out, L.g_tape, L.g_tape_bytes, st, true);
+  if (c->highway.static_dim > 0 && (rc = highway_gate_fwd(c, s.g, s.pg, L, M, s.st))) return rc;
+  return mlpg_fwd_impl(gen_out, (int64_t)c->T * s.d_out, s.d_out, s.y_hat_static, (int64_t)c->T * s.nS, s.nS, c->mlpg_table,
+                       &c->streams, &c->windows, c->B, c->T, s.stream, s.hw());
+}
+
+// Generator backward (loss_g.backward(), train.py:294-318) on dL/dy_hat_static summed in g_static, in order:
+//   the MSE term (train.py:294), whose pass stores its gradient into g_yhat when it sends one (not when y_hat = x);
+//   the MLPG adjoint: with no MSE gradient (mse_w == 0, the CLI default, train.py:15) nothing else adds to dL/dy_hat, so
+//     it writes the operand planes of the head's backward GEMMs directly; otherwise it accumulates onto g_yhat in fp32
+//     (highway: it solves with Tx * g_static and leaves dz for the gate's weight gradient);
+//   the gate's backward; the head (g) backward, whose input gradient is dL/dh of the SRU / LSTM stack's top layer;
+//   the stack's backward.
+static int generator_bwd(Step& s) {
+  const gantts_gan_step_t* c = s.c;
+  const StepLayout& L = s.L;
+  const int64_t M = s.M;
+  const int d_out = s.d_out, nS = s.nS;
+  const bool sru = c->sru.num_layers > 0, lstm = c->lstm.num_layers > 0;
+  const bool mse_grad = c->mse_w != 0.f && !lstm;
+  int rc;
+  if ((rc = launch_sse(s.y_hat, d_out, s.y, d_out, L.mask, M, d_out, L.scal + S_MSE_SCALE, mse_grad ? L.g_yhat : nullptr,
+                       d_out, &L.red[R_MSE], s.st)))
+    return rc;
+  bool direct = false;
+  if (!mse_grad) {
+    Planes gp;
+    if ((rc = mlp_bwd_gy_planes(&s.g, M, L.mlp_ws, L.mlp_ws_bytes, &gp))) return rc;
+    rc = mlpg_bwd_planes(L.g_static, (int64_t)c->T * nS, nS, gp.hi, gp.lo, gp.pitch, c->mlpg_table, &c->streams,
+                         &c->windows, c->B, c->T, s.stream, s.hw());
+    if (rc == GANTTS_OK) direct = true;
+    else if (rc != GANTTS_E_UNSUPPORTED) return rc;
+  }
+  if (!direct &&
+      (rc = mlpg_bwd_impl(L.g_static, (int64_t)c->T * nS, nS, L.g_yhat, (int64_t)c->T * d_out, d_out, c->mlpg_table,
+                          &c->streams, &c->windows, c->B, c->T, mse_grad ? 1 : 0, s.stream, s.hw())))
+    return rc;
+  if (c->highway.static_dim > 0 && (rc = highway_gate_bwd(c, s.g, s.pg, L, M, s.st))) return rc;
+  float* gx = sru ? L.sru.dx : (lstm ? L.lstm.dh : nullptr);
+  const int gx_rs = sru ? sru_ncols(c->sru) : (lstm ? lstm_ndir(c->lstm) * c->lstm.hidden : 0);
+  if ((rc = mlp_bwd_impl(&s.g, direct ? nullptr : L.g_yhat, d_out, nullptr, 0, M, L.g_tape, L.g_tape_bytes, gx, gx_rs, 0,
+                         s.pg.gW, s.pg.gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, -1, direct)))
+    return rc;
+  if (sru) return sru_stack_bwd(c, L, s.pg, s.x, M, s.seed, s.st);
+  if (lstm) return lstm_stack_bwd(c, L, s.pg, s.lengths, M, s.seed, s.st);
+  return GANTTS_OK;
+}
+
+// Discriminator forward into L.d_out.  stacked: the [real | fake] batch of 2M rows (train.py:261,265), real = the
+// adversarial columns of y's static features (real_cols), fake = those of y_hat_static; otherwise the fake rows alone
+// (the adversarial forward, train.py:307).  Unconditioned, the columns go straight into the operand planes of D's tape;
+// conditioned (train.py:254-256), D's input cat((x, columns), -1) is assembled in fp32 d_in, and the adversarial forward
+// re-uses the fake half the stacked one assembled.
+static int discriminator_fwd(Step& s, bool stacked) {
+  const StepLayout& L = s.L;
+  const int64_t M = s.M, rows = stacked ? 2 * M : M;
+  int rc;
+  if (!s.cond_w) {
+    Planes din;
+    if ((rc = mlp_tape_input_planes(&s.d, rows, L.d_tape, L.d_tape_bytes, &din))) return rc;
+    if (stacked) {
+      GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(2 * M * s.nA, 1024), 256, 0, s.st, s.y, s.d_out, s.real_cols, M,
+                        s.y_hat_static, s.nS, s.adv_cols, M, din.hi, din.lo, din.pitch);
+      GANTTS_LAUNCH_CHECK("gather_planes_kernel(real|fake)");
+    } else {
+      ColList none;
+      none.n = 0;
+      GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(M * s.nA, 1024), 256, 0, s.st, s.y_hat_static, s.nS, s.adv_cols, M,
+                        nullptr, 0, none, 0, din.hi, din.lo, din.pitch);
+      GANTTS_LAUNCH_CHECK("gather_planes_kernel(adv)");
+    }
+    return mlp_fwd_impl(&s.d, nullptr, 0, rows, L.d_out, 1, L.d_tape, L.d_tape_bytes, s.stream, true);
+  }
+  const int dD = s.dD;
+  if (stacked) {
+    gather_cols_list_kernel<<<blocks_1d(M * s.nA, 1024), 256, 0, s.st>>>(s.y, s.d_out, L.d_in + s.cond_w, dD, s.real_cols, M);
+    GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(real)");
+    gather_cols_list_kernel<<<blocks_1d(M * s.nA, 1024), 256, 0, s.st>>>(s.y_hat_static, s.nS, L.d_in + M * dD + s.cond_w,
+                                                                          dD, s.adv_cols, M);
+    GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(fake)");
+    for (int64_t half = 0; half < 2; ++half)
+      GANTTS_CUDA(cudaMemcpy2DAsync(L.d_in + half * M * dD, (size_t)dD * sizeof(float), s.x, (size_t)s.d_in * sizeof(float),
+                                    (size_t)s.cond_w * sizeof(float), (size_t)M, cudaMemcpyDeviceToDevice, s.st));
+  }
+  return gantts_mlp_fwd(&s.d, L.d_in + (stacked ? 0 : M * dD), dD, rows, L.d_out, 1, L.d_tape, L.d_tape_bytes, s.stream);
+}
+
+// Discriminator backward from dL/dD in g_dout, adding the gradient w.r.t. the fake rows' adversarial columns into
+// g_static.  stacked: loss_d.backward() on the [real | fake] batch, with D's parameter gradients; otherwise the
+// adversarial batch, input gradient only.  When the adversarial columns form one window of y_hat_static the last GEMM
+// adds its result straight into g_static (the scatter of the column gather's backward); otherwise it goes to g_din and a
+// scatter kernel follows.
+static int discriminator_bwd(Step& s, bool stacked) {
+  const StepLayout& L = s.L;
+  const int64_t M = s.M, skip = stacked ? M : 0;      // the real rows' input gradient is not needed
+  float* const* gW = stacked ? s.pd.gW : nullptr;
+  float* const* gb = stacked ? s.pd.gb : nullptr;
+  // in place: row r of the batch -> g_static[r - skip]
+  float* gx = s.adv_window ? L.g_static + s.adv_cols.c[0] - skip * (int64_t)s.nS : L.g_din;
+  int rc;
+  if ((rc = mlp_bwd_impl(&s.d, L.g_dout, 1, L.d_out, 1, skip + M, L.d_tape, L.d_tape_bytes, gx, s.adv_window ? s.nS : s.dD,
+                         skip, gW, gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, s.adv_window ? 1 : -1)))
+    return rc;
+  if (s.adv_window) return GANTTS_OK;
+  scatter_cols_list_add_kernel<<<blocks_1d(M * s.nA, 1024), 256, 0, s.st>>>(L.g_din + skip * s.dD + s.cond_w, s.dD,
+                                                                             L.g_static, s.nS, s.adv_cols, M);
+  GANTTS_LAUNCH_CHECK("scatter_cols_list_add_kernel");
+  return GANTTS_OK;
 }
 
 }  // namespace gantts
@@ -1167,265 +1307,123 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
     set_error("gan_step: workspace too small (%zu < %zu)", workspace_bytes, need);
     return GANTTS_E_WORKSPACE;
   }
-  cudaStream_t st = as_stream(stream);
-  StepLayout L;
-  layout(c, reinterpret_cast<char*>(al256(reinterpret_cast<uintptr_t>(workspace))), &L);
-  const int64_t M = (int64_t)c->B * c->T;
-  // d_in: the width (and row stride) of x -- the SRU stack's input width when there is one
-  const int Lg = c->g.num_layers, d_in = gen_in_width(c), d_out = c->g.dims[Lg];
-  const int dD = c->d.dims[0], nS = c->n_static;
-  const bool has_d = c->w_d > 0.f;
-  const bool has_adv = has_d && c->adv_w > 0.f;
-  // discriminator_linguistic_condition (train.py:254-256,302-303): D sees cat((x, y_adv), -1); the first
-  // cond_w columns of both halves of d_in are copies of x, the gradient w.r.t. them is discarded.
-  const int cond_w = (has_d && c->d_conditioned) ? d_in : 0;
-  const int nA = dD - cond_w;
-  ParamList pg, pd;
-  g_param_list(c, L.g_grads, &pg);
-  pd.n = 0;
-  pd.total = 0;
-  if (has_d) param_list(c->d, c->d_sumW, c->d_sumb, c->d_sqW, c->d_sqb, L.d_grads, &pd);
+  Step s;
+  s.c = c;
+  s.stream = stream;
+  s.st = as_stream(stream);
+  layout(c, reinterpret_cast<char*>(al256(reinterpret_cast<uintptr_t>(workspace))), &s.L);
+  const StepLayout& L = s.L;
+  const int64_t M = s.M = (int64_t)c->B * c->T;
+  s.x = x;
+  s.y = y;
+  s.lengths = lengths_dev;
+  s.y_hat = y_hat;
+  s.y_hat_static = y_hat_static;
+  s.seed = seed;
+  s.d_in = gen_in_width(c);
+  s.d_out = c->g.dims[c->g.num_layers];
+  s.dD = c->d.dims[0];
+  const int nS = s.nS = c->n_static;
+  s.has_d = c->w_d > 0.f;
+  s.has_adv = s.has_d && c->adv_w > 0.f;
+  // discriminator_linguistic_condition (train.py:254-256,302-303): D sees cat((x, y_adv), -1); the first cond_w columns
+  // of both halves of d_in are copies of x, the gradient w.r.t. them is discarded.
+  s.cond_w = (s.has_d && c->d_conditioned) ? s.d_in : 0;
+  s.nA = s.dD - s.cond_w;
+  s.g = c->g;
+  s.d = c->d;
+  g_param_list(c, &s.g, L.g_grads, &s.pg);
+  s.pd.n = 0;
+  s.pd.total = 0;
+  if (s.has_d) d_param_list(c, &s.d, L.d_grads, &s.pd);
   // In2OutHighwayNet: gate + combine around the MLPG (x_s = the first S columns of x)
-  const bool hw = c->highway.static_dim > 0;
-  HighwayArgs hwa{};
-  if (hw) {
-    char* cur = L.hw_dz;
+  s.hwa = HighwayArgs{};
+  if (c->highway.static_dim > 0) {
+    char* cur = L.hw.dz;
     const Planes dz = carve_planes(cur, M, nS);
-    hwa.x = x;
-    hwa.x_rs = d_in;
-    hwa.tx = L.hw_tx;
-    hwa.gx = L.hw_gx;
-    hwa.dz_hi = dz.hi;
-    hwa.dz_lo = dz.lo;
-    hwa.dz_pitch = dz.pitch;
-    hwa.S = nS;
+    s.hwa = HighwayArgs{x, s.d_in, L.hw.tx, L.hw.gx, dz.hi, dz.lo, dz.pitch, nS};
   }
-  const HighwayArgs* hwp = hw ? &hwa : nullptr;
-  ColList static_cols, adv_cols;
-  static_cols.n = c->n_static_cols;
-  for (int i = 0; i < c->n_static_cols; ++i) static_cols.c[i] = c->static_cols[i];
-  adv_cols.n = has_d ? c->n_adv : 0;
-  for (int i = 0; i < adv_cols.n; ++i) adv_cols.c[i] = c->adv_cols[i];
+  s.static_cols.n = c->n_static_cols;
+  for (int i = 0; i < c->n_static_cols; ++i) s.static_cols.c[i] = c->static_cols[i];
+  s.adv_cols.n = s.has_d ? c->n_adv : 0;
+  for (int i = 0; i < s.adv_cols.n; ++i) s.adv_cols.c[i] = c->adv_cols[i];
   // the adversarial columns are one contiguous window of y_hat_static (mgc with the first coefficients masked, the
   // hparams case): the discriminator's input gradient can be accumulated in place
-  bool adv_window = has_d && !cond_w && adv_cols.n >= 1;
-  for (int i = 1; i < adv_cols.n; ++i) adv_window = adv_window && adv_cols.c[i] == adv_cols.c[0] + i;
-  ColList real_cols;          // adversarial columns taken from y directly: static_cols o adv_cols
-  real_cols.n = adv_cols.n;
-  for (int i = 0; i < adv_cols.n; ++i) {
-    GANTTS_CHECK_ARG(adv_cols.c[i] >= 0 && adv_cols.c[i] < c->n_static_cols, "gan_step: adversarial column out of range");
-    real_cols.c[i] = static_cols.c[adv_cols.c[i]];
+  s.adv_window = s.has_d && !s.cond_w && s.adv_cols.n >= 1;
+  for (int i = 1; i < s.adv_cols.n; ++i) s.adv_window = s.adv_window && s.adv_cols.c[i] == s.adv_cols.c[0] + i;
+  s.real_cols.n = s.adv_cols.n;          // adversarial columns taken from y directly: static_cols o adv_cols
+  for (int i = 0; i < s.adv_cols.n; ++i) {
+    GANTTS_CHECK_ARG(s.adv_cols.c[i] >= 0 && s.adv_cols.c[i] < c->n_static_cols, "gan_step: adversarial column out of range");
+    s.real_cols.c[i] = s.static_cols.c[s.adv_cols.c[i]];
   }
-  gantts_mlp_t g = c->g, d = c->d;
-  g.seed = gantts_gan_step_seed(seed, 0);
-  // In2OutRNNHighwayNet: hidden2out's output feeds the MLPG, y_hat is x, and loss_mse sends no gradient into G
-  const bool lstm = c->lstm.num_layers > 0;
-  const float* gen_out = lstm ? L.lstm_out : y_hat;
-  const bool mse_grad = c->mse_w != 0.f && !lstm;
+  s.g.seed = gantts_gan_step_seed(seed, 0);
+  const cudaStream_t st = s.st;
 
-  RedCounts cnt{};
   if (phases & GANTTS_STEP_EVAL) {
     NvtxRange r_eval("gantts_gan_step/eval");
     // ---- "test" phase of train.py:481-486 (model.eval(), phase != "train" at :273,:315): forwards and losses only
     GANTTS_CHECK_ARG(phases == GANTTS_STEP_EVAL, "gan_step: GANTTS_STEP_EVAL cannot be combined with training phases");
-    g.dropout_p = 0.f;
-    d.dropout_p = 0.f;
-    if ((rc = gantts_sequence_mask(lengths_dev, L.mask, c->B, c->T, stream))) return rc;
-    GANTTS_PDL_LAUNCH((set_scales_kernel), 1, 32, 0, st, L.scal, inv_frames, has_adv ? c->adv_w : 0.f, c->mge_w, c->mse_w, 1, lengths_dev, c->B, c->T);
-    GANTTS_LAUNCH_CHECK("set_scales_kernel");
-    if (has_d) {      // (the eval path keeps the two-step gather of the discriminator input)
-      gather_cols_list_kernel<<<blocks_1d(M * nS, 1024), 256, 0, st>>>(y, d_out, L.y_static, nS, static_cols, M);
-      GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(y_static)");
-    }
-    if ((rc = generator_fwd(c, g, L, x, d_in, lengths_dev, M, y_hat, d_out, seed, false, st))) return rc;
-    if (hw && (rc = highway_gate_fwd(c, g, L, M, st))) return rc;
-    if ((rc = mlpg_fwd_impl(gen_out, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
-                            c->mlpg_table, &c->streams, &c->windows, c->B, c->T, stream, hwp)))
-      return rc;
-    if (has_d) {
-      gather_cols_list_kernel<<<blocks_1d(M * nA, 1024), 256, 0, st>>>(L.y_static, nS, L.d_in + cond_w, dD, adv_cols,
-                                                                       M);
-      GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(real)");
-      gather_cols_list_kernel<<<blocks_1d(M * nA, 1024), 256, 0, st>>>(y_hat_static, nS, L.d_in + M * dD + cond_w, dD,
-                                                                       adv_cols, M);
-      GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(fake)");
-      if (cond_w) {
-        GANTTS_CUDA(cudaMemcpy2DAsync(L.d_in, (size_t)dD * sizeof(float), x, (size_t)d_in * sizeof(float),
-                                      (size_t)cond_w * sizeof(float), (size_t)M, cudaMemcpyDeviceToDevice, st));
-        GANTTS_CUDA(cudaMemcpy2DAsync(L.d_in + M * dD, (size_t)dD * sizeof(float), x, (size_t)d_in * sizeof(float),
-                                      (size_t)cond_w * sizeof(float), (size_t)M, cudaMemcpyDeviceToDevice, st));
-      }
-      if ((rc = gantts_mlp_fwd(&d, L.d_in, dD, 2 * M, L.d_out, 1, L.d_tape, L.d_tape_bytes, stream))) return rc;
+    s.g.dropout_p = 0.f;
+    s.d.dropout_p = 0.f;
+    if ((rc = step_prologue(s, inv_frames, true))) return rc;
+    if ((rc = generator_fwd(s, false))) return rc;
+    if (s.has_d) {
+      if ((rc = discriminator_fwd(s, true))) return rc;
       if ((rc = launch_bce(L.d_out, L.mask, M, 2, 0, 1, L.scal + S_INV_T, nullptr, &L.red[R_REAL], &L.red[R_FAKE], st)))
         return rc;
-      cnt.n[R_REAL] = cnt.n[R_FAKE] = bce_blocks(M);
-      if (has_adv) {
-        if ((rc = launch_bce(L.d_out + M, L.mask, M, 1, 0, 0, L.scal + S_INV_T, nullptr, &L.red[R_ADV], nullptr, st)))
-          return rc;
-        cnt.n[R_ADV] = bce_blocks(M);
-      }
+      // the adversarial loss re-uses the fake half: no dropout and no D step in between
+      if (s.has_adv &&
+          (rc = launch_bce(L.d_out + M, L.mask, M, 1, 0, 0, L.scal + S_INV_T, nullptr, &L.red[R_ADV], nullptr, st)))
+        return rc;
     }
-    if ((rc = launch_sse(y_hat_static, nS, y, d_out, L.mask, M, nS, L.scal + S_MGE_SCALE, nullptr, 0, &L.red[R_MGE], st,
-                         &static_cols)))
+    if ((rc = launch_sse(y_hat_static, nS, y, s.d_out, L.mask, M, nS, L.scal + S_MGE_SCALE, nullptr, 0, &L.red[R_MGE], st,
+                         &s.static_cols)))
       return rc;
-    if ((rc = launch_sse(y_hat, d_out, y, d_out, L.mask, M, d_out, L.scal + S_MSE_SCALE, nullptr, 0, &L.red[R_MSE], st)))
+    if ((rc = launch_sse(y_hat, s.d_out, y, s.d_out, L.mask, M, s.d_out, L.scal + S_MSE_SCALE, nullptr, 0, &L.red[R_MSE],
+                         st)))
       return rc;
-    cnt.n[R_MGE] = sse_blocks(M, nS);
-    cnt.n[R_MSE] = sse_blocks(M, d_out);
-    GANTTS_PDL_LAUNCH((finalize_losses_kernel), 1, RED_THREADS, 0, st, L.scal, losses_dev, L.red, cnt, has_adv ? c->adv_w : 0.f, c->mge_w,
-                                                      c->mse_w, has_d ? 1 : 0);
-    GANTTS_LAUNCH_CHECK("finalize_losses_kernel");
-    return GANTTS_OK;
+    return step_finalize(s, losses_dev);
   }
 
   if (phases & 1) {
     NvtxRange r1("gantts_gan_step/phase1: G fwd, MLPG, MGE, D fwd+bwd");
-    // ---- prologue: mask, scales, y_static (train.py:528-535)
-    if ((rc = gantts_sequence_mask(lengths_dev, L.mask, c->B, c->T, stream))) return rc;
-    GANTTS_PDL_LAUNCH((set_scales_kernel), 1, 32, 0, st, L.scal, inv_frames, has_adv ? c->adv_w : 0.f, c->mge_w, c->mse_w, 0, lengths_dev, c->B, c->T);
-    GANTTS_LAUNCH_CHECK("set_scales_kernel");
-    if (has_d && cond_w) {      // only the conditioned-discriminator fallback still gathers from y_static
-      gather_cols_list_kernel<<<blocks_1d(M * nS, 1024), 256, 0, st>>>(y, d_out, L.y_static, nS, static_cols, M);
-      GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(y_static)");
-    }
-    // ---- apply_generator (train.py:336-355): G forward + MLPG
-    if ((rc = generator_fwd(c, g, L, x, d_in, lengths_dev, M, y_hat, d_out, seed, true, st))) return rc;
-    if (hw && (rc = highway_gate_fwd(c, g, L, M, st))) return rc;
-    if ((rc = mlpg_fwd_impl(gen_out, (int64_t)c->T * d_out, d_out, y_hat_static, (int64_t)c->T * nS, nS,
-                            c->mlpg_table, &c->streams, &c->windows, c->B, c->T, stream, hwp)))
-      return rc;
+    if ((rc = step_prologue(s, inv_frames, false))) return rc;
+    if ((rc = generator_fwd(s, true))) return rc;
     // MGE loss (train.py:291) and its gradient in one pass; the gradient INITIALISES g_static, the two discriminator
     // passes then accumulate their input gradients on top of it
-    if ((rc = launch_sse(y_hat_static, nS, y, d_out, L.mask, M, nS, L.scal + S_MGE_SCALE, L.g_static, nS,
-                         &L.red[R_MGE], st, &static_cols)))
+    if ((rc = launch_sse(y_hat_static, nS, y, s.d_out, L.mask, M, nS, L.scal + S_MGE_SCALE, L.g_static, nS, &L.red[R_MGE],
+                         st, &s.static_cols)))
       return rc;
-    if (has_d) {
-      // ---- update_discriminator (train.py:245-279): stacked real | fake batch of 2M rows
-      d.seed = gantts_gan_step_seed(seed, 1);
-      if (!cond_w) {
-        // selected columns of y (real) and y_hat_static (fake) straight into the discriminator's input planes
-        Planes din;
-        if ((rc = mlp_tape_input_planes(&d, 2 * M, L.d_tape, L.d_tape_bytes, &din))) return rc;
-        GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(2 * M * nA, 1024), 256, 0, st, y, d_out, real_cols, M, y_hat_static, nS,
-                                                                          adv_cols, M, din.hi, din.lo, din.pitch);
-        GANTTS_LAUNCH_CHECK("gather_planes_kernel(real|fake)");
-        if ((rc = mlp_fwd_impl(&d, nullptr, 0, 2 * M, L.d_out, 1, L.d_tape, L.d_tape_bytes, stream, true))) return rc;
-      } else {
-        gather_cols_list_kernel<<<blocks_1d(M * nA, 1024), 256, 0, st>>>(L.y_static, nS, L.d_in + cond_w, dD, adv_cols,
-                                                                         M);
-        GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(real)");
-        gather_cols_list_kernel<<<blocks_1d(M * nA, 1024), 256, 0, st>>>(y_hat_static, nS, L.d_in + M * dD + cond_w, dD,
-                                                                         adv_cols, M);
-        GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(fake)");
-        GANTTS_CUDA(cudaMemcpy2DAsync(L.d_in, (size_t)dD * sizeof(float), x, (size_t)d_in * sizeof(float),
-                                      (size_t)cond_w * sizeof(float), (size_t)M, cudaMemcpyDeviceToDevice, st));
-        GANTTS_CUDA(cudaMemcpy2DAsync(L.d_in + M * dD, (size_t)dD * sizeof(float), x, (size_t)d_in * sizeof(float),
-                                      (size_t)cond_w * sizeof(float), (size_t)M, cudaMemcpyDeviceToDevice, st));
-        if ((rc = gantts_mlp_fwd(&d, L.d_in, dD, 2 * M, L.d_out, 1, L.d_tape, L.d_tape_bytes, stream))) return rc;
-      }
+    if (s.has_d) {
+      // ---- update_discriminator (train.py:245-279)
+      s.d.seed = gantts_gan_step_seed(seed, 1);
+      if ((rc = discriminator_fwd(s, true))) return rc;
       // real and fake BCE terms, counts and dL/dD of both halves (train.py:262-270) in one launch
       if ((rc = launch_bce(L.d_out, L.mask, M, 2, 0, 1, L.scal + S_INV_T, L.g_dout, &L.red[R_REAL], &L.red[R_FAKE], st)))
         return rc;
-      // loss_d.backward(): D parameter gradients + gradient w.r.t. the (fake) D input (rows M..2M-1 only).  When the
-      // adversarial columns form one window of y_hat_static the last GEMM adds its result straight into g_static
-      // (the scatter of the column gather's backward); otherwise it goes to g_din and a scatter kernel follows.
-      if (adv_window) {
-        float* win = L.g_static + adv_cols.c[0] - M * (int64_t)nS;      // row r of the stacked batch -> g_static[r - M]
-        if ((rc = mlp_bwd_impl(&d, L.g_dout, 1, L.d_out, 1, 2 * M, L.d_tape, L.d_tape_bytes, win, nS, M, pd.gW, pd.gb, 0,
-                               L.mlp_ws, L.mlp_ws_bytes, stream, 1)))
-          return rc;
-      } else {
-        if ((rc = mlp_bwd_impl(&d, L.g_dout, 1, L.d_out, 1, 2 * M, L.d_tape, L.d_tape_bytes, L.g_din, dD, M, pd.gW,
-                               pd.gb, 0, L.mlp_ws, L.mlp_ws_bytes, stream)))
-          return rc;
-        scatter_cols_list_add_kernel<<<blocks_1d(M * nA, 1024), 256, 0, st>>>(L.g_din + M * dD + cond_w, dD, L.g_static,
-                                                                              nS, adv_cols, M);
-        GANTTS_LAUNCH_CHECK("scatter_cols_list_add_kernel(fake)");
-      }
+      if ((rc = discriminator_bwd(s, true))) return rc;
     }
   }
   if (phases & 2) {
     NvtxRange r2("gantts_gan_step/phase2: D step, adv D fwd+bwd, MLPG bwd, G bwd");
-    if (has_d) {
-      // ---- clip_grad_norm_ + Adagrad on D (train.py:275-276)
-      if ((rc = clip_opt_model(c, pd, L.opt_partial, L.scal + S_DSUMSQ, c->lr_d, c->wd_d, st)))
-        return rc;
-    }
+    // ---- clip_grad_norm_ + Adagrad on D (train.py:275-276)
+    if (s.has_d && (rc = clip_opt_model(c, s.pd, L.opt_partial, L.scal + S_DSUMSQ, c->lr_d, c->wd_d, st))) return rc;
     // ---- update_generator (train.py:282-320); the MGE term was evaluated in phase 1
-    if (has_adv) {
+    if (s.has_adv) {
       // third D forward: updated weights, fresh dropout mask (train.py:307)
-      d.seed = gantts_gan_step_seed(seed, 2);
-      if (!cond_w) {
-        Planes din;
-        if ((rc = mlp_tape_input_planes(&d, M, L.d_tape, L.d_tape_bytes, &din))) return rc;
-        ColList none;
-        none.n = 0;
-        GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(M * nA, 1024), 256, 0, st, y_hat_static, nS, adv_cols, M, nullptr, 0, none, 0,
-                                                                      din.hi, din.lo, din.pitch);
-        GANTTS_LAUNCH_CHECK("gather_planes_kernel(adv)");
-        if ((rc = mlp_fwd_impl(&d, nullptr, 0, M, L.d_out, 1, L.d_tape, L.d_tape_bytes, stream, true))) return rc;
-      } else if ((rc = gantts_mlp_fwd(&d, L.d_in + M * dD, dD, M, L.d_out, 1, L.d_tape, L.d_tape_bytes, stream))) {
-        return rc;
-      }
+      s.d.seed = gantts_gan_step_seed(seed, 2);
+      if ((rc = discriminator_fwd(s, false))) return rc;
       if ((rc = launch_bce(L.d_out, L.mask, M, 1, 0, 0, L.scal + S_ADV_SCALE, L.g_dout, &L.red[R_ADV], nullptr, st)))
         return rc;
-      if (adv_window) {
-        if ((rc = mlp_bwd_impl(&d, L.g_dout, 1, L.d_out, 1, M, L.d_tape, L.d_tape_bytes, L.g_static + adv_cols.c[0], nS, 0,
-                               nullptr, nullptr, 0, L.mlp_ws, L.mlp_ws_bytes, stream, 1)))
-          return rc;
-      } else {
-        if ((rc = gantts_mlp_bwd(&d, L.g_dout, 1, L.d_out, 1, M, L.d_tape, L.d_tape_bytes, L.g_din, dD, nullptr,
-                                 nullptr, 0, L.mlp_ws, L.mlp_ws_bytes, stream)))
-          return rc;
-        scatter_cols_list_add_kernel<<<blocks_1d(M * nA, 1024), 256, 0, st>>>(L.g_din + cond_w, dD, L.g_static, nS,
-                                                                              adv_cols, M);
-        GANTTS_LAUNCH_CHECK("scatter_cols_list_add_kernel(adv)");
-      }
+      if ((rc = discriminator_bwd(s, false))) return rc;
     }
-    // ---- loss_g.backward(): MSE term (train.py:294) + MLPG backward + generator backward on the summed gradient.
-    // With mse_w != 0 the MSE pass stores its gradient into g_yhat and the MLPG backward accumulates on top of it.
-    if ((rc = launch_sse(y_hat, d_out, y, d_out, L.mask, M, d_out, L.scal + S_MSE_SCALE, mse_grad ? L.g_yhat : nullptr,
-                         d_out, &L.red[R_MSE], st)))
-      return rc;
-    // no MSE gradient (mse_w == 0, the CLI default, train.py:15; or y_hat = x): nothing else adds to dL/dy_hat, so the
-    // MLPG backward writes the operand planes of the generator's backward GEMMs directly (no fp32 matrix, no conversion)
-    bool direct = false;
-    if (!mse_grad) {
-      Planes gp;
-      if ((rc = mlp_bwd_gy_planes(&g, M, L.mlp_ws, L.mlp_ws_bytes, &gp))) return rc;
-      rc = mlpg_bwd_planes(L.g_static, (int64_t)c->T * nS, nS, gp.hi, gp.lo, gp.pitch, c->mlpg_table, &c->streams,
-                           &c->windows, c->B, c->T, stream, hwp);
-      if (rc == GANTTS_OK) direct = true;
-      else if (rc != GANTTS_E_UNSUPPORTED) return rc;
-    }
-    // (highway: the adjoint solves with Tx * g_static and leaves dz for the gate's weight gradient)
-    if (!direct &&
-        (rc = mlpg_bwd_impl(L.g_static, (int64_t)c->T * nS, nS, L.g_yhat, (int64_t)c->T * d_out, d_out, c->mlpg_table,
-                            &c->streams, &c->windows, c->B, c->T, mse_grad ? 1 : 0, stream, hwp)))
-      return rc;
-    if (hw && (rc = highway_gate_bwd(c, g, L, M, st))) return rc;
-    // (SRU or LSTM stack: hidden2out's input gradient is dL/dh of the stack's top layer)
-    const bool sru = c->sru.num_layers > 0;
-    float* gx = sru ? L.sru_dx : (lstm ? L.lstm_dh : nullptr);
-    const int gx_rs = sru ? sru_ncols(c->sru) : (lstm ? lstm_ndir(c->lstm) * c->lstm.hidden : 0);
-    if ((rc = mlp_bwd_impl(&g, direct ? nullptr : L.g_yhat, d_out, nullptr, 0, M, L.g_tape, L.g_tape_bytes, gx, gx_rs, 0,
-                           pg.gW, pg.gb, 0, L.mlp_ws, L.mlp_ws_bytes, stream, -1, direct)))
-      return rc;
-    if (sru && (rc = sru_stack_bwd(c, L, pg, x, M, seed, st))) return rc;
-    if (lstm && (rc = lstm_stack_bwd(c, L, pg, lengths_dev, M, seed, st))) return rc;
+    if ((rc = generator_bwd(s))) return rc;
   }
   if (phases & 4) {
     NvtxRange r4("gantts_gan_step/phase4: G step, losses");
     // ---- clip_grad_norm_ + Adagrad on G (train.py:317-318), then the loss scalars
-    if ((rc = clip_opt_model(c, pg, L.opt_partial, L.scal + S_GSUMSQ, c->lr_g, c->wd_g, st)))
-      return rc;
-    if (has_d) cnt.n[R_REAL] = cnt.n[R_FAKE] = bce_blocks(M);
-    if (has_adv) cnt.n[R_ADV] = bce_blocks(M);
-    cnt.n[R_MGE] = sse_blocks(M, nS);
-    cnt.n[R_MSE] = sse_blocks(M, d_out);
-    GANTTS_PDL_LAUNCH((finalize_losses_kernel), 1, RED_THREADS, 0, st, L.scal, losses_dev, L.red, cnt, has_adv ? c->adv_w : 0.f, c->mge_w,
-                                                      c->mse_w, has_d ? 1 : 0);
-    GANTTS_LAUNCH_CHECK("finalize_losses_kernel");
+    if ((rc = clip_opt_model(c, s.pg, L.opt_partial, L.scal + S_GSUMSQ, c->lr_g, c->wd_g, st))) return rc;
+    return step_finalize(s, losses_dev);
   }
   return GANTTS_OK;
 }

@@ -55,17 +55,8 @@ def _check_lstm(lstm):
     return lstm
 
 
-def _lstm_tensors(lstm):
-    """[(layer, direction, [weight_ih, weight_hh, bias_ih, bias_hh])] of an nn.LSTM in its parameters() order."""
-    out = []
-    for k in range(lstm.num_layers):
-        for d, sfx in enumerate(["", "_reverse"][:2 if lstm.bidirectional else 1]):
-            out.append((k, d, [getattr(lstm, "%s_l%d%s" % (n, k, sfx)) for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")]))
-    return out
-
-
 def _fill_sru(desc, cells):
-    """The shape block of gantts_sru_stack_t from an SRU stack (rnn.SRU.rnn_lst); pointers are set by the caller."""
+    """The shape block of gantts_sru_stack_t from an SRU stack (rnn.SRU.rnn_lst)."""
     if len(cells) > _lib.MAX_SRU_LAYERS:
         raise RuntimeError("gantts_b200: at most %d SRU layers" % _lib.MAX_SRU_LAYERS)
     c0 = cells[0]
@@ -85,19 +76,14 @@ def _fill_sru(desc, cells):
 
 
 def _fill_mlp(desc, layers, p, last_act):
+    """The shape block of gantts_mlp_t (its tensors go into the step's tensor tables)."""
     if len(layers) > _lib.MAX_LAYERS:
         raise RuntimeError("gantts_b200: at most %d layers" % _lib.MAX_LAYERS)
     desc.num_layers = len(layers)
     desc.dims[0] = layers[0].weight.shape[1]
     for i, l in enumerate(layers):
-        ops.require_cuda(l.weight, l.bias)
-        if not (l.weight.is_contiguous() and l.bias.is_contiguous()):
-            raise RuntimeError("gantts_b200: parameters must be contiguous")
         desc.dims[i + 1] = l.weight.shape[0]
-        desc.W[i] = l.weight.data_ptr()
-        desc.b[i] = l.bias.data_ptr()
     desc.slope, desc.dropout_p, desc.last_act, desc.seed = ops.LEAKY_SLOPE, float(p), int(last_act), 0
-    return layers
 
 
 class FusedGanStep(object):
@@ -123,75 +109,38 @@ class FusedGanStep(object):
         parallel.broadcast_parameters(model_d, group=process_group)
         c = _lib.GanStepT()
         c.B, c.T = self.B, self.T
-        self._gate, self._sru, self._lstm, g_layers = _generator_parts(model_g)
-        self._g_layers = _fill_mlp(c.g, g_layers, getattr(model_g, "dropout_p", 0.0), _lib.ACT_NONE)
-        self._d_layers = _fill_mlp(c.d, list(model_d.layers) + [model_d.last_linear], model_d.dropout_p,
-                                   _lib.ACT_SIGMOID)
+        gate, sru, lstm, g_layers = _generator_parts(model_g)
+        _fill_mlp(c.g, g_layers, getattr(model_g, "dropout_p", 0.0), _lib.ACT_NONE)
+        _fill_mlp(c.d, list(model_d.layers) + [model_d.last_linear], model_d.dropout_p, _lib.ACT_SIGMOID)
         if getattr(model_g, "last_sigmoid", False) or not model_d.last_sigmoid:
             raise RuntimeError("FusedGanStep: generator must be linear-output, discriminator sigmoid-output")
-        self._sums, self._sqs = [], []      # Adagrad: state_sum | Adam: exp_avg, exp_avg_sq (model.parameters() order)
-
-        def new_state1(t):
-            a = torch.zeros_like(t)
-            self._sums.append(a)
-            a2 = None
-            if optimizer == "Adam":
-                a2 = torch.zeros_like(t)
-                self._sqs.append(a2)
-            return a, a2
-
-        def new_state(l):
-            (a, a2), (b, b2) = new_state1(l.weight), new_state1(l.bias)
-            return a, b, a2, b2
-        if self._gate is not None:
-            gt, h = self._gate, c.highway
-            ops.require_cuda(gt.weight, gt.bias)
-            if not (gt.weight.is_contiguous() and gt.bias.is_contiguous()):
-                raise RuntimeError("gantts_b200: parameters must be contiguous")
-            h.static_dim = int(model_g.static_dim)
-            h.W, h.b = gt.weight.data_ptr(), gt.bias.data_ptr()
-            a, b, a2, b2 = new_state(gt)
-            h.sumW, h.sumb = a.data_ptr(), b.data_ptr()
-            if a2 is not None:
-                h.sqW, h.sqb = a2.data_ptr(), b2.data_ptr()
-        if self._sru:
-            su = c.sru
-            _fill_sru(su, self._sru)
-            for i, cell in enumerate(self._sru):
-                ops.require_cuda(cell.weight, cell.bias)
-                if not (cell.weight.is_contiguous() and cell.bias.is_contiguous()):
-                    raise RuntimeError("gantts_b200: parameters must be contiguous")
-                su.W[i], su.b[i] = cell.weight.data_ptr(), cell.bias.data_ptr()
-                a, b, a2, b2 = new_state(cell)
-                su.sumW[i], su.sumb[i] = a.data_ptr(), b.data_ptr()
-                if a2 is not None:
-                    su.sqW[i], su.sqb[i] = a2.data_ptr(), b2.data_ptr()
-        if self._lstm is not None:
-            ls, lm = c.lstm, self._lstm
-            ls.num_layers, ls.in_dim, ls.hidden = lm.num_layers, lm.input_size, lm.hidden_size
-            ls.bidirectional = int(bool(lm.bidirectional))
-            ls.dropout = float(lm.dropout) if lm.num_layers > 1 else 0.0
-            for k, d, ts in _lstm_tensors(lm):
-                ops.require_cuda(*ts)
-                if not all(t.is_contiguous() for t in ts):
-                    raise RuntimeError("gantts_b200: parameters must be contiguous")
-                for t, sums, sqs in zip(ts, (ls.sumW_ih, ls.sumW_hh, ls.sumb_ih, ls.sumb_hh),
-                                        (ls.sqW_ih, ls.sqW_hh, ls.sqb_ih, ls.sqb_hh)):
-                    a, a2 = new_state1(t)
-                    sums[k][d] = a.data_ptr()
-                    if a2 is not None:
-                        sqs[k][d] = a2.data_ptr()
-            self._set_lstm_pointers(c)
-        # number of generator tensors (the MLP layers' state is added below): their optimiser state comes first in
-        # self._sums / self._sqs
-        self._ng = len(self._sums) + 2 * len(self._g_layers)
-        for layers, sw, sb, qw, qb in ((self._g_layers, c.g_sumW, c.g_sumb, c.g_sqW, c.g_sqb),
-                                       (self._d_layers, c.d_sumW, c.d_sumb, c.d_sqW, c.d_sqb)):
-            for i, l in enumerate(layers):
-                a, b, a2, b2 = new_state(l)
-                sw[i], sb[i] = a.data_ptr(), b.data_ptr()
-                if a2 is not None:
-                    qw[i], qb[i] = a2.data_ptr(), b2.data_ptr()
+        if gate is not None:
+            c.highway.static_dim = int(model_g.static_dim)
+        if sru:
+            _fill_sru(c.sru, sru)
+        if lstm is not None:
+            ls = c.lstm
+            ls.num_layers, ls.in_dim, ls.hidden = lstm.num_layers, lstm.input_size, lstm.hidden_size
+            ls.bidirectional = int(bool(lstm.bidirectional))
+            ls.dropout = float(lstm.dropout) if lstm.num_layers > 1 else 0.0
+        # the tensor tables, in model.parameters() order; the C step binds them to its stages from the shapes above
+        self._params = list(model_g.parameters()) + list(model_d.parameters())
+        self._ng = len(list(model_g.parameters()))          # generator tensors: their optimiser state comes first
+        ops.require_cuda(*self._params)
+        if not all(t.is_contiguous() for t in self._params):
+            raise RuntimeError("gantts_b200: parameters must be contiguous")
+        # Adagrad: state_sum | Adam: exp_avg, exp_avg_sq
+        self._sums = [torch.zeros_like(t) for t in self._params]
+        self._sqs = [torch.zeros_like(t) for t in self._params] if optimizer == "Adam" else []
+        for tab, lo, hi in ((c.g_tensors, 0, self._ng), (c.d_tensors, self._ng, len(self._params))):
+            if hi - lo > _lib.MAX_STEP_TENSORS:
+                raise RuntimeError("gantts_b200: a model of more than %d tensors" % _lib.MAX_STEP_TENSORS)
+            tab.n = hi - lo
+            for i in range(lo, hi):
+                tab.state[i - lo] = self._sums[i].data_ptr()
+                if self._sqs:
+                    tab.state2[i - lo] = self._sqs[i].data_ptr()
+        self._bind_params(c)
         nw = len(hp.windows)
         entries, n_static = multistream.mlpg_stream_entries(hp.stream_sizes, hp.has_dynamic_features,
                                                             [True] * len(hp.stream_sizes), nw)
@@ -235,11 +184,10 @@ class FusedGanStep(object):
         self._step = 0
         self._grad_views = {}
 
-    def _set_lstm_pointers(self, cfg):
-        ls = cfg.lstm
-        for k, d, ts in _lstm_tensors(self._lstm):
-            for t, dst in zip(ts, (ls.W_ih, ls.W_hh, ls.b_ih, ls.b_hh)):
-                dst[k][d] = t.data_ptr()
+    def _bind_params(self, cfg):
+        for tab, lo, hi in ((cfg.g_tensors, 0, self._ng), (cfg.d_tensors, self._ng, len(self._params))):
+            for i in range(lo, hi):
+                tab.param[i - lo] = self._params[i].data_ptr()
 
     def grad_buffer(self, which):
         """Flat fp32 gradient buffer (0 = generator, 1 = discriminator) as a tensor view."""
@@ -275,15 +223,7 @@ class FusedGanStep(object):
         if not lengths.is_cuda or lengths.dtype != torch.int64:
             raise RuntimeError("FusedGanStep: lengths must be a CUDA int64 tensor")
         self.cfg.adv_w = float(adv_w)
-        for desc, layers in ((self.cfg.g, self._g_layers), (self.cfg.d, self._d_layers)):
-            for i, l in enumerate(layers):      # parameters may have been re-allocated (load_state_dict keeps them)
-                desc.W[i], desc.b[i] = l.weight.data_ptr(), l.bias.data_ptr()
-        if self._gate is not None:
-            self.cfg.highway.W, self.cfg.highway.b = self._gate.weight.data_ptr(), self._gate.bias.data_ptr()
-        for i, cell in enumerate(self._sru):
-            self.cfg.sru.W[i], self.cfg.sru.b[i] = cell.weight.data_ptr(), cell.bias.data_ptr()
-        if self._lstm is not None:
-            self._set_lstm_pointers(self.cfg)
+        self._bind_params(self.cfg)             # parameters may have been re-allocated (load_state_dict keeps them)
         if train is None:
             if self.g.training != self.d.training:
                 raise RuntimeError("FusedGanStep: generator and discriminator disagree on train()/eval()")

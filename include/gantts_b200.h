@@ -294,8 +294,8 @@ int gantts_sru_bwd(const float* u, const float* x, const float* bias, const floa
  * update_generator :282-320, both clip_grad_norm_ + Adagrad steps) on `stream`, no host sync.
  *
  * MLP generator (g, linear output) and MLP discriminator (d, one sigmoid output, input = the
- * `adv_cols` columns of the static features).  Weights (g.W/g.b, d.W/d.b) and the Adagrad
- * accumulators are updated IN PLACE.  phases is a bit mask so that a data-parallel caller can
+ * `adv_cols` columns of the static features).  The tensors of g_tensors / d_tensors and their
+ * optimiser state are updated IN PLACE.  phases is a bit mask so that a data-parallel caller can
  * all-reduce the gradient buffers (gantts_gan_step_grad_buffer) between the pieces:
  *   1 = prologue, G forward, MLPG, D forward on [real | fake], loss_d backward  -> D gradients ready
  *   2 = D clip+Adagrad, MGE/MSE/ADV losses, third D forward, loss_g backward    -> G gradients ready
@@ -311,22 +311,18 @@ int gantts_sru_bwd(const float* u, const float* x, const float* bias, const floa
  * and in the backward, from g = dL/dy_hat_static:  dGx = Tx * g (into the MLPG adjoint and the stack's backward),
  * dz = g * Gx * Tx * (1 - Tx),  dT.weight = dz^T x_s,  dT.bias = sum over rows of dz (no gradient w.r.t. x).
  * Accepted layout: exactly one stream, dynamic, in_start = out_start = 0, sd = S; n_static = S; g.dims[0] >= S;
- * g.dims[L] = windows.n * S; non-null W, b and optimiser state.  The gate is part of the generator everywhere: its two
+ * g.dims[L] = windows.n * S; a 16-byte aligned T.bias.  The gate is part of the generator everywhere: its two
  * tensors come FIRST in the flat gradient buffer (model.parameters() order: T.weight, T.bias, then g's layers), in the
  * clip norm and in the optimiser step.  The eval phase runs the same forward and leaves the gate and its state untouched.
  */
 typedef struct {
   int static_dim;                          /* 0 = plain MLP generator; S > 0 = In2OutHighwayNet with S static columns */
-  const float* W;                          /* T.weight [S][S] (nn.Linear layout), updated in place */
-  const float* b;                          /* T.bias [S], 16-byte aligned, updated in place */
-  float *sumW, *sumb;                      /* Adagrad state_sum | Adam exp_avg */
-  float *sqW, *sqb;                        /* Adam exp_avg_sq (unused by Adagrad) */
 } gantts_highway_t;
 
 /* SRURNN generator (reference gantts/models.py:144-167, hparams.py `tts_acoustic` / `tts_duration`): num_layers > 0.
  * Then g is hidden2out alone (g.num_layers == 1, g.dims[0] = ncols = hidden * (bidirectional ? 2 : 1)) and the step
  * runs the SRU stack of gantts_sru_fwd in front of it.  Layer l has n_in = in_dim (l = 0) or ncols, k = 4 when
- * n_in != ncols else 3, weight W[l] [n_in][ncols * k] and bias b[l] [2 * ncols] = forget | reset (the SRUCell layout).
+ * n_in != ncols else 3, weight [n_in][ncols * k] and bias [2 * ncols] = forget | reset (the SRUCell layout).
  * In training, layer l multiplies its GEMM input (only: the highway term keeps the unmasked input) by the variational
  * mask gantts_dropout(ones[B][n_in], rnn_dropout, gantts_sru_mask_seed(seed, l, 0)) and, for every layer but the last,
  * g(c_t) by gantts_dropout(ones[B][ncols], dropout, gantts_sru_mask_seed(seed, l, 1)); both are shared over time.
@@ -340,12 +336,6 @@ typedef struct {
   int in_dim, hidden, bidirectional;
   int act;                                 /* 0 identity, 1 tanh, 2 relu */
   float dropout, rnn_dropout;              /* each in [0, 1) */
-  const float* W[GANTTS_MAX_SRU_LAYERS];   /* [n_in][ncols * k], updated in place */
-  const float* b[GANTTS_MAX_SRU_LAYERS];   /* [2 * ncols], updated in place */
-  float* sumW[GANTTS_MAX_SRU_LAYERS];      /* Adagrad state_sum | Adam exp_avg */
-  float* sumb[GANTTS_MAX_SRU_LAYERS];
-  float* sqW[GANTTS_MAX_SRU_LAYERS];       /* Adam exp_avg_sq (unused by Adagrad) */
-  float* sqb[GANTTS_MAX_SRU_LAYERS];
 } gantts_sru_stack_t;
 
 /* In2OutRNNHighwayNet generator (reference gantts/models.py:72-118, the RNN VC model of hparams.py): num_layers > 0,
@@ -358,7 +348,7 @@ typedef struct {
  * but sends no gradient into the generator.  In training the output of every layer but the last is multiplied by
  * gantts_dropout(ones[B * T][ndir * hidden], dropout, gantts_lstm_mask_seed(seed, layer)) (nn.LSTM's per-element
  * inter-layer dropout).  Layer l has n_in = in_dim (l = 0) or ndir * hidden and, per direction d (0 forward, 1 reverse),
- * the torch.nn.LSTM tensors W_ih[l][d] [4H][n_in], W_hh[l][d] [4H][H], b_ih[l][d], b_hh[l][d] [4H] (gates i, f, g, o).
+ * the torch.nn.LSTM tensors W_ih [4H][n_in], W_hh [4H][H], b_ih, b_hh [4H] (gates i, f, g, o).
  * In model.parameters() order the gate's two tensors come first, then per layer and direction W_ih, W_hh, b_ih, b_hh,
  * then hidden2out, in the flat gradient buffer, the clip norm and the optimiser step; b_ih and b_hh get the same
  * gradient and keep separate optimiser state.  B <= 128, hidden a multiple of 4.  LSTMRNN / GRURNN (an LSTM stack
@@ -369,28 +359,30 @@ typedef struct {
   int num_layers;                          /* 0 = no LSTM stack (all other generators) */
   int in_dim, hidden, bidirectional;
   float dropout;                           /* in [0, 1) */
-  const float* W_ih[GANTTS_MAX_LSTM_LAYERS][2];   /* updated in place, like every tensor below */
-  const float* W_hh[GANTTS_MAX_LSTM_LAYERS][2];
-  const float* b_ih[GANTTS_MAX_LSTM_LAYERS][2];
-  const float* b_hh[GANTTS_MAX_LSTM_LAYERS][2];
-  float* sumW_ih[GANTTS_MAX_LSTM_LAYERS][2];      /* Adagrad state_sum | Adam exp_avg */
-  float* sumW_hh[GANTTS_MAX_LSTM_LAYERS][2];
-  float* sumb_ih[GANTTS_MAX_LSTM_LAYERS][2];
-  float* sumb_hh[GANTTS_MAX_LSTM_LAYERS][2];
-  float* sqW_ih[GANTTS_MAX_LSTM_LAYERS][2];       /* Adam exp_avg_sq (unused by Adagrad) */
-  float* sqW_hh[GANTTS_MAX_LSTM_LAYERS][2];
-  float* sqb_ih[GANTTS_MAX_LSTM_LAYERS][2];
-  float* sqb_hh[GANTTS_MAX_LSTM_LAYERS][2];
 } gantts_lstm_stack_t;
 
+/* One model's tensors in model.parameters() order: what the step updates in place, and their optimiser state.  One table
+ * is one TensorList of the clip + optimiser kernels, so GANTTS_MAX_STEP_TENSORS is their tensor limit. */
+#define GANTTS_MAX_STEP_TENSORS 32
+typedef struct {
+  int n;
+  float* param[GANTTS_MAX_STEP_TENSORS];
+  float* state[GANTTS_MAX_STEP_TENSORS];   /* Adagrad state_sum | Adam exp_avg */
+  float* state2[GANTTS_MAX_STEP_TENSORS];  /* Adam exp_avg_sq (unused by Adagrad) */
+} gantts_step_tensors_t;
+
+/* The shape blocks (g, highway, sru, lstm, d) describe the two models; their tensors come from g_tensors and d_tensors
+ * alone: the W / b pointers of g and d are not read.  The step binds the tables to the stages from the shapes and
+ * rejects a table whose n differs from the count the shapes give, or with a null param or state (state2 under Adam). */
 typedef struct {
   int B, T;
   gantts_mlp_t g;                          /* generator: dims[0] = linguistic width, dims[L] = acoustic width */
+  gantts_highway_t highway;                /* static_dim = 0: no highway gate */
+  gantts_sru_stack_t sru;                  /* num_layers = 0: no SRU stack */
+  gantts_lstm_stack_t lstm;                /* num_layers = 0: no LSTM stack */
   gantts_mlp_t d;                          /* discriminator: dims[0] = n_adv, dims[L] = 1, last_act = SIGMOID */
-  float* g_sumW[GANTTS_MAX_LAYERS];        /* Adagrad state_sum per parameter tensor */
-  float* g_sumb[GANTTS_MAX_LAYERS];
-  float* d_sumW[GANTTS_MAX_LAYERS];
-  float* d_sumb[GANTTS_MAX_LAYERS];
+  gantts_step_tensors_t g_tensors;         /* generator tensors, model_g.parameters() order */
+  gantts_step_tensors_t d_tensors;         /* discriminator tensors, model_d.parameters() order (read when w_d > 0) */
   gantts_streams_t streams;                /* MLPG stream layout of the generator output */
   gantts_windows_t windows;
   const float* mlpg_table;                 /* device copy of gantts_mlpg_table(windows, T) */
@@ -404,19 +396,12 @@ typedef struct {
   float lr_g, lr_d, wd_g, wd_d, eps, max_norm;
   float w_d, mse_w, mge_w, adv_w;
   /* Optimiser of both models (reference train.py:784-789 getattr(optim, hp.optimizer_g)(...)): 0 = Adagrad
-   * (hparams.py:201-206; *_sum* = state_sum), 1 = Adam (hparams.py:125-130, the duration model: lr 1e-3,
-   * betas (0.5, 0.9), weight_decay 0, eps 1e-8, amsgrad off; *_sum* = exp_avg, *_sq* = exp_avg_sq, opt_step =
+   * (hparams.py:201-206; state = state_sum), 1 = Adam (hparams.py:125-130, the duration model: lr 1e-3,
+   * betas (0.5, 0.9), weight_decay 0, eps 1e-8, amsgrad off; state = exp_avg, state2 = exp_avg_sq, opt_step =
    * number of the step being taken, 1 for the first -- the bias corrections are computed on the host). */
   int optimizer;
   float beta1, beta2;
   int64_t opt_step;
-  float* g_sqW[GANTTS_MAX_LAYERS];
-  float* g_sqb[GANTTS_MAX_LAYERS];
-  float* d_sqW[GANTTS_MAX_LAYERS];
-  float* d_sqb[GANTTS_MAX_LAYERS];
-  gantts_highway_t highway;                /* static_dim = 0: plain MLP generator (all fields above keep their offsets) */
-  gantts_sru_stack_t sru;                  /* num_layers = 0: no SRU stack (all fields above keep their offsets) */
-  gantts_lstm_stack_t lstm;                /* num_layers = 0: no LSTM stack (all fields above keep their offsets) */
 } gantts_gan_step_t;
 #define GANTTS_OPT_ADAGRAD 0
 #define GANTTS_OPT_ADAM 1

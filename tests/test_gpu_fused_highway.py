@@ -6,13 +6,13 @@ Parity with injected dropout masks as in test_gpu_train_mode.py: the step's keep
 used and handed to the oracle port.  Tolerance: 1e-4 relative unless stated.  The last-but-one test is host-only (no
 mark): the highway block's configuration rules through the C ABI.
 """
-import ctypes
-
 import numpy as np
 import pytest
 import torch
 
 from conftest import WINDOWS, rel_err
+from fused_step_helpers import (FAKE, check_weights, config_checker, dev, fill_tables, loss_errors, make_batch, npy,  # noqa: F401
+                                ragged_lengths, resync_oracle, sd_numpy, step_config)
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
 
@@ -23,40 +23,10 @@ GOLD_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mse", "loss_mge", "lo
              "real_correct", "fake_correct")
 
 
-@pytest.fixture(scope="module")
-def dev():
-    import __graft_entry__
-    __graft_entry__.build()
-    return torch.device("cuda:0")
-
-
-def npy(t):
-    return t.detach().cpu().numpy()
-
-
-def ragged_lengths(B, T, seed):
-    rng = np.random.RandomState(seed)
-    return sorted([T] + [int(v) for v in rng.randint(T // 2, T, B - 1)], reverse=True)
-
-
-def make_batch(B, T, d_in, d_out, lens, seed):
-    g = torch.Generator().manual_seed(seed)
-    x = torch.randn(B, T, d_in, generator=g)
-    y = torch.randn(B, T, d_out, generator=g)
-    for b, n in enumerate(lens):
-        x[b, n:] = 0
-        y[b, n:] = 0
-    return x, y
-
-
 def vc_hp(width=177):
     from gantts_b200 import step as gstep
     return gstep.HParams(windows=WINDOWS, stream_sizes=[width], has_dynamic_features=[True], adversarial_streams=[True],
                          mask_nth_mgc_for_adv_loss=0, discriminator_linguistic_condition=False)
-
-
-def sd_numpy(m):
-    return {k: v.detach().cpu().numpy() for k, v in m.state_dict().items()}
 
 
 def vc_models(seed, p, dev, hidden=512, d_hidden=256, d_layers=2):
@@ -66,10 +36,6 @@ def vc_models(seed, p, dev, hidden=512, d_hidden=256, d_layers=2):
                                              dropout=p)
     md = gantts_b200.models.MLP(59, 1, d_layers, d_hidden, dropout=p, last_sigmoid=True)
     return mg, md
-
-
-def loss_errors(got, ref, keys):
-    return {k: abs(float(got[k]) - ref[k]) / max(abs(ref[k]), 1e-12) for k in keys}
 
 
 def step_masks(fs, M, g_hidden, d_hidden, p, dev, with_d=True):
@@ -84,12 +50,6 @@ def step_masks(fs, M, g_hidden, d_hidden, p, dev, with_d=True):
     dm = {"real": [m[:M].cpu() for m in stacked], "fake": [m[M:].cpu() for m in stacked],
           "adv": [m.cpu() for m in ops.mlp_dropout_masks(M, d_hidden, p, lib.gantts_gan_step_seed(s, 2), dev)]}
     return g, dm
-
-
-def check_weights(model, named, tag):
-    for k, v in model.state_dict().items():
-        d = np.abs(npy(v) - named[k].detach().numpy())
-        assert np.median(d) < 2e-6 and d.max() <= 0.0201, (tag, k, np.median(d), d.max())
 
 
 @pytest.mark.gpu
@@ -163,7 +123,7 @@ def test_fused_highway_vc_adversarial_train_mode_injected_masks(dev):
     assert g_err < 5e-4, g_err
     assert abs(got["real_correct"] - ref["real_correct"]) <= 3 and abs(got["fake_correct"] - ref["fake_correct"]) <= 3
     assert got["frames"] == float(sum(lens))
-    check_weights(mg, gen.named, "vc")
+    check_weights(mg, gen.named, "vc", median=2e-6)
 
 
 @pytest.mark.gpu
@@ -183,7 +143,6 @@ def test_fused_highway_cfg1_two_steps(dev, monkeypatch, mode):
     d_before = [q.detach().clone() for q in md.parameters()]
     fs = fused.FusedGanStep(mg, md, vc_hp(), B, T, w_d=0.0, mse_w=1.0, mge_w=1.0, seed=70)
     R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, T))
-    names = [n for n, _ in mg.named_parameters()]
     for it in range(2):
         lens = ragged_lengths(B, T, 20 + it)
         x, y = make_batch(B, T, 177, 177, lens, 30 + it)
@@ -197,12 +156,8 @@ def test_fused_highway_cfg1_two_steps(dev, monkeypatch, mode):
         errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), ys_ref.numpy())
         assert max(errs.values()) < 1e-4, (it, errs)
         assert got["loss_d"] == 0.0 and got["loss_adv"] == 0.0
-        check_weights(mg, gen.named, "cfg1 step %d" % it)
-        sums = dict(zip(names, fs._sums[:len(names)]))
-        with torch.no_grad():
-            for i, (k, t) in enumerate(gen.named.items()):
-                t.copy_(mg.state_dict()[k].cpu())
-                gen.sums[i].copy_(sums[k].cpu())
+        check_weights(mg, gen.named, "cfg1 step %d" % it, median=2e-6)
+        resync_oracle(fs, mg, md, gen, [], [])
     for a, b in zip(d_before, md.parameters()):
         assert torch.equal(a, b.detach())
 
@@ -316,75 +271,56 @@ def test_fused_highway_phase_split_is_bitwise_equal(dev):
         assert torch.equal(a, b)
 
 
-def _vc_step_config(lib):
-    """A valid In2OutHighwayNet configuration of gantts_gan_step_t (host pointers are placeholders: only the
-    configuration check and the workspace layout run)."""
-    from gantts_b200 import _lib
-    S, nw, fake = 59, 3, 1 << 20
-    c = _lib.GanStepT()
-    c.B, c.T = 2, 16
-    c.g.num_layers = 2
-    for i, v in enumerate((177, 64, nw * S)):
-        c.g.dims[i] = v
-    c.d.num_layers = 2
-    for i, v in enumerate((S, 32, 1)):
-        c.d.dims[i] = v
-    for m in (c.g, c.d):
-        for i in range(2):
-            m.W[i] = m.b[i] = fake
-    c.g.last_act, c.d.last_act = _lib.ACT_NONE, _lib.ACT_SIGMOID
-    c.streams = _lib.make_streams([(0, S, True, 0)])
-    c.windows = _lib.make_windows(WINDOWS)
-    c.mlpg_table = fake
-    c.n_static = c.n_static_cols = S
-    c.n_adv = S
-    for i in range(S):
-        c.static_cols[i] = c.adv_cols[i] = i
-    c.w_d, c.mge_w, c.adv_w, c.max_norm, c.lr_g, c.lr_d, c.eps = 1.0, 1.0, 1.0, 1.0, 0.01, 0.01, 1e-10
-    c.optimizer = _lib.OPT_ADAGRAD
-    h = c.highway
-    h.static_dim = S
-    h.W = h.b = h.sumW = h.sumb = fake
-    return c
+def _vc_step_config():
+    """A valid In2OutHighwayNet configuration of gantts_gan_step_t: G 177 -> 64 -> 3 S with the gate (S = 59), D S -> 32
+    -> 1 (host pointers are placeholders: only the configuration check and the workspace layout run)."""
+    S = 59
+    c = step_config((177, 64, 3 * S), (S, 32, 1), [(0, S, True, 0)], range(S), range(S))
+    c.highway.static_dim = S
+    return fill_tables(c, 2 + 2 * 2)
 
 
-def test_highway_step_config_rules():
+def test_highway_step_config_rules_on_tensor_tables():
     """gantts_gan_step_workspace_bytes (host-only) accepts the VC layout and rejects, with a message naming the rule,
     every highway configuration the gate + combine arithmetic does not describe."""
-    import __graft_entry__
-    __graft_entry__.build()
     from gantts_b200 import _lib, multistream, step as gstep
-    lib = _lib.load()
-    ws = lambda c: lib.gantts_gan_step_workspace_bytes(ctypes.byref(c))
-    err = lambda: lib.gantts_last_error_string().decode()
-    c = _vc_step_config(lib)
+    ws, err, rejected = config_checker()
+    c = _vc_step_config()
     assert ws(c) > 0, err()
+    with_gate = ws(c)
     c.highway.static_dim = 0                                   # the same config as a plain MLP generator
-    plain = ws(c)
-    c.highway.static_dim = 59
-    assert 0 < plain < ws(c)
+    c.g_tensors.n = 4
+    assert 0 < ws(c) < with_gate, err()
 
-    c = _vc_step_config(lib)                                   # the TTS layout: four streams, one of them static
-    hp = gstep.TTS_ACOUSTIC
-    entries, _ = multistream.mlpg_stream_entries(hp.stream_sizes, hp.has_dynamic_features, [True] * 4, 3)
-    c.streams = _lib.make_streams(entries)
-    assert ws(c) == 0 and "one dynamic stream" in err(), err()
+    def tts_streams(c):                                        # the TTS layout: four streams, one of them static
+        hp = gstep.TTS_ACOUSTIC
+        entries, _ = multistream.mlpg_stream_entries(hp.stream_sizes, hp.has_dynamic_features, [True] * 4, 3)
+        c.streams = _lib.make_streams(entries)
 
-    c = _vc_step_config(lib)
-    c.n_static = c.n_static_cols = 58
-    assert ws(c) == 0 and "n_static" in err(), err()
+    def n_static(c):
+        c.n_static = c.n_static_cols = 58
+    rejected(_vc_step_config, tts_streams, "one dynamic stream")
+    rejected(_vc_step_config, n_static, "n_static")
+    rejected(_vc_step_config, lambda c: c.g.dims.__setitem__(2, 176), "output width")
+    rejected(_vc_step_config, lambda c: c.g_tensors.param.__setitem__(0, None), "null generator tensor 0")
+    rejected(_vc_step_config, lambda c: c.g_tensors.param.__setitem__(1, FAKE + 4), "gate bias must be 16-byte aligned")
+    rejected(_vc_step_config, lambda c: c.g_tensors.state.__setitem__(1, None),
+             "null generator optimiser state of tensor 1")
 
-    c = _vc_step_config(lib)
-    c.g.dims[2] = 176
-    assert ws(c) == 0 and "output width" in err(), err()
 
-    c = _vc_step_config(lib)
-    c.highway.W = None
-    assert ws(c) == 0 and "null highway gate" in err(), err()
-
-    c = _vc_step_config(lib)
-    c.highway.sumb = None
-    assert ws(c) == 0 and "optimiser state" in err(), err()
+def test_step_tensor_table_rules():
+    """Each model's tensor table must hold exactly the tensors its shapes give, each with its optimiser state; the
+    discriminator's table is read only when there is a discriminator (w_d > 0)."""
+    ws, err, rejected = config_checker()
+    rejected(_vc_step_config, lambda c: setattr(c.g_tensors, "n", 4), "generator table has 4 tensors, its shapes give 6")
+    rejected(_vc_step_config, lambda c: setattr(c.g_tensors, "n", 7), "generator table has 7 tensors, its shapes give 6")
+    rejected(_vc_step_config, lambda c: setattr(c.d_tensors, "n", 0), "discriminator table has 0 tensors, its shapes give 4")
+    rejected(_vc_step_config, lambda c: c.d_tensors.param.__setitem__(2, None), "null discriminator tensor 2")
+    rejected(_vc_step_config, lambda c: c.d_tensors.state.__setitem__(3, None),
+             "null discriminator optimiser state of tensor 3")
+    c = _vc_step_config()
+    c.w_d, c.d_tensors.n = 0.0, 0
+    assert ws(c) > 0, err()
 
 
 @pytest.mark.gpu

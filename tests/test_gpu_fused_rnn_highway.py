@@ -9,14 +9,14 @@ test_gpu_fused_highway.py.  Tolerances: losses, gradient norms and y_hat_static 
 test_gpu_train_mode.py); y_hat is the input, bit for bit; post-step weights median |delta| < 5e-6 and max <= 0.0201 (a
 first Adagrad / Adam step moves a weight by lr * sign(g)).  The configuration-rule test is host-only (no mark).
 """
-import ctypes
-import os
-
 import numpy as np
 import pytest
 import torch
 
 from conftest import WINDOWS, rel_err
+from fused_step_helpers import (adv_loss_with, check_weights, config_checker, d_masks, dev, fill_tables,  # noqa: F401
+                                loss_errors, make_batch, npy, ragged_lengths, resync_oracle, sd_numpy, step_config,
+                                step_hp, use_adam)
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
 
@@ -30,43 +30,6 @@ KINDS = ("weight_ih", "weight_hh", "bias_ih", "bias_hh")
 def vc_ohp(width, cond=False):
     return dict(stream_sizes=[width], has_dynamic_features=[True], adversarial_streams=[True],
                 mask_nth_mgc_for_adv_loss=0, num_windows=3, discriminator_linguistic_condition=cond)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    import __graft_entry__
-    __graft_entry__.build()
-    return torch.device("cuda:0")
-
-
-def npy(t):
-    return t.detach().cpu().numpy()
-
-
-def step_hp(ohp):
-    from gantts_b200 import step as gstep
-    return gstep.HParams(windows=WINDOWS, stream_sizes=ohp["stream_sizes"], has_dynamic_features=ohp["has_dynamic_features"],
-                         adversarial_streams=ohp["adversarial_streams"], mask_nth_mgc_for_adv_loss=0,
-                         discriminator_linguistic_condition=ohp["discriminator_linguistic_condition"])
-
-
-def ragged_lengths(B, T, seed):
-    rng = np.random.RandomState(seed)
-    return sorted([T] + [int(v) for v in rng.randint(T // 2, T, B - 1)], reverse=True)
-
-
-def make_batch(B, T, d_in, d_out, lens, seed):
-    g = torch.Generator().manual_seed(seed)
-    x = torch.randn(B, T, d_in, generator=g)
-    y = torch.randn(B, T, d_out, generator=g)
-    for b, n in enumerate(lens):
-        x[b, n:] = 0
-        y[b, n:] = 0
-    return x, y
-
-
-def sd_numpy(m):
-    return {k: v.detach().cpu().numpy() for k, v in m.state_dict().items()}
 
 
 def rhw_models(seed, S, layers, hidden, bidir, p, d_hidden, d_layers, p_d, cond=False):
@@ -129,38 +92,6 @@ def lstm_masks(fs, mg, B, T, dev):
             for k in range(lm.num_layers - 1)]
 
 
-def d_masks(fs, M, d_hidden, p, dev):
-    from gantts_b200 import ops, _lib
-    lib = _lib.load()
-    s = fs.last_seed
-    stacked = ops.mlp_dropout_masks(2 * M, d_hidden, p, lib.gantts_gan_step_seed(s, 1), dev)
-    return {"real": [m[:M].cpu() for m in stacked], "fake": [m[M:].cpu() for m in stacked],
-            "adv": [m.cpu() for m in ops.mlp_dropout_masks(M, d_hidden, p, lib.gantts_gan_step_seed(s, 2), dev)]}
-
-
-def adv_loss_with(md, x, ys_ref, lens, ohp, adv_masks):
-    """loss_adv of the oracle's y_hat_static through the PRODUCT's updated discriminator (see test_gpu_fused_sru.py:
-    after D's first optimiser step, weights with near-zero gradients land 2 lr apart in the two implementations)."""
-    ps = list(md.parameters())
-    layers = [(w.detach().cpu(), b.detach().cpu()) for w, b in zip(ps[0::2], ps[1::2])]
-    fake_in = gp.get_selected_static_stream(ys_ref, ohp)
-    if ohp["discriminator_linguistic_condition"]:
-        fake_in = torch.cat((x, fake_in), -1)
-    mask = gp.sequence_mask(lens, x.size(1)).unsqueeze(-1)
-    D = gp.mlp_forward(fake_in, layers, last_sigmoid=True, masks=adv_masks)
-    return float(gp.bce_real(D, mask, mask.sum().item()))
-
-
-def loss_errors(got, ref, keys):
-    return {k: abs(float(got[k]) - ref[k]) / max(abs(ref[k]), 1e-12) for k in keys}
-
-
-def check_weights(model, named, tag):
-    for k, v in model.state_dict().items():
-        d = np.abs(npy(v) - named[k].detach().numpy())
-        assert np.median(d) < 5e-6 and d.max() <= 0.0201, (tag, k, np.median(d), d.max())
-
-
 def run_vs_oracle(dev, mg, md, ohp, B, T, steps, mse_w, p_d, d_hidden, seed, tag, optimizer="Adagrad"):
     """`steps` training steps of FusedGanStep, each against the oracle started from the product's weights and optimiser
     state, with the step's own masks injected."""
@@ -177,7 +108,6 @@ def run_vs_oracle(dev, mg, md, ohp, B, T, steps, mse_w, p_d, d_hidden, seed, tag
     mg.to(dev).train(), md.to(dev).train()
     fs = fused.FusedGanStep(mg, md, step_hp(ohp), B, T, w_d=1.0, mse_w=mse_w, mge_w=1.0, weight_decay=0.0, seed=seed,
                             optimizer=optimizer, optimizer_params=okw)
-    names = [n for n, _ in mg.named_parameters()]
     R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, T))
     in_dim = 3 * S
     for it in range(steps):
@@ -198,24 +128,7 @@ def run_vs_oracle(dev, mg, md, ohp, B, T, steps, mse_w, p_d, d_hidden, seed, tag
         assert torch.equal(fs.y_hat, xd)                                   # models.py:118: the input is y_hat
         assert abs(got["real_correct"] - ref["real_correct"]) <= 3 and abs(got["fake_correct"] - ref["fake_correct"]) <= 3
         check_weights(mg, gen.named, "%s step %d" % (tag, it))
-        # the next step starts from the product's weights and optimiser state
-        sd = fs.state_dict()
-        with torch.no_grad():
-            for i, n in enumerate(names):
-                gen.named[n].copy_(mg.state_dict()[n].cpu())
-            for r, q in zip(d_params, md.parameters()):
-                r.copy_(q.detach().cpu())
-            order = list(gen.named)
-            for key, params, keys, sums, opt in (("optimizer_g", None, names, gen.sums, g_opt),
-                                                 ("optimizer_d", d_params, None, d_sum, d_opt)):
-                st = sd[key]["state"]
-                for i in range(len(st)):
-                    j = order.index(keys[i]) if keys is not None else i      # oracle order of parameter i
-                    if opt is None:
-                        sums[j].copy_(st[i]["sum"].cpu())
-                    else:
-                        opt.m[j].copy_(st[i]["exp_avg"].cpu())
-                        opt.v[j].copy_(st[i]["exp_avg_sq"].cpu())
+        resync_oracle(fs, mg, md, gen, d_params, d_sum, g_opt, d_opt)        # the next step starts from the product's state
     return fs
 
 
@@ -457,108 +370,62 @@ def test_fused_step_still_rejects_grurnn_and_unsupported_lstms(dev):
 
 
 def _rhw_step_config():
-    """A valid In2OutRNNHighwayNet configuration of gantts_gan_step_t on the cfg3 layout (host pointers are
-    placeholders: only the configuration check and the workspace layout run)."""
-    from gantts_b200 import _lib
-    S, fake, H, nl = 59, 1 << 20, 16, 3
-    c = _lib.GanStepT()
-    c.B, c.T = 2, 16
-    c.g.num_layers = 1
-    c.g.dims[0], c.g.dims[1] = 2 * H, 3 * S
-    c.d.num_layers = 2
-    for i, v in enumerate((S, 32, 1)):
-        c.d.dims[i] = v
-    for m in (c.g, c.d):
-        for i in range(m.num_layers):
-            m.W[i] = m.b[i] = fake
-    c.g_sumW[0] = c.g_sumb[0] = fake
-    c.g.last_act, c.d.last_act = _lib.ACT_NONE, _lib.ACT_SIGMOID
-    c.streams = _lib.make_streams([(0, S, True, 0)])
-    c.windows = _lib.make_windows(WINDOWS)
-    c.mlpg_table = fake
-    c.n_static = c.n_static_cols = c.n_adv = S
-    for i in range(S):
-        c.static_cols[i] = c.adv_cols[i] = i
-    c.w_d, c.mge_w, c.adv_w, c.max_norm, c.lr_g, c.lr_d, c.eps = 1.0, 1.0, 1.0, 1.0, 0.01, 0.01, 1e-10
-    c.optimizer = _lib.OPT_ADAGRAD
-    h = c.highway
-    h.static_dim = S
-    h.W = h.b = h.sumW = h.sumb = fake
+    """A valid In2OutRNNHighwayNet configuration of gantts_gan_step_t on the cfg3 layout: the gate (S = 59), 3
+    bidirectional LSTM layers of 16 over 3 S, hidden2out 32 -> 3 S, D S -> 32 -> 1 (host pointers are placeholders: only
+    the configuration check and the workspace layout run)."""
+    S, H, nl = 59, 16, 3
+    c = step_config((2 * H, 3 * S), (S, 32, 1), [(0, S, True, 0)], range(S), range(S))
+    c.highway.static_dim = S
     ls = c.lstm
     ls.num_layers, ls.in_dim, ls.hidden, ls.bidirectional, ls.dropout = nl, 3 * S, H, 1, 0.5
-    for k in range(nl):
-        for d in range(2):
-            for f in ("W_ih", "W_hh", "b_ih", "b_hh", "sumW_ih", "sumW_hh", "sumb_ih", "sumb_hh"):
-                getattr(ls, f)[k][d] = fake
-    return c
+    return fill_tables(c, 2 + 8 * nl + 2)
 
 
-def test_rnn_highway_step_config_rules(tmp_path):
+def lstm_tensor(layer, direction, kind):
+    """Index in the generator's table of an LSTM tensor (kind 0..3: W_ih, W_hh, b_ih, b_hh), bidirectional stack."""
+    return 2 + 4 * (2 * layer + direction) + kind
+
+
+def test_rnn_highway_step_config_rules_on_tensor_tables():
     """gantts_gan_step_workspace_bytes (host-only) accepts the In2OutRNNHighwayNet layout and rejects, with a message
     naming the rule, every LSTM configuration the step does not implement; the LSTM mask seeds are a stream of their
-    own; the ctypes mirror of the appended block matches the header."""
-    import subprocess
-    import __graft_entry__
-    __graft_entry__.build()
+    own."""
     from gantts_b200 import _lib
+    ws, err, rejected = config_checker()
     lib = _lib.load()
-    ws = lambda c: lib.gantts_gan_step_workspace_bytes(ctypes.byref(c))
-    err = lambda: lib.gantts_last_error_string().decode()
     c = _rhw_step_config()
     assert ws(c) > 0, err()
     with_lstm = ws(c)
     c.lstm.num_layers = 0                         # the gate + a one-layer MLP on x: no LSTM workspace
     c.g.dims[0] = 3 * 59
+    c.g_tensors.n = 4
     assert 0 < ws(c) < with_lstm, err()
 
-    def rejected(mutate, needle):
-        c = _rhw_step_config()
-        mutate(c)
-        assert ws(c) == 0 and needle in err(), (needle, err())
-    rejected(lambda c: setattr(c.highway, "static_dim", 0), "highway gate")
-    rejected(lambda c: setattr(c.sru, "num_layers", 1), "mutually exclusive")
-    rejected(lambda c: setattr(c.lstm, "num_layers", _lib.MAX_LSTM_LAYERS + 1), "LSTM layer count")
-    rejected(lambda c: setattr(c.lstm, "num_layers", -1), "LSTM layer count")
-    rejected(lambda c: setattr(c.lstm, "hidden", 18), "multiple of 4")
-    rejected(lambda c: setattr(c, "B", 129), "LSTM_MAX_B")
-    rejected(lambda c: setattr(c.lstm, "dropout", 1.0), "LSTM dropout")
-    rejected(lambda c: setattr(c.lstm, "dropout", -0.1), "LSTM dropout")
-    rejected(lambda c: c.g.dims.__setitem__(0, 16), "hidden2out")
-    rejected(lambda c: setattr(c.g, "num_layers", 2), "hidden2out")
-    rejected(lambda c: setattr(c.lstm, "in_dim", 3 * 59 - 1), "in_dim")
+    def rej(mutate, needle):
+        rejected(_rhw_step_config, mutate, needle)
+    rej(lambda c: setattr(c.highway, "static_dim", 0), "highway gate")
+    rej(lambda c: setattr(c.sru, "num_layers", 1), "mutually exclusive")
+    rej(lambda c: setattr(c.lstm, "num_layers", _lib.MAX_LSTM_LAYERS + 1), "LSTM layer count")
+    rej(lambda c: setattr(c.lstm, "num_layers", -1), "LSTM layer count")
+    rej(lambda c: setattr(c.lstm, "hidden", 18), "multiple of 4")
+    rej(lambda c: setattr(c, "B", 129), "LSTM_MAX_B")
+    rej(lambda c: setattr(c.lstm, "dropout", 1.0), "LSTM dropout")
+    rej(lambda c: setattr(c.lstm, "dropout", -0.1), "LSTM dropout")
+    rej(lambda c: c.g.dims.__setitem__(0, 16), "hidden2out")
+    rej(lambda c: setattr(c.g, "num_layers", 2), "hidden2out")
+    rej(lambda c: setattr(c.lstm, "in_dim", 3 * 59 - 1), "in_dim")
 
     def narrow(c):                                # in_dim < S (with a matching hidden2out)
         c.lstm.in_dim = c.g.dims[1] = 40
-    rejected(narrow, "static_dim")
-    rejected(lambda c: c.lstm.W_hh[2].__setitem__(1, None), "null LSTM weight")
-    rejected(lambda c: c.lstm.b_ih[0].__setitem__(0, None), "null LSTM weight")
-    rejected(lambda c: c.lstm.sumb_hh[1].__setitem__(0, None), "optimiser state")
-
-    def adam(c):                                  # exp_avg_sq for every tensor but layer 2's reverse W_hh
-        c.optimizer, c.beta1, c.beta2 = _lib.OPT_ADAM, 0.5, 0.9
-        c.highway.sqW = c.highway.sqb = c.g_sqW[0] = c.g_sqb[0] = 1 << 20
-        for k in range(3):
-            for d in range(2):
-                for f in ("sqW_ih", "sqW_hh", "sqb_ih", "sqb_hh"):
-                    getattr(c.lstm, f)[k][d] = 1 << 20
-        c.lstm.sqW_hh[2][1] = None
-    rejected(adam, "exp_avg_sq for LSTM layer 2 direction 1")
+    rej(narrow, "static_dim")
+    rej(lambda c: c.g_tensors.param.__setitem__(lstm_tensor(2, 1, 1), None), "null generator tensor 23")
+    rej(lambda c: c.g_tensors.param.__setitem__(lstm_tensor(0, 0, 2), None), "null generator tensor 4")
+    rej(lambda c: c.g_tensors.state.__setitem__(lstm_tensor(1, 0, 3), None), "null generator optimiser state of tensor 13")
+    rej(lambda c: setattr(c.lstm, "num_layers", 2), "generator table has 28 tensors, its shapes give 20")
+    rej(lambda c: use_adam(c, missing=(lstm_tensor(2, 1, 1),)), "exp_avg_sq for generator tensor 23")
     # the seeds of the LSTM masks are a stream of their own
     for seed in (0, 5, 12345):
         lstm_seeds = {lib.gantts_lstm_mask_seed(seed, l) for l in range(_lib.MAX_LSTM_LAYERS)}
         others = {lib.gantts_gan_step_seed(seed, w) for w in range(4)}
         others |= {lib.gantts_sru_mask_seed(seed, l, w) for l in range(_lib.MAX_SRU_LAYERS) for w in range(2)}
         assert len(lstm_seeds) == _lib.MAX_LSTM_LAYERS and not lstm_seeds & others
-    # offsets of the appended block and inside it, against the C compiler's view of the header
-    fields = [("gantts_gan_step_t", "lstm", _lib.GanStepT.lstm.offset)]
-    for f in ("in_dim", "dropout", "W_ih", "b_hh", "sumW_ih", "sqb_hh"):
-        fields.append(("gantts_lstm_stack_t", f, getattr(_lib.LstmStackT, f).offset))
-    src = tmp_path / "layout.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "gantts_b200.h"\nint main(void) {\n'
-                   '  printf("%zu %zu", sizeof(gantts_gan_step_t), sizeof(gantts_lstm_stack_t));\n' +
-                   "".join('  printf(" %%zu", offsetof(%s, %s));\n' % (s, f) for s, f, _ in fields) + "  return 0;\n}\n")
-    exe = tmp_path / "layout"
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    subprocess.run(["gcc", "-I", os.path.join(root, "include"), "-o", str(exe), str(src)], check=True)
-    got = [int(v) for v in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
-    assert got == [ctypes.sizeof(_lib.GanStepT), ctypes.sizeof(_lib.LstmStackT)] + [o for _, _, o in fields]

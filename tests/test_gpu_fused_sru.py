@@ -9,13 +9,14 @@ the discriminator's masks come from gantts_gan_step_seed as in test_gpu_fused_hi
 and gradient norms 2e-4 relative; post-step weights median |delta| < 5e-6 and max <= 0.0201 (a first Adagrad / Adam
 step moves a weight by lr * sign(g)).  The configuration-rule test is host-only (no mark).
 """
-import ctypes
-
 import numpy as np
 import pytest
 import torch
 
 from conftest import WINDOWS, TTS_HP, rel_err
+from fused_step_helpers import (adv_loss_with, check_weights, config_checker, d_masks, dev, fill_tables,  # noqa: F401
+                                loss_errors, make_batch, npy, ragged_lengths, resync_oracle, sd_numpy, step_config,
+                                step_hp, use_adam)
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
 
@@ -24,45 +25,6 @@ DURATION_HP = dict(stream_sizes=[5], has_dynamic_features=[False], adversarial_s
                    mask_nth_mgc_for_adv_loss=0, num_windows=1, discriminator_linguistic_condition=True)
 LOSS_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mge", "loss_mse", "loss_adv", "loss_g")
 TOL = 2e-4
-
-
-@pytest.fixture(scope="module")
-def dev():
-    import __graft_entry__
-    __graft_entry__.build()
-    return torch.device("cuda:0")
-
-
-def npy(t):
-    return t.detach().cpu().numpy()
-
-
-def step_hp(ohp):
-    from gantts_b200 import step as gstep
-    return gstep.HParams(windows=WINDOWS[:ohp["num_windows"]], stream_sizes=ohp["stream_sizes"],
-                         has_dynamic_features=ohp["has_dynamic_features"],
-                         adversarial_streams=ohp["adversarial_streams"],
-                         mask_nth_mgc_for_adv_loss=ohp["mask_nth_mgc_for_adv_loss"],
-                         discriminator_linguistic_condition=ohp["discriminator_linguistic_condition"])
-
-
-def ragged_lengths(B, T, seed):
-    rng = np.random.RandomState(seed)
-    return sorted([T] + [int(v) for v in rng.randint(T // 2, T, B - 1)], reverse=True)
-
-
-def make_batch(B, T, d_in, d_out, lens, seed):
-    g = torch.Generator().manual_seed(seed)
-    x = torch.randn(B, T, d_in, generator=g)
-    y = torch.randn(B, T, d_out, generator=g)
-    for b, n in enumerate(lens):
-        x[b, n:] = 0
-        y[b, n:] = 0
-    return x, y
-
-
-def sd_numpy(m):
-    return {k: v.detach().cpu().numpy() for k, v in m.state_dict().items()}
 
 
 def sru_models(seed, in_dim, out_dim, layers, hidden, bidir, relu, p, rnn_p, d_hidden, d_layers, d_p, n_adv):
@@ -125,53 +87,6 @@ def sru_masks(fs, mg, B, dev):
     return out
 
 
-def d_masks(fs, M, d_hidden, p, dev):
-    from gantts_b200 import ops, _lib
-    lib = _lib.load()
-    s = fs.last_seed
-    stacked = ops.mlp_dropout_masks(2 * M, d_hidden, p, lib.gantts_gan_step_seed(s, 1), dev)
-    return {"real": [m[:M].cpu() for m in stacked], "fake": [m[M:].cpu() for m in stacked],
-            "adv": [m.cpu() for m in ops.mlp_dropout_masks(M, d_hidden, p, lib.gantts_gan_step_seed(s, 2), dev)]}
-
-
-def adv_loss_with(md, x, ys_ref, lens, ohp, adv_masks):
-    """loss_adv of the oracle's y_hat_static through the PRODUCT's updated discriminator.  The adversarial forward runs
-    after the discriminator's first Adagrad / Adam step, which moves every weight by about lr * sign(g): a weight whose
-    gradient is within rounding of zero lands 2 lr apart in the two implementations, and at the conditioned D's 483
-    inputs those few weights move loss_adv by a few 1e-4.  With the product's D on both sides the comparison isolates
-    the generator's output and the loss arithmetic."""
-    ps = list(md.parameters())
-    layers = [(w.detach().cpu(), b.detach().cpu()) for w, b in zip(ps[0::2], ps[1::2])]
-    fake_in = gp.get_selected_static_stream(ys_ref, ohp)
-    if ohp["discriminator_linguistic_condition"]:
-        fake_in = torch.cat((x, fake_in), -1)
-    mask = gp.sequence_mask(lens, x.size(1)).unsqueeze(-1)
-    D = gp.mlp_forward(fake_in, layers, last_sigmoid=True, masks=adv_masks)
-    return float(gp.bce_real(D, mask, mask.sum().item()))
-
-
-def loss_errors(got, ref, keys):
-    return {k: abs(float(got[k]) - ref[k]) / max(abs(ref[k]), 1e-12) for k in keys}
-
-
-def check_weights(params, ref_params, tag):
-    for i, (q, r) in enumerate(zip(params, ref_params)):
-        d = np.abs(npy(q) - r.detach().numpy())
-        assert np.median(d) < 5e-6 and d.max() <= 0.0201, (tag, i, np.median(d), d.max())
-
-
-def resync(mg, md, fs, gen, d_layers, d_sum):
-    """Start the oracle's next step from the product's weights and Adagrad state."""
-    with torch.no_grad():
-        for r, q in zip(gen.params(), mg.parameters()):
-            r.copy_(q.detach().cpu())
-        for r, q in zip([t for pair in d_layers for t in pair], md.parameters()):
-            r.copy_(q.detach().cpu())
-        ng = len(gen.params())
-        for r, s in zip(gen.sums + d_sum, fs._sums[:ng] + fs._sums[ng:]):
-            r.copy_(s.cpu())
-
-
 def run_vs_oracle(dev, mg, md, ohp, B, T, steps, mse_w, p_d, d_hidden, seed, tag, with_outputs=True):
     from gantts_b200 import fused
     in_dim = mg.gru.rnn_lst[0].n_in
@@ -199,8 +114,8 @@ def run_vs_oracle(dev, mg, md, ohp, B, T, steps, mse_w, p_d, d_hidden, seed, tag
             errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), ys_ref.numpy())
         assert max(errs.values()) < TOL, (tag, it, errs)
         assert abs(got["real_correct"] - ref["real_correct"]) <= 3 and abs(got["fake_correct"] - ref["fake_correct"]) <= 3
-        check_weights(list(mg.parameters()), gen.params(), "%s step %d" % (tag, it))
-        resync(mg, md, fs, gen, d_layers, d_sum)
+        check_weights(mg, gen.named, "%s step %d" % (tag, it))
+        resync_oracle(fs, mg, md, gen, [t for pair in d_layers for t in pair], d_sum)
     return fs
 
 
@@ -263,14 +178,9 @@ def test_fused_sru_tts_duration_adam_and_resume(dev):
         errs["y_hat"] = rel_err(npy(fs.y_hat), yh_ref.numpy())
         errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), ys_ref.numpy())
         assert max(errs.values()) < TOL, (it, errs)
-        sd = fs.state_dict()
-        for mod, params, key, st in ((mg, gen.params(), "optimizer_g", g_opt), (md, d_params, "optimizer_d", d_opt)):
-            check_weights(list(mod.parameters()), params, "tts_duration %s step %d" % (key, it))
-            with torch.no_grad():
-                for i, (q, r) in enumerate(zip(mod.parameters(), params)):
-                    r.copy_(q.detach().cpu())
-                    st.m[i].copy_(sd[key]["state"][i]["exp_avg"].cpu())
-                    st.v[i].copy_(sd[key]["state"][i]["exp_avg_sq"].cpu())
+        check_weights(mg, gen.named, "tts_duration optimizer_g step %d" % it)
+        check_weights(md, dict(zip([n for n, _ in md.named_parameters()], d_params)), "tts_duration optimizer_d step %d" % it)
+        resync_oracle(fs, mg, md, gen, d_params, None, g_opt, d_opt)
     snap = [q.detach().clone() for q in list(mg.parameters()) + list(md.parameters())]
     sd = fs.state_dict()
     lens = ragged_lengths(B, T, 60)
@@ -400,83 +310,52 @@ def test_fused_sru_rejects_sigmoid_output(dev):
 
 
 def _sru_step_config():
-    """A valid SRURNN configuration of gantts_gan_step_t on the tts_acoustic layout with a conditioned D (host pointers
-    are placeholders: only the configuration check and the workspace layout run)."""
-    from gantts_b200 import _lib, multistream, step as gstep
-    fake, in_dim, hidden, nl = 1 << 20, 40, 16, 3
-    c = _lib.GanStepT()
-    c.B, c.T = 2, 16
-    c.g.num_layers = 1
-    c.g.dims[0], c.g.dims[1] = 2 * hidden, 187
-    c.d.num_layers = 2
-    for i, v in enumerate((in_dim + 58, 32, 1)):
-        c.d.dims[i] = v
-    for m in (c.g, c.d):
-        for i in range(m.num_layers):
-            m.W[i] = m.b[i] = fake
-    c.g_sumW[0] = c.g_sumb[0] = fake
-    c.g.last_act, c.d.last_act = _lib.ACT_NONE, _lib.ACT_SIGMOID
+    """A valid SRURNN configuration of gantts_gan_step_t on the tts_acoustic layout with a conditioned D: 3 bidirectional
+    layers of 16 over in_dim 40, hidden2out 32 -> 187, D 40 + 58 -> 32 -> 1 (host pointers are placeholders: only the
+    configuration check and the workspace layout run)."""
+    from gantts_b200 import multistream, step as gstep
+    in_dim, hidden, nl = 40, 16, 3
     hp = gstep.TTS_ACOUSTIC
     entries, n_static = multistream.mlpg_stream_entries(hp.stream_sizes, hp.has_dynamic_features, [True] * 4, 3)
-    c.streams = _lib.make_streams(entries)
-    c.windows = _lib.make_windows(WINDOWS)
-    c.mlpg_table = fake
-    c.n_static = c.n_static_cols = n_static
-    for i in range(n_static):
-        c.static_cols[i] = i
-    c.n_adv = 58
-    for i in range(58):
-        c.adv_cols[i] = 2 + i
-    c.d_conditioned = 1
-    c.w_d, c.mge_w, c.adv_w, c.max_norm, c.lr_g, c.lr_d, c.eps = 1.0, 1.0, 1.0, 1.0, 0.01, 0.01, 1e-10
-    c.optimizer = _lib.OPT_ADAGRAD
+    c = step_config((2 * hidden, 187), (in_dim + 58, 32, 1), entries, range(n_static), range(2, 60), conditioned=True)
     s = c.sru
     s.num_layers, s.in_dim, s.hidden, s.bidirectional, s.act = nl, in_dim, hidden, 1, 2
     s.dropout, s.rnn_dropout = 0.2, 0.2
-    for i in range(nl):
-        s.W[i] = s.b[i] = s.sumW[i] = s.sumb[i] = fake
-    return c
+    return fill_tables(c, 2 * nl + 2)
 
 
-def test_sru_step_config_rules():
+def test_sru_step_config_rules_on_tensor_tables():
     """gantts_gan_step_workspace_bytes (host-only) accepts the SRURNN layout, lays out no SRU workspace without a stack,
-    and rejects, with a message naming the rule, every SRU configuration the step does not implement."""
-    import __graft_entry__
-    __graft_entry__.build()
+    and rejects, with a message naming the rule, every SRU configuration the step does not implement.  The generator's
+    table holds [weight, bias] of layers 0, 1, 2, then hidden2out's."""
     from gantts_b200 import _lib
+    ws, err, rejected = config_checker()
     lib = _lib.load()
-    ws = lambda c: lib.gantts_gan_step_workspace_bytes(ctypes.byref(c))
-    err = lambda: lib.gantts_last_error_string().decode()
-    assert lib.gantts_version() == 103
+    assert lib.gantts_version() == 104
     c = _sru_step_config()
     assert ws(c) > 0, err()
     with_sru = ws(c)
     c.sru.num_layers = 0                                # the same config without a stack: D then sees g.dims[0] columns
     c.d.dims[0] = 32 + 58
+    c.g_tensors.n = 2
     assert 0 < ws(c) < with_sru, err()
 
-    def rejected(mutate, needle):
-        c = _sru_step_config()
-        mutate(c)
-        assert ws(c) == 0 and needle in err(), (needle, err())
-    rejected(lambda c: setattr(c.highway, "static_dim", 59), "mutually exclusive")
-    rejected(lambda c: setattr(c.sru, "num_layers", _lib.MAX_SRU_LAYERS + 1), "SRU layer count")
-    rejected(lambda c: setattr(c.sru, "num_layers", -1), "SRU layer count")
-    rejected(lambda c: setattr(c.sru, "act", 3), "activation")
-    rejected(lambda c: setattr(c.sru, "dropout", 1.0), "dropout")
-    rejected(lambda c: setattr(c.sru, "rnn_dropout", -0.1), "dropout")
-    rejected(lambda c: c.g.dims.__setitem__(0, 31), "hidden2out")
-    rejected(lambda c: setattr(c.g, "num_layers", 2), "hidden2out")
-    rejected(lambda c: c.sru.W.__setitem__(2, None), "null SRU weight")
-    rejected(lambda c: c.sru.b.__setitem__(0, None), "null SRU weight")
-    rejected(lambda c: c.sru.sumb.__setitem__(1, None), "optimiser state")
-
-    def adam(c):                                         # exp_avg_sq for every SRU layer but the last
-        c.optimizer, c.beta1, c.beta2 = _lib.OPT_ADAM, 0.5, 0.9
-        for i in range(c.sru.num_layers - 1):
-            c.sru.sqW[i] = c.sru.sqb[i] = 1 << 20
-    rejected(adam, "exp_avg_sq for SRU layer 2")
-    rejected(lambda c: c.d.dims.__setitem__(0, 32 + 58), "discriminator input width")
+    def rej(mutate, needle):
+        rejected(_sru_step_config, mutate, needle)
+    rej(lambda c: setattr(c.highway, "static_dim", 59), "mutually exclusive")
+    rej(lambda c: setattr(c.sru, "num_layers", _lib.MAX_SRU_LAYERS + 1), "SRU layer count")
+    rej(lambda c: setattr(c.sru, "num_layers", -1), "SRU layer count")
+    rej(lambda c: setattr(c.sru, "act", 3), "activation")
+    rej(lambda c: setattr(c.sru, "dropout", 1.0), "dropout")
+    rej(lambda c: setattr(c.sru, "rnn_dropout", -0.1), "dropout")
+    rej(lambda c: c.g.dims.__setitem__(0, 31), "hidden2out")
+    rej(lambda c: setattr(c.g, "num_layers", 2), "hidden2out")
+    rej(lambda c: c.g_tensors.param.__setitem__(4, None), "null generator tensor 4")        # layer 2's weight
+    rej(lambda c: c.g_tensors.param.__setitem__(1, None), "null generator tensor 1")        # layer 0's bias
+    rej(lambda c: c.g_tensors.state.__setitem__(3, None), "null generator optimiser state of tensor 3")
+    rej(lambda c: setattr(c.sru, "num_layers", 2), "generator table has 8 tensors, its shapes give 6")
+    rej(lambda c: use_adam(c, missing=(4, 5)), "exp_avg_sq for generator tensor 4")           # layer 2's
+    rej(lambda c: c.d.dims.__setitem__(0, 32 + 58), "discriminator input width")
     # the seeds of the SRU masks are a stream of their own
     seeds = {lib.gantts_sru_mask_seed(5, l, w) for l in range(8) for w in range(2)}
     assert len(seeds) == 16 and not seeds & {lib.gantts_gan_step_seed(5, w) for w in range(3)}

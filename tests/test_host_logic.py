@@ -219,23 +219,28 @@ def test_distortion_struct_matches_header():
     assert names == [f for f, _ in _lib.DistortionColsT._fields_]
 
 
-def test_gan_step_struct_layout_matches_header(tmp_path):
-    """ctypes mirror of gantts_gan_step_t against the C compiler's view of include/gantts_b200.h: total size and the
-    offsets of the first / middle / last fields (incl. the optimiser block appended in round 2)."""
+def test_gan_step_struct_every_field_matches_header(tmp_path):
+    """ctypes mirror of gantts_gan_step_t and of the blocks it holds against the C compiler's view of
+    include/gantts_b200.h: the size of each struct and the offset of every field."""
     import ctypes
     import subprocess
     from gantts_b200 import _lib
-    fields = ["B", "g", "d", "g_sumW", "streams", "windows", "mlpg_table", "n_static", "static_cols", "adv_cols", "lr_g", "adv_w",
-              "optimizer", "beta1", "opt_step", "g_sqW", "d_sqb"]
+    structs = [("gantts_gan_step_t", _lib.GanStepT), ("gantts_step_tensors_t", _lib.StepTensorsT),
+               ("gantts_highway_t", _lib.HighwayT), ("gantts_sru_stack_t", _lib.SruStackT),
+               ("gantts_lstm_stack_t", _lib.LstmStackT), ("gantts_mlp_t", _lib.MlpT)]
+    lines, want = [], []
+    for cname, ct in structs:
+        lines.append('  printf(" %%zu", sizeof(%s));\n' % cname)
+        want.append(ctypes.sizeof(ct))
+        for f, _ in ct._fields_:
+            lines.append('  printf(" %%zu", offsetof(%s, %s));\n' % (cname, f))
+            want.append(getattr(ct, f).offset)
     src = tmp_path / "layout.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "gantts_b200.h"\nint main(void) {\n'
-                   '  printf("%zu", sizeof(gantts_gan_step_t));\n' +
-                   "".join('  printf(" %%zu", offsetof(gantts_gan_step_t, %s));\n' % f for f in fields) +
+    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "gantts_b200.h"\nint main(void) {\n' + "".join(lines) +
                    "  return 0;\n}\n")
     exe = tmp_path / "layout"
     subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), "-o", str(exe), str(src)], check=True)
     got = [int(v) for v in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
-    want = [ctypes.sizeof(_lib.GanStepT)] + [getattr(_lib.GanStepT, f).offset for f in fields]
     assert got == want
 
 
