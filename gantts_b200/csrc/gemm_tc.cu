@@ -696,11 +696,10 @@ static int launch_split(const float* src, int64_t rs, int64_t rows, int cols, co
 }
 
 // Output columns per tile: 64 or 128, as few column tiles as TC_MAX_BN allows, split evenly.
-static int pick_bn(int n, int cap_override = 0) {
-  const int cap = cap_override ? cap_override : TC_MAX_BN;
+static int pick_bn(int n) {
   int bn = (n + 63) / 64 * 64;
-  if (bn <= cap) return bn;
-  int tiles = (n + cap - 1) / cap;
+  if (bn <= TC_MAX_BN) return bn;
+  int tiles = (n + TC_MAX_BN - 1) / TC_MAX_BN;
   bn = ((n + tiles - 1) / tiles + 63) / 64 * 64;
   return bn;
 }
@@ -823,7 +822,7 @@ static int launch_bn(const CUtensorMap& mAh, const CUtensorMap& mAl, const CUten
 }
 
 // out[rows_a][cols_b] = epi(A * B^T)   (K-major planes A [rows_a][red], B [cols_b][red]).
-static int launch_gemm_kk_one(const Planes& A, const Planes& B, const EpiArgs& e, cudaStream_t st, int bn_cap = 0) {
+static int launch_gemm_kk(const Planes& A, const Planes& B, const EpiArgs& e, cudaStream_t st) {
   GemmParams p{};
   p.rows_a = A.rows;
   p.cols_b = (int)B.rows;
@@ -834,7 +833,7 @@ static int launch_gemm_kk_one(const Planes& A, const Planes& B, const EpiArgs& e
   }
   p.a_plane = TC_BM * 128u;
   p.red_chunk = (p.red + TC_KK_BK - 1) / TC_KK_BK * TC_KK_BK;
-  p.bn = pick_bn(p.cols_b, bn_cap);
+  p.bn = pick_bn(p.cols_b);
   p.num_a = (int)((p.rows_a + TC_BM - 1) / TC_BM);
   p.num_b = (p.cols_b + p.bn - 1) / p.bn;
   p.num_z = 1;
@@ -857,55 +856,6 @@ static int launch_gemm_kk_one(const Planes& A, const Planes& B, const EpiArgs& e
   }
   set_error("gemm_kk: bad epilogue %d", e.epi);
   return GANTTS_E_BADARG;
-}
-
-// Tail balancing, OPT-IN (GANTTS_B200_TAIL=1).  Each SM works through whole tiles, so a launch takes whole rounds
-// of tiles.  The rows of an incomplete last wave are cut off and given to a SECOND launch with narrower column tiles
-// (BN/2) so that they spread over more SMs.  The extra launch's fill and drain usually cost more than the part of a
-// wave it saves, so it stays off.
-static int use_tail() {
-  const char* e = getenv("GANTTS_B200_TAIL");
-  return e ? atoi(e) : 0;
-}
-
-static int launch_gemm_kk(const Planes& A, const Planes& B, const EpiArgs& e, cudaStream_t st) {
-  if (use_tail()) {
-    const int N = (int)B.rows;
-    const int bn = pick_bn(N);
-    const int num_b = (N + bn - 1) / bn;
-    const int units = num_sms();
-    const int64_t row_tiles = (A.rows + TC_BM - 1) / TC_BM;
-    const int64_t tiles = row_tiles * num_b;
-    const int64_t rounds = tiles / units, rem = tiles % units;
-    if (rounds >= 1 && rem > 0 && bn >= 128 && bn % 128 == 0) {
-      const double frac = (double)rem / units;
-      int best_k = 1;
-      double best = 1.0;
-      for (int k = 2; k <= 4; k *= 2) {
-        if (bn / k < 64) break;
-        const double cost = ceil(k * frac - 1e-9) / k + 0.04;        // + the second launch's fill/drain
-        if (cost < best) { best = cost; best_k = k; }
-      }
-      const int64_t main_row_tiles = rounds * units / num_b;
-      const int64_t main_rows = main_row_tiles * TC_BM;
-      if (best_k > 1 && main_rows > 0 && main_rows < A.rows) {
-        Planes A1 = A, A2 = A;
-        A1.rows = main_rows;
-        A2.rows = A.rows - main_rows;
-        A2.hi += main_rows * A.pitch;
-        A2.lo += main_rows * A.pitch;
-        EpiArgs e2 = e;
-        e2.row0 = e.row0 + main_rows;
-        if (e2.C) e2.C += main_rows * e.ldc;
-        if (e2.out_hi) { e2.out_hi += main_rows * e.out_pitch; e2.out_lo += main_rows * e.out_pitch; }
-        if (e2.code) e2.code += main_rows * e.code_pitch;
-        int rc = launch_gemm_kk_one(A1, B, e, st);
-        if (rc) return rc;
-        return launch_gemm_kk_one(A2, B, e2, st, bn / best_k);
-      }
-    }
-  }
-  return launch_gemm_kk_one(A, B, e, st);
 }
 
 // C[n][k] (+)= sum_m A[m][n] * B[m][k]  (MN-major planes A [red][rows_a], B [red][cols_b]);

@@ -436,6 +436,8 @@ gemv_partial_reduce_kernel(const float* __restrict__ partial, int blocks, int K,
 constexpr int GEMV_BLOCKS = 132 * 2;
 
 constexpr int MLP_COLSUM_CHUNKS = 128;
+// The backward walks down the stack with two gradient plane buffers, writing one while it reads the other.
+constexpr int MLP_GRAD_BUFS = 2;
 
 static int colsum_planes(const Planes& G, float* gb, int accumulate, float* partial, cudaStream_t st) {
   int chunks = MLP_COLSUM_CHUNKS;
@@ -512,8 +514,7 @@ extern "C" size_t gantts_mlp_workspace_bytes(const gantts_mlp_t* m, int64_t M) {
   for (int l = 0; l <= m->num_layers; ++l) maxd = m->dims[l] > maxd ? m->dims[l] : maxd;
   for (int l = 0; l < m->num_layers; ++l)       // one partial region per layer: reductions are deferred
     part += mn_partial_bytes(M, m->dims[l + 1], m->dims[l], nullptr, nullptr) + 256;
-  const int nbuf = chain_shape_ok(m, CHAIN_BWD_GRAD) && m->num_layers - 1 > 2 ? m->num_layers - 1 : 2;   // gradient plane buffers
-  return (size_t)2 * nbuf * plane_bytes(M, maxd) + part + (size_t)MLP_COLSUM_CHUNKS * maxd * sizeof(float) +
+  return (size_t)2 * MLP_GRAD_BUFS * plane_bytes(M, maxd) + part + (size_t)MLP_COLSUM_CHUNKS * maxd * sizeof(float) +
          (size_t)GEMV_BLOCKS * (GEMV_MAX_K + 1) * sizeof(float) + 4096;
 }
 
@@ -579,42 +580,6 @@ static int gantts::mlp_fwd_impl(const gantts_mlp_t* m, const float* x, int64_t x
     if (nb < 1) nb = 1;
     GANTTS_PDL_LAUNCH((split_weights_kernel), nb, 256, 0, st, wl);
     GANTTS_LAUNCH_CHECK("split_weights_kernel");
-  }
-  if (chain_shape_ok(m, CHAIN_FWD)) {
-    // narrow stack with a single output (the discriminator): ONE launch, activations stay on chip between layers
-    ChainParams cp{};
-    cp.M = M;
-    cp.num_layers = L - 1;
-    cp.slope = m->slope;
-    cp.keep_scale = m->dropout_p > 0.f ? 1.f / (1.f - m->dropout_p) : 1.f;
-    cp.thresh = m->dropout_p > 0.f ? (uint32_t)(m->dropout_p * 65536.f + 0.5f) : 0u;
-    cp.x_hi = t.H[0].hi;
-    cp.x_lo = t.H[0].lo;
-    cp.x_pitch = t.H[0].pitch;
-    cp.x_valid = m->dims[0];
-    for (int l = 0; l < L - 1; ++l) {
-      ChainLayer& cl = cp.L[l];
-      cl.N = pad64(m->dims[l + 1]);
-      cl.n_valid = m->dims[l + 1];
-      cl.K = pad64(m->dims[l]);
-      cl.k_valid = m->dims[l];
-      cl.w_hi = t.W[l].hi;
-      cl.w_lo = t.W[l].lo;
-      cl.w_pitch = t.W[l].pitch;
-      cl.bias = m->b[l];
-      cl.s_hi = t.H[l + 1].hi;                   // tape: H_{l+1} planes for the backward
-      cl.s_lo = t.H[l + 1].lo;
-      cl.s_pitch = t.H[l + 1].pitch;
-      cl.code = t.code[l + 1];
-      cl.code_pitch = t.code_pitch[l + 1];
-      cl.seed = layer_seed(m->seed, l);
-    }
-    cp.w_last = m->W[L - 1];
-    cp.b_last = m->b[L - 1];
-    cp.y = y;
-    cp.y_rs = y_rs;
-    cp.sigmoid = m->last_act == GANTTS_ACT_SIGMOID ? 1 : 0;
-    return launch_chain<false>(cp, st);
   }
   for (int l = 0; l < L; ++l) {
     EpiArgs e;
@@ -721,12 +686,8 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
   int maxd = 0;
   for (int l = 0; l <= L; ++l) maxd = m->dims[l] > maxd ? m->dims[l] : maxd;
   char* cur = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(workspace) + 255) / 256 * 256);
-  bool any_grad = false;
-  for (int l = 0; l < L; ++l) any_grad |= (gW && gW[l]) || (gb && gb[l]);
-  const bool chain = chain_shape_ok(m, any_grad ? CHAIN_BWD_GRAD : CHAIN_BWD_NOGRAD);
-  const int nbuf = chain_shape_ok(m, CHAIN_BWD_GRAD) && L - 1 > 2 ? L - 1 : 2;
-  char* gbuf[GANTTS_MAX_LAYERS];
-  for (int i = 0; i < nbuf; ++i) {
+  char* gbuf[MLP_GRAD_BUFS];
+  for (int i = 0; i < MLP_GRAD_BUFS; ++i) {
     gbuf[i] = cur;
     cur += 2 * plane_bytes(M, maxd);
   }
@@ -737,95 +698,6 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
 
   float* gemv_part = reinterpret_cast<float*>(partial_cur);
   partial_cur += ((size_t)GEMV_BLOCKS * (GEMV_MAX_K + 1) * sizeof(float) + 255) / 256 * 256;
-  if (chain) {
-    // dims[L] == 1, >= 2 hidden layers.  gW/gb of the single-output layer come from the GEMV backward kernel (it
-    // also leaves the head gradient planes gZ_{L-2} for the weight-gradient GEMM); the chain kernel recomputes the
-    // head on chip, walks gZ_{l-1} = (gZ_l W_l) * act'(H_l) down to the input gradient and writes the gradient
-    // planes the remaining weight-gradient GEMMs read.
-    const int Lh = L - 1;                      // hidden layers = MLP linear layers 0..Lh-1 in front of the GEMV
-    const bool want_w = gW != nullptr;
-    bool any_w = false;
-    for (int l = 0; l < L; ++l) any_w |= (gW && gW[l]) || (gb && gb[l]);
-    const float ks = m->dropout_p > 0.f ? 1.f / (1.f - m->dropout_p) : 1.f;
-    Planes Gl[GANTTS_MAX_LAYERS];              // Gl[l] = gradient planes w.r.t. the output of linear layer l
-    for (int l = 0; l < Lh; ++l) {
-      char* c = gbuf[l];
-      Gl[l] = carve_planes(c, M, m->dims[l + 1]);
-    }
-    float* gemv_part0 = gemv_part;
-    const int K1 = m->dims[Lh];
-    const bool want_last = (gW && gW[L - 1]) || (gb && gb[L - 1]);
-    if (any_w) {
-      // head planes (needed by gW of layer Lh-1) + gW/gb of the GEMV layer
-#define GANTTS_GEMV_BWD_ARGS2                                                                                    \
-  gy, gy_rs, y, y_rs, t.H[Lh].hi, t.H[Lh].lo, t.H[Lh].pitch, t.code[Lh], t.code_pitch[Lh], m->W[L - 1],         \
-      Gl[Lh - 1].hi, Gl[Lh - 1].lo, Gl[Lh - 1].pitch, gemv_part0, M, K1, m->last_act == GANTTS_ACT_SIGMOID ? 1 : 0, ks, \
-      m->slope * ks, m->dropout_p > 0.f ? 0.f : m->slope, want_last ? 1 : 0
-      if (K1 % 8 == 0 && K1 <= 256)
-        GANTTS_PDL_LAUNCH((gemv_bwd_vec_kernel<1, 4>), GEMV_BLOCKS, GEMV_THREADS, 0, st, GANTTS_GEMV_BWD_ARGS2);
-      else
-        gemv_bwd_kernel<<<GEMV_BLOCKS, GEMV_THREADS, 0, st>>>(GANTTS_GEMV_BWD_ARGS2);
-#undef GANTTS_GEMV_BWD_ARGS2
-      GANTTS_LAUNCH_CHECK("gemv_bwd_kernel");
-      if (want_last) {
-        GANTTS_PDL_LAUNCH((gemv_partial_reduce_kernel), (K1 + 1 + 31) / 32, 256, 0, st, gemv_part0, GEMV_BLOCKS, K1,
-                                                                      gW ? gW[L - 1] : nullptr,
-                                                                      gb ? gb[L - 1] : nullptr, accumulate);
-        GANTTS_LAUNCH_CHECK("gemv_partial_reduce_kernel");
-      }
-    }
-    ChainParams cp{};
-    cp.M = M;
-    cp.num_layers = Lh;                          // chain layer i applies W of MLP layer Lh-1-i
-    cp.slope = m->slope;
-    cp.keep_scale = ks;
-    cp.thresh = m->dropout_p > 0.f ? (uint32_t)(m->dropout_p * 65536.f + 0.5f) : 0u;
-    cp.gy = gy;
-    cp.gy_rs = gy_rs;
-    cp.yv = m->last_act == GANTTS_ACT_SIGMOID ? y : nullptr;
-    cp.yv_rs = y_rs;
-    cp.w_head = m->W[L - 1];
-    cp.head_valid = K1;
-    cp.code_head = t.code[Lh];
-    cp.code_head_pitch = t.code_pitch[Lh];
-    for (int i = 0; i < Lh; ++i) {
-      const int ml = Lh - 1 - i;                 // MLP layer whose transposed weights this chain layer multiplies by
-      ChainLayer& cl = cp.L[i];
-      cl.N = pad64(m->dims[ml]);
-      cl.n_valid = m->dims[ml];
-      cl.K = pad64(m->dims[ml + 1]);
-      cl.k_valid = m->dims[ml + 1];
-      cl.w_hi = t.Wt[ml].hi;
-      cl.w_lo = t.Wt[ml].lo;
-      cl.w_pitch = t.Wt[ml].pitch;
-      if (ml >= 1) {
-        cl.code = t.code[ml];
-        cl.code_pitch = t.code_pitch[ml];
-        if ((gW && gW[ml - 1]) || (gb && gb[ml - 1])) {   // gradient planes for the weight-gradient GEMM of layer ml-1
-          cl.s_hi = Gl[ml - 1].hi;
-          cl.s_lo = Gl[ml - 1].lo;
-          cl.s_pitch = Gl[ml - 1].pitch;
-        }
-      }
-    }
-    cp.C = gx ? gx + gx_row0 * gx_rs : nullptr;
-    cp.ldc = gx_rs;
-    cp.c_row0 = gx_row0;
-    cp.c_accumulate = gx_accumulate;
-    if ((rc = launch_chain<true>(cp, st))) return rc;
-    (void)want_w;
-    for (int l = Lh - 1; l >= 0; --l) {
-      float* gbl = (gb && gb[l]) ? gb[l] : nullptr;
-      if (gW && gW[l]) {
-        float* partial = reinterpret_cast<float*>(partial_cur);
-        partial_cur += mn_partial_bytes(M, m->dims[l + 1], m->dims[l], nullptr, nullptr) + 256;
-        if ((rc = launch_gemm_mn(Gl[l], t.H[l], gW[l], gbl, accumulate, partial, st, &rl))) return rc;
-      } else if (gbl) {
-        if ((rc = colsum_planes(Gl[l], gbl, accumulate, colpart, st))) return rc;
-      }
-    }
-    return flush_reduce(rl, accumulate, st);
-  }
   int pp = 0;
   int l_start = L - 1;
   char* c0 = gbuf[pp];

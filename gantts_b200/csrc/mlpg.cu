@@ -677,7 +677,7 @@ static SolveGrid solve_grid(int B, int T, int ncols) {
 }
 
 // which: 1 = forward, 2 = backward.  GANTTS_B200_MLPG_SOLVE is a bit mask of the directions that use the substitution
-// kernels (default 2: the backward uses the substitution kernels, the forward the FIR kernels).
+// kernels (default 3: both directions use them; the FIR kernels remain for windows wider than +-2 frames).
 static bool solve_taps(const gantts_windows_t* win, SolveTaps* tp, int which) {
   int hb = 0;
   tp->nw = win->n;

@@ -1,6 +1,6 @@
 """Where the drop-in path (tests/trainpy_mirror.train_step on the `gantts` alias, cfg2) spends its HOST time: cProfile of 20
 steps (top entries by cumulative and by own time) + GPU-busy time of the same steps from CUDA events with the host syncs
-removed (the modular GanTrainer.step, which has none).  Output: markdown on stdout (kept as profiles/r02_dropin.md)."""
+removed (the modular GanTrainer.step, which has none).  Output: markdown on stdout."""
 import cProfile
 import io
 import os

@@ -1,6 +1,6 @@
 """Same-box library bar for the recurrent generators (SURVEY.md 2.2 K8): torch-CUDA nn.LSTM (cuDNN) forward + backward at
 the BASELINE cfg3 / cfg5 shapes next to gantts_b200.rnn.lstm_forward on the same weights and inputs.  CUDA events,
-3 warm-ups + 5 timed iterations.  Prints one markdown table (copied into profiles/r02_lstm_vs_cudnn.md)."""
+3 warm-ups + 5 timed iterations.  Prints one markdown table."""
 import os
 import sys
 

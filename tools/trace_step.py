@@ -5,7 +5,7 @@
 Runs `--warmup` fused steps, then `--steps` more under the profiler with a synchronise after each, and splits the
 kernel list into steps (every step launches the same kernels).  Writes the launch list of the middle step in launch
 order with each kernel's duration.  The tensor-core GEMM launches are labelled with their shapes (the per-kind launch
-order in tools/per_launch.py) and get their executed TFLOP/s (3 x 2MNK for the bf16x3 split) and share of the step.
+order in KK and MN below) and get their executed TFLOP/s (3 x 2MNK for the bf16x3 split) and share of the step.
 Tracing adds host overhead between launches, so the step span here is not a bench value; compare kernel times and
 shares, and take step times from bench.py.
 """
@@ -17,9 +17,26 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 import bench  # noqa: E402
-from per_launch import KK, MN  # noqa: E402
+
+M = 32000
+# K-major launches (y = x W^T or gx = gz W) and MN-major launches (gW = gz^T x) of one step, in launch order per kind:
+# (label, rows, N, K, output kind)
+KK = [("G fwd 425->512 (+act, planes)", M, 512, 425, "planes"), ("G fwd 512->512", M, 512, 512, "planes"),
+      ("G fwd 512->512", M, 512, 512, "planes"), ("G fwd 512->187 (fp32 y_hat, ld 187)", M, 187, 512, "f32"),
+      ("D fwd 58->256, real|fake 2M rows", 2 * M, 256, 58, "planes"), ("D fwd 256->256, 2M rows", 2 * M, 256, 256, "planes"),
+      ("D fwd 256->256, 2M rows", 2 * M, 256, 256, "planes"),
+      ("D bwd gx3 = gz W", 2 * M, 256, 256, "planes"), ("D bwd gx2", 2 * M, 256, 256, "planes"),
+      ("D bwd gx1 (fake half, fp32, ld 58)", M, 58, 256, "f32"),
+      ("D(adv) fwd 58->256, M rows", M, 256, 58, "planes"), ("D(adv) fwd 256->256", M, 256, 256, "planes"),
+      ("D(adv) fwd 256->256", M, 256, 256, "planes"),
+      ("D(adv) bwd gx3", M, 256, 256, "planes"), ("D(adv) bwd gx2", M, 256, 256, "planes"),
+      ("D(adv) bwd gx1 -> += g_static window (fp32)", M, 58, 256, "f32"),
+      ("G bwd gx4 = gz W (512 wide)", M, 512, 187, "planes"), ("G bwd gx3", M, 512, 512, "planes"),
+      ("G bwd gx2", M, 512, 512, "planes")]
+MN = [("D bwd gW3 = gz^T h (256x256)", 2 * M, 256, 256), ("D bwd gW2", 2 * M, 256, 256), ("D bwd gW1 (256x58)", 2 * M, 256, 58),
+      ("G bwd gW4 (187x512)", M, 187, 512), ("G bwd gW3 (512x512)", M, 512, 512), ("G bwd gW2 (512x512)", M, 512, 512),
+      ("G bwd gW1 (512x425)", M, 512, 425)]
 
 
 def short(name):
@@ -109,7 +126,7 @@ def main():
               % (sum(1 for r in rows if r[3] is not None), gemm_us, gemm_us / tot if tot else 0.0,
                  gemm_fl / (gemm_us * 1e-6) / 1e12 if gemm_us else 0.0)]
     if unmatched:
-        lines.append("%d GEMM labels unused: the launch structure differs from tools/per_launch.py." % unmatched)
+        lines.append("%d GEMM labels unused: the launch structure differs from the KK and MN lists." % unmatched)
     text = "\n".join(lines) + "\n"
     print(text)
     if args.out:
