@@ -162,6 +162,9 @@ SIGNATURES = {
     "gantts_gan_step_grad_buffer": (_i, [ctypes.POINTER(GanStepT), _vp, _i, ctypes.POINTER(ctypes.c_void_p),
                                          ctypes.POINTER(ctypes.c_int64)]),
     "gantts_gan_step": (_i, [ctypes.POINTER(GanStepT), _i, _vp, _vp, _vp, _f, _u64, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "gantts_spoof_count_workspace_bytes": (_sz, [ctypes.POINTER(MlpT), _i64]),
+    "gantts_spoof_count": (_i, [ctypes.POINTER(MlpT), _vp, _i, ctypes.POINTER(ctypes.c_int), _i, _vp, _i, _i, _vp, _vp,
+                                _sz, _vp]),
     "gantts_lstm_workspace_bytes": (_sz, []),
     "gantts_lstm_layer_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
     "gantts_lstm_layer_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
@@ -179,7 +182,7 @@ SIGNATURES = {
     "gantts_lstm_mask_seed": (_u64, [_u64, _i]),
 }
 
-STEP_D, STEP_G, STEP_FINISH, STEP_EVAL = 1, 2, 4, 8
+STEP_D, STEP_G, STEP_FINISH, STEP_EVAL, STEP_D_ONLY = 1, 2, 4, 8, 16
 
 
 def load():

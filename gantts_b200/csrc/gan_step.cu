@@ -121,6 +121,23 @@ __global__ void set_scales_kernel(float* scal, float inv_frames, float adv_w, fl
   }
 }
 
+// Spoofing-rate count of reference train.py:549-558: sum over valid frames of [D_ref > 0.5], row r = b * T + t valid
+// when t < lengths[b].  One block in a fixed order; every partial sum is an integer below 2^24, so the float is exact.
+// The count is STORED (count[0] = n), not accumulated.
+__global__ void __launch_bounds__(RED_THREADS)
+spoof_count_kernel(const float* __restrict__ Dv, const int64_t* __restrict__ lengths, int B, int T, float* __restrict__ count) {
+  pdl_entry();
+  __shared__ float sm[32];
+  float v[1] = {0.f};
+  const int64_t rows = (int64_t)B * T;
+  for (int64_t r = threadIdx.x; r < rows; r += RED_THREADS) {
+    const int64_t t = r % T;
+    if (t < lengths[r / T] && Dv[r] > 0.5f) v[0] += 1.f;
+  }
+  block_sum<1>(v, sm);
+  if (threadIdx.x == 0) count[0] = v[0];
+}
+
 // Deferred reductions: every loss kernel of the step leaves per-block partial sums in its own slot; the single
 // finalize kernel at the end of the step reduces all of them (deterministic: fixed block order) -- no per-loss
 // "finish" launch on the way.
@@ -1106,13 +1123,14 @@ struct Step {
   const HighwayArgs* hw() const { return c->highway.static_dim > 0 ? &hwa : nullptr; }
 };
 
-// batch prologue (train.py:528-535): sequence mask and loss scales
-static int step_prologue(const Step& s, float inv_frames, bool eval) {
+// batch prologue (train.py:528-535): sequence mask and loss scales.  zero_norms: a step that steps neither model (eval)
+// or only D (D_ONLY) reports 0 for the gradient norm it does not compute, never an earlier step's value.
+static int step_prologue(const Step& s, float inv_frames, bool zero_norms) {
   const gantts_gan_step_t* c = s.c;
   int rc = gantts_sequence_mask(s.lengths, s.L.mask, c->B, c->T, s.stream);
   if (rc) return rc;
   GANTTS_PDL_LAUNCH((set_scales_kernel), 1, 32, 0, s.st, s.L.scal, inv_frames, s.has_adv ? c->adv_w : 0.f, c->mge_w, c->mse_w,
-                    eval ? 1 : 0, s.lengths, c->B, c->T);
+                    zero_norms ? 1 : 0, s.lengths, c->B, c->T);
   GANTTS_LAUNCH_CHECK("set_scales_kernel");
   return GANTTS_OK;
 }
@@ -1242,19 +1260,20 @@ static int discriminator_fwd(Step& s, bool stacked) {
 // g_static.  stacked: loss_d.backward() on the [real | fake] batch, with D's parameter gradients; otherwise the
 // adversarial batch, input gradient only.  When the adversarial columns form one window of y_hat_static the last GEMM
 // adds its result straight into g_static (the scatter of the column gather's backward); otherwise it goes to g_din and a
-// scatter kernel follows.
-static int discriminator_bwd(Step& s, bool stacked) {
+// scatter kernel follows.  input_grad = false (the D-only step, where nothing consumes dL/dy_hat_static): parameter
+// gradients alone.
+static int discriminator_bwd(Step& s, bool stacked, bool input_grad = true) {
   const StepLayout& L = s.L;
   const int64_t M = s.M, skip = stacked ? M : 0;      // the real rows' input gradient is not needed
   float* const* gW = stacked ? s.pd.gW : nullptr;
   float* const* gb = stacked ? s.pd.gb : nullptr;
   // in place: row r of the batch -> g_static[r - skip]
-  float* gx = s.adv_window ? L.g_static + s.adv_cols.c[0] - skip * (int64_t)s.nS : L.g_din;
+  float* gx = !input_grad ? nullptr : (s.adv_window ? L.g_static + s.adv_cols.c[0] - skip * (int64_t)s.nS : L.g_din);
   int rc;
   if ((rc = mlp_bwd_impl(&s.d, L.g_dout, 1, L.d_out, 1, skip + M, L.d_tape, L.d_tape_bytes, gx, s.adv_window ? s.nS : s.dD,
                          skip, gW, gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, s.adv_window ? 1 : -1)))
     return rc;
-  if (s.adv_window) return GANTTS_OK;
+  if (s.adv_window || !input_grad) return GANTTS_OK;
   scatter_cols_list_add_kernel<<<blocks_1d(M * s.nA, 1024), 256, 0, s.st>>>(L.g_din + skip * s.dD + s.cond_w, s.dD,
                                                                              L.g_static, s.nS, s.adv_cols, M);
   GANTTS_LAUNCH_CHECK("scatter_cols_list_add_kernel");
@@ -1301,6 +1320,14 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
                                void* stream) {
   int rc = check_step(c);
   if (rc) return rc;
+  // the discriminator warm-up (train.py --discriminator-warmup, :696 update_g = False): D steps, G is left alone
+  const bool d_only = (phases & GANTTS_STEP_D_ONLY) != 0;
+  if (d_only) {
+    GANTTS_CHECK_ARG(!(phases & GANTTS_STEP_EVAL),
+                     "gan_step: GANTTS_STEP_D_ONLY cannot be combined with GANTTS_STEP_EVAL (the test phase updates nothing)");
+    GANTTS_CHECK_ARG(c->w_d > 0.f, "gan_step: GANTTS_STEP_D_ONLY trains the discriminator and needs w_d > 0 (got %g)",
+                     (double)c->w_d);
+  }
   GANTTS_CHECK_ARG(x && y && lengths_dev && y_hat && y_hat_static && losses_dev, "gan_step: null pointer");
   size_t need = gantts_gan_step_workspace_bytes(c);
   if (!workspace || workspace_bytes < need) {
@@ -1325,7 +1352,7 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
   s.dD = c->d.dims[0];
   const int nS = s.nS = c->n_static;
   s.has_d = c->w_d > 0.f;
-  s.has_adv = s.has_d && c->adv_w > 0.f;
+  s.has_adv = s.has_d && c->adv_w > 0.f && !d_only;
   // discriminator_linguistic_condition (train.py:254-256,302-303): D sees cat((x, y_adv), -1); the first cond_w columns
   // of both halves of d_in are copies of x, the gradient w.r.t. them is discarded.
   s.cond_w = (s.has_d && c->d_conditioned) ? s.d_in : 0;
@@ -1387,12 +1414,16 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
 
   if (phases & 1) {
     NvtxRange r1("gantts_gan_step/phase1: G fwd, MLPG, MGE, D fwd+bwd");
-    if ((rc = step_prologue(s, inv_frames, false))) return rc;
+    if ((rc = step_prologue(s, inv_frames, d_only))) return rc;
     if ((rc = generator_fwd(s, true))) return rc;
     // MGE loss (train.py:291) and its gradient in one pass; the gradient INITIALISES g_static, the two discriminator
-    // passes then accumulate their input gradients on top of it
-    if ((rc = launch_sse(y_hat_static, nS, y, s.d_out, L.mask, M, nS, L.scal + S_MGE_SCALE, L.g_static, nS, &L.red[R_MGE],
-                         st, &s.static_cols)))
+    // passes then accumulate their input gradients on top of it.  D-only: forward values of MGE and MSE alone (the
+    // generator backward that would evaluate MSE does not run).
+    if ((rc = launch_sse(y_hat_static, nS, y, s.d_out, L.mask, M, nS, L.scal + S_MGE_SCALE, d_only ? nullptr : L.g_static, nS,
+                         &L.red[R_MGE], st, &s.static_cols)))
+      return rc;
+    if (d_only && (rc = launch_sse(y_hat, s.d_out, y, s.d_out, L.mask, M, s.d_out, L.scal + S_MSE_SCALE, nullptr, 0,
+                                   &L.red[R_MSE], st)))
       return rc;
     if (s.has_d) {
       // ---- update_discriminator (train.py:245-279)
@@ -1401,8 +1432,21 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
       // real and fake BCE terms, counts and dL/dD of both halves (train.py:262-270) in one launch
       if ((rc = launch_bce(L.d_out, L.mask, M, 2, 0, 1, L.scal + S_INV_T, L.g_dout, &L.red[R_REAL], &L.red[R_FAKE], st)))
         return rc;
-      if ((rc = discriminator_bwd(s, true))) return rc;
+      if ((rc = discriminator_bwd(s, true, !d_only))) return rc;
     }
+  }
+  if (d_only) {
+    // ---- update_generator is not called (train.py:562-566 with update_g = False): D's clip + optimiser step, then the
+    // loss scalars; no third D forward, no MLPG adjoint, no generator backward or step
+    if (phases & 2) {
+      NvtxRange r2("gantts_gan_step/phase2 (D only): D step");
+      if ((rc = clip_opt_model(c, s.pd, L.opt_partial, L.scal + S_DSUMSQ, c->lr_d, c->wd_d, st))) return rc;
+    }
+    if (phases & 4) {
+      NvtxRange r4("gantts_gan_step/phase4 (D only): losses");
+      return step_finalize(s, losses_dev);
+    }
+    return GANTTS_OK;
   }
   if (phases & 2) {
     NvtxRange r2("gantts_gan_step/phase2: D step, adv D fwd+bwd, MLPG bwd, G bwd");
@@ -1425,5 +1469,66 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
     if ((rc = clip_opt_model(c, s.pg, L.opt_partial, L.scal + S_GSUMSQ, c->lr_g, c->wd_g, st))) return rc;
     return step_finalize(s, losses_dev);
   }
+  return GANTTS_OK;
+}
+
+// ---- spoofing-rate count (train.py:549-558): D_ref on the adversarial columns of y_hat_static, dropout off
+// (train.py:445), no conditioning (train.py:554-555), no gradient.  Workspace: D_ref's tape, then its output [rows].
+static int check_spoof_d(const gantts_mlp_t* d, int64_t rows) {
+  GANTTS_CHECK_ARG(d, "spoof_count: null reference discriminator");
+  GANTTS_CHECK_ARG(d->num_layers >= 1 && d->num_layers <= GANTTS_MAX_LAYERS, "spoof_count: bad layer count %d", d->num_layers);
+  GANTTS_CHECK_ARG(d->dims[d->num_layers] == 1 && d->last_act == GANTTS_ACT_SIGMOID,
+                   "spoof_count: the reference discriminator must end in a single sigmoid output");
+  GANTTS_CHECK_ARG(rows >= 1 && rows < (1 << 24),
+                   "spoof_count: B * T = %lld frames, the float count is exact below 2^24", (long long)rows);
+  return GANTTS_OK;
+}
+
+extern "C" size_t gantts_spoof_count_workspace_bytes(const gantts_mlp_t* d, int64_t rows) {
+  if (check_spoof_d(d, rows)) return 0;
+  return al256(gantts_mlp_tape_bytes(d, rows)) + al256((size_t)rows * sizeof(float)) + 256;
+}
+
+extern "C" int gantts_spoof_count(const gantts_mlp_t* d, const float* y_hat_static, int n_static, const int* adv_cols,
+                                  int n_adv, const int64_t* lengths_dev, int B, int T, float* count_dev, void* ws,
+                                  size_t ws_bytes, void* stream) {
+  GANTTS_CHECK_ARG(B >= 1 && T >= 1, "spoof_count: bad batch shape");
+  const int64_t rows = (int64_t)B * T;
+  int rc = check_spoof_d(d, rows);
+  if (rc) return rc;
+  GANTTS_CHECK_ARG(y_hat_static && adv_cols && lengths_dev && count_dev, "spoof_count: null pointer");
+  GANTTS_CHECK_ARG(n_adv >= 1 && n_adv <= GANTTS_MAX_COLS && n_adv == d->dims[0],
+                   "spoof_count: %d adversarial columns != reference discriminator input width %d (it gets no "
+                   "linguistic conditioning, train.py:554-555)", n_adv, d->dims[0]);
+  GANTTS_CHECK_ARG(n_static >= 1, "spoof_count: bad n_static");
+  ColList cols;
+  cols.n = n_adv;
+  for (int i = 0; i < n_adv; ++i) {
+    GANTTS_CHECK_ARG(adv_cols[i] >= 0 && adv_cols[i] < n_static, "spoof_count: adversarial column %d out of range",
+                     adv_cols[i]);
+    cols.c[i] = adv_cols[i];
+  }
+  const size_t need = gantts_spoof_count_workspace_bytes(d, rows);
+  if (!ws || ws_bytes < need) {
+    set_error("spoof_count: workspace too small (%zu < %zu)", ws_bytes, need);
+    return GANTTS_E_WORKSPACE;
+  }
+  gantts_mlp_t m = *d;
+  m.dropout_p = 0.f;
+  char* base = reinterpret_cast<char*>(al256(reinterpret_cast<uintptr_t>(ws)));
+  const size_t tape_bytes = gantts_mlp_tape_bytes(&m, rows);
+  char* tape = base;
+  float* dout = reinterpret_cast<float*>(base + al256(tape_bytes));
+  const cudaStream_t st = as_stream(stream);
+  Planes din;
+  if ((rc = mlp_tape_input_planes(&m, rows, tape, tape_bytes, &din))) return rc;
+  ColList none;
+  none.n = 0;
+  GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(rows * n_adv, 1024), 256, 0, st, y_hat_static, (int64_t)n_static, cols,
+                    rows, nullptr, 0, none, 0, din.hi, din.lo, din.pitch);
+  GANTTS_LAUNCH_CHECK("gather_planes_kernel(spoof)");
+  if ((rc = mlp_fwd_impl(&m, nullptr, 0, rows, dout, 1, tape, tape_bytes, stream, true))) return rc;
+  GANTTS_PDL_LAUNCH((spoof_count_kernel), 1, RED_THREADS, 0, st, dout, lengths_dev, B, T, count_dev);
+  GANTTS_LAUNCH_CHECK("spoof_count_kernel");
   return GANTTS_OK;
 }

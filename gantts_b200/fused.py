@@ -86,12 +86,38 @@ def _fill_mlp(desc, layers, p, last_act):
     desc.slope, desc.dropout_p, desc.last_act, desc.seed = ops.LEAKY_SLOPE, float(p), int(last_act), 0
 
 
+def adversarial_columns(hp):
+    """Columns of y_hat_static the discriminator sees: get_selected_static_stream of reference train.py:232-242 (stream
+    select, then the first mask_nth_mgc_for_adv_loss columns dropped)."""
+    sizes = multistream.get_static_stream_sizes(hp.stream_sizes, hp.has_dynamic_features, len(hp.windows))
+    acols = multistream.select_stream_columns(sizes, hp.adversarial_streams)
+    if hp.mask_nth_mgc_for_adv_loss > 0:
+        acols = acols[hp.mask_nth_mgc_for_adv_loss:]
+    return [int(v) for v in acols]
+
+
+def check_reference_discriminator(model_ref, n_adv, who):
+    """The reference discriminator of the spoofing-rate count (train.py:549-558): an MLP with one sigmoid output whose
+    input is the n_adv adversarial columns alone."""
+    if not (hasattr(model_ref, "layers") and hasattr(model_ref, "last_linear")) or not model_ref.last_sigmoid:
+        raise RuntimeError("%s: the reference discriminator must be a sigmoid-output MLP" % who)
+    width = int(model_ref.layers[0].weight.shape[1] if len(model_ref.layers) else model_ref.last_linear.weight.shape[1])
+    if width != n_adv:
+        raise RuntimeError("%s: the reference discriminator takes %d inputs, but train.py:549-555 feeds it the %d "
+                           "adversarial columns alone (no linguistic conditioning)" % (who, width, n_adv))
+
+
 class FusedGanStep(object):
     def __init__(self, model_g, model_d, hp, B, T, w_d=1.0, mse_w=0.0, mge_w=1.0, lr=0.01, weight_decay=1e-7,
-                 max_norm=1.0, process_group=None, seed=None, optimizer="Adagrad", optimizer_params=None):
+                 max_norm=1.0, process_group=None, seed=None, optimizer="Adagrad", optimizer_params=None,
+                 reference_discriminator=None):
         """``optimizer`` / ``optimizer_params`` mirror ``getattr(optim, hp.optimizer_g)(params, **hp.optimizer_g_params)``
         of reference train.py:784-789 (one setting for both models): "Adagrad" (lr, weight_decay, eps; the defaults
-        are hparams.py:201-206) or "Adam" (lr, betas, eps, weight_decay; hparams.py:125-130)."""
+        are hparams.py:201-206) or "Adam" (lr, betas, eps, weight_decay; hparams.py:125-130).
+
+        ``reference_discriminator``: the frozen discriminator of the adversarial stage (train.py --checkpoint-r); every
+        step then counts the frames of the pre-update y_hat_static it takes for natural (train.py:549-558) into the
+        device scalar ``spoof_count``.  It runs with dropout off, sees no linguistic conditioning and is never updated."""
         lib = _lib.load()
         if optimizer not in ("Adagrad", "Adam"):
             raise RuntimeError("FusedGanStep: no native optimiser %r (Adagrad and Adam are the ones hparams.py uses)" % optimizer)
@@ -153,10 +179,7 @@ class FusedGanStep(object):
         c.n_static, c.n_static_cols = n_static, len(scols)
         for i, v in enumerate(scols):
             c.static_cols[i] = v
-        sizes = multistream.get_static_stream_sizes(hp.stream_sizes, hp.has_dynamic_features, nw)
-        acols = multistream.select_stream_columns(sizes, hp.adversarial_streams)
-        if hp.mask_nth_mgc_for_adv_loss > 0:
-            acols = acols[hp.mask_nth_mgc_for_adv_loss:]
+        acols = adversarial_columns(hp)
         c.n_adv = len(acols)
         for i, v in enumerate(acols):
             c.adv_cols[i] = v
@@ -181,8 +204,25 @@ class FusedGanStep(object):
         self.y_hat = torch.empty(self.B, self.T, c.g.dims[c.g.num_layers], dtype=torch.float32, device=dev)
         self.y_hat_static = torch.empty(self.B, self.T, n_static, dtype=torch.float32, device=dev)
         self._seed = int(seed) if seed is not None else ops.draw_seed() & ((1 << 60) - 1)
-        self._step = 0
+        self._step = 0                          # training calls: the seed stream
+        self._opt_steps = {"g": 0, "d": 0}      # optimiser steps per model (they differ after D-only steps)
         self._grad_views = {}
+        self.ref_d = reference_discriminator
+        if reference_discriminator is not None:
+            check_reference_discriminator(reference_discriminator, len(acols), "FusedGanStep")
+            ref_layers = list(reference_discriminator.layers) + [reference_discriminator.last_linear]
+            self._ref_params = [t for l in ref_layers for t in (l.weight, l.bias)]
+            ops.require_cuda(*self._ref_params)
+            if not all(t.is_contiguous() for t in self._ref_params):
+                raise RuntimeError("gantts_b200: parameters must be contiguous")
+            self._ref_desc = _lib.MlpT()
+            _fill_mlp(self._ref_desc, ref_layers, 0.0, _lib.ACT_SIGMOID)
+            self._adv_cols = (ctypes.c_int * len(acols))(*acols)
+            rbytes = lib.gantts_spoof_count_workspace_bytes(ctypes.byref(self._ref_desc), self.B * self.T)
+            if rbytes == 0:
+                raise RuntimeError("gantts_b200 spoof_count config rejected: %s" % lib.gantts_last_error_string().decode())
+            self._ref_ws = torch.empty(rbytes, dtype=torch.uint8, device=dev)
+            self.spoof_count = torch.zeros((), dtype=torch.float32, device=dev)
 
     def _bind_params(self, cfg):
         for tab, lo, hi in ((cfg.g_tensors, 0, self._ng), (cfg.d_tensors, self._ng, len(self._params))):
@@ -207,14 +247,19 @@ class FusedGanStep(object):
                                        self.y_hat_static.data_ptr(), self.losses.data_ptr(), self._ws.data_ptr(),
                                        self._ws.numel(), ops._stream()))
 
-    def step(self, x, y, lengths, frames=None, adv_w=1.0, train=None):
+    def step(self, x, y, lengths, frames=None, adv_w=1.0, train=None, update_g=True):
         """x (B,T,d_in), y (B,T,d_out) contiguous CUDA float32; lengths CUDA int64 (B,); frames = GLOBAL
         number of valid frames (host number; checked against the device-side count when the losses are read,
         see loss_dict).  Returns the device tensor of 12 loss scalars.
 
         ``train=None`` follows the models like the reference's train_loop does (train.py:481-486): both models
         in ``.train()`` -> training step; both in ``.eval()`` -> the "test" phase (forwards and losses only,
-        dropout off, parameters and Adagrad state untouched)."""
+        dropout off, parameters and Adagrad state untouched).
+
+        ``update_g=False`` is the discriminator warm-up step (train.py --discriminator-warmup, :696): the generator runs
+        forward in train mode, the discriminator is updated, the generator and its optimiser state are left alone.
+        loss_adv and g_grad_norm are then 0 and loss_g = mse_w loss_mse + mge_w loss_mge of the forward.  Ignored in
+        the test phase, which updates nothing."""
         ops.require_cuda(x, y)
         if not (x.is_contiguous() and y.is_contiguous()):
             raise RuntimeError("FusedGanStep: x and y must be contiguous")
@@ -240,26 +285,62 @@ class FusedGanStep(object):
             inv = 1.0 / float(frames)
         if not train:
             self._call(_lib.STEP_EVAL, x, y, lengths, inv, 0)
+            self._count_spoofed(lengths)
             return self.losses
+        if not update_g and not self.cfg.w_d > 0:
+            raise RuntimeError("FusedGanStep: update_g=False trains the discriminator alone and needs w_d > 0")
         seed = (self._seed + self._step) & ((1 << 61) - 1)
         self.last_seed = seed
         self._step += 1
-        self.cfg.opt_step = self._step          # Adam's bias corrections: the number of the step being taken
-        if world == 1:
-            self._call(7, x, y, lengths, inv, seed)
-        else:
-            self._call(1, x, y, lengths, inv, seed)
-            parallel.allreduce_sum_(self.grad_buffer(1), self.pg)
-            self._call(2, x, y, lengths, inv, seed)
-            parallel.allreduce_sum_(self.grad_buffer(0), self.pg)
+        # Adam's bias corrections: the number of the step each model is taking
+        self._opt_steps["d"] += 1
+        if update_g:
+            self._opt_steps["g"] += 1
+        n_g, n_d = self._opt_steps["g"], self._opt_steps["d"]
+        d_only = 0 if update_g else _lib.STEP_D_ONLY
+        if world == 1 and (n_g == n_d or d_only):
+            self.cfg.opt_step = n_d
+            self._call(7 | d_only, x, y, lengths, inv, seed)
+        elif world == 1:
+            self.cfg.opt_step = n_d
+            self._call(1 | 2, x, y, lengths, inv, seed)
+            self.cfg.opt_step = n_g
             self._call(4, x, y, lengths, inv, seed)
+        else:
+            self.cfg.opt_step = n_d
+            self._call(1 | d_only, x, y, lengths, inv, seed)
+            parallel.allreduce_sum_(self.grad_buffer(1), self.pg)
+            self._call(2 | d_only, x, y, lengths, inv, seed)
+            if update_g:
+                parallel.allreduce_sum_(self.grad_buffer(0), self.pg)
+            self.cfg.opt_step = n_g
+            self._call(4 | d_only, x, y, lengths, inv, seed)
+        self._count_spoofed(lengths)
         return self.losses
+
+    def _count_spoofed(self, lengths):
+        """spoof_count = frames of this step's y_hat_static (the pre-update generator's output) the reference
+        discriminator takes for natural (train.py:549-558); local to the rank, like `frames`."""
+        if self.ref_d is None:
+            return
+        lib = _lib.load()
+        d = self._ref_desc
+        for i, (w, b) in enumerate(zip(self._ref_params[0::2], self._ref_params[1::2])):
+            d.W[i], d.b[i] = w.data_ptr(), b.data_ptr()
+        ws = self._ref_ws
+        _lib.check(lib.gantts_spoof_count(ctypes.byref(d), self.y_hat_static.data_ptr(), self.y_hat_static.shape[-1],
+                                          self._adv_cols, len(self._adv_cols), lengths.data_ptr(), self.B, self.T,
+                                          self.spoof_count.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream()))
 
     def loss_dict(self):
         """Host copy of the 12 loss scalars (one synchronising read).  Single process: also verifies the `frames`
         the caller passed to step() against the device-side sum of the mask -- a wrong value would silently
-        rescale every loss and gradient."""
-        v = dict(zip(LOSS_NAMES, self.losses.tolist()))
+        rescale every loss and gradient.  With a reference discriminator the dict also holds "spoof_count"."""
+        if self.ref_d is None:
+            v = dict(zip(LOSS_NAMES, self.losses.tolist()))
+        else:
+            vals = torch.cat((self.losses, self.spoof_count.view(1))).tolist()
+            v = dict(zip(LOSS_NAMES + ("spoof_count",), vals))
         world = torch.distributed.get_world_size(self.pg) if (torch.distributed.is_available()
                                                               and torch.distributed.is_initialized()) else 1
         claim = getattr(self, "_frames_claim", None)
@@ -271,9 +352,9 @@ class FusedGanStep(object):
     # ---- checkpoint / resume (reference train.py:162-171 save_checkpoint, :174-199 load_checkpoint round-trip
     # optimizer.state_dict(); the layout below is torch.optim.Adagrad's, one entry per parameter in
     # model.parameters() order, so the files are interchangeable with the reference's)
-    def _opt_state(self, lo, hi, lr, wd):
+    def _opt_state(self, lo, hi, lr, wd, nstep):
         n = hi - lo
-        step = torch.tensor(float(self._step))
+        step = torch.tensor(float(nstep))
         if self.optimizer == "Adam":
             return {"state": {i: {"step": step.clone(), "exp_avg": self._sums[lo + i].detach().clone(),
                                   "exp_avg_sq": self._sqs[lo + i].detach().clone()} for i in range(n)},
@@ -288,18 +369,21 @@ class FusedGanStep(object):
 
     def state_dict(self):
         ng, n = self._ng, len(self._sums)
-        return {"optimizer_g": self._opt_state(0, ng, float(self.cfg.lr_g), float(self.cfg.wd_g)),
-                "optimizer_d": self._opt_state(ng, n, float(self.cfg.lr_d), float(self.cfg.wd_d)),
+        return {"optimizer_g": self._opt_state(0, ng, float(self.cfg.lr_g), float(self.cfg.wd_g), self._opt_steps["g"]),
+                "optimizer_d": self._opt_state(ng, n, float(self.cfg.lr_d), float(self.cfg.wd_d), self._opt_steps["d"]),
                 "step": self._step, "seed": self._seed}
 
     def load_state_dict(self, sd):
         ng, n = self._ng, len(self._sums)
+        step = int(sd.get("step", self._step))
         for key, lo, hi in (("optimizer_g", 0, ng), ("optimizer_d", ng, n)):
             st = sd[key]["state"]
             for i in range(hi - lo):
                 e = st.get(i, st.get(str(i)))
                 if e is None:
                     raise RuntimeError("FusedGanStep.load_state_dict: %s has no state for parameter %d" % (key, i))
+                if i == 0:              # each optimiser's own step count (the models differ after D-only steps)
+                    self._opt_steps[key[-1]] = int(float(e["step"])) if "step" in e else step
                 if self.optimizer == "Adam":
                     self._sums[lo + i].copy_(e["exp_avg"])
                     self._sqs[lo + i].copy_(e["exp_avg_sq"])
@@ -315,5 +399,5 @@ class FusedGanStep(object):
             else:
                 self.cfg.lr_d = float(grp.get("lr", self.cfg.lr_d))
                 self.cfg.wd_d = float(grp.get("weight_decay", self.cfg.wd_d))
-        self._step = int(sd.get("step", self._step))
+        self._step = step
         self._seed = int(sd.get("seed", self._seed))

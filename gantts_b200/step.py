@@ -54,8 +54,17 @@ class GanTrainer(object):
     """One-call GAN step over native ops.  ``step`` returns device scalars (no host sync)."""
 
     def __init__(self, model_g, model_d, hp, w_d=1.0, mse_w=0.0, mge_w=1.0, lr=0.01, weight_decay=1e-7,
-                 process_group=None, optimizer="Adagrad", optimizer_params=None):
+                 process_group=None, optimizer="Adagrad", optimizer_params=None, reference_discriminator=None):
+        """``reference_discriminator``: the frozen discriminator of the adversarial stage (train.py --checkpoint-r);
+        every step then returns ``out["spoof_count"]``, the frames of the pre-update y_hat_static it takes for natural
+        (train.py:549-558).  It is put in eval mode like train.py:445 does, sees no linguistic conditioning and is
+        never updated."""
+        from .fused import adversarial_columns, check_reference_discriminator
         self.g, self.d, self.hp = model_g, model_d, hp
+        self.ref_d = reference_discriminator
+        if reference_discriminator is not None:
+            check_reference_discriminator(reference_discriminator, len(adversarial_columns(hp)), "GanTrainer")
+            reference_discriminator.eval()
         self.w_d, self.mse_w, self.mge_w = float(w_d), float(mse_w), float(mge_w)
         okw = dict(optimizer_params) if optimizer_params is not None else dict(lr=lr, weight_decay=weight_decay)
         self.opt_g = make_optimizer(optimizer, model_g.parameters(), **okw)
@@ -68,13 +77,22 @@ class GanTrainer(object):
     def _allreduce(self, t):
         return parallel.allreduce_sum_(t, self.pg)
 
-    def step(self, x, y, lengths, R, adv_w=1.0, train=True):
+    def step(self, x, y, lengths, R, adv_w=1.0, train=True, update_g=True):
         """lengths: CUDA int64 tensor, or what train.py passes (a list of ints / 0-d tensors, sorted descending:
         ``cpu_sorted_lengths``, train.py:503).  The lengths go to the generator and to all three discriminator
         forwards like train.py:542-575 does (recurrent models honour them: packed-sequence semantics).
         ``train=False`` is the "test" phase (train.py:481-486,273,315): no backward, no optimiser step; call
-        ``model.eval()`` on the models to switch dropout off as the reference does."""
+        ``model.eval()`` on the models to switch dropout off as the reference does.
+        ``update_g=False`` is the discriminator warm-up step (train.py --discriminator-warmup, :696): update_generator
+        is not called, so there is no adversarial forward, no generator backward and no generator step; loss_mse /
+        loss_mge are the forward values, loss_adv = 0 and loss_g = mse_w loss_mse + mge_w loss_mge.  Ignored when
+        ``train=False``."""
         hp = self.hp
+        update_g = update_g or not train
+        if not update_g and not (self.w_d > 0 and self.d is not None):
+            raise RuntimeError("GanTrainer: update_g=False trains the discriminator alone and needs w_d > 0 and a "
+                               "discriminator")
+        grad_g = train and update_g
         nw = len(hp.windows)
         if torch.is_tensor(lengths):
             cpu_lengths = lengths
@@ -94,9 +112,14 @@ class GanTrainer(object):
         # copies of (y_hat, y_hat_static), whose .grad collects both contributions.  For the recurrent generators this
         # halves the LSTM backward work of a step (cfg3: 93 -> 47 ms).
         same = y_hat_static_g is y_hat_g
-        y_hat = y_hat_g.detach().requires_grad_(train)
-        y_hat_static = y_hat if same else y_hat_static_g.detach().requires_grad_(train)
+        y_hat = y_hat_g.detach().requires_grad_(grad_g)
+        y_hat_static = y_hat if same else y_hat_static_g.detach().requires_grad_(grad_g)
         out = {}
+        if self.ref_d is not None:
+            # spoofing rate (train.py:549-558): the reference D on the pre-update output, no conditioning, no gradient
+            with torch.no_grad():
+                target = self.ref_d(get_selected_static_stream(y_hat_static, hp), lengths=cpu_lengths)
+                out["spoof_count"] = ops.masked_bce(target, mask, 0)[1]
         # Global number of valid frames (data parallel: normalise by the GLOBAL count, sum grads)
         Tn = self._allreduce(mask.sum().reshape(1))
         if self.w_d > 0 and self.d is not None:
@@ -116,10 +139,10 @@ class GanTrainer(object):
             out.update(loss_d=loss_d.detach(), loss_real_d=loss_real.detach(), loss_fake_d=loss_fake.detach(),
                        real_correct=r[1].detach(), fake_correct=f[1].detach())
         sse_mge = ops._MaskedSSE.apply(y_hat_static, y_static, mask)
-        with torch.set_grad_enabled(train and self.mse_w != 0.0):           # a zero weight needs no backward kernel
+        with torch.set_grad_enabled(grad_g and self.mse_w != 0.0):          # a zero weight needs no backward kernel
             sse_mse = ops._MaskedSSE.apply(y_hat, y, mask)
         loss_mge, loss_mse = sse_mge[0] / Tn[0], sse_mse[0] / Tn[0]                                   # :291,294
-        if adv_w > 0 and self.w_d > 0 and self.d is not None:
+        if adv_w > 0 and self.w_d > 0 and self.d is not None and update_g:
             fake_in = get_selected_static_stream(y_hat_static, hp)
             if hp.discriminator_linguistic_condition:
                 fake_in = torch.cat((x, fake_in), -1)
@@ -128,7 +151,7 @@ class GanTrainer(object):
         else:
             loss_adv, adv_w = torch.zeros((), device=x.device), 0.0
         loss_g = (self.mse_w * loss_mse + self.mge_w * loss_mge) + adv_w * loss_adv                   # :314
-        if train:
+        if grad_g:
             loss_g.backward()                                                                         # :316
             heads, grads = [y_hat_static_g], [y_hat_static.grad]
             if not same and y_hat.grad is not None:

@@ -415,6 +415,16 @@ typedef struct {
 #define GANTTS_STEP_G 2
 #define GANTTS_STEP_FINISH 4
 #define GANTTS_STEP_EVAL 8
+/* Modifier of the training phases: the discriminator warm-up step (reference train.py --discriminator-warmup, :696
+ * update_g = False; train_loop :541-566 without update_generator).  With it the phases are
+ *   1 = prologue, G forward (train mode: its dropout is on), MLPG, MGE and MSE forward values, D forward on
+ *       [real | fake], BCE, D backward for its parameter gradients only (no gradient w.r.t. its input)
+ *   2 = D clip + optimiser step (no third D forward, no MLPG adjoint, no generator backward)
+ *   4 = loss scalars (no G clip / step: G's tensors and optimiser state are untouched)
+ * and the loss slots mean what they mean in the full step, except loss_adv = 0, loss_g = mse_w loss_mse + mge_w loss_mge
+ * and g_grad_norm = 0.  A data-parallel caller all-reduces the discriminator's buffer between 1 and 2 only.  Needs
+ * w_d > 0; cannot be combined with GANTTS_STEP_EVAL.  opt_step is D's Adam step number here. */
+#define GANTTS_STEP_D_ONLY 16
 
 /* Dropout seeds of the fused step, so a test can regenerate every keep mask with gantts_dropout():
  * forward `which` (0 generator, 1 stacked real|fake discriminator batch, 2 adversarial discriminator forward)
@@ -438,6 +448,18 @@ int gantts_gan_step(const gantts_gan_step_t* cfg, int phases, const float* x, co
                     const int64_t* lengths_dev, float inv_frames, uint64_t seed, float* y_hat,
                     float* y_hat_static, float* losses_dev, void* workspace, size_t workspace_bytes,
                     void* stream);
+
+/* Spoofing-rate count of reference train.py:549-558 (the adversarial stage's metric, logged as
+ * regard_fake_as_natural / total_num_frames): count_dev[0] = sum over b, t < lengths_dev[b] of [D_ref(x) > 0.5] with
+ * x = columns adv_cols[0..n_adv) of y_hat_static [B][T][n_static].  d is the frozen reference discriminator (its W / b
+ * are read, dropout_p is ignored: it runs in eval mode as train.py:445 puts it); it gets no linguistic conditioning
+ * (train.py:554-555), so d->dims[0] must equal n_adv, and it must end in one sigmoid output.  The count is stored, not
+ * accumulated, and is exact while B * T < 2^24 (checked).  Workspace: gantts_spoof_count_workspace_bytes(d, B * T)
+ * (0 = the descriptor is rejected). */
+size_t gantts_spoof_count_workspace_bytes(const gantts_mlp_t* d, int64_t rows);
+int gantts_spoof_count(const gantts_mlp_t* d, const float* y_hat_static, int n_static, const int* adv_cols, int n_adv,
+                       const int64_t* lengths_dev, int B, int T, float* count_dev, void* ws, size_t ws_bytes,
+                       void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Inference-time MLPG with real variances (replaces nnmnkwii.paramgen.mlpg as called by reference

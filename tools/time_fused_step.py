@@ -15,12 +15,18 @@ Workloads (full-length batches; mse_w = 0, mge_w = 1 unless stated):
 The two paths alternate in one process, round by round, each round timed with CUDA events after a warm-up; the GPU's
 name, power limit and maximum SM clock are queried in the same run (nvidia-smi, read-only).  Needs a CUDA device.
 
+--stage d_warmup and --spoof time the features of the five-stage recipe (train_gan.sh) instead of the modular path: in
+one process, round by round, the full fused step ("fused"), with --stage d_warmup the discriminator warm-up step
+(FusedGanStep.step(update_g=False): "fused_d_only"), and with --spoof the full step that also counts the spoofing rate of
+a reference discriminator (train.py:549-558: "fused_spoof").
+
 --dump-outputs DIR: after the timed loop, DIR/<workload>/ receives what the fused path's caller holds after its last
 step, as float32 .npy files: the loss vector, y_hat, y_hat_static, both flat gradient buffers and every updated
 parameter of both models.  Two builds run with the same arguments can then be compared array by array.
 
     python tools/time_fused_step.py [--workload vc|cfg1|tts_acoustic|tts_duration|cfg3|all] [--rounds R] [--steps K]
-                                    [--warmup W] [--json OUT] [--dump-outputs DIR]
+                                    [--warmup W] [--json OUT] [--dump-outputs DIR] [--stage adversarial|d_warmup]
+                                    [--spoof]
 """
 import argparse
 import json
@@ -100,7 +106,7 @@ def dump(out_dir, fs, mg, md):
         np.save(os.path.join(out_dir, k + ".npy"), t.detach().float().cpu().numpy())
 
 
-def run(name, w, rounds, steps, warmup, dev, dump_dir=None):
+def run(name, w, rounds, steps, warmup, dev, dump_dir=None, stage="adversarial", spoof=False):
     from gantts_b200 import fused, step as gstep
     from oracle import nnmnkwii_port as nnp
     B, T = w["B"], w["T"]
@@ -114,10 +120,20 @@ def run(name, w, rounds, steps, warmup, dev, dump_dir=None):
     kw = dict(w_d=w["w_d"], mse_w=w["mse_w"], mge_w=w["mge_w"], optimizer=w["optimizer"], optimizer_params=w["okw"])
     mg, md = models(w, dev)
     fs = fused.FusedGanStep(mg, md, hp, B, T, seed=1, **kw)
-    tr = gstep.GanTrainer(*models(w, dev), hp, **kw)
-    R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(hp.windows, T)).to(dev)
-    steps_of = {"fused": lambda: fs.step(x, y, lengths, adv_w=adv_w),
-                "modular": lambda: tr.step(x, y, lengths, R, adv_w=adv_w)}
+    steps_of = {"fused": lambda: fs.step(x, y, lengths, adv_w=adv_w)}
+    if stage == "d_warmup":
+        steps_of["fused_d_only"] = lambda: fs.step(x, y, lengths, adv_w=adv_w, update_g=False)
+    if spoof:
+        import gantts_b200
+        torch.manual_seed(99)
+        ref_d = gantts_b200.models.MLP(len(fused.adversarial_columns(hp)), 1, len(md.layers), 256, dropout=0.5,
+                                       last_sigmoid=True).to(dev)
+        fs_spoof = fused.FusedGanStep(*models(w, dev), hp, B, T, seed=2, reference_discriminator=ref_d, **kw)
+        steps_of["fused_spoof"] = lambda: fs_spoof.step(x, y, lengths, adv_w=adv_w)
+    if len(steps_of) == 1:
+        tr = gstep.GanTrainer(*models(w, dev), hp, **kw)
+        R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(hp.windows, T)).to(dev)
+        steps_of["modular"] = lambda: tr.step(x, y, lengths, R, adv_w=adv_w)
     for fn in steps_of.values():
         for _ in range(warmup):
             fn()
@@ -139,7 +155,11 @@ def run(name, w, rounds, steps, warmup, dev, dump_dir=None):
         med = float(np.median(v))
         out[k] = {"ms_per_step_median": round(med, 4), "ms_per_step_min": round(min(v), 4),
                   "ms_per_step_max": round(max(v), 4), "frames_per_s": round(B * T / med * 1e3, 1)}
-    out["speedup_fused_vs_modular"] = round(out["modular"]["ms_per_step_median"] / out["fused"]["ms_per_step_median"], 3)
+    for k in ms:
+        if k != "fused":
+            out["ratio_%s_vs_fused" % k] = round(out[k]["ms_per_step_median"] / out["fused"]["ms_per_step_median"], 3)
+    if "modular" in ms:
+        out["speedup_fused_vs_modular"] = round(out["modular"]["ms_per_step_median"] / out["fused"]["ms_per_step_median"], 3)
     return out
 
 
@@ -152,7 +172,15 @@ def main():
     ap.add_argument("--json", default=None, help="also write the results to this file")
     ap.add_argument("--dump-outputs", metavar="DIR", default=None,
                     help="write the fused path's outputs after the timed loop to DIR/<workload>/*.npy")
+    ap.add_argument("--stage", choices=("adversarial", "d_warmup"), default="adversarial",
+                    help="d_warmup: also time the discriminator warm-up step (update_g=False)")
+    ap.add_argument("--spoof", action="store_true",
+                    help="also time the full step with the spoofing-rate count of a reference discriminator")
     args = ap.parse_args()
+    if args.stage == "d_warmup" or args.spoof:
+        ok = [k for k, w in WORKLOADS.items() if w["w_d"] > 0]
+        if args.workload not in ok:
+            sys.exit("time_fused_step.py: --stage d_warmup / --spoof need a workload with a discriminator: %s" % ok)
     if not torch.cuda.is_available():
         sys.exit("time_fused_step.py: needs a CUDA device (there is no CPU path to time)")
     import __graft_entry__
@@ -162,7 +190,7 @@ def main():
     for name in (list(WORKLOADS) if args.workload == "all" else [args.workload]):
         w = WORKLOADS[name]
         rounds, steps, warmup = [d if a is None else a for a, d in zip((args.rounds, args.steps, args.warmup), w["runs"])]
-        r = run(name, w, rounds, steps, warmup, dev, args.dump_outputs)
+        r = run(name, w, rounds, steps, warmup, dev, args.dump_outputs, args.stage, args.spoof)
         print(json.dumps(r), flush=True)
         res["results"].append(r)
     print(json.dumps({"gpu": res["gpu"]}))
