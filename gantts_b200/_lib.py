@@ -130,6 +130,7 @@ SIGNATURES = {
     "gantts_profile_enable": (_i, [_i]),
     "gantts_profile_collect": (_i, [_vp, _vp, _vp]),
     "gantts_mlpg_table": (_i, [ctypes.POINTER(WindowsT), _i, _vp]),
+    "gantts_mlpg_table_device": (_i, [ctypes.POINTER(WindowsT), _i, _vp, _vp]),
     "gantts_mlpg_fwd": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, ctypes.POINTER(StreamsT),
                              ctypes.POINTER(WindowsT), _i, _i, _vp]),
     "gantts_mlpg_bwd": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, ctypes.POINTER(StreamsT),
@@ -162,6 +163,8 @@ SIGNATURES = {
     "gantts_gan_step_grad_buffer": (_i, [ctypes.POINTER(GanStepT), _vp, _i, ctypes.POINTER(ctypes.c_void_p),
                                          ctypes.POINTER(ctypes.c_int64)]),
     "gantts_gan_step": (_i, [ctypes.POINTER(GanStepT), _i, _vp, _vp, _vp, _f, _u64, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "gantts_gan_step_shaped": (_i, [ctypes.POINTER(GanStepT), _i, _i, _vp, _i, _vp, _vp, _vp, _f, _u64, _vp, _vp, _vp,
+                                    _vp, _sz, _vp]),
     "gantts_spoof_count_workspace_bytes": (_sz, [ctypes.POINTER(MlpT), _i64]),
     "gantts_spoof_count": (_i, [ctypes.POINTER(MlpT), _vp, _i, ctypes.POINTER(ctypes.c_int), _i, _vp, _i, _i, _vp, _vp,
                                 _sz, _vp]),

@@ -681,7 +681,7 @@ static void layout_lstm(const gantts_gan_step_t* c, int64_t M, Arena& a, LstmWs*
     w->h[l] = a.f32((size_t)M * nd * H);
     w->gates[l] = a.f32((size_t)M * n4);
     w->cells[l] = a.f32((size_t)M * nd * H);
-    const size_t pi = mn_partial_bytes(M, 4 * H, ni, nullptr, nullptr), ph = mn_partial_bytes(M, 4 * H, H, nullptr, nullptr);
+    const size_t pi = mn_partial_bytes_upto(M, 4 * H, ni), ph = mn_partial_bytes_upto(M, 4 * H, H);
     part_ih = pi > part_ih ? pi : part_ih;
     part_hh = ph > part_hh ? ph : part_hh;
   }
@@ -716,7 +716,7 @@ static void layout_highway(const gantts_gan_step_t* c, int64_t M, Arena& a, High
   w->gx = a.f32(on ? (size_t)M * S : 0);
   w->w = a.take(on ? 2 * plane_bytes(S, S) : 0);
   w->dz = a.take(on ? 2 * plane_bytes(M, S) : 0);
-  w->partial = reinterpret_cast<float*>(a.take(on ? mn_partial_bytes(M, S, S, nullptr, nullptr) : 0));
+  w->partial = reinterpret_cast<float*>(a.take(on ? mn_partial_bytes_upto(M, S, S) : 0));
 }
 
 // x_s: the first S columns of x's operand planes -- the generator MLP's tape input, or the LSTM stack's layer-0 input
@@ -778,7 +778,7 @@ static void layout_sru(const gantts_gan_step_t* c, int64_t M, Arena& a, SruWs* w
     w->c[l] = a.f32((size_t)M * nc);
     if (l < nl - 1) w->h[l] = a.f32((size_t)M * nc);
     w->w[l] = a.take(2 * plane_bytes(ni, ku) + 2 * plane_bytes(ku, ni));
-    w->partial[l] = reinterpret_cast<float*>(a.take(mn_partial_bytes(M, ni, ku, nullptr, nullptr)));
+    w->partial[l] = reinterpret_cast<float*>(a.take(mn_partial_bytes_upto(M, ni, ku)));
   }
   w->du = a.take(nl > 0 ? 2 * plane_bytes(M, maxku) : 0);
   w->dx = a.f32((size_t)M * nc);
@@ -801,7 +801,8 @@ static void sru_w_planes(const gantts_gan_step_t* c, const StepLayout& L, int l,
 // SRU stack forward (rnn.SRUCell per layer): the last layer's h goes unmasked into hidden2out's tape input planes, so
 // the caller runs hidden2out with mlp_fwd_impl(..., input_ready = true).  train = false: no masks.
 static int sru_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const ParamList& pg, const StepLayout& L,
-                         const float* x, int64_t M, uint64_t seed, bool train, cudaStream_t st) {
+                         const float* x, int B, int T, uint64_t seed, bool train, cudaStream_t st) {
+  const int64_t M = (int64_t)B * T;
   const gantts_sru_stack_t& s = c->sru;
   const int nl = s.num_layers, nc = sru_ncols(s);
   const float p_h = train ? s.dropout : 0.f, p_x = train ? s.rnn_dropout : 0.f;
@@ -832,7 +833,7 @@ static int sru_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, cons
   const Planes in0 = sru_in_planes(c, L, 0, M);
   if (p_x > 0.f) {
     GANTTS_PDL_LAUNCH((sru_mask_split_kernel), blocks_1d(M * s.in_dim, 1024), 256, 0, st, x, (int64_t)s.in_dim, M, s.in_dim,
-                      c->T, sru_mask(gantts_sru_mask_seed(seed, 0, 0), p_x), in0.hi, in0.lo, in0.pitch);
+                      T, sru_mask(gantts_sru_mask_seed(seed, 0, 0), p_x), in0.hi, in0.lo, in0.pitch);
     GANTTS_LAUNCH_CHECK("sru_mask_split_kernel");
   } else if ((rc = launch_split(x, s.in_dim, M, s.in_dim, in0, 0, st))) {
     return rc;
@@ -862,8 +863,8 @@ static int sru_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, cons
     p.pitch = out.pitch;
     p.mh = sru_mask(gantts_sru_mask_seed(seed, l, 1), last ? 0.f : p_h);      // SRU(): no output dropout on the last layer
     p.mx = sru_mask(gantts_sru_mask_seed(seed, l + 1, 0), last ? 0.f : p_x);
-    p.B = c->B;
-    p.T = c->T;
+    p.B = B;
+    p.T = T;
     p.d = s.hidden;
     p.bidir = s.bidirectional;
     p.act = s.act;
@@ -877,8 +878,9 @@ static int sru_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, cons
 //   dW = (x * mask_x)^T dU  (MN-major, lands in the [n_in][ncols k] parameter layout)
 //   dX = dU W^T             (K-major on W as stored; not for layer 0)
 // The layer below's dh = mask_x * dX + dx' is formed on load by its scan backward.
-static int sru_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const ParamList& pg, const float* x, int64_t M,
+static int sru_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const ParamList& pg, const float* x, int B, int T,
                          uint64_t seed, cudaStream_t st) {
+  const int64_t M = (int64_t)B * T;
   const gantts_sru_stack_t& s = c->sru;
   const int nl = s.num_layers, nc = sru_ncols(s);
   int rc;
@@ -903,13 +905,13 @@ static int sru_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const 
     p.du_pitch = du.pitch;
     p.dxp_out = (k == 3 && l > 0) ? L.sru.dxp : nullptr;
     p.dbias_part = L.sru.bpart;
-    p.B = c->B;
-    p.T = c->T;
+    p.B = B;
+    p.T = T;
     p.d = s.hidden;
     p.bidir = s.bidirectional;
     p.act = s.act;
     if ((rc = launch_sru_step_bwd(p, k, st))) return rc;
-    GANTTS_PDL_LAUNCH((sru_bias_reduce_kernel), (2 * nc + 255) / 256, 256, 0, st, L.sru.bpart, c->B, 2 * nc, pg.sru[l][BIAS].g);
+    GANTTS_PDL_LAUNCH((sru_bias_reduce_kernel), (2 * nc + 255) / 256, 256, 0, st, L.sru.bpart, B, 2 * nc, pg.sru[l][BIAS].g);
     GANTTS_LAUNCH_CHECK("sru_bias_reduce_kernel");
     if ((rc = launch_gemm_mn(sru_in_planes(c, L, l, M), du, pg.sru[l][WEIGHT].g, nullptr, 0, L.sru.partial[l], st, &rl))) return rc;
     if (l > 0) {
@@ -926,7 +928,7 @@ static int sru_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const 
 }
 
 static LstmParams lstm_layer_params(const gantts_gan_step_t* c, const ParamList& pg, const StepLayout& L, int l,
-                                    const int64_t* lengths) {
+                                    const int64_t* lengths, int B, int T) {
   const gantts_lstm_stack_t& s = c->lstm;
   LstmParams p{};
   p.W_hh = pg.lstm[l][0][W_HH].p;
@@ -938,8 +940,8 @@ static LstmParams lstm_layer_params(const gantts_gan_step_t* c, const ParamList&
   p.gates = L.lstm.gates[l];
   p.cells = L.lstm.cells[l];
   p.bar = L.lstm.bar;
-  p.B = c->B;
-  p.T = c->T;
+  p.B = B;
+  p.T = T;
   p.H = s.hidden;
   p.ndir = lstm_ndir(s);
   return p;
@@ -950,7 +952,8 @@ static LstmParams lstm_layer_params(const gantts_gan_step_t* c, const ParamList&
 // on the top layer the unmasked h into hidden2out's tape input planes, so the caller runs hidden2out with
 // mlp_fwd_impl(..., input_ready = true).  train = false: no masks.
 static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const ParamList& pg, const StepLayout& L,
-                          const float* x, const int64_t* lengths, int64_t M, uint64_t seed, bool train, cudaStream_t st) {
+                          const float* x, const int64_t* lengths, int B, int T, uint64_t seed, bool train, cudaStream_t st) {
+  const int64_t M = (int64_t)B * T;
   const gantts_lstm_stack_t& s = c->lstm;
   const int nl = s.num_layers, H = s.hidden, nd = lstm_ndir(s), G4 = 4 * H, nh = nd * H;
   const float p_drop = train ? s.dropout : 0.f;
@@ -1002,7 +1005,7 @@ static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, con
     e.ldc = (int64_t)nd * G4;
     e.bias = L.lstm.bias[l];
     if ((rc = launch_gemm_kk(lstm_in_planes(c, L, l, M), w, e, st))) return rc;
-    LstmParams p = lstm_layer_params(c, pg, L, l, lengths);
+    LstmParams p = lstm_layer_params(c, pg, L, l, lengths, B, T);
     p.xproj = L.lstm.xproj;
     if ((rc = lstm_run(false, p, st))) return rc;
     const Planes out = last ? top : lstm_in_planes(c, L, l + 1, M);
@@ -1022,7 +1025,8 @@ static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, con
 //   db_hh = db_ih (b_ih and b_hh enter xproj as one sum)
 // Each layer's split-K reductions go through one flush_reduce.
 static int lstm_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const ParamList& pg, const int64_t* lengths,
-                          int64_t M, uint64_t seed, cudaStream_t st) {
+                          int B, int T, uint64_t seed, cudaStream_t st) {
+  const int64_t M = (int64_t)B * T;
   const gantts_lstm_stack_t& s = c->lstm;
   const int nl = s.num_layers, H = s.hidden, nd = lstm_ndir(s), G4 = 4 * H, nh = nd * H;
   int rc;
@@ -1032,7 +1036,7 @@ static int lstm_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const
   const Planes hp = carve_planes(cur, M, H);
   ReduceList rl;
   for (int l = nl - 1; l >= 0; --l) {
-    LstmParams p = lstm_layer_params(c, pg, L, l, lengths);
+    LstmParams p = lstm_layer_params(c, pg, L, l, lengths, B, T);
     p.dh_out = L.lstm.dh;
     p.dxproj = L.lstm.xproj;
     if ((rc = lstm_run(true, p, st))) return rc;
@@ -1044,7 +1048,7 @@ static int lstm_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const
       dgd.lo += (int64_t)d * G4;
       dgd.cols = G4;
       if ((rc = launch_gemm_mn(dgd, in, pg.lstm[l][d][W_IH].g, pg.lstm[l][d][B_IH].g, 0, L.lstm.part[d][0], st, &rl))) return rc;
-      GANTTS_PDL_LAUNCH((lstm_hprev_planes_kernel), blocks_1d(M * H, 1024), 256, 0, st, L.lstm.h[l], lengths, c->B, c->T, H, nd,
+      GANTTS_PDL_LAUNCH((lstm_hprev_planes_kernel), blocks_1d(M * H, 1024), 256, 0, st, L.lstm.h[l], lengths, B, T, H, nd,
                         d, hp.hi, hp.lo, hp.pitch);
       GANTTS_LAUNCH_CHECK("lstm_hprev_planes_kernel");
       if ((rc = launch_gemm_mn(dgd, hp, pg.lstm[l][d][W_HH].g, nullptr, 0, L.lstm.part[d][1], st, &rl))) return rc;
@@ -1071,6 +1075,10 @@ static int lstm_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const
   return GANTTS_OK;
 }
 
+// The workspace is laid out once for the configured (B, T), the capacity: a call of shape (b, t) uses the first
+// M = b * t rows of every per-row buffer, and the split-K partials are sized for every M up to the capacity.  So the flat
+// gradient buffers (gantts_gan_step_grad_buffer) and every buffer one call leaves for the next (phases 1|2 then 4) sit at
+// the same offsets whatever the call's shape.
 static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
   const int64_t M = (int64_t)c->B * c->T;
   const int dD = c->d.dims[0];
@@ -1090,7 +1098,7 @@ static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
   L->g_tape = a.take(L->g_tape_bytes);
   L->d_tape_bytes = gantts_mlp_tape_bytes(&c->d, 2 * M);
   L->d_tape = a.take(L->d_tape_bytes);
-  const size_t gb = gantts_mlp_workspace_bytes(&c->g, M), db = gantts_mlp_workspace_bytes(&c->d, 2 * M);
+  const size_t gb = mlp_workspace_bytes(&c->g, M, true), db = mlp_workspace_bytes(&c->d, 2 * M, true);
   L->mlp_ws_bytes = gb > db ? gb : db;
   L->mlp_ws = a.take(L->mlp_ws_bytes);
   L->red = reinterpret_cast<RedWs*>(a.take(R_COUNT * sizeof(RedWs)));
@@ -1105,6 +1113,8 @@ static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
 struct Step {
   const gantts_gan_step_t* c;
   StepLayout L;
+  int B, T;                 // the call's shape (<= the configured capacity c->B, c->T), M = B * T
+  const float* table;       // MLPG table of the call's T
   gantts_mlp_t g, d;      // local copies: parameters from the tables, per-forward dropout and seed
   ParamList pg, pd;
   const float *x, *y;
@@ -1127,10 +1137,10 @@ struct Step {
 // or only D (D_ONLY) reports 0 for the gradient norm it does not compute, never an earlier step's value.
 static int step_prologue(const Step& s, float inv_frames, bool zero_norms) {
   const gantts_gan_step_t* c = s.c;
-  int rc = gantts_sequence_mask(s.lengths, s.L.mask, c->B, c->T, s.stream);
+  int rc = gantts_sequence_mask(s.lengths, s.L.mask, s.B, s.T, s.stream);
   if (rc) return rc;
   GANTTS_PDL_LAUNCH((set_scales_kernel), 1, 32, 0, s.st, s.L.scal, inv_frames, s.has_adv ? c->adv_w : 0.f, c->mge_w, c->mse_w,
-                    zero_norms ? 1 : 0, s.lengths, c->B, c->T);
+                    zero_norms ? 1 : 0, s.lengths, s.B, s.T);
   GANTTS_LAUNCH_CHECK("set_scales_kernel");
   return GANTTS_OK;
 }
@@ -1160,19 +1170,19 @@ static int generator_fwd(Step& s, bool train) {
   const float* gen_out = s.y_hat;
   int rc;
   if (c->lstm.num_layers > 0) {
-    if ((rc = lstm_stack_fwd(c, s.g, s.pg, L, s.x, s.lengths, M, s.seed, train, s.st))) return rc;
+    if ((rc = lstm_stack_fwd(c, s.g, s.pg, L, s.x, s.lengths, s.B, s.T, s.seed, train, s.st))) return rc;
     if ((rc = mlp_fwd_impl(&s.g, nullptr, 0, M, L.lstm.out, s.d_out, L.g_tape, L.g_tape_bytes, s.st, true))) return rc;
     GANTTS_CUDA(cudaMemcpyAsync(s.y_hat, s.x, (size_t)M * s.d_in * sizeof(float), cudaMemcpyDeviceToDevice, s.st));
     gen_out = L.lstm.out;
   } else if (c->sru.num_layers > 0) {
-    if ((rc = sru_stack_fwd(c, s.g, s.pg, L, s.x, M, s.seed, train, s.st))) return rc;
+    if ((rc = sru_stack_fwd(c, s.g, s.pg, L, s.x, s.B, s.T, s.seed, train, s.st))) return rc;
     if ((rc = mlp_fwd_impl(&s.g, nullptr, 0, M, s.y_hat, s.d_out, L.g_tape, L.g_tape_bytes, s.st, true))) return rc;
   } else if ((rc = gantts_mlp_fwd(&s.g, s.x, s.d_in, M, s.y_hat, s.d_out, L.g_tape, L.g_tape_bytes, s.st))) {
     return rc;
   }
   if (c->highway.static_dim > 0 && (rc = highway_gate_fwd(c, s.g, s.pg, L, M, s.st))) return rc;
-  return mlpg_fwd_impl(gen_out, (int64_t)c->T * s.d_out, s.d_out, s.y_hat_static, (int64_t)c->T * s.nS, s.nS, c->mlpg_table,
-                       &c->streams, &c->windows, c->B, c->T, s.stream, s.hw());
+  return mlpg_fwd_impl(gen_out, (int64_t)s.T * s.d_out, s.d_out, s.y_hat_static, (int64_t)s.T * s.nS, s.nS, s.table,
+                       &c->streams, &c->windows, s.B, s.T, s.stream, s.hw());
 }
 
 // Generator backward (loss_g.backward(), train.py:294-318) on dL/dy_hat_static summed in g_static, in order:
@@ -1197,14 +1207,14 @@ static int generator_bwd(Step& s) {
   if (!mse_grad) {
     Planes gp;
     if ((rc = mlp_bwd_gy_planes(&s.g, M, L.mlp_ws, L.mlp_ws_bytes, &gp))) return rc;
-    rc = mlpg_bwd_planes(L.g_static, (int64_t)c->T * nS, nS, gp.hi, gp.lo, gp.pitch, c->mlpg_table, &c->streams,
-                         &c->windows, c->B, c->T, s.stream, s.hw());
+    rc = mlpg_bwd_planes(L.g_static, (int64_t)s.T * nS, nS, gp.hi, gp.lo, gp.pitch, s.table, &c->streams,
+                         &c->windows, s.B, s.T, s.stream, s.hw());
     if (rc == GANTTS_OK) direct = true;
     else if (rc != GANTTS_E_UNSUPPORTED) return rc;
   }
   if (!direct &&
-      (rc = mlpg_bwd_impl(L.g_static, (int64_t)c->T * nS, nS, L.g_yhat, (int64_t)c->T * d_out, d_out, c->mlpg_table,
-                          &c->streams, &c->windows, c->B, c->T, mse_grad ? 1 : 0, s.stream, s.hw())))
+      (rc = mlpg_bwd_impl(L.g_static, (int64_t)s.T * nS, nS, L.g_yhat, (int64_t)s.T * d_out, d_out, s.table,
+                          &c->streams, &c->windows, s.B, s.T, mse_grad ? 1 : 0, s.stream, s.hw())))
     return rc;
   if (c->highway.static_dim > 0 && (rc = highway_gate_bwd(c, s.g, s.pg, L, M, s.st))) return rc;
   float* gx = sru ? L.sru.dx : (lstm ? L.lstm.dh : nullptr);
@@ -1212,8 +1222,8 @@ static int generator_bwd(Step& s) {
   if ((rc = mlp_bwd_impl(&s.g, direct ? nullptr : L.g_yhat, d_out, nullptr, 0, M, L.g_tape, L.g_tape_bytes, gx, gx_rs, 0,
                          s.pg.gW, s.pg.gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, -1, direct)))
     return rc;
-  if (sru) return sru_stack_bwd(c, L, s.pg, s.x, M, s.seed, s.st);
-  if (lstm) return lstm_stack_bwd(c, L, s.pg, s.lengths, M, s.seed, s.st);
+  if (sru) return sru_stack_bwd(c, L, s.pg, s.x, s.B, s.T, s.seed, s.st);
+  if (lstm) return lstm_stack_bwd(c, L, s.pg, s.lengths, s.B, s.T, s.seed, s.st);
   return GANTTS_OK;
 }
 
@@ -1318,8 +1328,21 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
                                const int64_t* lengths_dev, float inv_frames, uint64_t seed, float* y_hat,
                                float* y_hat_static, float* losses_dev, void* workspace, size_t workspace_bytes,
                                void* stream) {
+  GANTTS_CHECK_ARG(c, "gan_step: null config");
+  return gantts_gan_step_shaped(c, c->B, c->T, c->mlpg_table, phases, x, y, lengths_dev, inv_frames, seed, y_hat,
+                                y_hat_static, losses_dev, workspace, workspace_bytes, stream);
+}
+
+extern "C" int gantts_gan_step_shaped(const gantts_gan_step_t* c, int B, int T, const float* mlpg_table, int phases,
+                                      const float* x, const float* y, const int64_t* lengths_dev, float inv_frames,
+                                      uint64_t seed, float* y_hat, float* y_hat_static, float* losses_dev, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
   int rc = check_step(c);
   if (rc) return rc;
+  // the call's shape is at most the configured one, the capacity the workspace was laid out for
+  GANTTS_CHECK_ARG(B >= 1 && B <= c->B, "gan_step_shaped: batch size B = %d must be in [1, configured B = %d]", B, c->B);
+  GANTTS_CHECK_ARG(T >= 1 && T <= c->T, "gan_step_shaped: padded length T = %d must be in [1, configured T = %d]", T, c->T);
+  GANTTS_CHECK_ARG(mlpg_table, "gan_step_shaped: null MLPG table (it must be gantts_mlpg_table(windows, T) of the call's T)");
   // the discriminator warm-up (train.py --discriminator-warmup, :696 update_g = False): D steps, G is left alone
   const bool d_only = (phases & GANTTS_STEP_D_ONLY) != 0;
   if (d_only) {
@@ -1336,11 +1359,14 @@ extern "C" int gantts_gan_step(const gantts_gan_step_t* c, int phases, const flo
   }
   Step s;
   s.c = c;
+  s.B = B;
+  s.T = T;
+  s.table = mlpg_table;
   s.stream = stream;
   s.st = as_stream(stream);
   layout(c, reinterpret_cast<char*>(al256(reinterpret_cast<uintptr_t>(workspace))), &s.L);
   const StepLayout& L = s.L;
-  const int64_t M = s.M = (int64_t)c->B * c->T;
+  const int64_t M = s.M = (int64_t)B * T;
   s.x = x;
   s.y = y;
   s.lengths = lengths_dev;

@@ -875,6 +875,18 @@ static size_t mn_partial_bytes(int64_t red, int rows_a, int cols_b, int* splits_
   return ((size_t)splits * ((size_t)rows_a * cols_b + rows_a) * sizeof(float) + 255) / 256 * 256;
 }
 
+// Bytes that cover mn_partial_bytes(red, ...) for EVERY red in [1, red_max]: the split count is not monotone in red (the
+// rounding of the chunk can give a shorter reduction more splits), but it never exceeds min(num_sms / tiles, blocks).
+static size_t mn_partial_bytes_upto(int64_t red_max, int rows_a, int cols_b) {
+  const int bn = pick_bn(cols_b);
+  const int tiles = ((rows_a + TC_BM - 1) / TC_BM) * ((cols_b + bn - 1) / bn);
+  const int64_t blocks = (red_max + TC_MN_BK - 1) / TC_MN_BK;
+  int64_t splits = num_sms() / tiles;
+  if (splits > blocks) splits = blocks;
+  if (splits < 1) splits = 1;
+  return ((size_t)splits * ((size_t)rows_a * cols_b + rows_a) * sizeof(float) + 255) / 256 * 256;
+}
+
 // Deferred deterministic split reductions: several (partial -> out) jobs summed by ONE launch.
 constexpr int REDUCE_MAX_JOBS = 2 * GANTTS_MAX_LAYERS;
 struct ReduceList {

@@ -507,16 +507,22 @@ extern "C" size_t gantts_mlp_tape_bytes(const gantts_mlp_t* m, int64_t M) {
   return carve_tape(m, M, nullptr, nullptr) + 512;
 }
 
-extern "C" size_t gantts_mlp_workspace_bytes(const gantts_mlp_t* m, int64_t M) {
+namespace gantts {
+// upto = false: the workspace of M rows; true: enough for every row count in [1, M]
+static size_t mlp_workspace_bytes(const gantts_mlp_t* m, int64_t M, bool upto) {
   if (!m || m->num_layers < 1 || m->num_layers > GANTTS_MAX_LAYERS || M < 1) return 0;
   int maxd = 0;
   size_t part = 0;
   for (int l = 0; l <= m->num_layers; ++l) maxd = m->dims[l] > maxd ? m->dims[l] : maxd;
   for (int l = 0; l < m->num_layers; ++l)       // one partial region per layer: reductions are deferred
-    part += mn_partial_bytes(M, m->dims[l + 1], m->dims[l], nullptr, nullptr) + 256;
+    part += (upto ? mn_partial_bytes_upto(M, m->dims[l + 1], m->dims[l])
+                  : mn_partial_bytes(M, m->dims[l + 1], m->dims[l], nullptr, nullptr)) + 256;
   return (size_t)2 * MLP_GRAD_BUFS * plane_bytes(M, maxd) + part + (size_t)MLP_COLSUM_CHUNKS * maxd * sizeof(float) +
          (size_t)GEMV_BLOCKS * (GEMV_MAX_K + 1) * sizeof(float) + 4096;
 }
+}  // namespace gantts
+
+extern "C" size_t gantts_mlp_workspace_bytes(const gantts_mlp_t* m, int64_t M) { return mlp_workspace_bytes(m, M, false); }
 
 // input_ready: the caller has already written the input planes into the tape (mlp_tape_input_planes) -- the fused
 // step gathers the discriminator's input columns straight into planes instead of gathering to fp32 and splitting.

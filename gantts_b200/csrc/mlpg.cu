@@ -817,6 +817,142 @@ extern "C" int gantts_mlpg_table(const gantts_windows_t* win, int T, float* tabl
   return GANTTS_OK;
 }
 
+// ---------------------------------------------------------------------------- the table built on the device
+// gantts_mlpg_table's arithmetic, operation for operation: every product, sum and difference in float64 through the
+// _rn intrinsics (no FMA contraction, which the host build does not emit either), IEEE division and square root.  Only
+// the parallel structure differs, and no value depends on it.
+namespace gantts {
+
+constexpr int TABLE_DEV_THREADS = 256;
+constexpr int TABLE_DEV_MAX_WARPS = 32;       // row solves in flight: scratch = warps x 32 x T doubles
+
+// band[d * T + j] = P[j + d][j]: each entry sums its terms in the host's order (window, then frame r ascending: one
+// (k1, k2) pair per frame), then thread 0 factors P = L L^T in place, column by column.
+__global__ void __launch_bounds__(TABLE_DEV_THREADS)
+mlpg_table_factor_kernel(gantts_windows_t win, int T, int hb, double* __restrict__ band) {
+  for (int64_t e = threadIdx.x; e < (int64_t)(hb + 1) * T; e += TABLE_DEV_THREADS) {
+    const int d = (int)(e / T), j = (int)(e - (int64_t)d * T), i = j + d;
+    double acc = 0.0;
+    if (i < T) {
+      for (int w = 0; w < win.n; ++w) {
+        const int l = win.l[w], u = win.u[w];
+        const int r0 = i - u > 0 ? i - u : 0, r1 = j + l < T - 1 ? j + l : T - 1;
+        for (int r = r0; r <= r1; ++r)
+          acc = __dadd_rn(acc, __dmul_rn((double)win.coef[w][i - r + l], (double)win.coef[w][j - r + l]));
+      }
+    }
+    band[e] = acc;
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  double* L = band;
+  for (int j = 0; j < T; ++j) {
+    double d = L[j];
+    for (int k = 1; k <= hb && j - k >= 0; ++k) {
+      const double v = L[(int64_t)k * T + (j - k)];
+      d = __dsub_rn(d, __dmul_rn(v, v));
+    }
+    d = __dsqrt_rn(d);          // P not positive definite: NaN (the host builder rejects such windows)
+    L[j] = d;
+    for (int i = j + 1; i <= j + hb && i < T; ++i) {
+      double s = L[(int64_t)(i - j) * T + j];
+      for (int k = 1; k <= hb; ++k) {
+        const int c = j - k;
+        if (c < 0 || i - c > hb) continue;
+        s = __dsub_rn(s, __dmul_rn(L[(int64_t)(i - c) * T + c], L[(int64_t)(j - c) * T + c]));
+      }
+      L[(int64_t)(i - j) * T + j] = __ddiv_rn(s, d);
+    }
+  }
+}
+
+__device__ __forceinline__ double band_at(const double* __restrict__ L, int T, int hb, int i, int j) {   // L[i][j], i >= j
+  const int d = i - j;
+  return (i < T && j >= 0 && d >= 0 && d <= hb) ? L[(int64_t)d * T + j] : 0.0;
+}
+
+// One lane per table row t: x = P^-1 e_t by the host's forward substitution (zeros before t) and backward substitution,
+// stopped once the FIR taps of the row are written (x[i] for i < t - K does not feed them).  The 32 lanes of a warp walk
+// the same frame i together (a lane whose row starts later contributes its zeros), so the scratch column z[i][lane] of
+// the forward values is read and written in whole rows.
+__global__ void __launch_bounds__(32 * 4)
+mlpg_table_rows_kernel(int T, int hb, const double* __restrict__ L, double* __restrict__ zbuf, int nwarps,
+                       float* __restrict__ table) {
+  const int lane = threadIdx.x & 31;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (warp >= nwarps) return;
+  double* z = zbuf + (int64_t)warp * T * 32 + lane;
+  for (int t0 = warp * 32; t0 < T; t0 += nwarps * 32) {
+    const int t = t0 + lane;
+    const bool on = t < T;
+    if (on) {
+      float* row = table + (int64_t)t * TABW;
+      for (int j = 0; j < TABW; ++j) row[j] = 0.f;
+      row[52] = __double2float_rn(__ddiv_rn(1.0, band_at(L, T, hb, t, t)));
+      row[53] = __double2float_rn(band_at(L, T, hb, t, t - 1));
+      row[54] = __double2float_rn(band_at(L, T, hb, t, t - 2));
+      row[56] = __double2float_rn(band_at(L, T, hb, t + 1, t));
+      row[57] = __double2float_rn(band_at(L, T, hb, t + 2, t));
+    }
+    double p[GANTTS_MAX_WINDOW_TAPS] = {0.0, 0.0, 0.0, 0.0, 0.0};   // p[k - 1] = x[i - k] (forward) / x[i + k] (backward)
+    for (int i = t0; i < T; ++i) {
+      double x = 0.0;
+      if (i >= t) {
+        double s = i == t ? 1.0 : 0.0;
+#pragma unroll
+        for (int k = 1; k < GANTTS_MAX_WINDOW_TAPS; ++k)
+          if (k <= hb && i - k >= t) s = __dsub_rn(s, __dmul_rn(L[(int64_t)k * T + (i - k)], p[k - 1]));
+        x = __ddiv_rn(s, L[i]);
+      }
+#pragma unroll
+      for (int k = GANTTS_MAX_WINDOW_TAPS - 1; k > 0; --k) p[k] = p[k - 1];
+      p[0] = x;
+      z[(int64_t)i * 32] = x;
+    }
+#pragma unroll
+    for (int k = 0; k < GANTTS_MAX_WINDOW_TAPS; ++k) p[k] = 0.0;
+    const int stop = t0 - K_HALF > 0 ? t0 - K_HALF : 0;
+    for (int i = T - 1; i >= stop; --i) {
+      double s = i >= t0 ? z[(int64_t)i * 32] : 0.0;      // x[i] = 0 before the row's start
+#pragma unroll
+      for (int k = 1; k < GANTTS_MAX_WINDOW_TAPS; ++k)
+        if (k <= hb && i + k < T) s = __dsub_rn(s, __dmul_rn(L[(int64_t)k * T + i], p[k - 1]));
+      const double x = __ddiv_rn(s, L[i]);
+#pragma unroll
+      for (int k = GANTTS_MAX_WINDOW_TAPS - 1; k > 0; --k) p[k] = p[k - 1];
+      p[0] = x;
+      const int j = i - t + K_HALF;
+      if (on && j >= 0 && j < NTAPS) table[(int64_t)t * TABW + j] = __double2float_rn(x);
+    }
+  }
+}
+
+}  // namespace gantts
+
+extern "C" int gantts_mlpg_table_device(const gantts_windows_t* win, int T, float* table_dev, void* stream) {
+  GANTTS_CHECK_ARG(win && table_dev && T >= 1, "mlpg_table_device: bad arguments");
+  GANTTS_CHECK_ARG(win->n >= 1 && win->n <= GANTTS_MAX_WINDOWS, "mlpg_table_device: bad window count");
+  int hb = 0;
+  for (int w = 0; w < win->n; ++w) {
+    GANTTS_CHECK_ARG(win->l[w] >= 0 && win->l[w] <= HALO && win->u[w] >= 0 && win->u[w] <= HALO,
+                     "mlpg_table_device: window %d taps out of range", w);
+    hb = win->l[w] + win->u[w] > hb ? win->l[w] + win->u[w] : hb;
+  }
+  static_assert(2 * HALO < GANTTS_MAX_WINDOW_TAPS, "the row solves keep hb <= 2 HALO previous values");
+  const cudaStream_t st = as_stream(stream);
+  const int groups = (T + 31) / 32, warps = groups < TABLE_DEV_MAX_WARPS ? groups : TABLE_DEV_MAX_WARPS;
+  const size_t band_bytes = (size_t)(hb + 1) * T * sizeof(double), z_bytes = (size_t)warps * 32 * T * sizeof(double);
+  void* scratch = nullptr;
+  GANTTS_CUDA(cudaMallocAsync(&scratch, band_bytes + z_bytes, st));
+  double* band = static_cast<double*>(scratch);
+  mlpg_table_factor_kernel<<<1, TABLE_DEV_THREADS, 0, st>>>(*win, T, hb, band);
+  GANTTS_LAUNCH_CHECK("mlpg_table_factor_kernel");
+  mlpg_table_rows_kernel<<<(warps + 3) / 4, 32 * 4, 0, st>>>(T, hb, band, band + (size_t)(hb + 1) * T, warps, table_dev);
+  GANTTS_LAUNCH_CHECK("mlpg_table_rows_kernel");
+  GANTTS_CUDA(cudaFreeAsync(scratch, st));
+  return GANTTS_OK;
+}
+
 namespace gantts {
 static int check_highway(const HighwayArgs* hw, int ncols, int64_t bs, int64_t ts, int T) {
   if (!hw) return GANTTS_OK;

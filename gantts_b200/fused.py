@@ -4,10 +4,16 @@ single host synchronisation (SURVEY.md 8f row 3).  Not drop-in for train.py (whi
 functions); offered next to the compatible modular path (gantts_b200.step.GanTrainer), which also runs
 the LSTMRNN / GRURNN generators.
 
+The step is built for a (B, T) that is its capacity: each call trains on its own mini-batch shape (b, t), b <= B and
+t <= T, with exactly the arithmetic of a step built for (b, t) -- so the batches of train.py's collate_fn, padded to their
+own max_len with a short last batch, map onto it one by one.
+
 Data parallel: utterance shards, the two flat gradient buffers are SUM all-reduced (NCCL via
 torch.distributed on the same stream) between the phases of the step; losses are normalised by the
-GLOBAL number of valid frames.
+GLOBAL number of valid frames.  Every rank pads its shard to the GLOBAL max_len of the mini-batch (the same t on every
+rank; b may differ), as the MLPG and the SRU's reverse direction depend on the padded length.
 """
+import collections
 import ctypes
 
 import numpy as np
@@ -172,8 +178,11 @@ class FusedGanStep(object):
                                                             [True] * len(hp.stream_sizes), nw)
         c.streams = _lib.make_streams(entries)
         c.windows = _lib.make_windows(hp.windows)
+        # the host table of the configured T (it also validates the windows); other padded lengths get tables built on
+        # the device (ops.mlpg_table_device, bit-identical), kept in a small LRU cache
         self._table = ops.mlpg_table(hp.windows, self.T, dev)
         c.mlpg_table = self._table.data_ptr()
+        self._tables = collections.OrderedDict()
         scols = multistream.static_feature_columns(nw, hp.stream_sizes, hp.has_dynamic_features,
                                                    [True] * len(hp.stream_sizes))
         c.n_static, c.n_static_cols = n_static, len(scols)
@@ -201,8 +210,12 @@ class FusedGanStep(object):
             raise RuntimeError("gantts_b200 gan_step config rejected: %s" % lib.gantts_last_error_string().decode())
         self._ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         self.losses = torch.zeros(len(LOSS_NAMES), dtype=torch.float32, device=dev)
-        self.y_hat = torch.empty(self.B, self.T, c.g.dims[c.g.num_layers], dtype=torch.float32, device=dev)
-        self.y_hat_static = torch.empty(self.B, self.T, n_static, dtype=torch.float32, device=dev)
+        # y_hat / y_hat_static are (b, t, .) views of these buffers after a call of shape (b, t); the buffers themselves
+        # at the configured shape
+        self._y_hat_buf = torch.empty(self.B, self.T, c.g.dims[c.g.num_layers], dtype=torch.float32, device=dev)
+        self._y_hat_static_buf = torch.empty(self.B, self.T, n_static, dtype=torch.float32, device=dev)
+        self.y_hat, self.y_hat_static = self._y_hat_buf, self._y_hat_static_buf
+        self._shape = (self.B, self.T, self._table.data_ptr())      # (b, t, MLPG table) of the next native call
         self._seed = int(seed) if seed is not None else ops.draw_seed() & ((1 << 60) - 1)
         self._step = 0                          # training calls: the seed stream
         self._opt_steps = {"g": 0, "d": 0}      # optimiser steps per model (they differ after D-only steps)
@@ -240,17 +253,47 @@ class FusedGanStep(object):
             self._grad_views[which] = self._ws[off:off + 4 * cnt.value].view(torch.float32)
         return self._grad_views[which]
 
+    TABLE_CACHE = 64            # device-built MLPG tables kept (one per padded length t != T)
+
+    def _mlpg_table(self, t):
+        """The MLPG table of padded length t: the host one for the configured T, else built on the device once."""
+        if t == self.T:
+            return self._table
+        tab = self._tables.get(t)
+        if tab is None:
+            tab = ops.mlpg_table_device(self.hp.windows, t, self.device)
+            self._tables[t] = tab
+            if len(self._tables) > self.TABLE_CACHE:
+                self._tables.popitem(last=False)
+        else:
+            self._tables.move_to_end(t)
+        return tab
+
+    def _set_shape(self, b, t):
+        """y_hat / y_hat_static as (b, t, .) views of their buffers (the buffers themselves at the configured shape)."""
+        if (b, t) == (self.B, self.T):
+            self.y_hat, self.y_hat_static = self._y_hat_buf, self._y_hat_static_buf
+        elif tuple(self.y_hat.shape[:2]) != (b, t):
+            self.y_hat, self.y_hat_static = (buf.view(-1)[:b * t * buf.shape[2]].view(b, t, buf.shape[2])
+                                             for buf in (self._y_hat_buf, self._y_hat_static_buf))
+
     def _call(self, phases, x, y, lengths, inv_frames, seed):
         lib = _lib.load()
-        _lib.check(lib.gantts_gan_step(ctypes.byref(self.cfg), phases, x.data_ptr(), y.data_ptr(),
-                                       lengths.data_ptr(), inv_frames, seed, self.y_hat.data_ptr(),
-                                       self.y_hat_static.data_ptr(), self.losses.data_ptr(), self._ws.data_ptr(),
-                                       self._ws.numel(), ops._stream()))
+        b, t, table = self._shape
+        _lib.check(lib.gantts_gan_step_shaped(ctypes.byref(self.cfg), b, t, table, phases,
+                                              x.data_ptr(), y.data_ptr(), lengths.data_ptr(), inv_frames, seed,
+                                              self.y_hat.data_ptr(), self.y_hat_static.data_ptr(), self.losses.data_ptr(),
+                                              self._ws.data_ptr(), self._ws.numel(), ops._stream()))
 
     def step(self, x, y, lengths, frames=None, adv_w=1.0, train=None, update_g=True):
-        """x (B,T,d_in), y (B,T,d_out) contiguous CUDA float32; lengths CUDA int64 (B,); frames = GLOBAL
-        number of valid frames (host number; checked against the device-side count when the losses are read,
-        see loss_dict).  Returns the device tensor of 12 loss scalars.
+        """x (b,t,d_in), y (b,t,d_out) contiguous CUDA float32 with 1 <= b <= B and 1 <= t <= T of the configured (B, T);
+        lengths CUDA int64 (b,); frames = GLOBAL number of valid frames (host number; checked against the device-side
+        count when the losses are read, see loss_dict).  Returns the device tensor of 12 loss scalars; y_hat and
+        y_hat_static are then (b, t, .) views.
+
+        Each mini-batch may have its own shape, like the batches of train.py's collate_fn (padded to their own max_len,
+        the last one shorter): the call computes exactly what a step built for (b, t) computes from the same state and
+        seed.  MLPG solves over the padded length t, so padding a batch further changes its result.
 
         ``train=None`` follows the models like the reference's train_loop does (train.py:481-486): both models
         in ``.train()`` -> training step; both in ``.eval()`` -> the "test" phase (forwards and losses only,
@@ -263,10 +306,18 @@ class FusedGanStep(object):
         ops.require_cuda(x, y)
         if not (x.is_contiguous() and y.is_contiguous()):
             raise RuntimeError("FusedGanStep: x and y must be contiguous")
-        if tuple(x.shape[:2]) != (self.B, self.T) or tuple(y.shape[:2]) != (self.B, self.T):
-            raise RuntimeError("FusedGanStep: batch shape differs from the configured (B, T)")
+        if x.dim() != 3 or y.dim() != 3 or tuple(x.shape[:2]) != tuple(y.shape[:2]):
+            raise RuntimeError("FusedGanStep: x and y must be (b, t, .) batches of the same shape")
+        b, t = int(x.shape[0]), int(x.shape[1])
+        if not (1 <= b <= self.B and 1 <= t <= self.T):
+            raise RuntimeError("FusedGanStep: batch shape (%d, %d) exceeds the configured (B, T) = (%d, %d)"
+                               % (b, t, self.B, self.T))
         if not lengths.is_cuda or lengths.dtype != torch.int64:
             raise RuntimeError("FusedGanStep: lengths must be a CUDA int64 tensor")
+        if tuple(lengths.shape) != (b,):
+            raise RuntimeError("FusedGanStep: lengths must have shape (b,) = (%d,)" % b)
+        self._set_shape(b, t)
+        self._shape = (b, t, self._mlpg_table(t).data_ptr())
         self.cfg.adv_w = float(adv_w)
         self._bind_params(self.cfg)             # parameters may have been re-allocated (load_state_dict keeps them)
         if train is None:
@@ -328,8 +379,9 @@ class FusedGanStep(object):
         for i, (w, b) in enumerate(zip(self._ref_params[0::2], self._ref_params[1::2])):
             d.W[i], d.b[i] = w.data_ptr(), b.data_ptr()
         ws = self._ref_ws
-        _lib.check(lib.gantts_spoof_count(ctypes.byref(d), self.y_hat_static.data_ptr(), self.y_hat_static.shape[-1],
-                                          self._adv_cols, len(self._adv_cols), lengths.data_ptr(), self.B, self.T,
+        b, t, n_static = self.y_hat_static.shape
+        _lib.check(lib.gantts_spoof_count(ctypes.byref(d), self.y_hat_static.data_ptr(), n_static,
+                                          self._adv_cols, len(self._adv_cols), lengths.data_ptr(), b, t,
                                           self.spoof_count.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream()))
 
     def loss_dict(self):

@@ -110,6 +110,19 @@ def mlpg_table(windows, T, device):
     return t
 
 
+def mlpg_table_device(windows, T, device):
+    """mlpg_table_full_host(windows, T) built on `device` instead: a (T, GANTTS_MLPG_TABLE_COLS) float32 CUDA tensor,
+    bit-identical to the host table, enqueued on the current stream with no host synchronisation.  It does not repeat the
+    host builder's checks that P is positive definite and P^-1 decays within the taps: validate a window set once with
+    the host builder."""
+    lib = _lib.load()
+    w = _lib.make_windows(windows)
+    with torch.cuda.device(device):
+        tab = torch.empty(int(T), _lib.MLPG_TABLE_COLS, dtype=torch.float32, device=device)
+        _lib.check(lib.gantts_mlpg_table_device(ctypes.byref(w), int(T), tab.data_ptr(), _stream()))
+    return tab
+
+
 def _validate_R(R, windows, T):
     """One-time check per (num_windows, T) that a dense R handed in by the caller really is
     (W^T W)^-1 W^T for the registered windows (the kernels never read R on the hot path)."""

@@ -89,6 +89,14 @@ typedef struct {
  */
 int gantts_mlpg_table(const gantts_windows_t* windows, int T, float* table_host);
 
+/* The same table built on the device and enqueued on `stream` (no host synchronisation, no host copy): table_dev[T *
+ * GANTTS_MLPG_TABLE_COLS] is bit for bit what gantts_mlpg_table writes -- one thread factors the band in the host's
+ * operation order, then one thread per row t solves P x = e_t, all in float64 without FMA contraction.  Scratch memory is
+ * allocated stream-ordered and freed on the stream.  The windows are checked like gantts_mlpg_table's; the two numerical
+ * conditions it reports (P positive definite, P^-1 decayed at lag K) are properties of the windows that the host builder
+ * verifies -- validate a window set once with it. */
+int gantts_mlpg_table_device(const gantts_windows_t* windows, int T, float* table_dev, void* stream);
+
 /* out[b,t,out_col] = MLPG(in[b,:,stream cols]) for dynamic streams, copy for static ones.
  * in:  float32 [B][T][*] with element strides (in_bstride, in_tstride), unit column stride.
  * out: float32 [B][T][*] with element strides (out_bstride, out_tstride). */
@@ -448,6 +456,18 @@ int gantts_gan_step(const gantts_gan_step_t* cfg, int phases, const float* x, co
                     const int64_t* lengths_dev, float inv_frames, uint64_t seed, float* y_hat,
                     float* y_hat_static, float* losses_dev, void* workspace, size_t workspace_bytes,
                     void* stream);
+/* The same step on a mini-batch of its own shape (B, T), 1 <= B <= cfg->B and 1 <= T <= cfg->T: the configured (B, T) is
+ * the capacity the workspace is laid out for, and gantts_gan_step is this call with (cfg->B, cfg->T, cfg->mlpg_table).
+ * x [B][T][*], y, y_hat, y_hat_static [B][T][*] and lengths_dev [B] are contiguous at the call's shape; mlpg_table is the
+ * device table of the call's T (gantts_mlpg_table or gantts_mlpg_table_device).  The arithmetic is exactly that of a step
+ * configured for (B, T): dropout masks and split-K plans follow the call's rows M = B * T, and the MLPG solves over T.
+ * The flat gradient buffers and whatever one call leaves for the next (phases 1|2 then 4 of the same shape) sit at the
+ * same offsets for every shape, so gantts_gan_step_grad_buffer holds for all of them.  The shape and the table are
+ * checked before any device work. */
+int gantts_gan_step_shaped(const gantts_gan_step_t* cfg, int B, int T, const float* mlpg_table, int phases,
+                           const float* x, const float* y, const int64_t* lengths_dev, float inv_frames, uint64_t seed,
+                           float* y_hat, float* y_hat_static, float* losses_dev, void* workspace,
+                           size_t workspace_bytes, void* stream);
 
 /* Spoofing-rate count of reference train.py:549-558 (the adversarial stage's metric, logged as
  * regard_fake_as_natural / total_num_frames): count_dev[0] = sum over b, t < lengths_dev[b] of [D_ref(x) > 0.5] with
