@@ -111,7 +111,8 @@ class GanStepT(ctypes.Structure):
                 ("w_d", ctypes.c_float), ("mse_w", ctypes.c_float), ("mge_w", ctypes.c_float),
                 ("adv_w", ctypes.c_float),
                 ("optimizer", ctypes.c_int), ("beta1", ctypes.c_float), ("beta2", ctypes.c_float),
-                ("opt_step", ctypes.c_int64)]
+                ("opt_step", ctypes.c_int64),
+                ("d_lstm", LstmStackT)]
 
 
 OPT_ADAGRAD, OPT_ADAM = 0, 1
@@ -183,6 +184,7 @@ SIGNATURES = {
     "gantts_mlp_layer_seed": (_u64, [_u64, _i]),
     "gantts_sru_mask_seed": (_u64, [_u64, _i, _i]),
     "gantts_lstm_mask_seed": (_u64, [_u64, _i]),
+    "gantts_d_lstm_mask_seed": (_u64, [_u64, _i, _i]),
 }
 
 STEP_D, STEP_G, STEP_FINISH, STEP_EVAL, STEP_D_ONLY = 1, 2, 4, 8, 16

@@ -395,7 +395,7 @@ struct SruWs {
   float* bpart;           // [B][2 * ncols] bias-gradient partials
 };
 
-// LSTM generator (zero bytes otherwise); per layer l:
+// LSTM stack of the generator, or of the discriminator at 2M rows (zero bytes otherwise); per layer l:
 struct LstmWs {
   char* in[GANTTS_MAX_LSTM_LAYERS];      // planes of the GEMM input [M][n_in]: x (l = 0), else h_{l-1} * mask_{l-1}
   char* w[GANTTS_MAX_LSTM_LAYERS];       // planes of W_ih of both directions [ndir 4H][n_in], then [n_in][ndir 4H]
@@ -410,6 +410,7 @@ struct LstmWs {
   char* hp;               // planes of hprev [M][H]
   float* part[2][2];      // split-K partials per direction: [d][0] dW_ih | db_ih, [d][1] dW_hh (one layer at a time)
   unsigned int* bar;      // grid-barrier counters of the recurrence
+  int64_t* lengths;       // discriminator: [2B] lengths of the stacked [real | fake] batch, the call's lengths twice
 };
 
 struct StepLayout {
@@ -434,6 +435,7 @@ struct StepLayout {
   HighwayWs hw;
   SruWs sru;
   LstmWs lstm;
+  LstmWs d_lstm;
   size_t total;
 };
 
@@ -446,6 +448,11 @@ static inline int lstm_nin(const gantts_lstm_stack_t& s, int l) { return l == 0 
 // width of x: the SRU or LSTM stack's input, else the generator MLP's
 static inline int gen_in_width(const gantts_gan_step_t* c) {
   return c->sru.num_layers > 0 ? c->sru.in_dim : (c->lstm.num_layers > 0 ? c->lstm.in_dim : c->g.dims[0]);
+}
+
+// width of the discriminator's input: the LSTM stack's, else the MLP's
+static inline int d_in_width(const gantts_gan_step_t* c) {
+  return c->d_lstm.num_layers > 0 ? c->d_lstm.in_dim : c->d.dims[0];
 }
 
 // tensor pl->n of table t: the next `size` elements of the model's flat gradient buffer (flat nullptr: counts only)
@@ -473,6 +480,16 @@ static void bind_mlp(const gantts_step_tensors_t& t, gantts_mlp_t* m, float* fla
   }
 }
 
+// [W_ih, W_hh, b_ih, b_hh] of every layer and direction of an LSTM stack into pl->lstm (none when ls.num_layers = 0)
+static void bind_lstm(const gantts_step_tensors_t& t, const gantts_lstm_stack_t& ls, float* flat, ParamList* pl) {
+  const int64_t G4 = 4 * (int64_t)ls.hidden;
+  for (int l = 0; l < ls.num_layers; ++l)
+    for (int d = 0; d < lstm_ndir(ls); ++d) {
+      const int64_t sizes[4] = {G4 * lstm_nin(ls, l), G4 * ls.hidden, G4, G4};
+      for (int i = 0; i < 4; ++i) pl->lstm[l][d][i] = take_tensor(t, sizes[i], flat, pl);
+    }
+}
+
 // The generator's table bound from the shapes, in model.parameters() order: [weight, bias] of every SRU layer, or
 // [T.weight, T.bias] of the highway gate and then [W_ih, W_hh, b_ih, b_hh] of every LSTM layer and direction; then the
 // MLP layers (hidden2out alone after a stack).  pl->n is the tensor count the shapes give, pl->total the elements.
@@ -490,20 +507,24 @@ static void g_param_list(const gantts_gan_step_t* c, gantts_mlp_t* g, float* fla
     pl->gate[WEIGHT] = take_tensor(t, S * S, flat, pl);
     pl->gate[BIAS] = take_tensor(t, S, flat, pl);
   }
-  const gantts_lstm_stack_t& ls = c->lstm;
-  const int64_t G4 = 4 * (int64_t)ls.hidden;
-  for (int l = 0; l < ls.num_layers; ++l)
-    for (int d = 0; d < lstm_ndir(ls); ++d) {
-      const int64_t sizes[4] = {G4 * lstm_nin(ls, l), G4 * ls.hidden, G4, G4};
-      for (int i = 0; i < 4; ++i) pl->lstm[l][d][i] = take_tensor(t, sizes[i], flat, pl);
-    }
+  bind_lstm(t, c->lstm, flat, pl);
   bind_mlp(t, g, flat, pl);
 }
 
+// The discriminator's table: [W_ih, W_hh, b_ih, b_hh] of every LSTM layer and direction (LSTMRNN / GRURNN), then the MLP
+// layers (hidden2out alone after a stack).
 static void d_param_list(const gantts_gan_step_t* c, gantts_mlp_t* d, float* flat, ParamList* pl) {
   pl->n = 0;
   pl->total = 0;
+  bind_lstm(c->d_tensors, c->d_lstm, flat, pl);
   bind_mlp(c->d_tensors, d, flat, pl);
+}
+
+static int64_t d_param_count(const gantts_gan_step_t* c) {
+  ParamList pl;
+  gantts_mlp_t d = c->d;
+  d_param_list(c, &d, nullptr, &pl);
+  return pl.total;
 }
 
 static int64_t g_param_count(const gantts_gan_step_t* c) {
@@ -511,12 +532,6 @@ static int64_t g_param_count(const gantts_gan_step_t* c) {
   gantts_mlp_t g = c->g;
   g_param_list(c, &g, nullptr, &pl);
   return pl.total;
-}
-
-static int64_t mlp_param_count(const gantts_mlp_t& m) {
-  int64_t n = 0;
-  for (int l = 0; l < m.num_layers; ++l) n += (int64_t)m.dims[l + 1] * m.dims[l] + m.dims[l + 1];
-  return n;
 }
 
 static inline int bce_blocks(int64_t rows) { return grid_for(rows, RED_THREADS); }
@@ -629,12 +644,33 @@ static int check_step(const gantts_gan_step_t* c) {
                      "gan_step: with an SRU stack g is hidden2out alone: 1 layer of input width %d (got %d layer(s), input "
                      "width %d)", nc, c->g.num_layers, c->g.dims[0]);
   }
+  const gantts_lstm_stack_t& dl = c->d_lstm;
+  GANTTS_CHECK_ARG(dl.num_layers >= 0 && dl.num_layers <= GANTTS_MAX_LSTM_LAYERS,
+                   "gan_step: discriminator LSTM layer count %d not in [0, %d] (train larger stacks with GanTrainer)",
+                   dl.num_layers, GANTTS_MAX_LSTM_LAYERS);
   if (c->w_d > 0.f) {
     GANTTS_CHECK_ARG(c->d.num_layers >= 1 && c->d.num_layers <= GANTTS_MAX_LAYERS, "gan_step: bad discriminator");
+    if (dl.num_layers > 0) {
+      // LSTMRNN / GRURNN with last_sigmoid (models.py:170-213): the LSTM stack, then hidden2out as a one-layer MLP
+      GANTTS_CHECK_ARG(dl.bidirectional == 0 || dl.bidirectional == 1, "gan_step: bad discriminator LSTM bidirectional %d",
+                       dl.bidirectional);
+      GANTTS_CHECK_ARG(dl.hidden >= 4 && dl.hidden % 4 == 0,
+                       "gan_step: discriminator LSTM hidden size %d is not a positive multiple of 4 (train it with GanTrainer)",
+                       dl.hidden);
+      GANTTS_CHECK_ARG(2 * c->B <= LSTM_MAX_B,
+                       "gan_step: a recurrent discriminator runs the stacked [real | fake] batch of 2B sequences, at most "
+                       "LSTM_MAX_B = %d, so B <= %d (B = %d); GanTrainer runs real and fake separately", LSTM_MAX_B,
+                       LSTM_MAX_B / 2, c->B);
+      GANTTS_CHECK_ARG(dl.dropout >= 0.f && dl.dropout < 1.f, "gan_step: discriminator LSTM dropout out of [0, 1)");
+      const int nh = lstm_ndir(dl) * dl.hidden;
+      GANTTS_CHECK_ARG(c->d.num_layers == 1 && c->d.dims[0] == nh,
+                       "gan_step: with a discriminator LSTM stack d is hidden2out alone: 1 layer of input width %d (got %d "
+                       "layer(s), input width %d)", nh, c->d.num_layers, c->d.dims[0]);
+    }
     const int cond_w = c->d_conditioned ? gen_in_width(c) : 0;
-    GANTTS_CHECK_ARG(c->n_adv >= 1 && c->n_adv <= GANTTS_MAX_COLS && c->d.dims[0] == cond_w + c->n_adv,
+    GANTTS_CHECK_ARG(c->n_adv >= 1 && c->n_adv <= GANTTS_MAX_COLS && d_in_width(c) == cond_w + c->n_adv,
                      "gan_step: discriminator input width %d != %d conditioning + %d adversarial columns",
-                     c->d.dims[0], cond_w, c->n_adv);
+                     d_in_width(c), cond_w, c->n_adv);
     GANTTS_CHECK_ARG(c->d.dims[c->d.num_layers] == 1 && c->d.last_act == GANTTS_ACT_SIGMOID,
                      "gan_step: discriminator must end in a single sigmoid output");
   }
@@ -665,11 +701,15 @@ static int check_step(const gantts_gan_step_t* c) {
   if (h.static_dim > 0)
     GANTTS_CHECK_ARG((reinterpret_cast<uintptr_t>(pl.gate[BIAS].p) & 15) == 0,
                      "gan_step: highway gate bias must be 16-byte aligned");
-  return c->w_d > 0.f ? check_table(c, c->d_tensors, 2 * c->d.num_layers, "discriminator") : GANTTS_OK;
+  if (!(c->w_d > 0.f)) return GANTTS_OK;
+  gantts_mlp_t d = c->d;
+  d_param_list(c, &d, nullptr, &pl);
+  return check_table(c, c->d_tensors, pl.n, "discriminator");
 }
 
-static void layout_lstm(const gantts_gan_step_t* c, int64_t M, Arena& a, LstmWs* w) {
-  const gantts_lstm_stack_t& ls = c->lstm;
+// out_cols: width of the head's fp32 output kept in w->out (the generator's hidden2out); seqs: sequences whose lengths
+// w->lengths holds (the discriminator's stacked batch; 0 = none)
+static void layout_lstm(const gantts_lstm_stack_t& ls, int64_t M, int out_cols, int64_t seqs, Arena& a, LstmWs* w) {
   const int nl = ls.num_layers, H = nl > 0 ? ls.hidden : 0, nd = lstm_ndir(ls), n4 = nd * 4 * H;
   const bool on = nl > 0;
   size_t part_ih = 0, part_hh = 0;
@@ -686,7 +726,7 @@ static void layout_lstm(const gantts_gan_step_t* c, int64_t M, Arena& a, LstmWs*
     part_hh = ph > part_hh ? ph : part_hh;
   }
   w->xproj = a.f32((size_t)M * n4);
-  w->out = a.f32(on ? (size_t)M * c->g.dims[c->g.num_layers] : 0);
+  w->out = a.f32(on ? (size_t)M * out_cols : 0);
   w->dh = a.f32((size_t)M * nd * H);
   w->dg = a.take(on ? 2 * plane_bytes(M, n4) : 0);
   w->hp = a.take(on ? 2 * plane_bytes(M, H) : 0);
@@ -695,18 +735,35 @@ static void layout_lstm(const gantts_gan_step_t* c, int64_t M, Arena& a, LstmWs*
     w->part[d][1] = reinterpret_cast<float*>(a.take(d < nd ? part_hh : 0));
   }
   w->bar = reinterpret_cast<unsigned int*>(a.take(on ? 256 : 0));
+  w->lengths = reinterpret_cast<int64_t*>(a.take(on ? (size_t)seqs * sizeof(int64_t) : 0));
 }
 
+// One LSTM stack of the step: the generator's (In2OutRNNHighwayNet) or the discriminator's (LSTMRNN / GRURNN), with its
+// workspace, its tensors and the stream its inter-layer masks are drawn from.
+struct LstmStack {
+  const gantts_lstm_stack_t* s;
+  const LstmWs* w;
+  const Bound (*p)[2][4];   // ParamList::lstm: [layer][direction] W_ih, W_hh, b_ih, b_hh
+  int which;                // 0: gantts_lstm_mask_seed; 1, 2: gantts_d_lstm_mask_seed(seed, which, layer)
+  uint64_t mask_seed(uint64_t seed, int l) const {
+    return which == 0 ? gantts_lstm_mask_seed(seed, l) : gantts_d_lstm_mask_seed(seed, which, l);
+  }
+};
+
 // LSTM layer l's workspace: planes of its GEMM input, and of W_ih of both directions [ndir 4H][n_in] then transposed
-static Planes lstm_in_planes(const gantts_gan_step_t* c, const StepLayout& L, int l, int64_t M) {
-  char* cur = L.lstm.in[l];
-  return carve_planes(cur, M, lstm_nin(c->lstm, l));
+static Planes lstm_in_planes(const LstmStack& k, int l, int64_t M) {
+  char* cur = k.w->in[l];
+  return carve_planes(cur, M, lstm_nin(*k.s, l));
 }
-static void lstm_w_planes(const gantts_gan_step_t* c, const StepLayout& L, int l, Planes* w, Planes* wt) {
-  const int ni = lstm_nin(c->lstm, l), n4 = lstm_ndir(c->lstm) * 4 * c->lstm.hidden;
-  char* cur = L.lstm.w[l];
+static void lstm_w_planes(const LstmStack& k, int l, Planes* w, Planes* wt) {
+  const int ni = lstm_nin(*k.s, l), n4 = lstm_ndir(*k.s) * 4 * k.s->hidden;
+  char* cur = k.w->w[l];
   *w = carve_planes(cur, n4, ni);
   *wt = carve_planes(cur, ni, n4);
+}
+
+static LstmStack g_lstm(const gantts_gan_step_t* c, const StepLayout& L, const ParamList& pg) {
+  return LstmStack{&c->lstm, &L.lstm, pg.lstm, 0};
 }
 
 static void layout_highway(const gantts_gan_step_t* c, int64_t M, Arena& a, HighwayWs* w) {
@@ -724,7 +781,7 @@ static void layout_highway(const gantts_gan_step_t* c, int64_t M, Arena& a, High
 static int gate_input_planes(const gantts_gan_step_t* c, const gantts_mlp_t& g, const StepLayout& L, int64_t M,
                              Planes* xs) {
   if (c->lstm.num_layers > 0) {
-    *xs = lstm_in_planes(c, L, 0, M);
+    *xs = lstm_in_planes(LstmStack{&c->lstm, &L.lstm, nullptr, 0}, 0, M);
   } else {
     int rc = mlp_tape_input_planes(&g, M, L.g_tape, L.g_tape_bytes, xs);
     if (rc) return rc;
@@ -927,19 +984,18 @@ static int sru_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const 
   return flush_reduce(rl, 0, st);
 }
 
-static LstmParams lstm_layer_params(const gantts_gan_step_t* c, const ParamList& pg, const StepLayout& L, int l,
-                                    const int64_t* lengths, int B, int T) {
-  const gantts_lstm_stack_t& s = c->lstm;
+static LstmParams lstm_layer_params(const LstmStack& k, int l, const int64_t* lengths, int B, int T) {
+  const gantts_lstm_stack_t& s = *k.s;
   LstmParams p{};
-  p.W_hh = pg.lstm[l][0][W_HH].p;
+  p.W_hh = k.p[l][0][W_HH].p;
   if (s.bidirectional)      // the two directions' tensors are 4-byte aligned: their distance is a whole number of floats
-    p.W_hh_dir = ((int64_t)reinterpret_cast<uintptr_t>(pg.lstm[l][1][W_HH].p) - (int64_t)reinterpret_cast<uintptr_t>(pg.lstm[l][0][W_HH].p)) /
+    p.W_hh_dir = ((int64_t)reinterpret_cast<uintptr_t>(k.p[l][1][W_HH].p) - (int64_t)reinterpret_cast<uintptr_t>(k.p[l][0][W_HH].p)) /
                  (int64_t)sizeof(float);
   p.lengths = lengths;
-  p.h_out = L.lstm.h[l];
-  p.gates = L.lstm.gates[l];
-  p.cells = L.lstm.cells[l];
-  p.bar = L.lstm.bar;
+  p.h_out = k.w->h[l];
+  p.gates = k.w->gates[l];
+  p.cells = k.w->cells[l];
+  p.bar = k.w->bar;
   p.B = B;
   p.T = T;
   p.H = s.hidden;
@@ -947,14 +1003,15 @@ static LstmParams lstm_layer_params(const gantts_gan_step_t* c, const ParamList&
   return p;
 }
 
-// LSTM stack forward (nn.LSTM on packed sequences, per-element dropout between layers): per layer one xproj GEMM over
-// both directions, the cooperative recurrence, and one kernel that writes the next GEMM's operand planes of h * mask --
-// on the top layer the unmasked h into hidden2out's tape input planes, so the caller runs hidden2out with
-// mlp_fwd_impl(..., input_ready = true).  train = false: no masks.
-static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, const ParamList& pg, const StepLayout& L,
-                          const float* x, const int64_t* lengths, int B, int T, uint64_t seed, bool train, cudaStream_t st) {
+// LSTM stack forward (nn.LSTM on packed sequences, per-element dropout between layers) over B sequences of T steps: per
+// layer one xproj GEMM over both directions, the cooperative recurrence, and one kernel that writes the next GEMM's operand
+// planes of h * mask -- on the top layer the unmasked h into `top`, the head's tape input planes, so the caller runs the
+// head with mlp_fwd_impl(..., input_ready = true).  x (row stride x_rs) is split into layer 0's input planes here; x =
+// nullptr: the caller has written them.  train = false: no masks.
+static int lstm_stack_fwd(const LstmStack& k, const float* x, int64_t x_rs, const Planes& top, const int64_t* lengths,
+                          int B, int T, uint64_t seed, bool train, cudaStream_t st) {
   const int64_t M = (int64_t)B * T;
-  const gantts_lstm_stack_t& s = c->lstm;
+  const gantts_lstm_stack_t& s = *k.s;
   const int nl = s.num_layers, H = s.hidden, nd = lstm_ndir(s), G4 = 4 * H, nh = nd * H;
   const float p_drop = train ? s.dropout : 0.f;
   int rc;
@@ -968,10 +1025,10 @@ static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, con
     bl.len = G4;
     for (int l = 0; l < nl; ++l) {
       Planes w, wt;
-      lstm_w_planes(c, L, l, &w, &wt);
+      lstm_w_planes(k, l, &w, &wt);
       for (int d = 0; d < nd; ++d) {
         const int i = l * nd + d;
-        wl.W[i] = pg.lstm[l][d][W_IH].p;
+        wl.W[i] = k.p[l][d][W_IH].p;
         wl.N[i] = G4;
         wl.K[i] = lstm_nin(s, l);
         wl.hi[i] = w.hi + (int64_t)d * G4 * w.pitch;
@@ -981,9 +1038,9 @@ static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, con
         wl.tlo[i] = wt.lo + (int64_t)d * G4;
         wl.tpitch[i] = wt.pitch;
         wl.off[i + 1] = wl.off[i] + (int64_t)((G4 + 31) / 32) * ((wl.K[i] + 31) / 32);
-        bl.a[i] = pg.lstm[l][d][B_IH].p;
-        bl.b[i] = pg.lstm[l][d][B_HH].p;
-        bl.out[i] = L.lstm.bias[l] + (int64_t)d * G4;
+        bl.a[i] = k.p[l][d][B_IH].p;
+        bl.b[i] = k.p[l][d][B_HH].p;
+        bl.out[i] = k.w->bias[l] + (int64_t)d * G4;
       }
     }
     const int nb = (int)(wl.off[wl.n] < num_sms() * 8 ? wl.off[wl.n] : num_sms() * 8);
@@ -992,85 +1049,113 @@ static int lstm_stack_fwd(const gantts_gan_step_t* c, const gantts_mlp_t& g, con
     GANTTS_PDL_LAUNCH((lstm_bias_sum_kernel), (bl.n * G4 + 255) / 256, 256, 0, st, bl);
     GANTTS_LAUNCH_CHECK("lstm_bias_sum_kernel");
   }
-  if ((rc = launch_split(x, s.in_dim, M, s.in_dim, lstm_in_planes(c, L, 0, M), 0, st))) return rc;
-  Planes top;
-  if ((rc = mlp_tape_input_planes(&g, M, L.g_tape, L.g_tape_bytes, &top))) return rc;
+  if (x && (rc = launch_split(x, x_rs, M, s.in_dim, lstm_in_planes(k, 0, M), 0, st))) return rc;
   for (int l = 0; l < nl; ++l) {
     const bool last = l == nl - 1;
     Planes w, wt;
-    lstm_w_planes(c, L, l, &w, &wt);
+    lstm_w_planes(k, l, &w, &wt);
     EpiArgs e;
     e.epi = EPI_F32;
-    e.C = L.lstm.xproj;
+    e.C = k.w->xproj;
     e.ldc = (int64_t)nd * G4;
-    e.bias = L.lstm.bias[l];
-    if ((rc = launch_gemm_kk(lstm_in_planes(c, L, l, M), w, e, st))) return rc;
-    LstmParams p = lstm_layer_params(c, pg, L, l, lengths, B, T);
-    p.xproj = L.lstm.xproj;
+    e.bias = k.w->bias[l];
+    if ((rc = launch_gemm_kk(lstm_in_planes(k, l, M), w, e, st))) return rc;
+    LstmParams p = lstm_layer_params(k, l, lengths, B, T);
+    p.xproj = k.w->xproj;
     if ((rc = lstm_run(false, p, st))) return rc;
-    const Planes out = last ? top : lstm_in_planes(c, L, l + 1, M);
+    const Planes out = last ? top : lstm_in_planes(k, l + 1, M);
     const float pl = last ? 0.f : p_drop;             // nn.LSTM: no dropout on the last layer's output
-    GANTTS_PDL_LAUNCH((lstm_planes_kernel), blocks_1d(M * nh, 1024), 256, 0, st, L.lstm.h[l], M, nh,
-                      gantts_lstm_mask_seed(seed, l), pl > 0.f ? (uint32_t)(pl * 65536.f + 0.5f) : 0u,
+    GANTTS_PDL_LAUNCH((lstm_planes_kernel), blocks_1d(M * nh, 1024), 256, 0, st, k.w->h[l], M, nh,
+                      k.mask_seed(seed, l), pl > 0.f ? (uint32_t)(pl * 65536.f + 0.5f) : 0u,
                       pl > 0.f ? 1.f / (1.f - pl) : 1.f, out.hi, out.lo, out.pitch);
     GANTTS_LAUNCH_CHECK("lstm_planes_kernel");
   }
   return GANTTS_OK;
 }
 
-// LSTM stack backward from dL/dh of the top layer in L.lstm.dh (hidden2out's input gradient), top layer first:
+// Layer 0's input gradient of a stack backward: columns [col0, col0 + cols) of dX_0 = dgates W_ih for the rows
+// [row0, rows) into C (row r -> C + (r - row0) * ldc), stored or added (the discriminator's adversarial input columns of
+// the fake rows, into g_static or g_din).
+struct LstmInGrad {
+  int64_t row0;
+  int col0, cols;
+  float* C;
+  int64_t ldc;
+  int accumulate;
+};
+
+// LSTM stack backward from dL/dh of the top layer in k.w->dh (the head's input gradient), top layer first:
 //   recurrence backward -> dgates (fp32, in the xproj buffer) -> dgates planes
 //   per direction: dW_ih and db_ih = dgates_d^T in (MN-major, ones-tile bias), dW_hh = dgates_d^T hprev_d (MN-major)
 //   dX = dgates W_ih, times the mask of the layer below in the GEMM epilogue (not for layer 0)
 //   db_hh = db_ih (b_ih and b_hh enter xproj as one sum)
-// Each layer's split-K reductions go through one flush_reduce.
-static int lstm_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const ParamList& pg, const int64_t* lengths,
-                          int B, int T, uint64_t seed, cudaStream_t st) {
+// Each layer's split-K reductions go through one flush_reduce.  param_grads = false: the input gradients alone (the
+// discriminator's adversarial pass); din: layer 0's input gradient, or none.
+static int lstm_stack_bwd(const LstmStack& k, const int64_t* lengths, int B, int T, uint64_t seed, bool param_grads,
+                          const LstmInGrad* din, cudaStream_t st) {
   const int64_t M = (int64_t)B * T;
-  const gantts_lstm_stack_t& s = c->lstm;
+  const gantts_lstm_stack_t& s = *k.s;
   const int nl = s.num_layers, H = s.hidden, nd = lstm_ndir(s), G4 = 4 * H, nh = nd * H;
   int rc;
-  char* cur = L.lstm.dg;
+  char* cur = k.w->dg;
   const Planes dg = carve_planes(cur, M, (int64_t)nd * G4);
-  cur = L.lstm.hp;
+  cur = k.w->hp;
   const Planes hp = carve_planes(cur, M, H);
   ReduceList rl;
   for (int l = nl - 1; l >= 0; --l) {
-    LstmParams p = lstm_layer_params(c, pg, L, l, lengths, B, T);
-    p.dh_out = L.lstm.dh;
-    p.dxproj = L.lstm.xproj;
+    LstmParams p = lstm_layer_params(k, l, lengths, B, T);
+    p.dh_out = k.w->dh;
+    p.dxproj = k.w->xproj;
     if ((rc = lstm_run(true, p, st))) return rc;
-    if ((rc = launch_split(L.lstm.xproj, (int64_t)nd * G4, M, nd * G4, dg, 0, st))) return rc;
-    const Planes in = lstm_in_planes(c, L, l, M);
-    for (int d = 0; d < nd; ++d) {
+    if ((rc = launch_split(k.w->xproj, (int64_t)nd * G4, M, nd * G4, dg, 0, st))) return rc;
+    const Planes in = lstm_in_planes(k, l, M);
+    for (int d = 0; d < nd && param_grads; ++d) {
       Planes dgd = dg;
       dgd.hi += (int64_t)d * G4;
       dgd.lo += (int64_t)d * G4;
       dgd.cols = G4;
-      if ((rc = launch_gemm_mn(dgd, in, pg.lstm[l][d][W_IH].g, pg.lstm[l][d][B_IH].g, 0, L.lstm.part[d][0], st, &rl))) return rc;
-      GANTTS_PDL_LAUNCH((lstm_hprev_planes_kernel), blocks_1d(M * H, 1024), 256, 0, st, L.lstm.h[l], lengths, B, T, H, nd,
+      if ((rc = launch_gemm_mn(dgd, in, k.p[l][d][W_IH].g, k.p[l][d][B_IH].g, 0, k.w->part[d][0], st, &rl))) return rc;
+      GANTTS_PDL_LAUNCH((lstm_hprev_planes_kernel), blocks_1d(M * H, 1024), 256, 0, st, k.w->h[l], lengths, B, T, H, nd,
                         d, hp.hi, hp.lo, hp.pitch);
       GANTTS_LAUNCH_CHECK("lstm_hprev_planes_kernel");
-      if ((rc = launch_gemm_mn(dgd, hp, pg.lstm[l][d][W_HH].g, nullptr, 0, L.lstm.part[d][1], st, &rl))) return rc;
+      if ((rc = launch_gemm_mn(dgd, hp, k.p[l][d][W_HH].g, nullptr, 0, k.w->part[d][1], st, &rl))) return rc;
     }
     if (l > 0) {
       Planes w, wt;
-      lstm_w_planes(c, L, l, &w, &wt);
+      lstm_w_planes(k, l, &w, &wt);
       EpiArgs e;
       e.epi = EPI_F32;
-      e.C = L.lstm.dh;
+      e.C = k.w->dh;
       e.ldc = nh;
       if (s.dropout > 0.f) {      // dh_{l-1} = mask_{l-1} * dX: LeakyReLU with slope 1 is the identity, then the mask
         e.act = GANTTS_ACT_LEAKY_DROPOUT;
         e.slope = 1.f;
         e.p = s.dropout;
-        e.seed = gantts_lstm_mask_seed(seed, l - 1);
+        e.seed = k.mask_seed(seed, l - 1);
       }
       if ((rc = launch_gemm_kk(dg, wt, e, st))) return rc;
+    } else if (din) {
+      // the rows [row0, M) of dgates against the rows [col0, col0 + cols) of W_ih^T's planes
+      Planes w, wt;
+      lstm_w_planes(k, 0, &w, &wt);
+      Planes a = dg;
+      a.hi += din->row0 * dg.pitch;
+      a.lo += din->row0 * dg.pitch;
+      a.rows = M - din->row0;
+      wt.hi += (int64_t)din->col0 * wt.pitch;
+      wt.lo += (int64_t)din->col0 * wt.pitch;
+      wt.rows = din->cols;
+      EpiArgs e;
+      e.epi = EPI_F32;
+      e.C = din->C;
+      e.ldc = din->ldc;
+      e.accumulate = din->accumulate;
+      if ((rc = launch_gemm_kk(a, wt, e, st))) return rc;
     }
+    if (!param_grads) continue;
     if ((rc = flush_reduce(rl, 0, st))) return rc;
     for (int d = 0; d < nd; ++d)
-      GANTTS_CUDA(cudaMemcpyAsync(pg.lstm[l][d][B_HH].g, pg.lstm[l][d][B_IH].g, (size_t)G4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      GANTTS_CUDA(cudaMemcpyAsync(k.p[l][d][B_HH].g, k.p[l][d][B_IH].g, (size_t)G4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
   }
   return GANTTS_OK;
 }
@@ -1081,7 +1166,7 @@ static int lstm_stack_bwd(const gantts_gan_step_t* c, const StepLayout& L, const
 // the same offsets whatever the call's shape.
 static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
   const int64_t M = (int64_t)c->B * c->T;
-  const int dD = c->d.dims[0];
+  const int dD = d_in_width(c);
   *L = StepLayout{};      // the buffers of absent layers stay null
   Arena a{base};
   L->scal = a.f32(S_COUNT);
@@ -1093,7 +1178,7 @@ static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
   L->g_static = a.f32((size_t)M * c->n_static);
   L->g_yhat = a.f32((size_t)M * c->g.dims[c->g.num_layers]);
   L->g_grads = a.f32(g_param_count(c));
-  L->d_grads = a.f32(mlp_param_count(c->d));
+  L->d_grads = a.f32(d_param_count(c));
   L->g_tape_bytes = gantts_mlp_tape_bytes(&c->g, M);
   L->g_tape = a.take(L->g_tape_bytes);
   L->d_tape_bytes = gantts_mlp_tape_bytes(&c->d, 2 * M);
@@ -1105,7 +1190,8 @@ static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
   L->opt_partial = a.f32(OPT_MAX_BLOCKS);
   layout_highway(c, M, a, &L->hw);
   layout_sru(c, M, a, &L->sru);
-  layout_lstm(c, M, a, &L->lstm);
+  layout_lstm(c->lstm, M, c->g.dims[c->g.num_layers], 0, a, &L->lstm);
+  layout_lstm(c->d_lstm, 2 * M, 0, 2 * (int64_t)c->B, a, &L->d_lstm);
   L->total = (size_t)(a.cur - base) + 256;
 }
 
@@ -1124,6 +1210,7 @@ struct Step {
   int d_in, d_out, dD, nS;  // d_in: the width (and row stride) of x -- the SRU or LSTM stack's input width when there is one
   int cond_w, nA;           // conditioning columns of D's input (copies of x), adversarial columns
   bool has_d, has_adv;
+  bool train;               // dropout on (every call but the eval phase)
   bool adv_window;          // the adversarial columns are one contiguous window of y_hat_static
   HighwayArgs hwa;
   ColList static_cols, adv_cols, real_cols;
@@ -1131,6 +1218,9 @@ struct Step {
   void* stream;
   cudaStream_t st;
   const HighwayArgs* hw() const { return c->highway.static_dim > 0 ? &hwa : nullptr; }
+  bool d_rnn() const { return c->d_lstm.num_layers > 0; }
+  // the discriminator's LSTM stack in forward `which` (1 stacked, 2 adversarial)
+  LstmStack d_lstm(int which) const { return LstmStack{&c->d_lstm, &L.d_lstm, pd.lstm, which}; }
 };
 
 // batch prologue (train.py:528-535): sequence mask and loss scales.  zero_norms: a step that steps neither model (eval)
@@ -1170,7 +1260,9 @@ static int generator_fwd(Step& s, bool train) {
   const float* gen_out = s.y_hat;
   int rc;
   if (c->lstm.num_layers > 0) {
-    if ((rc = lstm_stack_fwd(c, s.g, s.pg, L, s.x, s.lengths, s.B, s.T, s.seed, train, s.st))) return rc;
+    Planes top;
+    if ((rc = mlp_tape_input_planes(&s.g, M, L.g_tape, L.g_tape_bytes, &top))) return rc;
+    if ((rc = lstm_stack_fwd(g_lstm(c, L, s.pg), s.x, s.d_in, top, s.lengths, s.B, s.T, s.seed, train, s.st))) return rc;
     if ((rc = mlp_fwd_impl(&s.g, nullptr, 0, M, L.lstm.out, s.d_out, L.g_tape, L.g_tape_bytes, s.st, true))) return rc;
     GANTTS_CUDA(cudaMemcpyAsync(s.y_hat, s.x, (size_t)M * s.d_in * sizeof(float), cudaMemcpyDeviceToDevice, s.st));
     gen_out = L.lstm.out;
@@ -1223,8 +1315,23 @@ static int generator_bwd(Step& s) {
                          s.pg.gW, s.pg.gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, -1, direct)))
     return rc;
   if (sru) return sru_stack_bwd(c, L, s.pg, s.x, s.B, s.T, s.seed, s.st);
-  if (lstm) return lstm_stack_bwd(c, L, s.pg, s.lengths, s.B, s.T, s.seed, s.st);
+  if (lstm) return lstm_stack_bwd(g_lstm(c, L, s.pg), s.lengths, s.B, s.T, s.seed, true, nullptr, s.st);
   return GANTTS_OK;
+}
+
+// A recurrent discriminator's LSTM stack on the stacked batch (2B sequences: the lengths twice) or the adversarial one,
+// from x (the conditioned input d_in, row stride dD) or from input planes the caller gathered (x = nullptr), up to the
+// top h in hidden2out's tape input planes.
+static int discriminator_stack_fwd(Step& s, bool stacked, const float* x, const Planes& top) {
+  const int64_t* lengths = s.lengths;
+  if (stacked) {
+    lengths = s.L.d_lstm.lengths;
+    for (int half = 0; half < 2; ++half)
+      GANTTS_CUDA(cudaMemcpyAsync(s.L.d_lstm.lengths + half * s.B, s.lengths, (size_t)s.B * sizeof(int64_t),
+                                  cudaMemcpyDeviceToDevice, s.st));
+  }
+  return lstm_stack_fwd(s.d_lstm(stacked ? 1 : 2), x, s.dD, top, lengths, stacked ? 2 * s.B : s.B, s.T, s.seed, s.train,
+                        s.st);
 }
 
 // Discriminator forward into L.d_out.  stacked: the [real | fake] batch of 2M rows (train.py:261,265), real = the
@@ -1236,9 +1343,11 @@ static int discriminator_fwd(Step& s, bool stacked) {
   const StepLayout& L = s.L;
   const int64_t M = s.M, rows = stacked ? 2 * M : M;
   int rc;
+  Planes tape_in;
+  if ((rc = mlp_tape_input_planes(&s.d, rows, L.d_tape, L.d_tape_bytes, &tape_in))) return rc;
+  // a recurrent D (LSTMRNN / GRURNN): its stack reads the input planes, hidden2out the stack's top h in the tape
+  const Planes din = s.d_rnn() ? lstm_in_planes(s.d_lstm(stacked ? 1 : 2), 0, rows) : tape_in;
   if (!s.cond_w) {
-    Planes din;
-    if ((rc = mlp_tape_input_planes(&s.d, rows, L.d_tape, L.d_tape_bytes, &din))) return rc;
     if (stacked) {
       GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(2 * M * s.nA, 1024), 256, 0, s.st, s.y, s.d_out, s.real_cols, M,
                         s.y_hat_static, s.nS, s.adv_cols, M, din.hi, din.lo, din.pitch);
@@ -1250,6 +1359,7 @@ static int discriminator_fwd(Step& s, bool stacked) {
                         nullptr, 0, none, 0, din.hi, din.lo, din.pitch);
       GANTTS_LAUNCH_CHECK("gather_planes_kernel(adv)");
     }
+    if (s.d_rnn() && (rc = discriminator_stack_fwd(s, stacked, nullptr, tape_in))) return rc;
     return mlp_fwd_impl(&s.d, nullptr, 0, rows, L.d_out, 1, L.d_tape, L.d_tape_bytes, s.stream, true);
   }
   const int dD = s.dD;
@@ -1262,6 +1372,10 @@ static int discriminator_fwd(Step& s, bool stacked) {
     for (int64_t half = 0; half < 2; ++half)
       GANTTS_CUDA(cudaMemcpy2DAsync(L.d_in + half * M * dD, (size_t)dD * sizeof(float), s.x, (size_t)s.d_in * sizeof(float),
                                     (size_t)s.cond_w * sizeof(float), (size_t)M, cudaMemcpyDeviceToDevice, s.st));
+  }
+  if (s.d_rnn()) {
+    if ((rc = discriminator_stack_fwd(s, stacked, L.d_in + (stacked ? 0 : M * dD), tape_in))) return rc;
+    return mlp_fwd_impl(&s.d, nullptr, 0, rows, L.d_out, 1, L.d_tape, L.d_tape_bytes, s.stream, true);
   }
   return gantts_mlp_fwd(&s.d, L.d_in + (stacked ? 0 : M * dD), dD, rows, L.d_out, 1, L.d_tape, L.d_tape_bytes, s.stream);
 }
@@ -1280,9 +1394,27 @@ static int discriminator_bwd(Step& s, bool stacked, bool input_grad = true) {
   // in place: row r of the batch -> g_static[r - skip]
   float* gx = !input_grad ? nullptr : (s.adv_window ? L.g_static + s.adv_cols.c[0] - skip * (int64_t)s.nS : L.g_din);
   int rc;
-  if ((rc = mlp_bwd_impl(&s.d, L.g_dout, 1, L.d_out, 1, skip + M, L.d_tape, L.d_tape_bytes, gx, s.adv_window ? s.nS : s.dD,
-                         skip, gW, gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, s.adv_window ? 1 : -1)))
+  if (s.d_rnn()) {
+    // hidden2out's backward gives dL/dh of the stack's top layer; the stack's backward computes the parameter gradients
+    // on the stacked pass only, and the input gradient w.r.t. the adversarial columns of the fake rows alone
+    const LstmStack k = s.d_lstm(stacked ? 1 : 2);
+    const int nh = lstm_ndir(s.c->d_lstm) * s.c->d_lstm.hidden;
+    if ((rc = mlp_bwd_impl(&s.d, L.g_dout, 1, L.d_out, 1, skip + M, L.d_tape, L.d_tape_bytes, k.w->dh, nh, 0, gW, gb, 0,
+                           L.mlp_ws, L.mlp_ws_bytes, s.stream, 0)))
+      return rc;
+    // row r of the batch -> row r - skip of g_static's adversarial window (in place), else of g_din's adversarial columns
+    LstmInGrad din{};
+    if (input_grad) {
+      const int64_t rs = s.adv_window ? s.nS : s.dD;
+      din = LstmInGrad{skip, s.cond_w, s.nA, (s.adv_window ? gx : gx + s.cond_w) + skip * rs, rs, s.adv_window ? 1 : 0};
+    }
+    if ((rc = lstm_stack_bwd(k, stacked ? L.d_lstm.lengths : s.lengths, stacked ? 2 * s.B : s.B, s.T, s.seed, stacked,
+                             input_grad ? &din : nullptr, s.st)))
+      return rc;
+  } else if ((rc = mlp_bwd_impl(&s.d, L.g_dout, 1, L.d_out, 1, skip + M, L.d_tape, L.d_tape_bytes, gx, s.adv_window ? s.nS : s.dD,
+                                skip, gW, gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, s.adv_window ? 1 : -1))) {
     return rc;
+  }
   if (s.adv_window || !input_grad) return GANTTS_OK;
   scatter_cols_list_add_kernel<<<blocks_1d(M * s.nA, 1024), 256, 0, s.st>>>(L.g_din + skip * s.dD + s.cond_w, s.dD,
                                                                              L.g_static, s.nS, s.adv_cols, M);
@@ -1305,6 +1437,12 @@ extern "C" uint64_t gantts_lstm_mask_seed(uint64_t seed, int layer) {
   return gantts_mlp_layer_seed(gantts_gan_step_seed(seed, 3), 2 * GANTTS_MAX_SRU_LAYERS + layer);
 }
 
+// after every generator LSTM index 2 * GANTTS_MAX_SRU_LAYERS + layer of the same stream
+extern "C" uint64_t gantts_d_lstm_mask_seed(uint64_t seed, int which, int layer) {
+  return gantts_mlp_layer_seed(gantts_gan_step_seed(seed, 3),
+                               2 * GANTTS_MAX_SRU_LAYERS + GANTTS_MAX_LSTM_LAYERS * which + layer);
+}
+
 extern "C" size_t gantts_gan_step_workspace_bytes(const gantts_gan_step_t* c) {
   if (check_step(c)) return 0;
   StepLayout L;
@@ -1320,7 +1458,7 @@ extern "C" int gantts_gan_step_grad_buffer(const gantts_gan_step_t* c, void* wor
   StepLayout L;
   layout(c, reinterpret_cast<char*>(al256(reinterpret_cast<uintptr_t>(workspace))), &L);
   *ptr = which == 0 ? L.g_grads : L.d_grads;
-  *count = which == 0 ? g_param_count(c) : mlp_param_count(c->d);
+  *count = which == 0 ? g_param_count(c) : d_param_count(c);
   return GANTTS_OK;
 }
 
@@ -1373,9 +1511,10 @@ extern "C" int gantts_gan_step_shaped(const gantts_gan_step_t* c, int B, int T, 
   s.y_hat = y_hat;
   s.y_hat_static = y_hat_static;
   s.seed = seed;
+  s.train = !(phases & GANTTS_STEP_EVAL);
   s.d_in = gen_in_width(c);
   s.d_out = c->g.dims[c->g.num_layers];
-  s.dD = c->d.dims[0];
+  s.dD = d_in_width(c);
   const int nS = s.nS = c->n_static;
   s.has_d = c->w_d > 0.f;
   s.has_adv = s.has_d && c->adv_w > 0.f && !d_only;

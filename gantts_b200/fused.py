@@ -1,5 +1,5 @@
 """Fused GAN step: ONE C call (gantts_gan_step) per mini-batch for an MLP, In2OutHighwayNet, In2OutRNNHighwayNet or
-SRURNN generator + MLP discriminator -- the whole of reference train.py:528-580 enqueued on the current stream without a
+SRURNN generator + MLP, LSTMRNN or GRURNN discriminator -- the whole of reference train.py:528-580 enqueued on the current stream without a
 single host synchronisation (SURVEY.md 8f row 3).  Not drop-in for train.py (which owns its step
 functions); offered next to the compatible modular path (gantts_b200.step.GanTrainer), which also runs
 the LSTMRNN / GRURNN generators.
@@ -44,8 +44,20 @@ def _generator_parts(model_g):
                        "are); train it with gantts_b200.step.GanTrainer" % type(model_g).__name__)
 
 
+def _discriminator_parts(model_d):
+    """(nn.LSTM or None, [MLP layers..., last layer]) of a discriminator the fused step runs: an MLP, or an LSTMRNN / GRURNN
+    (reference train.py:774 builds the class hp.discriminator names; GRURNN keeps its nn.LSTM as .gru) whose last layer is
+    hidden2out."""
+    if isinstance(model_d, models._LSTMNet):
+        return _check_lstm(getattr(model_d, model_d._rnn_attr)), [model_d.hidden2out]
+    if hasattr(model_d, "layers") and hasattr(model_d, "last_linear"):
+        return None, list(model_d.layers) + [model_d.last_linear]
+    raise RuntimeError("FusedGanStep: discriminator %s is not supported (MLP, LSTMRNN and GRURNN are); train it with "
+                       "gantts_b200.step.GanTrainer" % type(model_d).__name__)
+
+
 def _check_lstm(lstm):
-    """The nn.LSTM of an In2OutRNNHighwayNet, if the fused step implements it."""
+    """An nn.LSTM of a generator or discriminator, if the fused step implements it."""
     why = None
     if getattr(lstm, "proj_size", 0) > 0:
         why = "proj_size > 0"
@@ -79,6 +91,13 @@ def _fill_sru(desc, cells):
     desc.act = int(c0.activation_type)
     desc.dropout = float(c0.dropout) if len(cells) > 1 else 0.0
     desc.rnn_dropout = float(c0.rnn_dropout)
+
+
+def _fill_lstm(desc, lstm):
+    """The shape block of gantts_lstm_stack_t from an nn.LSTM (its tensors go into the step's tensor tables)."""
+    desc.num_layers, desc.in_dim, desc.hidden = lstm.num_layers, lstm.input_size, lstm.hidden_size
+    desc.bidirectional = int(bool(lstm.bidirectional))
+    desc.dropout = float(lstm.dropout) if lstm.num_layers > 1 else 0.0
 
 
 def _fill_mlp(desc, layers, p, last_act):
@@ -142,8 +161,9 @@ class FusedGanStep(object):
         c = _lib.GanStepT()
         c.B, c.T = self.B, self.T
         gate, sru, lstm, g_layers = _generator_parts(model_g)
+        d_lstm, d_layers = _discriminator_parts(model_d)
         _fill_mlp(c.g, g_layers, getattr(model_g, "dropout_p", 0.0), _lib.ACT_NONE)
-        _fill_mlp(c.d, list(model_d.layers) + [model_d.last_linear], model_d.dropout_p, _lib.ACT_SIGMOID)
+        _fill_mlp(c.d, d_layers, getattr(model_d, "dropout_p", 0.0), _lib.ACT_SIGMOID)
         if getattr(model_g, "last_sigmoid", False) or not model_d.last_sigmoid:
             raise RuntimeError("FusedGanStep: generator must be linear-output, discriminator sigmoid-output")
         if gate is not None:
@@ -151,10 +171,9 @@ class FusedGanStep(object):
         if sru:
             _fill_sru(c.sru, sru)
         if lstm is not None:
-            ls = c.lstm
-            ls.num_layers, ls.in_dim, ls.hidden = lstm.num_layers, lstm.input_size, lstm.hidden_size
-            ls.bidirectional = int(bool(lstm.bidirectional))
-            ls.dropout = float(lstm.dropout) if lstm.num_layers > 1 else 0.0
+            _fill_lstm(c.lstm, lstm)
+        if d_lstm is not None:
+            _fill_lstm(c.d_lstm, d_lstm)
         # the tensor tables, in model.parameters() order; the C step binds them to its stages from the shapes above
         self._params = list(model_g.parameters()) + list(model_d.parameters())
         self._ng = len(list(model_g.parameters()))          # generator tensors: their optimiser state comes first

@@ -410,6 +410,18 @@ typedef struct {
   int optimizer;
   float beta1, beta2;
   int64_t opt_step;
+  /* Recurrent discriminator (reference LSTMRNN models.py:193-213, or GRURNN :170-190 -- also an nn.LSTM -- with
+   * last_sigmoid=True; train.py:774 builds the class hp.discriminator names): num_layers > 0.  num_layers = 0 (a zero-filled
+   * block) is the MLP discriminator above.  Then d is hidden2out alone (d.num_layers == 1, d.dims[0] = ndir * hidden,
+   * d.dims[1] = 1, last_act = SIGMOID), in_dim = the discriminator's input width (n_adv, plus the conditioning columns when
+   * d_conditioned), and every discriminator forward runs the stack with the packed-sequence semantics of
+   * gantts_lstm_layer_fwd on lengths_dev (train.py:261,265,307 pass `lengths`).  The stacked [real | fake] forward runs 2B
+   * sequences, so the configured B is at most 64 (LSTM_MAX_B / 2).  In training the output of every layer but the last is
+   * multiplied by gantts_dropout(ones[rows][ndir * hidden], dropout, gantts_d_lstm_mask_seed(seed, which, layer)), rows = 2B
+   * T on the stacked forward (which = 1) and B T on the adversarial one (which = 2).  The d_tensors table is
+   * model_d.parameters(): per layer and direction W_ih, W_hh, b_ih, b_hh, then hidden2out's weight and bias; b_ih and b_hh
+   * get the same gradient.  Only the adversarial columns of the fake rows receive an input gradient. */
+  gantts_lstm_stack_t d_lstm;
 } gantts_gan_step_t;
 #define GANTTS_OPT_ADAGRAD 0
 #define GANTTS_OPT_ADAM 1
@@ -447,6 +459,10 @@ uint64_t gantts_sru_mask_seed(uint64_t seed, int layer, int which);
 /* Seed of the inter-layer dropout mask on the output of LSTM layer `layer` in a step called with `seed`: a stream of its
  * own, apart from the three MLP forwards and every SRU mask. */
 uint64_t gantts_lstm_mask_seed(uint64_t seed, int layer);
+/* Seed of the inter-layer dropout mask on the output of the recurrent discriminator's layer `layer` in forward `which`
+ * (1 stacked real|fake batch, 2 adversarial forward) of a step called with `seed`: a stream of its own, apart from every
+ * seed above. */
+uint64_t gantts_d_lstm_mask_seed(uint64_t seed, int which, int layer);
 
 size_t gantts_gan_step_workspace_bytes(const gantts_gan_step_t* cfg);
 /* Flat gradient buffer inside `workspace` (which: 0 = generator, 1 = discriminator). */

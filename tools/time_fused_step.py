@@ -20,13 +20,17 @@ one process, round by round, the full fused step ("fused"), with --stage d_warmu
 (FusedGanStep.step(update_g=False): "fused_d_only"), and with --spoof the full step that also counts the spoofing rate of
 a reference discriminator (train.py:549-558: "fused_spoof").
 
+--rnn-d replaces the MLP discriminator of vc and tts_acoustic by a recurrent one, LSTMRNN(n, 1, 2, 256,
+bidirectional=True, dropout=0.5, last_sigmoid=True) with n = 59 (vc) or 425 + 58 conditioning + adversarial inputs
+(tts_acoustic), and times the fused step against the modular path as above.
+
 --dump-outputs DIR: after the timed loop, DIR/<workload>/ receives what the fused path's caller holds after its last
 step, as float32 .npy files: the loss vector, y_hat, y_hat_static, both flat gradient buffers and every updated
 parameter of both models.  Two builds run with the same arguments can then be compared array by array.
 
     python tools/time_fused_step.py [--workload vc|cfg1|tts_acoustic|tts_duration|cfg3|all] [--rounds R] [--steps K]
                                     [--warmup W] [--json OUT] [--dump-outputs DIR] [--stage adversarial|d_warmup]
-                                    [--spoof]
+                                    [--spoof] [--rnn-d]
 """
 import argparse
 import json
@@ -78,7 +82,7 @@ def hparams(name):
                          mask_nth_mgc_for_adv_loss=0, discriminator_linguistic_condition=False)
 
 
-def models(w, dev):
+def models(w, dev, rnn_d=False):
     import gantts_b200
     M = gantts_b200.models
     torch.manual_seed(1234)
@@ -93,6 +97,9 @@ def models(w, dev):
         mg = M.In2OutRNNHighwayNet(in_dim=177, out_dim=177, static_dim=59, num_hidden=3, hidden_dim=512,
                                    bidirectional=True, dropout=0.5)
         md = M.MLP(59, 1, 2, 256, dropout=0.5, last_sigmoid=True)
+    if rnn_d:
+        torch.manual_seed(4321)
+        md = M.LSTMRNN(md.layers[0].weight.shape[1], 1, 2, 256, bidirectional=True, dropout=0.5, last_sigmoid=True)
     return mg.to(dev).train(), md.to(dev).train()
 
 
@@ -106,7 +113,7 @@ def dump(out_dir, fs, mg, md):
         np.save(os.path.join(out_dir, k + ".npy"), t.detach().float().cpu().numpy())
 
 
-def run(name, w, rounds, steps, warmup, dev, dump_dir=None, stage="adversarial", spoof=False):
+def run(name, w, rounds, steps, warmup, dev, dump_dir=None, stage="adversarial", spoof=False, rnn_d=False):
     from gantts_b200 import fused, step as gstep
     from oracle import nnmnkwii_port as nnp
     B, T = w["B"], w["T"]
@@ -118,7 +125,7 @@ def run(name, w, rounds, steps, warmup, dev, dump_dir=None, stage="adversarial",
     lengths = torch.full((B,), T, dtype=torch.int64, device=dev)
     adv_w = 1.0 if w["w_d"] > 0 else 0.0
     kw = dict(w_d=w["w_d"], mse_w=w["mse_w"], mge_w=w["mge_w"], optimizer=w["optimizer"], optimizer_params=w["okw"])
-    mg, md = models(w, dev)
+    mg, md = models(w, dev, rnn_d)
     fs = fused.FusedGanStep(mg, md, hp, B, T, seed=1, **kw)
     steps_of = {"fused": lambda: fs.step(x, y, lengths, adv_w=adv_w)}
     if stage == "d_warmup":
@@ -131,7 +138,7 @@ def run(name, w, rounds, steps, warmup, dev, dump_dir=None, stage="adversarial",
         fs_spoof = fused.FusedGanStep(*models(w, dev), hp, B, T, seed=2, reference_discriminator=ref_d, **kw)
         steps_of["fused_spoof"] = lambda: fs_spoof.step(x, y, lengths, adv_w=adv_w)
     if len(steps_of) == 1:
-        tr = gstep.GanTrainer(*models(w, dev), hp, **kw)
+        tr = gstep.GanTrainer(*models(w, dev, rnn_d), hp, **kw)
         R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(hp.windows, T)).to(dev)
         steps_of["modular"] = lambda: tr.step(x, y, lengths, R, adv_w=adv_w)
     for fn in steps_of.values():
@@ -150,7 +157,8 @@ def run(name, w, rounds, steps, warmup, dev, dump_dir=None, stage="adversarial",
             ms[k].append(a.elapsed_time(b) / steps)
     if dump_dir:
         dump(os.path.join(dump_dir, name), fs, mg, md)
-    out = {"workload": name, "B": B, "T": T, "rounds": rounds, "steps_per_round": steps}
+    out = {"workload": name, "B": B, "T": T, "rounds": rounds, "steps_per_round": steps,
+           "discriminator": type(md).__name__}
     for k, v in ms.items():
         med = float(np.median(v))
         out[k] = {"ms_per_step_median": round(med, 4), "ms_per_step_min": round(min(v), 4),
@@ -176,7 +184,11 @@ def main():
                     help="d_warmup: also time the discriminator warm-up step (update_g=False)")
     ap.add_argument("--spoof", action="store_true",
                     help="also time the full step with the spoofing-rate count of a reference discriminator")
+    ap.add_argument("--rnn-d", action="store_true",
+                    help="vc / tts_acoustic with an LSTMRNN discriminator (2 x 256 bidirectional) instead of the MLP")
     args = ap.parse_args()
+    if args.rnn_d and args.workload not in ("vc", "tts_acoustic"):
+        sys.exit("time_fused_step.py: --rnn-d times the vc and tts_acoustic workloads")
     if args.stage == "d_warmup" or args.spoof:
         ok = [k for k, w in WORKLOADS.items() if w["w_d"] > 0]
         if args.workload not in ok:
@@ -190,7 +202,7 @@ def main():
     for name in (list(WORKLOADS) if args.workload == "all" else [args.workload]):
         w = WORKLOADS[name]
         rounds, steps, warmup = [d if a is None else a for a, d in zip((args.rounds, args.steps, args.warmup), w["runs"])]
-        r = run(name, w, rounds, steps, warmup, dev, args.dump_outputs, args.stage, args.spoof)
+        r = run(name, w, rounds, steps, warmup, dev, args.dump_outputs, args.stage, args.spoof, args.rnn_d)
         print(json.dumps(r), flush=True)
         res["results"].append(r)
     print(json.dumps({"gpu": res["gpu"]}))
