@@ -708,10 +708,12 @@ static int check_step(const gantts_gan_step_t* c) {
 }
 
 // out_cols: width of the head's fp32 output kept in w->out (the generator's hidden2out); seqs: sequences whose lengths
-// w->lengths holds (the discriminator's stacked batch; 0 = none)
-static void layout_lstm(const gantts_lstm_stack_t& ls, int64_t M, int out_cols, int64_t seqs, Arena& a, LstmWs* w) {
+// w->lengths holds (the discriminator's stacked batch; 0 = none).  bwd = false: a stack that only runs forward (the
+// spoofing-rate count's reference discriminator) -- no dh, dgates or hprev planes and no split-K partials.
+static void layout_lstm(const gantts_lstm_stack_t& ls, int64_t M, int out_cols, int64_t seqs, Arena& a, LstmWs* w,
+                        bool bwd = true) {
   const int nl = ls.num_layers, H = nl > 0 ? ls.hidden : 0, nd = lstm_ndir(ls), n4 = nd * 4 * H;
-  const bool on = nl > 0;
+  const bool on = nl > 0, on_bwd = on && bwd;
   size_t part_ih = 0, part_hh = 0;
   for (int l = 0; l < nl; ++l) {
     const int ni = lstm_nin(ls, l);
@@ -727,12 +729,12 @@ static void layout_lstm(const gantts_lstm_stack_t& ls, int64_t M, int out_cols, 
   }
   w->xproj = a.f32((size_t)M * n4);
   w->out = a.f32(on ? (size_t)M * out_cols : 0);
-  w->dh = a.f32((size_t)M * nd * H);
-  w->dg = a.take(on ? 2 * plane_bytes(M, n4) : 0);
-  w->hp = a.take(on ? 2 * plane_bytes(M, H) : 0);
+  w->dh = a.f32(bwd ? (size_t)M * nd * H : 0);
+  w->dg = a.take(on_bwd ? 2 * plane_bytes(M, n4) : 0);
+  w->hp = a.take(on_bwd ? 2 * plane_bytes(M, H) : 0);
   for (int d = 0; d < 2; ++d) {
-    w->part[d][0] = reinterpret_cast<float*>(a.take(d < nd ? part_ih : 0));
-    w->part[d][1] = reinterpret_cast<float*>(a.take(d < nd ? part_hh : 0));
+    w->part[d][0] = reinterpret_cast<float*>(a.take(bwd && d < nd ? part_ih : 0));
+    w->part[d][1] = reinterpret_cast<float*>(a.take(bwd && d < nd ? part_hh : 0));
   }
   w->bar = reinterpret_cast<unsigned int*>(a.take(on ? 256 : 0));
   w->lengths = reinterpret_cast<int64_t*>(a.take(on ? (size_t)seqs * sizeof(int64_t) : 0));
@@ -1694,6 +1696,119 @@ extern "C" int gantts_spoof_count(const gantts_mlp_t* d, const float* y_hat_stat
   GANTTS_LAUNCH_CHECK("gather_planes_kernel(spoof)");
   if ((rc = mlp_fwd_impl(&m, nullptr, 0, rows, dout, 1, tape, tape_bytes, stream, true))) return rc;
   GANTTS_PDL_LAUNCH((spoof_count_kernel), 1, RED_THREADS, 0, st, dout, lengths_dev, B, T, count_dev);
+  GANTTS_LAUNCH_CHECK("spoof_count_kernel");
+  return GANTTS_OK;
+}
+
+// ---- the same count with a recurrent reference discriminator (LSTMRNN / GRURNN with last_sigmoid, train.py:779-781
+// builds it from hp.discriminator like D): the adversarial columns go into layer 0's input planes, the LSTM stack runs
+// forward with dropout off over the B packed sequences, its top h goes into hidden2out's tape input planes, and the
+// one-output sigmoid head and the threshold count follow.  Workspace, laid out at the call's B * T rows: the stack's
+// forward buffers (layout_lstm without the backward ones), hidden2out's tape, its output [rows].
+struct SpoofLstmLayout {
+  LstmWs lstm;
+  char* tape;
+  size_t tape_bytes;
+  float* dout;
+  size_t total;
+};
+
+static void layout_spoof_lstm(const gantts_lstm_stack_t& ls, const gantts_mlp_t& head, int64_t rows, char* base,
+                              SpoofLstmLayout* L) {
+  *L = SpoofLstmLayout{};
+  Arena a{base};
+  layout_lstm(ls, rows, 0, 0, a, &L->lstm, false);
+  L->tape_bytes = gantts_mlp_tape_bytes(&head, rows);
+  L->tape = a.take(L->tape_bytes);
+  L->dout = a.f32((size_t)rows);
+  L->total = (size_t)(a.cur - base);
+}
+
+static int check_spoof_lstm(const gantts_lstm_stack_t* ls, const gantts_mlp_t* head, int B, int T) {
+  GANTTS_CHECK_ARG(ls && head, "spoof_count_lstm: null reference discriminator");
+  GANTTS_CHECK_ARG(ls->num_layers >= 1 && ls->num_layers <= GANTTS_MAX_LSTM_LAYERS,
+                   "spoof_count_lstm: LSTM layer count %d not in [1, %d] (count with GanTrainer)", ls->num_layers,
+                   GANTTS_MAX_LSTM_LAYERS);
+  GANTTS_CHECK_ARG(ls->hidden >= 4 && ls->hidden % 4 == 0,
+                   "spoof_count_lstm: LSTM hidden size %d is not a positive multiple of 4", ls->hidden);
+  GANTTS_CHECK_ARG(ls->bidirectional == 0 || ls->bidirectional == 1, "spoof_count_lstm: bad LSTM bidirectional %d",
+                   ls->bidirectional);
+  GANTTS_CHECK_ARG(ls->in_dim >= 1, "spoof_count_lstm: bad LSTM in_dim %d", ls->in_dim);
+  GANTTS_CHECK_ARG(B >= 1 && T >= 1, "spoof_count_lstm: bad batch shape");
+  GANTTS_CHECK_ARG(B <= LSTM_MAX_B, "spoof_count_lstm: an LSTM stack runs at most LSTM_MAX_B = %d sequences (B = %d)",
+                   LSTM_MAX_B, B);
+  GANTTS_CHECK_ARG((int64_t)B * T < (1 << 24), "spoof_count_lstm: B * T = %lld frames, the float count is exact below 2^24",
+                   (long long)B * T);
+  const int nh = lstm_ndir(*ls) * ls->hidden;
+  GANTTS_CHECK_ARG(head->num_layers == 1 && head->dims[0] == nh && head->dims[1] == 1 && head->last_act == GANTTS_ACT_SIGMOID,
+                   "spoof_count_lstm: the head must be hidden2out alone, 1 layer of %d -> 1 with a sigmoid (got %d "
+                   "layer(s), input width %d)", nh, head->num_layers, head->dims[0]);
+  return GANTTS_OK;
+}
+
+extern "C" size_t gantts_spoof_count_lstm_workspace_bytes(const gantts_lstm_stack_t* ls, const gantts_mlp_t* head, int B,
+                                                          int T) {
+  if (check_spoof_lstm(ls, head, B, T)) return 0;
+  SpoofLstmLayout L;
+  layout_spoof_lstm(*ls, *head, (int64_t)B * T, nullptr, &L);
+  return L.total + 256;
+}
+
+extern "C" int gantts_spoof_count_lstm(const gantts_lstm_stack_t* ls, const float* const* lstm_tensors, int n_tensors,
+                                       const gantts_mlp_t* head, const float* y_hat_static, int n_static,
+                                       const int* adv_cols, int n_adv, const int64_t* lengths_dev, int B, int T,
+                                       float* count_dev, void* ws, size_t ws_bytes, void* stream) {
+  int rc = check_spoof_lstm(ls, head, B, T);
+  if (rc) return rc;
+  GANTTS_CHECK_ARG(lstm_tensors && y_hat_static && adv_cols && lengths_dev && count_dev && head->W[0] && head->b[0],
+                   "spoof_count_lstm: null pointer");
+  const int want = 4 * lstm_ndir(*ls) * ls->num_layers;
+  GANTTS_CHECK_ARG(n_tensors == want,
+                   "spoof_count_lstm: %d LSTM tensors, the stack has %d (W_ih, W_hh, b_ih, b_hh per layer and direction)",
+                   n_tensors, want);
+  for (int i = 0; i < n_tensors; ++i) GANTTS_CHECK_ARG(lstm_tensors[i], "spoof_count_lstm: null pointer (LSTM tensor %d)", i);
+  GANTTS_CHECK_ARG(n_adv >= 1 && n_adv <= GANTTS_MAX_COLS && n_adv == ls->in_dim,
+                   "spoof_count_lstm: %d adversarial columns != reference discriminator input width %d (it gets no "
+                   "linguistic conditioning, train.py:554-555)", n_adv, ls->in_dim);
+  GANTTS_CHECK_ARG(n_static >= 1, "spoof_count_lstm: bad n_static");
+  ColList cols;
+  cols.n = n_adv;
+  for (int i = 0; i < n_adv; ++i) {
+    GANTTS_CHECK_ARG(adv_cols[i] >= 0 && adv_cols[i] < n_static, "spoof_count_lstm: adversarial column %d out of range",
+                     adv_cols[i]);
+    cols.c[i] = adv_cols[i];
+  }
+  const size_t need = gantts_spoof_count_lstm_workspace_bytes(ls, head, B, T);
+  if (!ws || ws_bytes < need) {
+    set_error("spoof_count_lstm: workspace too small (%zu < %zu)", ws_bytes, need);
+    return GANTTS_E_WORKSPACE;
+  }
+  const int64_t rows = (int64_t)B * T;
+  SpoofLstmLayout L;
+  layout_spoof_lstm(*ls, *head, rows, reinterpret_cast<char*>(al256(reinterpret_cast<uintptr_t>(ws))), &L);
+  // the stack's tensors in model.parameters() order, bound like a step's tables (no gradients, no optimiser state)
+  gantts_step_tensors_t t{};
+  t.n = n_tensors;
+  for (int i = 0; i < n_tensors; ++i) t.param[i] = const_cast<float*>(lstm_tensors[i]);
+  ParamList pl;
+  pl.n = 0;
+  pl.total = 0;
+  bind_lstm(t, *ls, nullptr, &pl);
+  const LstmStack k{ls, &L.lstm, pl.lstm, 0};     // eval mode: the mask stream is never drawn
+  gantts_mlp_t m = *head;
+  m.dropout_p = 0.f;
+  const cudaStream_t st = as_stream(stream);
+  const Planes in0 = lstm_in_planes(k, 0, rows);
+  ColList none;
+  none.n = 0;
+  GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(rows * n_adv, 1024), 256, 0, st, y_hat_static, (int64_t)n_static, cols,
+                    rows, nullptr, 0, none, 0, in0.hi, in0.lo, in0.pitch);
+  GANTTS_LAUNCH_CHECK("gather_planes_kernel(spoof lstm)");
+  Planes top;
+  if ((rc = mlp_tape_input_planes(&m, rows, L.tape, L.tape_bytes, &top))) return rc;
+  if ((rc = lstm_stack_fwd(k, nullptr, 0, top, lengths_dev, B, T, 0, false, st))) return rc;
+  if ((rc = mlp_fwd_impl(&m, nullptr, 0, rows, L.dout, 1, L.tape, L.tape_bytes, stream, true))) return rc;
+  GANTTS_PDL_LAUNCH((spoof_count_kernel), 1, RED_THREADS, 0, st, L.dout, lengths_dev, B, T, count_dev);
   GANTTS_LAUNCH_CHECK("spoof_count_kernel");
   return GANTTS_OK;
 }

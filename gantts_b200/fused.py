@@ -56,7 +56,7 @@ def _discriminator_parts(model_d):
                        "gantts_b200.step.GanTrainer" % type(model_d).__name__)
 
 
-def _check_lstm(lstm):
+def _check_lstm(lstm, who="FusedGanStep"):
     """An nn.LSTM of a generator or discriminator, if the fused step implements it."""
     why = None
     if getattr(lstm, "proj_size", 0) > 0:
@@ -68,8 +68,8 @@ def _check_lstm(lstm):
     elif lstm.num_layers > _lib.MAX_LSTM_LAYERS:
         why = "%d layers (at most %d)" % (lstm.num_layers, _lib.MAX_LSTM_LAYERS)
     if why is not None:
-        raise RuntimeError("FusedGanStep: an nn.LSTM with %s is not supported; train it with gantts_b200.step.GanTrainer"
-                           % why)
+        raise RuntimeError("%s: an nn.LSTM with %s is not supported%s" % (
+            who, why, "; train it with gantts_b200.step.GanTrainer" if who == "FusedGanStep" else ""))
     return lstm
 
 
@@ -122,11 +122,17 @@ def adversarial_columns(hp):
 
 
 def check_reference_discriminator(model_ref, n_adv, who):
-    """The reference discriminator of the spoofing-rate count (train.py:549-558): an MLP with one sigmoid output whose
-    input is the n_adv adversarial columns alone."""
-    if not (hasattr(model_ref, "layers") and hasattr(model_ref, "last_linear")) or not model_ref.last_sigmoid:
-        raise RuntimeError("%s: the reference discriminator must be a sigmoid-output MLP" % who)
-    width = int(model_ref.layers[0].weight.shape[1] if len(model_ref.layers) else model_ref.last_linear.weight.shape[1])
+    """The reference discriminator of the spoofing-rate count (train.py:549-558): an MLP, or an LSTMRNN / GRURNN
+    (train.py:779-781 builds it from hp.discriminator like D), with one sigmoid output and whose input is the n_adv
+    adversarial columns alone."""
+    if isinstance(model_ref, models._LSTMNet):
+        if not model_ref.last_sigmoid:
+            raise RuntimeError("%s: the reference discriminator must have a sigmoid output (last_sigmoid=True)" % who)
+        width = int(_check_lstm(getattr(model_ref, model_ref._rnn_attr), who).input_size)
+    elif not (hasattr(model_ref, "layers") and hasattr(model_ref, "last_linear")) or not model_ref.last_sigmoid:
+        raise RuntimeError("%s: the reference discriminator must be a sigmoid-output MLP, LSTMRNN or GRURNN" % who)
+    else:
+        width = int(model_ref.layers[0].weight.shape[1] if len(model_ref.layers) else model_ref.last_linear.weight.shape[1])
     if width != n_adv:
         raise RuntimeError("%s: the reference discriminator takes %d inputs, but train.py:549-555 feeds it the %d "
                            "adversarial columns alone (no linguistic conditioning)" % (who, width, n_adv))
@@ -142,7 +148,9 @@ class FusedGanStep(object):
 
         ``reference_discriminator``: the frozen discriminator of the adversarial stage (train.py --checkpoint-r); every
         step then counts the frames of the pre-update y_hat_static it takes for natural (train.py:549-558) into the
-        device scalar ``spoof_count``.  It runs with dropout off, sees no linguistic conditioning and is never updated."""
+        device scalar ``spoof_count``.  It runs with dropout off, sees no linguistic conditioning and is never updated.
+        It is an MLP, or an LSTMRNN / GRURNN (train.py:779-781 builds it from hp.discriminator like D) of at most 3 layers
+        and a configured B of at most 128, whose stack runs over the call's packed sequences."""
         lib = _lib.load()
         if optimizer not in ("Adagrad", "Adam"):
             raise RuntimeError("FusedGanStep: no native optimiser %r (Adagrad and Adam are the ones hparams.py uses)" % optimizer)
@@ -242,15 +250,30 @@ class FusedGanStep(object):
         self.ref_d = reference_discriminator
         if reference_discriminator is not None:
             check_reference_discriminator(reference_discriminator, len(acols), "FusedGanStep")
-            ref_layers = list(reference_discriminator.layers) + [reference_discriminator.last_linear]
+            self._ref_lstm = None
+            if isinstance(reference_discriminator, models._LSTMNet):
+                # LSTMRNN / GRURNN: its nn.LSTM's tensors (model.parameters() order), then hidden2out as the head
+                ref_rnn = getattr(reference_discriminator, reference_discriminator._rnn_attr)
+                self._ref_lstm = _lib.LstmStackT()
+                _fill_lstm(self._ref_lstm, ref_rnn)
+                ref_layers = [reference_discriminator.hidden2out]
+                self._ref_rnn_params = list(ref_rnn.parameters())
+            else:
+                ref_layers = list(reference_discriminator.layers) + [reference_discriminator.last_linear]
+                self._ref_rnn_params = []
             self._ref_params = [t for l in ref_layers for t in (l.weight, l.bias)]
-            ops.require_cuda(*self._ref_params)
-            if not all(t.is_contiguous() for t in self._ref_params):
+            ops.require_cuda(*(self._ref_rnn_params + self._ref_params))
+            if not all(t.is_contiguous() for t in self._ref_rnn_params + self._ref_params):
                 raise RuntimeError("gantts_b200: parameters must be contiguous")
             self._ref_desc = _lib.MlpT()
             _fill_mlp(self._ref_desc, ref_layers, 0.0, _lib.ACT_SIGMOID)
             self._adv_cols = (ctypes.c_int * len(acols))(*acols)
-            rbytes = lib.gantts_spoof_count_workspace_bytes(ctypes.byref(self._ref_desc), self.B * self.T)
+            if self._ref_lstm is not None:
+                # laid out for the configured (B, T), which holds every call's (b, t); refuses B > 128
+                rbytes = lib.gantts_spoof_count_lstm_workspace_bytes(ctypes.byref(self._ref_lstm),
+                                                                     ctypes.byref(self._ref_desc), self.B, self.T)
+            else:
+                rbytes = lib.gantts_spoof_count_workspace_bytes(ctypes.byref(self._ref_desc), self.B * self.T)
             if rbytes == 0:
                 raise RuntimeError("gantts_b200 spoof_count config rejected: %s" % lib.gantts_last_error_string().decode())
             self._ref_ws = torch.empty(rbytes, dtype=torch.uint8, device=dev)
@@ -399,6 +422,14 @@ class FusedGanStep(object):
             d.W[i], d.b[i] = w.data_ptr(), b.data_ptr()
         ws = self._ref_ws
         b, t, n_static = self.y_hat_static.shape
+        if self._ref_lstm is not None:
+            tensors = (ctypes.c_void_p * len(self._ref_rnn_params))(*[p.data_ptr() for p in self._ref_rnn_params])
+            _lib.check(lib.gantts_spoof_count_lstm(ctypes.byref(self._ref_lstm), tensors, len(self._ref_rnn_params),
+                                                   ctypes.byref(d), self.y_hat_static.data_ptr(), n_static,
+                                                   self._adv_cols, len(self._adv_cols), lengths.data_ptr(), b, t,
+                                                   self.spoof_count.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                   ops._stream()))
+            return
         _lib.check(lib.gantts_spoof_count(ctypes.byref(d), self.y_hat_static.data_ptr(), n_static,
                                           self._adv_cols, len(self._adv_cols), lengths.data_ptr(), b, t,
                                           self.spoof_count.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream()))

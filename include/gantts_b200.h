@@ -496,6 +496,20 @@ size_t gantts_spoof_count_workspace_bytes(const gantts_mlp_t* d, int64_t rows);
 int gantts_spoof_count(const gantts_mlp_t* d, const float* y_hat_static, int n_static, const int* adv_cols, int n_adv,
                        const int64_t* lengths_dev, int B, int T, float* count_dev, void* ws, size_t ws_bytes,
                        void* stream);
+/* The same count with a recurrent reference discriminator: LSTMRNN, or GRURNN (also an nn.LSTM), with last_sigmoid=True
+ * -- train.py:779-781 builds it from hp.discriminator like D, so with a recurrent D it is recurrent too.  ls is its nn.LSTM
+ * (1..GANTTS_MAX_LSTM_LAYERS layers, hidden a multiple of 4; dropout is ignored: eval mode), lstm_tensors its n_tensors =
+ * 4 ndir num_layers tensors in model.parameters() order (per layer and direction W_ih, W_hh, b_ih, b_hh), head its
+ * hidden2out (1 layer of ndir hidden -> 1, last_act = SIGMOID, W[0] / b[0] read).  The stack runs with the packed-sequence
+ * semantics of gantts_lstm_layer_fwd on lengths_dev (train.py:554-555 passes the lengths), so frames at or beyond a sequence's
+ * length have h = 0; the count masks them out.  ls->in_dim must equal n_adv (no linguistic conditioning), B <= 128 and
+ * B * T < 2^24.  Workspace: gantts_spoof_count_lstm_workspace_bytes(ls, head, B, T) of the call's shape, or of any larger
+ * one (0 = the descriptor is rejected); it is separate from the step's. */
+size_t gantts_spoof_count_lstm_workspace_bytes(const gantts_lstm_stack_t* ls, const gantts_mlp_t* head, int B, int T);
+int gantts_spoof_count_lstm(const gantts_lstm_stack_t* ls, const float* const* lstm_tensors, int n_tensors,
+                            const gantts_mlp_t* head, const float* y_hat_static, int n_static, const int* adv_cols,
+                            int n_adv, const int64_t* lengths_dev, int B, int T, float* count_dev, void* ws,
+                            size_t ws_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Inference-time MLPG with real variances (replaces nnmnkwii.paramgen.mlpg as called by reference

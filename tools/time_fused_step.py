@@ -18,7 +18,8 @@ name, power limit and maximum SM clock are queried in the same run (nvidia-smi, 
 --stage d_warmup and --spoof time the features of the five-stage recipe (train_gan.sh) instead of the modular path: in
 one process, round by round, the full fused step ("fused"), with --stage d_warmup the discriminator warm-up step
 (FusedGanStep.step(update_g=False): "fused_d_only"), and with --spoof the full step that also counts the spoofing rate of
-a reference discriminator (train.py:549-558: "fused_spoof").
+a reference discriminator (train.py:549-558: "fused_spoof").  The reference discriminator has D's class and shape on the
+adversarial columns alone (train.py:779-781), so with --rnn-d it is an LSTMRNN too.
 
 --rnn-d replaces the MLP discriminator of vc and tts_acoustic by a recurrent one, LSTMRNN(n, 1, 2, 256,
 bidirectional=True, dropout=0.5, last_sigmoid=True) with n = 59 (vc) or 425 + 58 conditioning + adversarial inputs
@@ -103,6 +104,21 @@ def models(w, dev, rnn_d=False):
     return mg.to(dev).train(), md.to(dev).train()
 
 
+def reference_discriminator(md, n_adv, dev):
+    """The spoofing-rate discriminator: D's class and shape (train.py:779-781 builds it from hp.discriminator like D) on
+    the n_adv adversarial columns alone, since train.py:554-555 feeds it no conditioning."""
+    import gantts_b200
+    M = gantts_b200.models
+    torch.manual_seed(99)
+    if isinstance(md, M._LSTMNet):
+        rnn = getattr(md, md._rnn_attr)
+        ref_d = type(md)(n_adv, 1, rnn.num_layers, rnn.hidden_size, bidirectional=rnn.bidirectional, dropout=rnn.dropout,
+                         last_sigmoid=True)
+    else:
+        ref_d = M.MLP(n_adv, 1, len(md.layers), md.layers[0].weight.shape[0], dropout=md.dropout_p, last_sigmoid=True)
+    return ref_d.to(dev)
+
+
 def dump(out_dir, fs, mg, md):
     os.makedirs(out_dir, exist_ok=True)
     arrays = {"losses": fs.losses, "y_hat": fs.y_hat, "y_hat_static": fs.y_hat_static,
@@ -131,11 +147,8 @@ def run(name, w, rounds, steps, warmup, dev, dump_dir=None, stage="adversarial",
     if stage == "d_warmup":
         steps_of["fused_d_only"] = lambda: fs.step(x, y, lengths, adv_w=adv_w, update_g=False)
     if spoof:
-        import gantts_b200
-        torch.manual_seed(99)
-        ref_d = gantts_b200.models.MLP(len(fused.adversarial_columns(hp)), 1, len(md.layers), 256, dropout=0.5,
-                                       last_sigmoid=True).to(dev)
-        fs_spoof = fused.FusedGanStep(*models(w, dev), hp, B, T, seed=2, reference_discriminator=ref_d, **kw)
+        ref_d = reference_discriminator(md, len(fused.adversarial_columns(hp)), dev)
+        fs_spoof = fused.FusedGanStep(*models(w, dev, rnn_d), hp, B, T, seed=2, reference_discriminator=ref_d, **kw)
         steps_of["fused_spoof"] = lambda: fs_spoof.step(x, y, lengths, adv_w=adv_w)
     if len(steps_of) == 1:
         tr = gstep.GanTrainer(*models(w, dev, rnn_d), hp, **kw)
