@@ -12,7 +12,8 @@
 // (SWIZZLE_128B, full/empty mbarriers per stage) across all of the CTA's tiles; warpgroups 1-2: whole tiles in turn,
 // one wgmma.m64n{BN}k16 per product and 64-row block.  Each warpgroup stages its accumulators through its own
 // shared-memory tile so that each epilogue thread owns 16 consecutive columns of one row (bias / LeakyReLU / dropout /
-// sigmoid, 16-byte stores); that epilogue runs while the other warpgroup's MMAs keep the tensor cores busy.
+// sigmoid, 16-byte stores); that epilogue runs while the other warpgroup's MMAs keep the tensor cores busy.  By default
+// the kernel runs cooperatively instead (COOP): both warpgroups on every tile, 64 rows each (see the kernel).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -141,27 +142,38 @@ __device__ __forceinline__ void dropout16(float (&v)[16], uint64_t seed, uint32_
 // (warp_row), the rows its wgmma fragments hold.
 __device__ __forceinline__ int64_t warp_row(int64_t row0, int l) { return row0 + (l & 15) + 64 * (l >> 4); }
 
+// Slot l (0-31) of a warp's epilogue pass: which output row and which 16-column chunk of the pass it holds.  Ping-pong
+// tiles (COOP = false): the warp holds 16 rows of both 64-row blocks, a pass is one chunk of 32 rows (warp_row).
+// Cooperative tiles (COOP = true): the warp holds 16 rows of one block, a pass is two chunks of those 16 rows.
+template <bool COOP>
+__device__ __forceinline__ int64_t slot_row(int64_t row0, int l) { return COOP ? row0 + (l & 15) : warp_row(row0, l); }
+template <bool COOP>
+__device__ __forceinline__ int slot_chunk(int l) { return COOP ? (l >> 4) : 0; }
+
+// `col` is the first column of the pass; slot l covers columns col + 16 slot_chunk(l) ...
+template <bool COOP>
 __device__ __forceinline__ void epilogue_f32_staged(const GemmParams& p, const uint32_t (&r)[16], int64_t row0,
                                                     int lane, int col, int z, const float* __restrict__ bias_s,
                                                     float* scr) {
-  const int64_t row = warp_row(row0, lane);
+  const int64_t row = slot_row<COOP>(row0, lane);
+  const int lcol = col + 16 * slot_chunk<COOP>(lane);
   float v[16];
 #pragma unroll
   for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
   if (p.bias) {
     if (bias_s) {
 #pragma unroll
-      for (int j = 0; j < 16; ++j) v[j] += bias_s[col + j];
+      for (int j = 0; j < 16; ++j) v[j] += bias_s[lcol + j];
     } else {
 #pragma unroll
       for (int j = 0; j < 16; ++j)
-        if (col + j < p.cols_b) v[j] += __ldg(p.bias + col + j);
+        if (lcol + j < p.cols_b) v[j] += __ldg(p.bias + lcol + j);
     }
   }
   if (p.act == GANTTS_ACT_LEAKY_DROPOUT) {
 #pragma unroll
     for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], v[j] * p.slope);
-    if (p.thresh) dropout16(v, p.seed, (uint32_t)(row + p.row0), p.cols_b, col, p.thresh, p.keep_scale);
+    if (p.thresh) dropout16(v, p.seed, (uint32_t)(row + p.row0), p.cols_b, lcol, p.thresh, p.keep_scale);
   } else if (p.act == GANTTS_ACT_SIGMOID) {
 #pragma unroll
     for (int j = 0; j < 16; ++j) v[j] = 1.f / (1.f + expf(-v[j]));
@@ -173,18 +185,19 @@ __device__ __forceinline__ void epilogue_f32_staged(const GemmParams& p, const u
   __syncwarp();
   float* cbase = p.C + (int64_t)z * p.c_zstride;
   const int j = lane & 15, hr = lane >> 4;
-  const bool col_ok = col + j < p.cols_b;
-  float* q0 = cbase + col + j;
   // accumulate (the discriminator's input gradient added into its window of g_static): all loads of a half are issued
   // before its first store -- interleaved `*q = *q + val` serialises load -> store round trips per warp (the compiler
-  // must assume the store aliases the next load)
+  // must assume the store aliases the next load).  Slots 16h .. 16h + 15 all lie in chunk slot_chunk(16h).
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
+    const int c = col + 16 * slot_chunk<COOP>(16 * h) + j;
+    const bool col_ok = c < p.cols_b;
+    float* q0 = cbase + c;
     float old[8];
     if (p.accumulate) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        const int64_t rw = warp_row(row0, 2 * (8 * h + i) + hr);
+        const int64_t rw = slot_row<COOP>(row0, 2 * (8 * h + i) + hr);
         old[i] = (col_ok && rw < p.rows_a) ? __ldcg(q0 + rw * p.ldc) : 0.f;
       }
     }
@@ -192,7 +205,7 @@ __device__ __forceinline__ void epilogue_f32_staged(const GemmParams& p, const u
     for (int i = 0; i < 8; ++i) {
       const int rr = 2 * (8 * h + i) + hr;
       const float val = scr[rr * 16 + 4 * ((j >> 2) ^ ((rr >> 1) & 3)) + (j & 3)];
-      const int64_t rw = warp_row(row0, rr);
+      const int64_t rw = slot_row<COOP>(row0, rr);
       if (col_ok && rw < p.rows_a) q0[rw * p.ldc] = p.accumulate ? old[i] + val : val;
     }
   }
@@ -302,18 +315,22 @@ __device__ __forceinline__ uint32_t epilogue_chunk16(const GemmParams& p, const 
   return code;
 }
 
-// The reduction of one 128 x BN tile (two 64-row blocks) by one warpgroup: for each smem stage, BK/16 steps of
-// hi*hi, hi*lo, lo*hi (and, with DB, the two ones-tile MMAs of the bias gradient) into `acc`.  Stage s is released
-// once the wgmma group of stage s + 1 has been issued and stage s's group has completed (wait_group 1), so one stage's
-// MMAs are always in flight.  After the last stage is issued the other warpgroup is told (turn_other) that it may
-// start its next tile's MMAs.
-template <bool MN, int BN, bool DB>
+// The reduction of one 128 x BN tile by one warpgroup: for each smem stage, BK/16 steps of hi*hi, hi*lo, lo*hi (and,
+// with DB, the two ones-tile MMAs of the bias gradient) into `acc`.  Ping-pong (COOP = false): the warpgroup issues both
+// 64-row blocks into acc[0], acc[1].  Cooperative (COOP = true): it issues the one block `blk` into acc[0] while the other
+// warpgroup issues the other block from the same stages.  Stage s is released (one arrive per warp) once the wgmma group
+// of stage s + 1 has been issued and stage s's group has completed (wait_group 1), so one stage's MMAs are always in
+// flight.  Ping-pong: after the last stage is issued the other warpgroup is told (turn_other) that it may start its next
+// tile's MMAs.
+template <bool MN, int BN, bool DB, bool COOP>
 __device__ __forceinline__ void mma_tile(const GemmParams& p, float (&acc)[2][BN / 2], float (&accdb)[2][4],
                                          uint32_t base, uint32_t full0, uint32_t empty0, uint32_t turn_other,
-                                         uint64_t d_ones, int nk, uint32_t& s, uint32_t& ph, int lane) {
+                                         uint64_t d_ones, int nk, uint32_t& s, uint32_t& ph, int lane, int blk) {
   constexpr int BK = MN ? TC_MN_BK : TC_KK_BK;
+  constexpr int HB = COOP ? 1 : 2;               // 64-row blocks this warpgroup issues
   constexpr uint32_t kstep = MN ? 2048u : 32u;   // K = 16: 16 rows of 128 B (MN-major), 32 B inside the row (K-major)
   const uint32_t a_half = MN ? p.atom_bytes : 8192u;  // rows 64-127 of A: the next MN atom / 64 rows of 128 B
+  const uint32_t a_off = COOP ? (uint32_t)blk * a_half : 0u;
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
   uint32_t prev = 0;
@@ -328,9 +345,9 @@ __device__ __forceinline__ void mma_tile(const GemmParams& p, float (&acc)[2][BN
       const uint64_t db_hi = ptx::make_smem_desc(sb_hi + k * kstep, p.atom_bytes, 1024u);
       const uint64_t db_lo = ptx::make_smem_desc(sb_lo + k * kstep, p.atom_bytes, 1024u);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const uint64_t da_hi = ptx::make_smem_desc(sa_hi + h * a_half + k * kstep, p.atom_bytes, 1024u);
-        const uint64_t da_lo = ptx::make_smem_desc(sa_lo + h * a_half + k * kstep, p.atom_bytes, 1024u);
+      for (int h = 0; h < HB; ++h) {
+        const uint64_t da_hi = ptx::make_smem_desc(sa_hi + a_off + h * a_half + k * kstep, p.atom_bytes, 1024u);
+        const uint64_t da_lo = ptx::make_smem_desc(sa_lo + a_off + h * a_half + k * kstep, p.atom_bytes, 1024u);
         if constexpr (BN == 128) {
           ptx::wgmma_m64n128k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_hi, db_hi);
           ptx::wgmma_m64n128k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_hi, db_lo);
@@ -356,7 +373,7 @@ __device__ __forceinline__ void mma_tile(const GemmParams& p, float (&acc)[2][BN
     if (++s == (uint32_t)p.num_stages) { s = 0; ph ^= 1; }
   }
   __syncwarp();
-  if (lane == 0) ptx::mbar_arrive(turn_other);
+  if (!COOP && lane == 0) ptx::mbar_arrive(turn_other);
   ptx::wgmma_wait<0>();
   ptx::fence_regs(acc[0]);
   ptx::fence_regs(acc[1]);
@@ -371,7 +388,13 @@ __device__ __forceinline__ void mma_tile(const GemmParams& p, float (&acc)[2][BN
 // through the stage ring continuously across the CTA's tiles.  Warpgroups 1 and 2 take the CTA's tiles in turn (even,
 // odd), each with its own accumulators: a warpgroup runs its tile's epilogue while the other one's MMAs use the tensor
 // cores, and a pair of `turn` mbarriers keeps their MMA phases in tile order.
-template <bool MN, int EPI, int BN>
+// COOP (the default): warpgroups 1 and 2 instead take every tile together, warpgroup w issuing rows 64w .. 64w + 63 from
+// the same ring stages, which are released when both have arrived; each then runs the epilogue of its 64 rows while the
+// producer refills the ring for the next tile.  Two warpgroups issuing MMAs side by side keep the tensor cores busier
+// than one at a time, and each epilogue covers half a tile; ping-pong's overlap of one tile's epilogue with the next
+// tile's MMAs is given up.  On the cfg2 step every launch is faster this way.  An output element's products are the same
+// MMAs in the same order.
+template <bool MN, int EPI, int BN, bool COOP>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                    const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
@@ -394,7 +417,7 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.num_stages; ++s) {
       ptx::mbar_init(full0 + 8 * s, 1);
-      ptx::mbar_init(empty0 + 8 * s, TC_WG_WARPS);      // one arrive per warp of the consuming warpgroup
+      ptx::mbar_init(empty0 + 8 * s, COOP ? 2 * TC_WG_WARPS : TC_WG_WARPS);   // one arrive per consuming warp
     }
     ptx::mbar_init(turn0, TC_WG_WARPS);
     ptx::mbar_init(turn0 + 8, TC_WG_WARPS);
@@ -465,17 +488,19 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
 
   // ---------------------------------------------------------------- MMA + epilogue warpgroups
   ptx::setmaxnreg_inc<TC_CONSUMER_REGS>();
-  const int wg = (warp >> 2) - 1;                        // takes the CTA's tiles i with i % 2 == wg
+  const int wg = (warp >> 2) - 1;          // ping-pong: takes the CTA's tiles i with i % 2 == wg; COOP: rows 64 wg ..
   const int q = warp & 3;
   const uint32_t turn_mine = turn0 + 8 * wg, turn_other = turn0 + 8 * (wg ^ 1);
   float* const wbuf = reinterpret_cast<float*>(gbase + p.epi_off) + (warp - 4) * TC_WARP_BUF_FLOATS;
   const uint64_t d_ones = ptx::make_smem_desc(base + p.ones_off, 0u, 1024u);
+  constexpr int HB = COOP ? 1 : 2;                       // 64-row blocks per warpgroup and tile
+  constexpr int CPP = COOP ? 2 : 1;                      // 16-column chunks per epilogue pass
   uint32_t s = 0, ph = 0;
   int i = 0;
   for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++i) {
     const int z = t / tiles_ab, rem = t - z * tiles_ab;
     const int nk = k_blocks(z);
-    if ((i & 1) != wg) {                                 // the other warpgroup's tile: skip its stages
+    if (!COOP && (i & 1) != wg) {                        // the other warpgroup's tile: skip its stages
       const uint32_t adv = s + (uint32_t)nk;
       ph ^= (adv / (uint32_t)p.num_stages) & 1u;
       s = adv % (uint32_t)p.num_stages;
@@ -484,49 +509,55 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
     const int ta = rem / p.num_b, tb = rem % p.num_b;
     const int a0 = ta * TC_BM, b0 = tb * BN;
     // warpgroup 0 goes first; afterwards each waits for the other to have issued its previous tile
-    ptx::mbar_wait(turn_mine, ((uint32_t)(i >> 1) & 1u) ^ (wg == 0 ? 1u : 0u));
+    if (!COOP) ptx::mbar_wait(turn_mine, ((uint32_t)(i >> 1) & 1u) ^ (wg == 0 ? 1u : 0u));
     float acc[2][BN / 2];
     float accdb[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
     const bool do_db = MN && p.db != nullptr && tb == 0;
     if (do_db)
-      mma_tile<MN, BN, MN>(p, acc, accdb, base, full0, empty0, turn_other, d_ones, nk, s, ph, lane);
+      mma_tile<MN, BN, MN, COOP>(p, acc, accdb, base, full0, empty0, turn_other, d_ones, nk, s, ph, lane, wg);
     else
-      mma_tile<MN, BN, false>(p, acc, accdb, base, full0, empty0, turn_other, d_ones, nk, s, ph, lane);
+      mma_tile<MN, BN, false, COOP>(p, acc, accdb, base, full0, empty0, turn_other, d_ones, nk, s, ph, lane, wg);
+    // first row of this warp in the tile's 64-row block 0 (ping-pong) or in the warpgroup's block (COOP)
+    const int64_t row0 = (int64_t)a0 + (COOP ? 64 * wg : 0) + 16 * q;
     if (do_db && (lane & 3) == 0) {
       // m64n8 layout: lane holds rows lane/4 and lane/4 + 8 of its warp's 16, columns 0-1 (all columns are equal)
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t r = (int64_t)a0 + 64 * h + 16 * q + (lane >> 2);
+      for (int h = 0; h < HB; ++h) {
+        const int64_t r = row0 + 64 * h + (lane >> 2);
         if (r < p.rows_a) p.db[(int64_t)z * p.rows_a + r] = accdb[h][0];
         if (r + 8 < p.rows_a) p.db[(int64_t)z * p.rows_a + r + 8] = accdb[h][2];
       }
     }
     // ------------------------------------------------------------ epilogue.  Warp q holds rows 16q .. 16q + 15 of
-    // both 64-row blocks; per 16-column chunk its fragments go through the warp's own shared-memory buffer
-    // [32][TC_WARP_PITCH] (lane l = row warp_row(a0 + 16q, l)) so that each lane owns 16 consecutive columns of one row.
-    const int64_t row0 = (int64_t)a0 + 16 * q;
-    const int64_t row = warp_row(row0, lane);
+    // both 64-row blocks (COOP: of its warpgroup's block); per pass its fragments go through the warp's own
+    // shared-memory buffer [32][TC_WARP_PITCH] so that lane l owns 16 consecutive columns of one row: row
+    // slot_row(row0, l), chunk slot_chunk(l) of the pass.
+    const int64_t row = slot_row<COOP>(row0, lane);
     const bool row_ok = row < p.rows_a;
-    uint32_t codes[BN / 16];
-    uint32_t code_out[BN / 16];
+    // derivative code words of the lane's chunk in each pass: chunk CPP k + slot_chunk(lane) of the tile
+    constexpr int PASSES = BN / (16 * CPP);
+    uint32_t codes[PASSES];
+    uint32_t code_out[PASSES];
 #pragma unroll
-    for (int k = 0; k < BN / 16; ++k) {
+    for (int k = 0; k < PASSES; ++k) {
+      const int c = b0 + 16 * (CPP * k + slot_chunk<COOP>(lane));
       codes[k] = code_out[k] = 0u;
-      if (EPI == EPI_PLANES_BWD && row_ok && b0 + 16 * k < p.cols_b)
-        codes[k] = __ldg(p.code + row * p.code_pitch + ((b0 + 16 * k) >> 4));
+      if (EPI == EPI_PLANES_BWD && row_ok && c < p.cols_b) codes[k] = __ldg(p.code + row * p.code_pitch + (c >> 4));
     }
 #pragma unroll
-    for (int k = 0; k < BN / 16; ++k) {
-      __syncwarp();                                      // the previous chunk has been read out of the buffer
-      // m64nN layout: register 4j + 2g + e is row 16q + lane / 4 + 8g, column 8j + 2 (lane % 4) + e
+    for (int k = 0; k < PASSES; ++k) {
+      __syncwarp();                                      // the previous pass has been read out of the buffer
+      // m64nN layout: register 4j + 2g + e is row 16q + lane / 4 + 8g, column 8j + 2 (lane % 4) + e.  Slots 16h ..
+      // 16h + 15 take block h's rows of chunk k (ping-pong) or the warp's rows of chunk 2k + h (COOP).
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int jj = 0; jj < 2; ++jj) {
-          const int j = 2 * k + jj;
+          const int blk = COOP ? 0 : h;
+          const int j = 2 * (CPP * k + (COOP ? h : 0)) + jj;
           float* w = wbuf + (16 * h + (lane >> 2)) * TC_WARP_PITCH + 8 * jj + 2 * (lane & 3);
-          *reinterpret_cast<float2*>(w) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
-          *reinterpret_cast<float2*>(w + 8 * TC_WARP_PITCH) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+          *reinterpret_cast<float2*>(w) = make_float2(acc[blk][4 * j], acc[blk][4 * j + 1]);
+          *reinterpret_cast<float2*>(w + 8 * TC_WARP_PITCH) = make_float2(acc[blk][4 * j + 2], acc[blk][4 * j + 3]);
         }
       __syncwarp();
       uint32_t rr[16];
@@ -537,18 +568,19 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
         rr[4 * m] = __float_as_uint(f.x); rr[4 * m + 1] = __float_as_uint(f.y);
         rr[4 * m + 2] = __float_as_uint(f.z); rr[4 * m + 3] = __float_as_uint(f.w);
       }
-      const int col = b0 + 16 * k;
+      const int col = b0 + 16 * CPP * k;                 // first column of the pass
+      const int lcol = col + 16 * slot_chunk<COOP>(lane);
       if (EPI == EPI_F32 && p.f32_stage) {             // whole warp takes part; rows beyond rows_a masked at the store
         __syncwarp();                                    // the buffer becomes the transpose scratch
-        if (col < p.cols_b) epilogue_f32_staged(p, rr, row0, lane, col, z, bias_s, wbuf);
-      } else if (row_ok && col < p.cols_b) {
-        code_out[k] = epilogue_chunk16<EPI>(p, rr, row, col, z, bias_s, codes[k]);
+        if (col < p.cols_b) epilogue_f32_staged<COOP>(p, rr, row0, lane, col, z, bias_s, wbuf);
+      } else if (row_ok && lcol < p.cols_b) {
+        code_out[k] = epilogue_chunk16<EPI>(p, rr, row, lcol, z, bias_s, codes[k]);
       }
     }
     if (EPI == EPI_PLANES_FWD && p.code != nullptr && row_ok) {
       uint32_t* cpp = p.code + row * p.code_pitch + (b0 >> 4);
       bool vec = false;
-      if constexpr (BN == 128) {
+      if constexpr (BN == 128 && !COOP) {
         vec = (p.code_pitch & 3) == 0;
         if (vec) {
           // whole 16-byte groups inside the (4-word padded) row: vector stores
@@ -558,8 +590,10 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
       }
       if (!vec) {
 #pragma unroll
-        for (int k = 0; k < BN / 16; ++k)
-          if (b0 + 16 * k < p.cols_b) cpp[k] = code_out[k];
+        for (int k = 0; k < PASSES; ++k) {
+          const int ck = CPP * k + slot_chunk<COOP>(lane);
+          if (b0 + 16 * ck < p.cols_b) cpp[ck] = code_out[k];
+        }
       }
     }
   }
@@ -774,7 +808,14 @@ static size_t plan_smem(GemmParams& p, const EpiArgs& e) {
   return (size_t)p.bar_off + 256 + 1024;
 }
 
-template <bool MN, int EPI, int BN>
+// Tiles run cooperatively (both MMA warpgroups on every tile) unless GANTTS_B200_GEMM_COOP=0 selects the ping-pong
+// schedule; both give the same bits.  Read per call so that tests can switch it.
+static int use_coop() {
+  const char* e = getenv("GANTTS_B200_GEMM_COOP");
+  return e ? atoi(e) : 1;
+}
+
+template <bool MN, int EPI, int BN, bool COOP>
 static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const CUtensorMap& mBh,
                          const CUtensorMap& mBl, const GemmParams& p, size_t smem, cudaStream_t st) {
   if (smem > TC_SMEM_MAX) {
@@ -790,7 +831,7 @@ static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const C
   static bool attr[64] = {};
   const int dev = current_device();
   if (dev < 0 || dev >= 64 || !attr[dev]) {
-    GANTTS_CUDA(cudaFuncSetAttribute(gemm_bf16x3_kernel<MN, EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    GANTTS_CUDA(cudaFuncSetAttribute(gemm_bf16x3_kernel<MN, EPI, BN, COOP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)TC_SMEM_MAX));
     if (dev >= 0 && dev < 64) attr[dev] = true;
   }
@@ -807,7 +848,7 @@ static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const C
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
   cfg.numAttrs = use_pdl() ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_bf16x3_kernel<MN, EPI, BN>, mAh, mAl, mBh, mBl, p);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_bf16x3_kernel<MN, EPI, BN, COOP>, mAh, mAl, mBh, mBl, p);
   prof_end(st);
   if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchKernelEx(gemm)");
   GANTTS_LAUNCH_CHECK("gemm_bf16x3_kernel");
@@ -817,8 +858,12 @@ static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const C
 template <bool MN, int EPI>
 static int launch_bn(const CUtensorMap& mAh, const CUtensorMap& mAl, const CUtensorMap& mBh, const CUtensorMap& mBl,
                      const GemmParams& p, size_t smem, cudaStream_t st) {
-  if (p.bn == 64) return launch_kernel<MN, EPI, 64>(mAh, mAl, mBh, mBl, p, smem, st);
-  return launch_kernel<MN, EPI, 128>(mAh, mAl, mBh, mBl, p, smem, st);
+  if (use_coop()) {
+    if (p.bn == 64) return launch_kernel<MN, EPI, 64, true>(mAh, mAl, mBh, mBl, p, smem, st);
+    return launch_kernel<MN, EPI, 128, true>(mAh, mAl, mBh, mBl, p, smem, st);
+  }
+  if (p.bn == 64) return launch_kernel<MN, EPI, 64, false>(mAh, mAl, mBh, mBl, p, smem, st);
+  return launch_kernel<MN, EPI, 128, false>(mAh, mAl, mBh, mBl, p, smem, st);
 }
 
 // out[rows_a][cols_b] = epi(A * B^T)   (K-major planes A [rows_a][red], B [cols_b][red]).

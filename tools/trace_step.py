@@ -67,15 +67,11 @@ def label_gemms(kernels, scale):
     return out, len(kk) + len(mn)
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", default="cfg2", choices=[k for k, v in bench.WORKLOADS.items() if v["kind"] == "mlp"])
-    ap.add_argument("--warmup", type=int, default=10)
-    ap.add_argument("--steps", type=int, default=3)
-    ap.add_argument("--out", default=None, help="markdown file for the launch list (default: stdout only)")
-    args = ap.parse_args()
+def capture(args):
+    """Runs args.warmup fused steps, then args.steps under the profiler.  Returns (per-step kernel lists [[(name, us)]],
+    workload dict, us from first start to last end of the middle step)."""
     if not torch.cuda.is_available():
-        raise SystemExit("trace_step.py: no CUDA device")
+        raise SystemExit("%s: no CUDA device" % os.path.basename(sys.argv[0]))
     import __graft_entry__
     __graft_entry__.build()
     from gantts_b200 import fused, step as gstep
@@ -105,11 +101,25 @@ def main():
            and not e.name.startswith(("Memcpy", "Memset", "[memory]"))]
     evs.sort(key=lambda e: e.time_range.start)
     if not evs or len(evs) % args.steps:
-        raise SystemExit("trace_step.py: %d kernels over %d steps do not split into equal steps" % (len(evs), args.steps))
+        raise SystemExit("%s: %d kernels over %d steps do not split into equal steps"
+                         % (os.path.basename(sys.argv[0]), len(evs), args.steps))
     per = len(evs) // args.steps
+    steps = [[(e.name, e.time_range.end - e.time_range.start) for e in evs[per * i: per * (i + 1)]]
+             for i in range(args.steps)]
     mid = evs[per * (args.steps // 2): per * (args.steps // 2 + 1)]
-    kernels = [(e.name, e.time_range.end - e.time_range.start) for e in mid]
-    span = mid[-1].time_range.end - mid[0].time_range.start
+    return steps, w, mid[-1].time_range.end - mid[0].time_range.start
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", default="cfg2", choices=[k for k, v in bench.WORKLOADS.items() if v["kind"] == "mlp"])
+    ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=3)
+    ap.add_argument("--out", default=None, help="markdown file for the launch list (default: stdout only)")
+    args = ap.parse_args()
+    steps, w, span = capture(args)
+    kernels = steps[args.steps // 2]
+    per = len(kernels)
     rows, unmatched = label_gemms(kernels, w["B"] * w["T"] // 32000)
     tot = sum(us for _, us, _, _ in rows)
     gemm_us = sum(us for _, us, _, f in rows if f is not None)
