@@ -45,7 +45,7 @@ void prof_end(cudaStream_t st);
 
 static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
-// Programmatic dependent launch for the small streaming kernels of the fused step (the tensor-core GEMMs already use it):
+// Programmatic dependent launch for the tensor-core GEMMs and the small streaming kernels of the fused step:
 // a kernel launched through GANTTS_PDL_LAUNCH may become resident while its predecessor in the stream is still in its last
 // wave; pdl_entry() at the top of the kernel (a) lets ITS successor do the same and (b) blocks until every prerequisite
 // grid has completed and its writes are visible -- nothing the predecessor produced is touched before that.  Without the

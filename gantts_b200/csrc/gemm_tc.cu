@@ -9,14 +9,13 @@
 //   MN = false : C[M][N] = A[M][K] * B[N][K]^T   both operands K-major   (layer forward, gx = gz W)
 //   MN = true  : C[N][K] = A[M][N]^T * B[M][K]   both operands MN-major  (gW = gz^T x, split over M)
 // warpgroup 0: one TMA producer thread filling a smem ring of `num_stages` {A_hi, A_lo, B_hi, B_lo} tiles
-// (SWIZZLE_128B, full/empty mbarriers per stage) across all of the CTA's tiles; warpgroups 1-2: whole tiles in turn,
-// one wgmma.m64n{BN}k16 per product and 64-row block.  Each warpgroup stages its accumulators through its own
-// shared-memory tile so that each epilogue thread owns 16 consecutive columns of one row (bias / LeakyReLU / dropout /
-// sigmoid, 16-byte stores); that epilogue runs while the other warpgroup's MMAs keep the tensor cores busy.  By default
-// the kernel runs cooperatively instead (COOP): both warpgroups on every tile, 64 rows each (see the kernel).
+// (SWIZZLE_128B, full/empty mbarriers per stage) across all of the CTA's tiles; warpgroups 1-2: every tile together,
+// warpgroup w issuing one wgmma.m64n{BN}k16 per product for rows 64w .. 64w + 63.  Each warpgroup stages its
+// accumulators through its warps' shared-memory buffers so that each epilogue thread owns 16 consecutive columns of one
+// row (bias / LeakyReLU / dropout / sigmoid, 16-byte stores); that epilogue runs while the producer refills the ring
+// for the CTA's next tile.
 #include <cuda.h>
 #include <cuda_bf16.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -25,7 +24,7 @@ namespace gantts {
 
 constexpr int TC_WG_WARPS = 4;      // warps of one MMA + epilogue warpgroup
 constexpr int TC_THREADS = 128 + 2 * 32 * TC_WG_WARPS;   // warpgroup 0 TMA, warpgroups 1-2 MMA + epilogue
-constexpr int TC_BM = 128;          // output rows per tile (one warpgroup: two wgmma m64 row blocks)
+constexpr int TC_BM = 128;          // output rows per tile (two wgmma m64 row blocks, one per MMA warpgroup)
 constexpr int TC_WARP_PITCH = 20;   // floats per row of a warp's epilogue buffer (float4-aligned, conflict-free reads)
 constexpr int TC_WARP_BUF_FLOATS = 32 * TC_WARP_PITCH;   // one 32-row x 16-column chunk (>= the 2 KB fp32 scratch)
 constexpr int TC_MAX_BN = 128;      // output columns per tile
@@ -60,7 +59,9 @@ struct GemmParams {
   // EPI_F32 output
   float* C;
   int64_t ldc, c_zstride;
-  int vec_ok, accumulate;
+  int vec_ok;           // C 16-byte aligned, ldc % 4 == 0, no accumulate: float4 stores from registers;
+                        // 0 = through the warp's buffer as a transpose scratch (epilogue_f32_smem)
+  int accumulate;
   // planes output (EPI_PLANES_*)
   __nv_bfloat16 *out_hi, *out_lo;
   int64_t out_pitch;
@@ -69,8 +70,6 @@ struct GemmParams {
   uint32_t* code;
   int64_t code_pitch;   // words per row
   uint32_t bias_off;    // byte offset (from the aligned smem base) of the staged bias vector, 0 = none
-  int f32_stage;        // EPI_F32 with an unaligned row stride: write back through the warp's buffer as a transpose
-                        // scratch (epilogue_f32_staged), 0 = store straight from registers
   // MN-major only: column sums of A (= bias gradient) via an extra N=8 MMA against a tile of ones
   float* db;            // [num_z][rows_a] partial sums, or null
   uint32_t ones_off;    // byte offset of the all-ones bf16 tile from the aligned smem base
@@ -133,30 +132,18 @@ __device__ __forceinline__ void dropout16(float (&v)[16], uint64_t seed, uint32_
   }
 }
 
-// EPI_F32 for outputs whose row stride is not a multiple of 4 floats (y_hat: ld 187, the discriminator input
-// gradient: ld 58, weight-gradient partials of 425- and 58-wide layers).  Straight from registers a thread can
-// only issue 16 scalar stores per chunk and a warp store touches 32 rows = 32 sectors.  Here the warp's 32 x 16 tile
-// goes through a private 2 KB shared-memory scratch (float4 writes, XOR-swizzled: conflict-free) and is written back
-// with lanes 0-15 / 16-31 covering two whole 64-byte row segments per store instruction.  Same arithmetic, same
-// order.  Default on (GANTTS_B200_F32_STAGE=0 disables).  The warp's rows are row0 + (l % 16) + 64 (l / 16) for l < 32
-// (warp_row), the rows its wgmma fragments hold.
-__device__ __forceinline__ int64_t warp_row(int64_t row0, int l) { return row0 + (l & 15) + 64 * (l >> 4); }
-
-// Slot l (0-31) of a warp's epilogue pass: which output row and which 16-column chunk of the pass it holds.  Ping-pong
-// tiles (COOP = false): the warp holds 16 rows of both 64-row blocks, a pass is one chunk of 32 rows (warp_row).
-// Cooperative tiles (COOP = true): the warp holds 16 rows of one block, a pass is two chunks of those 16 rows.
-template <bool COOP>
-__device__ __forceinline__ int64_t slot_row(int64_t row0, int l) { return COOP ? row0 + (l & 15) : warp_row(row0, l); }
-template <bool COOP>
-__device__ __forceinline__ int slot_chunk(int l) { return COOP ? (l >> 4) : 0; }
-
-// `col` is the first column of the pass; slot l covers columns col + 16 slot_chunk(l) ...
-template <bool COOP>
-__device__ __forceinline__ void epilogue_f32_staged(const GemmParams& p, const uint32_t (&r)[16], int64_t row0,
-                                                    int lane, int col, int z, const float* __restrict__ bias_s,
-                                                    float* scr) {
-  const int64_t row = slot_row<COOP>(row0, lane);
-  const int lcol = col + 16 * slot_chunk<COOP>(lane);
+// EPI_F32 for every output that is not vec_ok: row strides that are not a multiple of 4 floats (y_hat: ld 187, the
+// discriminator input gradient: ld 58, weight-gradient partials of 425- and 58-wide layers) and accumulating outputs.
+// Straight from registers a thread could only issue 16 scalar stores per chunk and a warp store would touch 32 rows =
+// 32 sectors.  Here the warp's 32 x 16 tile goes through a private 2 KB shared-memory scratch (float4 writes,
+// XOR-swizzled: conflict-free) and is written back with lanes 0-15 / 16-31 covering two whole 64-byte row segments per
+// store instruction.  Slot l (0-31) of the pass holds row row0 + (l % 16) and the 16 columns from col + 16 (l / 16):
+// the warp's 16 rows of its warpgroup's 64-row block, two 16-column chunks per pass.
+__device__ __forceinline__ void epilogue_f32_smem(const GemmParams& p, const uint32_t (&r)[16], int64_t row0,
+                                                  int lane, int col, int z, const float* __restrict__ bias_s,
+                                                  float* scr) {
+  const int64_t row = row0 + (lane & 15);
+  const int lcol = col + 16 * (lane >> 4);
   float v[16];
 #pragma unroll
   for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
@@ -187,26 +174,31 @@ __device__ __forceinline__ void epilogue_f32_staged(const GemmParams& p, const u
   const int j = lane & 15, hr = lane >> 4;
   // accumulate (the discriminator's input gradient added into its window of g_static): all loads of a half are issued
   // before its first store -- interleaved `*q = *q + val` serialises load -> store round trips per warp (the compiler
-  // must assume the store aliases the next load).  Slots 16h .. 16h + 15 all lie in chunk slot_chunk(16h).
+  // must assume the store aliases the next load).  Slots 16h .. 16h + 15 all lie in chunk h; slot 16h + 2i + hr holds
+  // row row0 + 2i + hr.  Each element's address and bounds check are computed once for its load and its store: ptxas
+  // then predicates the stores instead of branching around each one and recomputing its address.
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int c = col + 16 * slot_chunk<COOP>(16 * h) + j;
+    const int c = col + 16 * h + j;
     const bool col_ok = c < p.cols_b;
-    float* q0 = cbase + c;
+    float* q[8];
+    bool ok[8];
     float old[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int64_t rw = row0 + 2 * i + hr;
+      q[i] = cbase + c + rw * p.ldc;
+      ok[i] = col_ok && rw < p.rows_a;
+    }
     if (p.accumulate) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int64_t rw = slot_row<COOP>(row0, 2 * (8 * h + i) + hr);
-        old[i] = (col_ok && rw < p.rows_a) ? __ldcg(q0 + rw * p.ldc) : 0.f;
-      }
+      for (int i = 0; i < 8; ++i) old[i] = ok[i] ? __ldcg(q[i]) : 0.f;
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int rr = 2 * (8 * h + i) + hr;
       const float val = scr[rr * 16 + 4 * ((j >> 2) ^ ((rr >> 1) & 3)) + (j & 3)];
-      const int64_t rw = slot_row<COOP>(row0, rr);
-      if (col_ok && rw < p.rows_a) q0[rw * p.ldc] = p.accumulate ? old[i] + val : val;
+      if (ok[i]) *q[i] = p.accumulate ? old[i] + val : val;
     }
   }
   __syncwarp();
@@ -242,15 +234,16 @@ __device__ __forceinline__ uint32_t epilogue_chunk16(const GemmParams& p, const 
 #pragma unroll
       for (int j = 0; j < 16; ++j) v[j] = 1.f / (1.f + expf(-v[j]));
     }
+    // only vec_ok outputs get here (the others are staged): float4 stores, scalar ones for the column tail
 #pragma unroll
     for (int j = 0; j < 16; j += 4) {
       const int c = col + j;
-      if (p.vec_ok && c + 3 < p.cols_b) {
+      if (c + 3 < p.cols_b) {
         *reinterpret_cast<float4*>(crow + c) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
       } else {
 #pragma unroll
         for (int e = 0; e < 4; ++e)
-          if (c + e < p.cols_b) crow[c + e] = p.accumulate ? crow[c + e] + v[j + e] : v[j + e];
+          if (c + e < p.cols_b) crow[c + e] = v[j + e];
       }
     }
   } else if (EPI == EPI_PLANES_FWD) {
@@ -315,24 +308,21 @@ __device__ __forceinline__ uint32_t epilogue_chunk16(const GemmParams& p, const 
   return code;
 }
 
-// The reduction of one 128 x BN tile by one warpgroup: for each smem stage, BK/16 steps of hi*hi, hi*lo, lo*hi (and,
-// with DB, the two ones-tile MMAs of the bias gradient) into `acc`.  Ping-pong (COOP = false): the warpgroup issues both
-// 64-row blocks into acc[0], acc[1].  Cooperative (COOP = true): it issues the one block `blk` into acc[0] while the other
-// warpgroup issues the other block from the same stages.  Stage s is released (one arrive per warp) once the wgmma group
-// of stage s + 1 has been issued and stage s's group has completed (wait_group 1), so one stage's MMAs are always in
-// flight.  Ping-pong: after the last stage is issued the other warpgroup is told (turn_other) that it may start its next
-// tile's MMAs.
-template <bool MN, int BN, bool DB, bool COOP>
-__device__ __forceinline__ void mma_tile(const GemmParams& p, float (&acc)[2][BN / 2], float (&accdb)[2][4],
-                                         uint32_t base, uint32_t full0, uint32_t empty0, uint32_t turn_other,
-                                         uint64_t d_ones, int nk, uint32_t& s, uint32_t& ph, int lane, int blk) {
+// One warpgroup's share of the reduction of a 128 x BN tile: the 64-row block `blk`, for each smem stage BK/16 steps
+// of hi*hi, hi*lo, lo*hi (and, with DB, the two ones-tile MMAs of the bias gradient) into `acc`, while the other
+// warpgroup issues the other block from the same stages.  Stage s is released (one arrive per warp) once the wgmma
+// group of stage s + 1 has been issued and stage s's group has completed (wait_group 1), so one stage's MMAs are always
+// in flight.
+template <bool MN, int BN, bool DB>
+__device__ __forceinline__ void mma_tile(const GemmParams& p, float (&acc)[BN / 2], float (&accdb)[4], uint32_t base,
+                                         uint32_t full0, uint32_t empty0, uint64_t d_ones, int nk, uint32_t& s,
+                                         uint32_t& ph, int lane, int blk) {
   constexpr int BK = MN ? TC_MN_BK : TC_KK_BK;
-  constexpr int HB = COOP ? 1 : 2;               // 64-row blocks this warpgroup issues
   constexpr uint32_t kstep = MN ? 2048u : 32u;   // K = 16: 16 rows of 128 B (MN-major), 32 B inside the row (K-major)
   const uint32_t a_half = MN ? p.atom_bytes : 8192u;  // rows 64-127 of A: the next MN atom / 64 rows of 128 B
-  const uint32_t a_off = COOP ? (uint32_t)blk * a_half : 0u;
+  const uint32_t a_off = (uint32_t)blk * a_half;
 #pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   uint32_t prev = 0;
 #pragma unroll 1
   for (int kb = 0; kb < nk; ++kb) {
@@ -344,23 +334,20 @@ __device__ __forceinline__ void mma_tile(const GemmParams& p, float (&acc)[2][BN
     for (int k = 0; k < BK / 16; ++k) {
       const uint64_t db_hi = ptx::make_smem_desc(sb_hi + k * kstep, p.atom_bytes, 1024u);
       const uint64_t db_lo = ptx::make_smem_desc(sb_lo + k * kstep, p.atom_bytes, 1024u);
-#pragma unroll
-      for (int h = 0; h < HB; ++h) {
-        const uint64_t da_hi = ptx::make_smem_desc(sa_hi + a_off + h * a_half + k * kstep, p.atom_bytes, 1024u);
-        const uint64_t da_lo = ptx::make_smem_desc(sa_lo + a_off + h * a_half + k * kstep, p.atom_bytes, 1024u);
-        if constexpr (BN == 128) {
-          ptx::wgmma_m64n128k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_hi, db_hi);
-          ptx::wgmma_m64n128k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_hi, db_lo);
-          ptx::wgmma_m64n128k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_lo, db_hi);
-        } else {
-          ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_hi, db_hi);
-          ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_hi, db_lo);
-          ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc[h], da_lo, db_hi);
-        }
-        if constexpr (DB) {
-          ptx::wgmma_m64n8k16<MN ? 1 : 0>(accdb[h], da_hi, d_ones);
-          ptx::wgmma_m64n8k16<MN ? 1 : 0>(accdb[h], da_lo, d_ones);
-        }
+      const uint64_t da_hi = ptx::make_smem_desc(sa_hi + a_off + k * kstep, p.atom_bytes, 1024u);
+      const uint64_t da_lo = ptx::make_smem_desc(sa_lo + a_off + k * kstep, p.atom_bytes, 1024u);
+      if constexpr (BN == 128) {
+        ptx::wgmma_m64n128k16<MN ? 1 : 0, MN ? 1 : 0>(acc, da_hi, db_hi);
+        ptx::wgmma_m64n128k16<MN ? 1 : 0, MN ? 1 : 0>(acc, da_hi, db_lo);
+        ptx::wgmma_m64n128k16<MN ? 1 : 0, MN ? 1 : 0>(acc, da_lo, db_hi);
+      } else {
+        ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc, da_hi, db_hi);
+        ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc, da_hi, db_lo);
+        ptx::wgmma_m64n64k16<MN ? 1 : 0, MN ? 1 : 0>(acc, da_lo, db_hi);
+      }
+      if constexpr (DB) {
+        ptx::wgmma_m64n8k16<MN ? 1 : 0>(accdb, da_hi, d_ones);
+        ptx::wgmma_m64n8k16<MN ? 1 : 0>(accdb, da_lo, d_ones);
       }
     }
     ptx::wgmma_commit();
@@ -373,28 +360,20 @@ __device__ __forceinline__ void mma_tile(const GemmParams& p, float (&acc)[2][BN
     if (++s == (uint32_t)p.num_stages) { s = 0; ph ^= 1; }
   }
   __syncwarp();
-  if (!COOP && lane == 0) ptx::mbar_arrive(turn_other);
   ptx::wgmma_wait<0>();
-  ptx::fence_regs(acc[0]);
-  ptx::fence_regs(acc[1]);
-  ptx::fence_regs(accdb[0]);
-  ptx::fence_regs(accdb[1]);
+  ptx::fence_regs(acc);
+  ptx::fence_regs(accdb);
   __syncwarp();
   if (lane == 0) ptx::mbar_arrive(empty0 + 8 * prev);
 }
 
 // Persistent kernel: CTA b walks the tiles b, b + gridDim.x, ... (numbering: z-slice of the reduction, then row tile,
 // then column tile, so the column tiles of one row tile are neighbours).  Warpgroup 0: one TMA producer thread runs
-// through the stage ring continuously across the CTA's tiles.  Warpgroups 1 and 2 take the CTA's tiles in turn (even,
-// odd), each with its own accumulators: a warpgroup runs its tile's epilogue while the other one's MMAs use the tensor
-// cores, and a pair of `turn` mbarriers keeps their MMA phases in tile order.
-// COOP (the default): warpgroups 1 and 2 instead take every tile together, warpgroup w issuing rows 64w .. 64w + 63 from
-// the same ring stages, which are released when both have arrived; each then runs the epilogue of its 64 rows while the
-// producer refills the ring for the next tile.  Two warpgroups issuing MMAs side by side keep the tensor cores busier
-// than one at a time, and each epilogue covers half a tile; ping-pong's overlap of one tile's epilogue with the next
-// tile's MMAs is given up.  On the cfg2 step every launch is faster this way.  An output element's products are the same
-// MMAs in the same order.
-template <bool MN, int EPI, int BN, bool COOP>
+// through the stage ring continuously across the CTA's tiles.  Warpgroups 1 and 2 take every tile together,
+// warpgroup w issuing rows 64w .. 64w + 63 from the same ring stages, which are released when both have arrived; each
+// then runs the epilogue of its 64 rows while the producer refills the ring for the next tile.  Two warpgroups issuing
+// MMAs side by side keep the tensor cores busy, and each epilogue covers half a tile.
+template <bool MN, int EPI, int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                    const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
@@ -404,7 +383,7 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
   const uint32_t raw = ptx::smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* const gbase = smem_raw + (base - raw);
-  const uint32_t full0 = base + p.bar_off, empty0 = full0 + 8 * TC_MAX_STAGES, turn0 = empty0 + 8 * TC_MAX_STAGES;
+  const uint32_t full0 = base + p.bar_off, empty0 = full0 + 8 * TC_MAX_STAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_ab = p.num_a * p.num_b;
   const int tiles = tiles_ab * p.num_z;
@@ -417,10 +396,8 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.num_stages; ++s) {
       ptx::mbar_init(full0 + 8 * s, 1);
-      ptx::mbar_init(empty0 + 8 * s, COOP ? 2 * TC_WG_WARPS : TC_WG_WARPS);   // one arrive per consuming warp
+      ptx::mbar_init(empty0 + 8 * s, 2 * TC_WG_WARPS);   // one arrive per consuming warp
     }
-    ptx::mbar_init(turn0, TC_WG_WARPS);
-    ptx::mbar_init(turn0 + 8, TC_WG_WARPS);
     ptx::fence_barrier_init();
     ptx::prefetch_tensormap(&tmAh);
     ptx::prefetch_tensormap(&tmAl);
@@ -488,59 +465,43 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
 
   // ---------------------------------------------------------------- MMA + epilogue warpgroups
   ptx::setmaxnreg_inc<TC_CONSUMER_REGS>();
-  const int wg = (warp >> 2) - 1;          // ping-pong: takes the CTA's tiles i with i % 2 == wg; COOP: rows 64 wg ..
+  const int wg = (warp >> 2) - 1;          // rows 64 wg .. 64 wg + 63 of every tile
   const int q = warp & 3;
-  const uint32_t turn_mine = turn0 + 8 * wg, turn_other = turn0 + 8 * (wg ^ 1);
   float* const wbuf = reinterpret_cast<float*>(gbase + p.epi_off) + (warp - 4) * TC_WARP_BUF_FLOATS;
   const uint64_t d_ones = ptx::make_smem_desc(base + p.ones_off, 0u, 1024u);
-  constexpr int HB = COOP ? 1 : 2;                       // 64-row blocks per warpgroup and tile
-  constexpr int CPP = COOP ? 2 : 1;                      // 16-column chunks per epilogue pass
   uint32_t s = 0, ph = 0;
-  int i = 0;
-  for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++i) {
+  for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
     const int z = t / tiles_ab, rem = t - z * tiles_ab;
     const int nk = k_blocks(z);
-    if (!COOP && (i & 1) != wg) {                        // the other warpgroup's tile: skip its stages
-      const uint32_t adv = s + (uint32_t)nk;
-      ph ^= (adv / (uint32_t)p.num_stages) & 1u;
-      s = adv % (uint32_t)p.num_stages;
-      continue;
-    }
     const int ta = rem / p.num_b, tb = rem % p.num_b;
     const int a0 = ta * TC_BM, b0 = tb * BN;
-    // warpgroup 0 goes first; afterwards each waits for the other to have issued its previous tile
-    if (!COOP) ptx::mbar_wait(turn_mine, ((uint32_t)(i >> 1) & 1u) ^ (wg == 0 ? 1u : 0u));
-    float acc[2][BN / 2];
-    float accdb[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+    float acc[BN / 2];
+    float accdb[4] = {0.f, 0.f, 0.f, 0.f};
     const bool do_db = MN && p.db != nullptr && tb == 0;
     if (do_db)
-      mma_tile<MN, BN, MN, COOP>(p, acc, accdb, base, full0, empty0, turn_other, d_ones, nk, s, ph, lane, wg);
+      mma_tile<MN, BN, MN>(p, acc, accdb, base, full0, empty0, d_ones, nk, s, ph, lane, wg);
     else
-      mma_tile<MN, BN, false, COOP>(p, acc, accdb, base, full0, empty0, turn_other, d_ones, nk, s, ph, lane, wg);
-    // first row of this warp in the tile's 64-row block 0 (ping-pong) or in the warpgroup's block (COOP)
-    const int64_t row0 = (int64_t)a0 + (COOP ? 64 * wg : 0) + 16 * q;
+      mma_tile<MN, BN, false>(p, acc, accdb, base, full0, empty0, d_ones, nk, s, ph, lane, wg);
+    const int64_t row0 = (int64_t)a0 + 64 * wg + 16 * q;   // first row of this warp in the tile
     if (do_db && (lane & 3) == 0) {
       // m64n8 layout: lane holds rows lane/4 and lane/4 + 8 of its warp's 16, columns 0-1 (all columns are equal)
-#pragma unroll
-      for (int h = 0; h < HB; ++h) {
-        const int64_t r = row0 + 64 * h + (lane >> 2);
-        if (r < p.rows_a) p.db[(int64_t)z * p.rows_a + r] = accdb[h][0];
-        if (r + 8 < p.rows_a) p.db[(int64_t)z * p.rows_a + r + 8] = accdb[h][2];
-      }
+      const int64_t r = row0 + (lane >> 2);
+      if (r < p.rows_a) p.db[(int64_t)z * p.rows_a + r] = accdb[0];
+      if (r + 8 < p.rows_a) p.db[(int64_t)z * p.rows_a + r + 8] = accdb[2];
     }
-    // ------------------------------------------------------------ epilogue.  Warp q holds rows 16q .. 16q + 15 of
-    // both 64-row blocks (COOP: of its warpgroup's block); per pass its fragments go through the warp's own
-    // shared-memory buffer [32][TC_WARP_PITCH] so that lane l owns 16 consecutive columns of one row: row
-    // slot_row(row0, l), chunk slot_chunk(l) of the pass.
-    const int64_t row = slot_row<COOP>(row0, lane);
+    // ------------------------------------------------------------ epilogue.  Warp q holds rows 16q .. 16q + 15 of its
+    // warpgroup's 64-row block; per pass of two 16-column chunks its fragments go through the warp's own shared-memory
+    // buffer [32][TC_WARP_PITCH] so that lane l owns 16 consecutive columns of one row: row row0 + (l % 16), chunk
+    // l / 16 of the pass.
+    const int64_t row = row0 + (lane & 15);
     const bool row_ok = row < p.rows_a;
-    // derivative code words of the lane's chunk in each pass: chunk CPP k + slot_chunk(lane) of the tile
-    constexpr int PASSES = BN / (16 * CPP);
+    // derivative code words of the lane's chunk in each pass: chunk 2k + lane / 16 of the tile
+    constexpr int PASSES = BN / 32;
     uint32_t codes[PASSES];
     uint32_t code_out[PASSES];
 #pragma unroll
     for (int k = 0; k < PASSES; ++k) {
-      const int c = b0 + 16 * (CPP * k + slot_chunk<COOP>(lane));
+      const int c = b0 + 16 * (2 * k + (lane >> 4));
       codes[k] = code_out[k] = 0u;
       if (EPI == EPI_PLANES_BWD && row_ok && c < p.cols_b) codes[k] = __ldg(p.code + row * p.code_pitch + (c >> 4));
     }
@@ -548,16 +509,15 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
     for (int k = 0; k < PASSES; ++k) {
       __syncwarp();                                      // the previous pass has been read out of the buffer
       // m64nN layout: register 4j + 2g + e is row 16q + lane / 4 + 8g, column 8j + 2 (lane % 4) + e.  Slots 16h ..
-      // 16h + 15 take block h's rows of chunk k (ping-pong) or the warp's rows of chunk 2k + h (COOP).
+      // 16h + 15 take the warp's rows of chunk 2k + h.
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int jj = 0; jj < 2; ++jj) {
-          const int blk = COOP ? 0 : h;
-          const int j = 2 * (CPP * k + (COOP ? h : 0)) + jj;
+          const int j = 2 * (2 * k + h) + jj;
           float* w = wbuf + (16 * h + (lane >> 2)) * TC_WARP_PITCH + 8 * jj + 2 * (lane & 3);
-          *reinterpret_cast<float2*>(w) = make_float2(acc[blk][4 * j], acc[blk][4 * j + 1]);
-          *reinterpret_cast<float2*>(w + 8 * TC_WARP_PITCH) = make_float2(acc[blk][4 * j + 2], acc[blk][4 * j + 3]);
+          *reinterpret_cast<float2*>(w) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(w + 8 * TC_WARP_PITCH) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
       __syncwarp();
       uint32_t rr[16];
@@ -568,32 +528,21 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
         rr[4 * m] = __float_as_uint(f.x); rr[4 * m + 1] = __float_as_uint(f.y);
         rr[4 * m + 2] = __float_as_uint(f.z); rr[4 * m + 3] = __float_as_uint(f.w);
       }
-      const int col = b0 + 16 * CPP * k;                 // first column of the pass
-      const int lcol = col + 16 * slot_chunk<COOP>(lane);
-      if (EPI == EPI_F32 && p.f32_stage) {             // whole warp takes part; rows beyond rows_a masked at the store
+      const int col = b0 + 32 * k;                       // first column of the pass
+      const int lcol = col + 16 * (lane >> 4);
+      if (EPI == EPI_F32 && !p.vec_ok) {                 // whole warp takes part; rows beyond rows_a masked at the store
         __syncwarp();                                    // the buffer becomes the transpose scratch
-        if (col < p.cols_b) epilogue_f32_staged<COOP>(p, rr, row0, lane, col, z, bias_s, wbuf);
+        if (col < p.cols_b) epilogue_f32_smem(p, rr, row0, lane, col, z, bias_s, wbuf);
       } else if (row_ok && lcol < p.cols_b) {
         code_out[k] = epilogue_chunk16<EPI>(p, rr, row, lcol, z, bias_s, codes[k]);
       }
     }
     if (EPI == EPI_PLANES_FWD && p.code != nullptr && row_ok) {
       uint32_t* cpp = p.code + row * p.code_pitch + (b0 >> 4);
-      bool vec = false;
-      if constexpr (BN == 128 && !COOP) {
-        vec = (p.code_pitch & 3) == 0;
-        if (vec) {
-          // whole 16-byte groups inside the (4-word padded) row: vector stores
-          reinterpret_cast<uint4*>(cpp)[0] = make_uint4(code_out[0], code_out[1], code_out[2], code_out[3]);
-          reinterpret_cast<uint4*>(cpp)[1] = make_uint4(code_out[4], code_out[5], code_out[6], code_out[7]);
-        }
-      }
-      if (!vec) {
 #pragma unroll
-        for (int k = 0; k < PASSES; ++k) {
-          const int ck = CPP * k + slot_chunk<COOP>(lane);
-          if (b0 + 16 * ck < p.cols_b) cpp[ck] = code_out[k];
-        }
+      for (int k = 0; k < PASSES; ++k) {
+        const int ck = 2 * k + (lane >> 4);
+        if (b0 + 16 * ck < p.cols_b) cpp[ck] = code_out[k];
       }
     }
   }
@@ -777,26 +726,9 @@ static void fill_epilogue(GemmParams& p, const EpiArgs& e) {
   p.row0 = e.row0;
 }
 
-// Stage fp32 output tiles with unaligned row strides through shared memory (GANTTS_B200_F32_STAGE=0 disables).  Read per
-// call so that tests can switch it.
-static int use_f32_stage() {
-  const char* e = getenv("GANTTS_B200_F32_STAGE");
-  return e ? atoi(e) : 1;
-}
-
-static int use_pdl() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("GANTTS_B200_PDL");
-    v = e ? atoi(e) : 1;
-  }
-  return v;
-}
-
 // Shared-memory plan of one launch (offsets from the 1024-aligned base): as many ring stages as fit next to the 8
 // per-warp epilogue buffers (20 KB), the ones tile, the bias vector and the mbarriers.  Returns the dynamic smem bytes.
 static size_t plan_smem(GemmParams& p, const EpiArgs& e) {
-  p.f32_stage = (use_f32_stage() && e.epi == EPI_F32 && !p.vec_ok && p.C) ? 1 : 0;
   const uint32_t epi = 2 * TC_WG_WARPS * TC_WARP_BUF_FLOATS * 4;
   const uint32_t fixed = 1024 + epi + TC_ONES_SMEM + TC_BIAS_SMEM + 256;
   p.num_stages = (int)((TC_SMEM_MAX - fixed) / p.stage_bytes);
@@ -808,14 +740,7 @@ static size_t plan_smem(GemmParams& p, const EpiArgs& e) {
   return (size_t)p.bar_off + 256 + 1024;
 }
 
-// Tiles run cooperatively (both MMA warpgroups on every tile) unless GANTTS_B200_GEMM_COOP=0 selects the ping-pong
-// schedule; both give the same bits.  Read per call so that tests can switch it.
-static int use_coop() {
-  const char* e = getenv("GANTTS_B200_GEMM_COOP");
-  return e ? atoi(e) : 1;
-}
-
-template <bool MN, int EPI, int BN, bool COOP>
+template <bool MN, int EPI, int BN>
 static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const CUtensorMap& mBh,
                          const CUtensorMap& mBl, const GemmParams& p, size_t smem, cudaStream_t st) {
   if (smem > TC_SMEM_MAX) {
@@ -831,26 +756,15 @@ static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const C
   static bool attr[64] = {};
   const int dev = current_device();
   if (dev < 0 || dev >= 64 || !attr[dev]) {
-    GANTTS_CUDA(cudaFuncSetAttribute(gemm_bf16x3_kernel<MN, EPI, BN, COOP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    GANTTS_CUDA(cudaFuncSetAttribute(gemm_bf16x3_kernel<MN, EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)TC_SMEM_MAX));
     if (dev >= 0 && dev < 64) attr[dev] = true;
   }
   const int tiles = p.num_a * p.num_b * p.num_z;
   const int grid = tiles < num_sms() ? tiles : num_sms();
   prof_begin(MN ? PROF_GEMM_MN : PROF_GEMM_KK, 2.0 * (double)p.rows_a * p.cols_b * (double)p.red, st);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = use_pdl() ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_bf16x3_kernel<MN, EPI, BN, COOP>, mAh, mAl, mBh, mBl, p);
+  GANTTS_PDL_LAUNCH((gemm_bf16x3_kernel<MN, EPI, BN>), (unsigned)grid, TC_THREADS, smem, st, mAh, mAl, mBh, mBl, p);
   prof_end(st);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchKernelEx(gemm)");
   GANTTS_LAUNCH_CHECK("gemm_bf16x3_kernel");
   return GANTTS_OK;
 }
@@ -858,12 +772,8 @@ static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const C
 template <bool MN, int EPI>
 static int launch_bn(const CUtensorMap& mAh, const CUtensorMap& mAl, const CUtensorMap& mBh, const CUtensorMap& mBl,
                      const GemmParams& p, size_t smem, cudaStream_t st) {
-  if (use_coop()) {
-    if (p.bn == 64) return launch_kernel<MN, EPI, 64, true>(mAh, mAl, mBh, mBl, p, smem, st);
-    return launch_kernel<MN, EPI, 128, true>(mAh, mAl, mBh, mBl, p, smem, st);
-  }
-  if (p.bn == 64) return launch_kernel<MN, EPI, 64, false>(mAh, mAl, mBh, mBl, p, smem, st);
-  return launch_kernel<MN, EPI, 128, false>(mAh, mAl, mBh, mBl, p, smem, st);
+  if (p.bn == 64) return launch_kernel<MN, EPI, 64>(mAh, mAl, mBh, mBl, p, smem, st);
+  return launch_kernel<MN, EPI, 128>(mAh, mAl, mBh, mBl, p, smem, st);
 }
 
 // out[rows_a][cols_b] = epi(A * B^T)   (K-major planes A [rows_a][red], B [cols_b][red]).
