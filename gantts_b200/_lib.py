@@ -173,6 +173,7 @@ SIGNATURES = {
     "gantts_spoof_count_lstm": (_i, [ctypes.POINTER(LstmStackT), _vp, _i, ctypes.POINTER(MlpT), _vp, _i,
                                      ctypes.POINTER(ctypes.c_int), _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
     "gantts_lstm_workspace_bytes": (_sz, []),
+    "gantts_lstm_layer_supported": (_i, [_i, _i, _i]),
     "gantts_lstm_layer_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
     "gantts_lstm_layer_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
     "gantts_lstm_hprev": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),

@@ -627,6 +627,8 @@ static int check_step(const gantts_gan_step_t* c) {
     GANTTS_CHECK_ARG(ls.in_dim == c->g.dims[1],
                      "gan_step: LSTM in_dim %d != hidden2out output width %d (the model returns its input as y_hat)",
                      ls.in_dim, c->g.dims[1]);
+    // refused here rather than by the first backward, after a forward has run
+    if (int rc = lstm_check_trainable(ls.hidden, lstm_ndir(ls))) return rc;
   }
   const gantts_sru_stack_t& s = c->sru;
   GANTTS_CHECK_ARG(s.num_layers >= 0 && s.num_layers <= GANTTS_MAX_SRU_LAYERS, "gan_step: SRU layer count %d not in [0, %d]",
@@ -666,6 +668,7 @@ static int check_step(const gantts_gan_step_t* c) {
       GANTTS_CHECK_ARG(c->d.num_layers == 1 && c->d.dims[0] == nh,
                        "gan_step: with a discriminator LSTM stack d is hidden2out alone: 1 layer of input width %d (got %d "
                        "layer(s), input width %d)", nh, c->d.num_layers, c->d.dims[0]);
+      if (int rc = lstm_check_trainable(dl.hidden, lstm_ndir(dl))) return rc;
     }
     const int cond_w = c->d_conditioned ? gen_in_width(c) : 0;
     GANTTS_CHECK_ARG(c->n_adv >= 1 && c->n_adv <= GANTTS_MAX_COLS && d_in_width(c) == cond_w + c->n_adv,

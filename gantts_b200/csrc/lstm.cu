@@ -560,18 +560,52 @@ static int lstm_pick_hs(int H, int ndir, int* slices) {
   return 0;
 }
 
-template <int HS>
-static int lstm_launch(bool bwd, LstmParams& p, cudaStream_t st) {
-  const int H = p.H;
+static int lstm_use_reg() {
+  static int v = -1;
+  if (v < 0) {
+    const char* e = getenv("GANTTS_B200_LSTM_REG");
+    v = e ? atoi(e) : 1;
+  }
+  return v;
+}
+
+// The kernel lstm_run launches for one layer: HS hidden units per CTA, `slices` CTAs per direction, register-resident
+// (HS = 8, H <= 512, unless GANTTS_B200_LSTM_REG=0) or shared-memory kernels, and its dynamic shared memory.
+struct LstmPlan {
+  int hs, slices;
+  bool reg;
   size_t smem;
-  if (!bwd)
-    smem = ((size_t)4 * HS * (H + 4) + (size_t)LSTM_BC * H + LSTM_BC * 4 * HS + LSTM_MAX_B * HS) * sizeof(float);
-  else
-    smem = ((size_t)HS * (4 * H + 4) + (size_t)LSTM_BC * (4 * H + 4) + LSTM_THREADS + 2 * LSTM_MAX_B * HS) * sizeof(float);
-  if (smem > 227 * 1024) {
-    set_error("lstm: hidden size %d needs %zu B of shared memory (> 227 KB)", H, smem);
+};
+
+// GANTTS_E_UNSUPPORTED, with the error set, when the current device cannot run the recurrence of this shape.
+static int lstm_plan(bool bwd, int H, int ndir, LstmPlan* pl) {
+  pl->hs = lstm_pick_hs(H, ndir, &pl->slices);
+  if (pl->hs == 0) {
+    set_error("lstm: hidden size %d x %d directions does not fit one wave of CTAs", H, ndir);
     return GANTTS_E_UNSUPPORTED;
   }
+  const size_t HS = pl->hs;
+  pl->reg = HS == 8 && H <= 512 && lstm_use_reg();
+  if (pl->reg) {
+    const size_t KR = H <= 256 ? 32 : 64, RPT = 4 * H <= 4 * LSTM_THREADS ? 4 : 8;
+    pl->smem = (!bwd ? LSTM_BC * 8 * KR + 8 * LSTM_BC * 32 + LSTM_MAX_B * 8
+                     : LSTM_BC * RPT * LSTM_THREADS + 8 * 64 + 2 * LSTM_MAX_B * 8) * sizeof(float);
+  } else if (!bwd) {
+    pl->smem = (4 * HS * (H + 4) + (size_t)LSTM_BC * H + LSTM_BC * 4 * HS + LSTM_MAX_B * HS) * sizeof(float);
+  } else {
+    pl->smem = (HS * (4 * H + 4) + (size_t)LSTM_BC * (4 * H + 4) + LSTM_THREADS + 2 * LSTM_MAX_B * HS) * sizeof(float);
+  }
+  if (pl->smem > 227 * 1024) {
+    set_error("lstm: the %s of hidden size %d x %d directions (%d units per CTA) needs %zu B of shared memory per CTA, "
+              "more than the 227 KB limit", bwd ? "backward" : "forward", H, ndir, pl->hs, pl->smem);
+    return GANTTS_E_UNSUPPORTED;
+  }
+  return GANTTS_OK;
+}
+
+template <int HS>
+static int lstm_launch(bool bwd, LstmParams& p, size_t smem, cudaStream_t st) {
+  const int H = p.H;
   void* fn = bwd ? (void*)lstm_bwd_kernel<HS> : (void*)lstm_fwd_kernel<HS>;
   GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   GANTTS_CUDA(cudaMemsetAsync(p.bar, 0, 4 * sizeof(unsigned int), st));
@@ -586,29 +620,14 @@ static int lstm_launch(bool bwd, LstmParams& p, cudaStream_t st) {
   return GANTTS_OK;
 }
 
-static int lstm_use_reg() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("GANTTS_B200_LSTM_REG");
-    v = e ? atoi(e) : 1;
-  }
-  return v;
-}
-
 // Register-resident kernels: HS = 8 and H <= 512 (64 weights per thread).
-static int lstm_launch_reg(bool bwd, LstmParams& p, cudaStream_t st) {
+static int lstm_launch_reg(bool bwd, LstmParams& p, size_t smem, cudaStream_t st) {
   const int H = p.H;
   void* fn;
-  size_t smem;
-  if (!bwd) {
-    const int KR = H <= 256 ? 32 : 64;
-    fn = KR == 32 ? (void*)lstm_fwd_reg_kernel<32> : (void*)lstm_fwd_reg_kernel<64>;
-    smem = ((size_t)LSTM_BC * 8 * KR + 8 * LSTM_BC * 32 + LSTM_MAX_B * 8) * sizeof(float);
-  } else {
-    const int RPT = 4 * H <= 4 * LSTM_THREADS ? 4 : 8;
-    fn = RPT == 4 ? (void*)lstm_bwd_reg_kernel<4> : (void*)lstm_bwd_reg_kernel<8>;
-    smem = ((size_t)LSTM_BC * RPT * LSTM_THREADS + 8 * 64 + 2 * LSTM_MAX_B * 8) * sizeof(float);
-  }
+  if (!bwd)
+    fn = H <= 256 ? (void*)lstm_fwd_reg_kernel<32> : (void*)lstm_fwd_reg_kernel<64>;
+  else
+    fn = 4 * H <= 4 * LSTM_THREADS ? (void*)lstm_bwd_reg_kernel<4> : (void*)lstm_bwd_reg_kernel<8>;
   GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   GANTTS_CUDA(cudaMemsetAsync(p.bar, 0, 4 * sizeof(unsigned int), st));
   void* args[] = {&p};
@@ -624,12 +643,19 @@ static int lstm_launch_reg(bool bwd, LstmParams& p, cudaStream_t st) {
 // One layer's recurrence (forward or backward) in one cooperative launch; p.slices is chosen here.  The barrier
 // counters at p.bar are zeroed on the stream before the launch.
 static int lstm_run(bool bwd, LstmParams& p, cudaStream_t st) {
-  const int hs = lstm_pick_hs(p.H, p.ndir, &p.slices);
-  if (hs == 8 && p.H <= 512 && lstm_use_reg()) return lstm_launch_reg(bwd, p, st);
-  if (hs == 8) return lstm_launch<8>(bwd, p, st);
-  if (hs == 16) return lstm_launch<16>(bwd, p, st);
-  set_error("lstm: hidden size %d x %d directions does not fit one wave of CTAs", p.H, p.ndir);
-  return GANTTS_E_UNSUPPORTED;
+  LstmPlan pl;
+  const int rc = lstm_plan(bwd, p.H, p.ndir, &pl);
+  if (rc) return rc;
+  p.slices = pl.slices;
+  if (pl.reg) return lstm_launch_reg(bwd, p, pl.smem, st);
+  return pl.hs == 8 ? lstm_launch<8>(bwd, p, pl.smem, st) : lstm_launch<16>(bwd, p, pl.smem, st);
+}
+
+// A layer that trains needs both launches; the backward is the larger one, but check both.
+static int lstm_check_trainable(int H, int ndir) {
+  LstmPlan pl;
+  int rc = lstm_plan(false, H, ndir, &pl);
+  return rc ? rc : lstm_plan(true, H, ndir, &pl);
 }
 
 // ---------------------------------------------------------------------------- LSTM stack of the fused GAN step
@@ -706,6 +732,12 @@ __global__ void lstm_bias_sum_kernel(LstmBiasList bl) {
 using namespace gantts;
 
 extern "C" size_t gantts_lstm_workspace_bytes(void) { return 256; }
+
+extern "C" int gantts_lstm_layer_supported(int H, int ndir, int train) {
+  GANTTS_CHECK_ARG(H >= 4 && (H % 4) == 0 && (ndir == 1 || ndir == 2), "lstm: bad H/ndir (H must be a multiple of 4)");
+  LstmPlan pl;
+  return train ? lstm_check_trainable(H, ndir) : lstm_plan(false, H, ndir, &pl);
+}
 
 extern "C" int gantts_lstm_layer_fwd(const float* xproj, const float* W_hh, const int64_t* lengths_dev, float* h_out,
                                      float* gates, float* cells, int B, int T, int H, int ndir, void* workspace,

@@ -121,6 +121,9 @@ def lstm_forward(lstm, x, lengths, training, engine=None):
     B, T, _ = x.shape
     lens = lengths_tensor(lengths, B, T, x.device)
     ndir = 2 if lstm.bidirectional else 1
+    if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in lstm.parameters())):
+        # a layer whose backward this device cannot run is refused before its forward, not in loss.backward()
+        _lib.check(_lib.load().gantts_lstm_layer_supported(lstm.hidden_size, ndir, 1))
     h = x
     for k in range(lstm.num_layers):
         sfx = ["", "_reverse"][:ndir]

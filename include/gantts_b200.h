@@ -265,6 +265,10 @@ int gantts_clip_adam_step(float* const* params, float* const* grads, float* cons
  * shared memory, one grid barrier per step).  workspace: gantts_lstm_workspace_bytes() bytes.
  */
 size_t gantts_lstm_workspace_bytes(void);
+/* GANTTS_OK when the current device runs the forward of a layer of hidden size H and ndir directions and, with train != 0,
+ * its backward too; otherwise GANTTS_E_UNSUPPORTED and the error string names the limit (one wave of CTAs, or the
+ * shared memory per CTA).  The kernel, and so the limit, depends on H, ndir and the device's SM count. */
+int gantts_lstm_layer_supported(int H, int ndir, int train);
 int gantts_lstm_layer_fwd(const float* xproj, const float* W_hh, const int64_t* lengths_dev, float* h_out,
                           float* gates, float* cells, int B, int T, int H, int ndir, void* workspace,
                           size_t workspace_bytes, void* stream);
