@@ -96,6 +96,12 @@ class StepTensorsT(ctypes.Structure):
                 ("state2", ctypes.c_void_p * MAX_STEP_TENSORS)]
 
 
+class OptimizerT(ctypes.Structure):
+    _fields_ = [("own", ctypes.c_int), ("optimizer", ctypes.c_int),
+                ("beta1", ctypes.c_float), ("beta2", ctypes.c_float), ("eps", ctypes.c_float),
+                ("opt_step", ctypes.c_int64)]
+
+
 class GanStepT(ctypes.Structure):
     _fields_ = [("B", ctypes.c_int), ("T", ctypes.c_int),
                 ("g", MlpT), ("highway", HighwayT), ("sru", SruStackT), ("lstm", LstmStackT), ("d", MlpT),
@@ -111,6 +117,7 @@ class GanStepT(ctypes.Structure):
                 ("w_d", ctypes.c_float), ("mse_w", ctypes.c_float), ("mge_w", ctypes.c_float),
                 ("adv_w", ctypes.c_float),
                 ("optimizer", ctypes.c_int), ("beta1", ctypes.c_float), ("beta2", ctypes.c_float),
+                ("d_opt", OptimizerT),
                 ("opt_step", ctypes.c_int64),
                 ("d_lstm", LstmStackT)]
 

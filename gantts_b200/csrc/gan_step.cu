@@ -557,38 +557,51 @@ static int launch_sse(const float* a, int64_t a_rs, const float* b, int64_t b_rs
   return GANTTS_OK;
 }
 
+// One model's optimiser: the step's top-level fields for the generator, d_opt for the discriminator when it has its own
+struct OptSpec {
+  int kind;
+  float beta1, beta2, eps;
+  int64_t step;
+};
+static OptSpec g_opt_spec(const gantts_gan_step_t* c) { return {c->optimizer, c->beta1, c->beta2, c->eps, c->opt_step}; }
+static OptSpec d_opt_spec(const gantts_gan_step_t* c) {
+  const gantts_optimizer_t& o = c->d_opt;
+  return o.own ? OptSpec{o.optimizer, o.beta1, o.beta2, o.eps, o.opt_step} : g_opt_spec(c);
+}
+
 // clip_grad_norm_ + optimiser step over one model's parameter list: two launches (partials, update), no finish kernel
-static int clip_opt_model(const gantts_gan_step_t* c, const ParamList& pl, float* partial, float* sumsq_out, float lr, float wd,
-                          cudaStream_t st) {
+static int clip_opt_model(const gantts_gan_step_t* c, const OptSpec& o, const ParamList& pl, float* partial, float* sumsq_out,
+                          float lr, float wd, cudaStream_t st) {
   TensorList tl;
-  const bool adam = c->optimizer == GANTTS_OPT_ADAM;
+  const bool adam = o.kind == GANTTS_OPT_ADAM;
   int rc = fill(tl, pl.p, pl.g, pl.s, adam ? pl.s2 : nullptr, pl.sizes, 0, pl.n);
   if (rc) return rc;
   const int nb = blocks_for(tl.off[tl.n], OPT_MAX_BLOCKS);
   GANTTS_PDL_LAUNCH((sumsq_partial_kernel), nb, OPT_THREADS, 0, st, tl, partial);
   GANTTS_LAUNCH_CHECK("sumsq_partial_kernel");
   if (adam) {
-    GANTTS_CHECK_ARG(c->opt_step >= 1, "gan_step: Adam needs opt_step >= 1 (the number of the step being taken)");
-    const double t = (double)c->opt_step;
-    const float step_size = (float)((double)lr / (1.0 - pow((double)c->beta1, t)));
-    const float inv_sqrt_bc2 = (float)(1.0 / sqrt(1.0 - pow((double)c->beta2, t)));
-    GANTTS_PDL_LAUNCH((clip_adam_partials_kernel), nb, OPT_THREADS, 0, st, tl, partial, nb, sumsq_out, c->max_norm, c->beta1, c->beta2,
-                      wd, c->eps, step_size, inv_sqrt_bc2);
+    GANTTS_CHECK_ARG(o.step >= 1, "gan_step: Adam needs opt_step >= 1 (the number of the step being taken)");
+    const double t = (double)o.step;
+    const float step_size = (float)((double)lr / (1.0 - pow((double)o.beta1, t)));
+    const float inv_sqrt_bc2 = (float)(1.0 / sqrt(1.0 - pow((double)o.beta2, t)));
+    GANTTS_PDL_LAUNCH((clip_adam_partials_kernel), nb, OPT_THREADS, 0, st, tl, partial, nb, sumsq_out, c->max_norm, o.beta1, o.beta2,
+                      wd, o.eps, step_size, inv_sqrt_bc2);
     GANTTS_LAUNCH_CHECK("clip_adam_partials_kernel");
   } else {
-    GANTTS_PDL_LAUNCH((clip_adagrad_partials_kernel), nb, OPT_THREADS, 0, st, tl, partial, nb, sumsq_out, c->max_norm, lr, wd, c->eps);
+    GANTTS_PDL_LAUNCH((clip_adagrad_partials_kernel), nb, OPT_THREADS, 0, st, tl, partial, nb, sumsq_out, c->max_norm, lr, wd, o.eps);
     GANTTS_LAUNCH_CHECK("clip_adagrad_partials_kernel");
   }
   return GANTTS_OK;
 }
 
-// a model's table: the tensor count its shapes give, every tensor and its optimiser state non-null
-static int check_table(const gantts_gan_step_t* c, const gantts_step_tensors_t& t, int want, const char* model) {
+// a model's table: the tensor count its shapes give, every tensor and its optimiser state non-null (exp_avg_sq too when
+// that model's optimiser is Adam)
+static int check_table(const gantts_step_tensors_t& t, int want, int kind, const char* model) {
   GANTTS_CHECK_ARG(t.n == want, "gan_step: the %s table has %d tensors, its shapes give %d", model, t.n, want);
   for (int i = 0; i < t.n; ++i) {
     GANTTS_CHECK_ARG(t.param[i], "gan_step: null %s tensor %d", model, i);
     GANTTS_CHECK_ARG(t.state[i], "gan_step: null %s optimiser state of tensor %d", model, i);
-    if (c->optimizer == GANTTS_OPT_ADAM)
+    if (kind == GANTTS_OPT_ADAM)
       GANTTS_CHECK_ARG(t.state2[i], "gan_step: Adam needs exp_avg_sq for %s tensor %d", model, i);
   }
   return GANTTS_OK;
@@ -600,6 +613,21 @@ static int check_step(const gantts_gan_step_t* c) {
   GANTTS_CHECK_ARG(c->optimizer == GANTTS_OPT_ADAGRAD || c->optimizer == GANTTS_OPT_ADAM, "gan_step: unknown optimizer %d", c->optimizer);
   if (c->optimizer == GANTTS_OPT_ADAM)
     GANTTS_CHECK_ARG(c->beta1 >= 0.f && c->beta1 < 1.f && c->beta2 >= 0.f && c->beta2 < 1.f, "gan_step: Adam betas out of range");
+  const gantts_optimizer_t& dopt = c->d_opt;
+  GANTTS_CHECK_ARG(dopt.own == 0 || dopt.own == 1, "gan_step: d_opt.own must be 0 (follow the step's optimiser) or 1 (got %d)",
+                   dopt.own);
+  if (dopt.own) {
+    GANTTS_CHECK_ARG(dopt.optimizer == GANTTS_OPT_ADAGRAD || dopt.optimizer == GANTTS_OPT_ADAM,
+                     "gan_step: unknown discriminator optimizer %d (d_opt.optimizer)", dopt.optimizer);
+    if (dopt.optimizer == GANTTS_OPT_ADAM) {
+      GANTTS_CHECK_ARG(dopt.beta1 >= 0.f && dopt.beta1 < 1.f && dopt.beta2 >= 0.f && dopt.beta2 < 1.f,
+                       "gan_step: discriminator Adam betas out of range (d_opt.beta1 %g, d_opt.beta2 %g: each in [0, 1))",
+                       (double)dopt.beta1, (double)dopt.beta2);
+      GANTTS_CHECK_ARG(dopt.opt_step >= 1,
+                       "gan_step: discriminator Adam needs d_opt.opt_step >= 1 (the number of the step being taken; got %lld)",
+                       (long long)dopt.opt_step);
+    }
+  }
   GANTTS_CHECK_ARG(c->g.num_layers >= 1 && c->g.num_layers <= GANTTS_MAX_LAYERS, "gan_step: bad generator");
   GANTTS_CHECK_ARG(c->n_static >= 1 && c->n_static <= GANTTS_MAX_COLS, "gan_step: bad n_static");
   GANTTS_CHECK_ARG(c->n_static_cols == c->n_static, "gan_step: static column list must have n_static entries");
@@ -699,7 +727,7 @@ static int check_step(const gantts_gan_step_t* c) {
   ParamList pl;
   gantts_mlp_t g = c->g;
   g_param_list(c, &g, nullptr, &pl);
-  int rc = check_table(c, c->g_tensors, pl.n, "generator");
+  int rc = check_table(c->g_tensors, pl.n, c->optimizer, "generator");
   if (rc) return rc;
   if (h.static_dim > 0)
     GANTTS_CHECK_ARG((reinterpret_cast<uintptr_t>(pl.gate[BIAS].p) & 15) == 0,
@@ -707,7 +735,7 @@ static int check_step(const gantts_gan_step_t* c) {
   if (!(c->w_d > 0.f)) return GANTTS_OK;
   gantts_mlp_t d = c->d;
   d_param_list(c, &d, nullptr, &pl);
-  return check_table(c, c->d_tensors, pl.n, "discriminator");
+  return check_table(c->d_tensors, pl.n, d_opt_spec(c).kind, "discriminator");
 }
 
 // out_cols: width of the head's fp32 output kept in w->out (the generator's hidden2out); seqs: sequences whose lengths
@@ -1610,7 +1638,7 @@ extern "C" int gantts_gan_step_shaped(const gantts_gan_step_t* c, int B, int T, 
     // loss scalars; no third D forward, no MLPG adjoint, no generator backward or step
     if (phases & 2) {
       NvtxRange r2("gantts_gan_step/phase2 (D only): D step");
-      if ((rc = clip_opt_model(c, s.pd, L.opt_partial, L.scal + S_DSUMSQ, c->lr_d, c->wd_d, st))) return rc;
+      if ((rc = clip_opt_model(c, d_opt_spec(c), s.pd, L.opt_partial, L.scal + S_DSUMSQ, c->lr_d, c->wd_d, st))) return rc;
     }
     if (phases & 4) {
       NvtxRange r4("gantts_gan_step/phase4 (D only): losses");
@@ -1621,7 +1649,8 @@ extern "C" int gantts_gan_step_shaped(const gantts_gan_step_t* c, int B, int T, 
   if (phases & 2) {
     NvtxRange r2("gantts_gan_step/phase2: D step, adv D fwd+bwd, MLPG bwd, G bwd");
     // ---- clip_grad_norm_ + Adagrad on D (train.py:275-276)
-    if (s.has_d && (rc = clip_opt_model(c, s.pd, L.opt_partial, L.scal + S_DSUMSQ, c->lr_d, c->wd_d, st))) return rc;
+    if (s.has_d && (rc = clip_opt_model(c, d_opt_spec(c), s.pd, L.opt_partial, L.scal + S_DSUMSQ, c->lr_d, c->wd_d, st)))
+      return rc;
     // ---- update_generator (train.py:282-320); the MGE term was evaluated in phase 1
     if (s.has_adv) {
       // third D forward: updated weights, fresh dropout mask (train.py:307)
@@ -1636,7 +1665,7 @@ extern "C" int gantts_gan_step_shaped(const gantts_gan_step_t* c, int B, int T, 
   if (phases & 4) {
     NvtxRange r4("gantts_gan_step/phase4: G step, losses");
     // ---- clip_grad_norm_ + Adagrad on G (train.py:317-318), then the loss scalars
-    if ((rc = clip_opt_model(c, s.pg, L.opt_partial, L.scal + S_GSUMSQ, c->lr_g, c->wd_g, st))) return rc;
+    if ((rc = clip_opt_model(c, g_opt_spec(c), s.pg, L.opt_partial, L.scal + S_GSUMSQ, c->lr_g, c->wd_g, st))) return rc;
     return step_finalize(s, losses_dev);
   }
   return GANTTS_OK;

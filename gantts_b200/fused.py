@@ -24,6 +24,7 @@ from . import models
 from . import multistream
 from . import ops
 from . import parallel
+from .optim import OptimizerState
 
 LOSS_NAMES = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mse", "loss_mge", "loss_adv", "loss_g",
               "real_correct", "fake_correct", "frames", "d_grad_norm", "g_grad_norm")
@@ -138,13 +139,28 @@ def check_reference_discriminator(model_ref, n_adv, who):
                            "adversarial columns alone (no linguistic conditioning)" % (who, width, n_adv))
 
 
+def _optimizer_hyper(kind, params, lr, weight_decay):
+    """The hyper-parameters of one model's optimiser: ``params`` over the defaults of its kind (Adagrad: the step's
+    ``lr`` / ``weight_decay`` arguments; Adam: lr 1e-3, weight_decay 0)."""
+    hyper = dict(lr=lr, weight_decay=weight_decay) if kind == "Adagrad" else dict(lr=1e-3, weight_decay=0.0)
+    hyper.update(params or {})
+    return hyper
+
+
 class FusedGanStep(object):
     def __init__(self, model_g, model_d, hp, B, T, w_d=1.0, mse_w=0.0, mge_w=1.0, lr=0.01, weight_decay=1e-7,
                  max_norm=1.0, process_group=None, seed=None, optimizer="Adagrad", optimizer_params=None,
-                 reference_discriminator=None):
-        """``optimizer`` / ``optimizer_params`` mirror ``getattr(optim, hp.optimizer_g)(params, **hp.optimizer_g_params)``
-        of reference train.py:784-789 (one setting for both models): "Adagrad" (lr, weight_decay, eps; the defaults
-        are hparams.py:201-206) or "Adam" (lr, betas, eps, weight_decay; hparams.py:125-130).
+                 reference_discriminator=None, optimizer_d=None, optimizer_d_params=None):
+        """``optimizer`` / ``optimizer_params`` and ``optimizer_d`` / ``optimizer_d_params`` mirror
+        ``getattr(optim, hp.optimizer_g)(model_g.parameters(), **hp.optimizer_g_params)`` and the same for ``_d`` of
+        reference train.py:796-799: "Adagrad" (lr, weight_decay, eps; lr and weight_decay default to the ``lr`` /
+        ``weight_decay`` arguments, hparams.py:201-206) or "Adam" (lr, betas, eps, weight_decay; lr 1e-3 and
+        weight_decay 0 by default, hparams.py:125-130).  ``optimizer_d=None`` gives the discriminator the generator's
+        kind; ``optimizer_d_params=None`` gives it the generator's parameters when the kinds agree, else its kind's
+        defaults.  ``opt_g`` / ``opt_d`` hold each model's hyper-parameters and state with torch.optim's
+        ``param_groups``, ``state_dict()`` and ``load_state_dict()``: every step reads lr, weight_decay, eps and betas
+        from the groups, so train.py's exp_lr_scheduler (:323-333), save_checkpoint and load_checkpoint (:162-171,
+        :651-658) work on them as written.
 
         ``reference_discriminator``: the frozen discriminator of the adversarial stage (train.py --checkpoint-r); every
         step then counts the frames of the pre-update y_hat_static it takes for natural (train.py:549-558) into the
@@ -152,14 +168,15 @@ class FusedGanStep(object):
         It is an MLP, or an LSTMRNN / GRURNN (train.py:779-781 builds it from hp.discriminator like D) of at most 3 layers
         and a configured B of at most 128, whose stack runs over the call's packed sequences."""
         lib = _lib.load()
-        if optimizer not in ("Adagrad", "Adam"):
-            raise RuntimeError("FusedGanStep: no native optimiser %r (Adagrad and Adam are the ones hparams.py uses)" % optimizer)
-        self.optimizer = optimizer
-        okw = dict(optimizer_params or {})
-        if optimizer == "Adam":
-            lr, weight_decay = okw.get("lr", 1e-3), okw.get("weight_decay", 0.0)
-        else:
-            lr, weight_decay = okw.get("lr", lr), okw.get("weight_decay", weight_decay)
+        kind_d = optimizer if optimizer_d is None else optimizer_d
+        for kind in (optimizer, kind_d):
+            if kind not in ("Adagrad", "Adam"):
+                raise RuntimeError("FusedGanStep: no native optimiser %r (Adagrad and Adam are the ones hparams.py uses)"
+                                   % kind)
+        if optimizer_d_params is None and kind_d == optimizer:
+            optimizer_d_params = optimizer_params
+        hyper_g = _optimizer_hyper(optimizer, optimizer_params, lr, weight_decay)
+        hyper_d = _optimizer_hyper(kind_d, optimizer_d_params, lr, weight_decay)
         self.g, self.d, self.hp, self.pg = model_g, model_d, hp, process_group
         self.B, self.T = int(B), int(T)
         dev = next(model_g.parameters()).device
@@ -188,17 +205,24 @@ class FusedGanStep(object):
         ops.require_cuda(*self._params)
         if not all(t.is_contiguous() for t in self._params):
             raise RuntimeError("gantts_b200: parameters must be contiguous")
-        # Adagrad: state_sum | Adam: exp_avg, exp_avg_sq
-        self._sums = [torch.zeros_like(t) for t in self._params]
-        self._sqs = [torch.zeros_like(t) for t in self._params] if optimizer == "Adam" else []
-        for tab, lo, hi in ((c.g_tensors, 0, self._ng), (c.d_tensors, self._ng, len(self._params))):
-            if hi - lo > _lib.MAX_STEP_TENSORS:
+        # each model's optimiser state -- Adagrad: state_sum | Adam: exp_avg, exp_avg_sq -- in model.parameters() order
+        opts = []
+        for tab, params, kind, hyper in ((c.g_tensors, self._params[:self._ng], optimizer, hyper_g),
+                                         (c.d_tensors, self._params[self._ng:], kind_d, hyper_d)):
+            if len(params) > _lib.MAX_STEP_TENSORS:
                 raise RuntimeError("gantts_b200: a model of more than %d tensors" % _lib.MAX_STEP_TENSORS)
-            tab.n = hi - lo
-            for i in range(lo, hi):
-                tab.state[i - lo] = self._sums[i].data_ptr()
-                if self._sqs:
-                    tab.state2[i - lo] = self._sqs[i].data_ptr()
+            state = [torch.zeros_like(t) for t in params]
+            state2 = [torch.zeros_like(t) for t in params] if kind == "Adam" else []
+            tab.n = len(params)
+            for i, t in enumerate(state):
+                tab.state[i] = t.data_ptr()
+            for i, t in enumerate(state2):
+                tab.state2[i] = t.data_ptr()
+            opts.append(OptimizerState(kind, params, state, state2, **hyper))
+        self.opt_g, self.opt_d = opts
+        # the state tensors of both models (G's first); _sqs holds exp_avg_sq of the Adam models only
+        self._sums = self.opt_g._state + self.opt_d._state
+        self._sqs = self.opt_g._state2 + self.opt_d._state2
         self._bind_params(c)
         nw = len(hp.windows)
         entries, n_static = multistream.mlpg_stream_entries(hp.stream_sizes, hp.has_dynamic_features,
@@ -220,18 +244,10 @@ class FusedGanStep(object):
         for i, v in enumerate(acols):
             c.adv_cols[i] = v
         c.d_conditioned = 1 if hp.discriminator_linguistic_condition else 0
-        c.lr_g = c.lr_d = float(lr)
-        c.wd_g = c.wd_d = float(weight_decay)
         c.max_norm = float(max_norm)
-        if optimizer == "Adam":
-            betas = okw.get("betas", (0.9, 0.999))
-            self._betas = (float(betas[0]), float(betas[1]))          # as given (the C struct holds them as float32)
-            c.optimizer, c.beta1, c.beta2, c.eps = _lib.OPT_ADAM, float(betas[0]), float(betas[1]), float(okw.get("eps", 1e-8))
-        else:
-            c.optimizer, c.eps = _lib.OPT_ADAGRAD, float(okw.get("eps", 1e-10))
-        c.opt_step = 1
-        c.w_d, c.mse_w, c.mge_w, c.adv_w = float(w_d), float(mse_w), float(mge_w), 1.0
         self.cfg = c
+        self._set_optimizers(1, 1)
+        c.w_d, c.mse_w, c.mge_w, c.adv_w = float(w_d), float(mse_w), float(mge_w), 1.0
         nbytes = lib.gantts_gan_step_workspace_bytes(ctypes.byref(c))
         if nbytes == 0:
             raise RuntimeError("gantts_b200 gan_step config rejected: %s" % lib.gantts_last_error_string().decode())
@@ -245,7 +261,6 @@ class FusedGanStep(object):
         self._shape = (self.B, self.T, self._table.data_ptr())      # (b, t, MLPG table) of the next native call
         self._seed = int(seed) if seed is not None else ops.draw_seed() & ((1 << 60) - 1)
         self._step = 0                          # training calls: the seed stream
-        self._opt_steps = {"g": 0, "d": 0}      # optimiser steps per model (they differ after D-only steps)
         self._grad_views = {}
         self.ref_d = reference_discriminator
         if reference_discriminator is not None:
@@ -278,6 +293,27 @@ class FusedGanStep(object):
                 raise RuntimeError("gantts_b200 spoof_count config rejected: %s" % lib.gantts_last_error_string().decode())
             self._ref_ws = torch.empty(rbytes, dtype=torch.uint8, device=dev)
             self.spoof_count = torch.zeros((), dtype=torch.float32, device=dev)
+
+    @property
+    def _opt_steps(self):
+        """Optimiser steps per model (they differ after D-only steps)."""
+        return {"g": self.opt_g.steps, "d": self.opt_d.steps}
+
+    def _set_optimizers(self, n_g, n_d):
+        """The optimiser fields of the C config from opt_g / opt_d's groups; n_g, n_d = the number of the step each
+        model would take (Adam's bias corrections).  The discriminator always has its own block."""
+        c = self.cfg
+        for opt, n, d in ((self.opt_g, n_g, False), (self.opt_d, n_d, True)):
+            grp = opt.param_groups[0]
+            kind = _lib.OPT_ADAM if opt.kind == "Adam" else _lib.OPT_ADAGRAD
+            b1, b2 = grp["betas"] if opt.kind == "Adam" else (0.0, 0.0)
+            if d:
+                c.lr_d, c.wd_d = float(grp["lr"]), float(grp["weight_decay"])
+                o = c.d_opt
+                o.own, o.optimizer, o.beta1, o.beta2, o.eps, o.opt_step = 1, kind, b1, b2, float(grp["eps"]), n
+            else:
+                c.lr_g, c.wd_g = float(grp["lr"]), float(grp["weight_decay"])
+                c.optimizer, c.beta1, c.beta2, c.eps, c.opt_step = kind, b1, b2, float(grp["eps"]), n
 
     def _bind_params(self, cfg):
         for tab, lo, hi in ((cfg.g_tensors, 0, self._ng), (cfg.d_tensors, self._ng, len(self._params))):
@@ -385,29 +421,22 @@ class FusedGanStep(object):
         seed = (self._seed + self._step) & ((1 << 61) - 1)
         self.last_seed = seed
         self._step += 1
-        # Adam's bias corrections: the number of the step each model is taking
-        self._opt_steps["d"] += 1
-        if update_g:
-            self._opt_steps["g"] += 1
-        n_g, n_d = self._opt_steps["g"], self._opt_steps["d"]
+        # the hyper-parameters as the groups hold them now, and the number of the step each model takes (Adam's bias
+        # corrections; G's is not read by a D-only step)
+        self._set_optimizers(self.opt_g.steps + 1, self.opt_d.steps + 1)
         d_only = 0 if update_g else _lib.STEP_D_ONLY
-        if world == 1 and (n_g == n_d or d_only):
-            self.cfg.opt_step = n_d
+        if world == 1:
             self._call(7 | d_only, x, y, lengths, inv, seed)
-        elif world == 1:
-            self.cfg.opt_step = n_d
-            self._call(1 | 2, x, y, lengths, inv, seed)
-            self.cfg.opt_step = n_g
-            self._call(4, x, y, lengths, inv, seed)
         else:
-            self.cfg.opt_step = n_d
             self._call(1 | d_only, x, y, lengths, inv, seed)
             parallel.allreduce_sum_(self.grad_buffer(1), self.pg)
             self._call(2 | d_only, x, y, lengths, inv, seed)
             if update_g:
                 parallel.allreduce_sum_(self.grad_buffer(0), self.pg)
-            self.cfg.opt_step = n_g
             self._call(4 | d_only, x, y, lengths, inv, seed)
+        self.opt_d.steps += 1
+        if update_g:
+            self.opt_g.steps += 1
         self._count_spoofed(lengths)
         return self.losses
 
@@ -452,54 +481,16 @@ class FusedGanStep(object):
         return v
 
     # ---- checkpoint / resume (reference train.py:162-171 save_checkpoint, :174-199 load_checkpoint round-trip
-    # optimizer.state_dict(); the layout below is torch.optim.Adagrad's, one entry per parameter in
-    # model.parameters() order, so the files are interchangeable with the reference's)
-    def _opt_state(self, lo, hi, lr, wd, nstep):
-        n = hi - lo
-        step = torch.tensor(float(nstep))
-        if self.optimizer == "Adam":
-            return {"state": {i: {"step": step.clone(), "exp_avg": self._sums[lo + i].detach().clone(),
-                                  "exp_avg_sq": self._sqs[lo + i].detach().clone()} for i in range(n)},
-                    "param_groups": [{"lr": lr, "betas": self._betas,
-                                      "eps": float(self.cfg.eps), "weight_decay": wd, "amsgrad": False, "maximize": False,
-                                      "foreach": None, "capturable": False, "differentiable": False, "fused": None,
-                                      "params": list(range(n))}]}
-        return {"state": {i: {"step": step.clone(), "sum": self._sums[lo + i].detach().clone()} for i in range(n)},
-                "param_groups": [{"lr": lr, "lr_decay": 0, "eps": float(self.cfg.eps), "weight_decay": wd,
-                                  "initial_accumulator_value": 0, "foreach": None, "maximize": False,
-                                  "differentiable": False, "fused": None, "params": list(range(n))}]}
-
+    # optimizer.state_dict()): one torch.optim layout per model, opt_g's and opt_d's own, so each entry is
+    # interchangeable with a torch.optim.Adagrad / Adam over that model's parameters
     def state_dict(self):
-        ng, n = self._ng, len(self._sums)
-        return {"optimizer_g": self._opt_state(0, ng, float(self.cfg.lr_g), float(self.cfg.wd_g), self._opt_steps["g"]),
-                "optimizer_d": self._opt_state(ng, n, float(self.cfg.lr_d), float(self.cfg.wd_d), self._opt_steps["d"]),
+        return {"optimizer_g": self.opt_g.state_dict(), "optimizer_d": self.opt_d.state_dict(),
                 "step": self._step, "seed": self._seed}
 
     def load_state_dict(self, sd):
-        ng, n = self._ng, len(self._sums)
         step = int(sd.get("step", self._step))
-        for key, lo, hi in (("optimizer_g", 0, ng), ("optimizer_d", ng, n)):
-            st = sd[key]["state"]
-            for i in range(hi - lo):
-                e = st.get(i, st.get(str(i)))
-                if e is None:
-                    raise RuntimeError("FusedGanStep.load_state_dict: %s has no state for parameter %d" % (key, i))
-                if i == 0:              # each optimiser's own step count (the models differ after D-only steps)
-                    self._opt_steps[key[-1]] = int(float(e["step"])) if "step" in e else step
-                if self.optimizer == "Adam":
-                    self._sums[lo + i].copy_(e["exp_avg"])
-                    self._sqs[lo + i].copy_(e["exp_avg_sq"])
-                else:
-                    self._sums[lo + i].copy_(e["sum"])
-            grp = (sd[key].get("param_groups") or [{}])[0]
-            if self.optimizer == "Adam" and "betas" in grp:
-                self._betas = (float(grp["betas"][0]), float(grp["betas"][1]))
-                self.cfg.beta1, self.cfg.beta2 = self._betas
-            if key == "optimizer_g":
-                self.cfg.lr_g = float(grp.get("lr", self.cfg.lr_g))
-                self.cfg.wd_g = float(grp.get("weight_decay", self.cfg.wd_g))
-            else:
-                self.cfg.lr_d = float(grp.get("lr", self.cfg.lr_d))
-                self.cfg.wd_d = float(grp.get("weight_decay", self.cfg.wd_d))
+        for key, opt in (("optimizer_g", self.opt_g), ("optimizer_d", self.opt_d)):
+            opt.steps = step                    # an entry without "step" counts every training call
+            opt.load_state_dict(sd[key])
         self._step = step
         self._seed = int(sd.get("seed", self._seed))

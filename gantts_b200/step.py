@@ -54,8 +54,16 @@ class GanTrainer(object):
     """One-call GAN step over native ops.  ``step`` returns device scalars (no host sync)."""
 
     def __init__(self, model_g, model_d, hp, w_d=1.0, mse_w=0.0, mge_w=1.0, lr=0.01, weight_decay=1e-7,
-                 process_group=None, optimizer="Adagrad", optimizer_params=None, reference_discriminator=None):
-        """``reference_discriminator``: the frozen discriminator of the adversarial stage (train.py --checkpoint-r);
+                 process_group=None, optimizer="Adagrad", optimizer_params=None, reference_discriminator=None,
+                 optimizer_d=None, optimizer_d_params=None):
+        """``optimizer`` / ``optimizer_params`` and ``optimizer_d`` / ``optimizer_d_params`` are hp.optimizer_g /
+        hp.optimizer_g_params and hp.optimizer_d / hp.optimizer_d_params of reference train.py:796-799: ``opt_g`` and
+        ``opt_d`` are ClipAdagrad or ClipAdam with torch.optim's ``param_groups`` / ``state_dict()``, so train.py's
+        exp_lr_scheduler, save_checkpoint and load_checkpoint take them as they are.  ``optimizer_d=None`` gives D the
+        generator's kind; ``optimizer_d_params=None`` gives D the generator's parameters when the kinds agree, else
+        ``lr`` / ``weight_decay`` as the generator would get them.
+
+        ``reference_discriminator``: the frozen discriminator of the adversarial stage (train.py --checkpoint-r);
         every step then returns ``out["spoof_count"]``, the frames of the pre-update y_hat_static it takes for natural
         (train.py:549-558).  It is put in eval mode like train.py:445 does, sees no linguistic conditioning and is
         never updated."""
@@ -67,8 +75,13 @@ class GanTrainer(object):
             reference_discriminator.eval()
         self.w_d, self.mse_w, self.mge_w = float(w_d), float(mse_w), float(mge_w)
         okw = dict(optimizer_params) if optimizer_params is not None else dict(lr=lr, weight_decay=weight_decay)
+        kind_d = optimizer if optimizer_d is None else optimizer_d
+        if optimizer_d_params is not None:
+            okw_d = dict(optimizer_d_params)
+        else:
+            okw_d = okw if kind_d == optimizer else dict(lr=lr, weight_decay=weight_decay)
         self.opt_g = make_optimizer(optimizer, model_g.parameters(), **okw)
-        self.opt_d = make_optimizer(optimizer, model_d.parameters(), **okw) if model_d is not None else None
+        self.opt_d = make_optimizer(kind_d, model_d.parameters(), **okw_d) if model_d is not None else None
         self.pg = process_group
         parallel.broadcast_parameters(model_g, group=process_group)
         if model_d is not None:

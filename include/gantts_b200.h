@@ -383,9 +383,22 @@ typedef struct {
   float* state2[GANTTS_MAX_STEP_TENSORS];  /* Adam exp_avg_sq (unused by Adagrad) */
 } gantts_step_tensors_t;
 
+/* The discriminator's own optimiser (reference train.py:796-799 builds optimizer_d from hp.optimizer_d and
+ * hp.optimizer_d_params, apart from optimizer_g).  own = 0 (a zero-filled block): the discriminator follows the step's
+ * optimizer, beta1, beta2, eps and opt_step like the generator.  own = 1: it steps with the kind, betas, eps and step
+ * number below (opt_step = number of D's step being taken, 1 for the first; read under Adam only), and the step's
+ * top-level fields are the generator's alone.  Its lr and weight decay are lr_d / wd_d either way. */
+typedef struct {
+  int own;                                 /* 0: follow the step's optimiser fields; 1: the fields below */
+  int optimizer;                           /* GANTTS_OPT_ADAGRAD | GANTTS_OPT_ADAM */
+  float beta1, beta2, eps;
+  int64_t opt_step;
+} gantts_optimizer_t;
+
 /* The shape blocks (g, highway, sru, lstm, d) describe the two models; their tensors come from g_tensors and d_tensors
  * alone: the W / b pointers of g and d are not read.  The step binds the tables to the stages from the shapes and
- * rejects a table whose n differs from the count the shapes give, or with a null param or state (state2 under Adam). */
+ * rejects a table whose n differs from the count the shapes give, or with a null param or state (state2 where that
+ * model's optimiser is Adam). */
 typedef struct {
   int B, T;
   gantts_mlp_t g;                          /* generator: dims[0] = linguistic width, dims[L] = acoustic width */
@@ -407,12 +420,14 @@ typedef struct {
                                               cat((x, y_adv), -1), d.dims[0] = g.dims[0] + n_adv */
   float lr_g, lr_d, wd_g, wd_d, eps, max_norm;
   float w_d, mse_w, mge_w, adv_w;
-  /* Optimiser of both models (reference train.py:784-789 getattr(optim, hp.optimizer_g)(...)): 0 = Adagrad
-   * (hparams.py:201-206; state = state_sum), 1 = Adam (hparams.py:125-130, the duration model: lr 1e-3,
-   * betas (0.5, 0.9), weight_decay 0, eps 1e-8, amsgrad off; state = exp_avg, state2 = exp_avg_sq, opt_step =
-   * number of the step being taken, 1 for the first -- the bias corrections are computed on the host). */
+  /* Optimiser of the generator, and of the discriminator unless d_opt.own (reference train.py:796-799
+   * getattr(optim, hp.optimizer_g)(...)): 0 = Adagrad (hparams.py:201-206; state = state_sum), 1 = Adam
+   * (hparams.py:125-130, the duration model: lr 1e-3, betas (0.5, 0.9), weight_decay 0, eps 1e-8, amsgrad off; state =
+   * exp_avg, state2 = exp_avg_sq, opt_step = number of the step being taken, 1 for the first -- the bias corrections
+   * are computed on the host).  With d_opt.own = 0, opt_step is the discriminator's number under GANTTS_STEP_D_ONLY. */
   int optimizer;
   float beta1, beta2;
+  gantts_optimizer_t d_opt;                /* zero-filled: the discriminator shares the fields around it */
   int64_t opt_step;
   /* Recurrent discriminator (reference LSTMRNN models.py:193-213, or GRURNN :170-190 -- also an nn.LSTM -- with
    * last_sigmoid=True; train.py:774 builds the class hp.discriminator names): num_layers > 0.  num_layers = 0 (a zero-filled
@@ -447,7 +462,8 @@ typedef struct {
  *   4 = loss scalars (no G clip / step: G's tensors and optimiser state are untouched)
  * and the loss slots mean what they mean in the full step, except loss_adv = 0, loss_g = mse_w loss_mse + mge_w loss_mge
  * and g_grad_norm = 0.  A data-parallel caller all-reduces the discriminator's buffer between 1 and 2 only.  Needs
- * w_d > 0; cannot be combined with GANTTS_STEP_EVAL.  opt_step is D's Adam step number here. */
+ * w_d > 0; cannot be combined with GANTTS_STEP_EVAL.  D's Adam step number is d_opt.opt_step, or opt_step when
+ * d_opt.own = 0. */
 #define GANTTS_STEP_D_ONLY 16
 
 /* Dropout seeds of the fused step, so a test can regenerate every keep mask with gantts_dropout():
