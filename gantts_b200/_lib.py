@@ -46,6 +46,10 @@ class DistortionColsT(ctypes.Structure):
                 ("mse_start", ctypes.c_int), ("mse_count", ctypes.c_int)]
 
 
+METRIC_ACOUSTIC, METRIC_DURATION, METRIC_VC = 0, 1, 2
+LOG_UPDATE_D, LOG_UPDATE_G, LOG_SPOOF = 1, 2, 4
+LOG_N, LOG_FRAMES, LOG_LOSSES, LOG_SPOOFED, LOG_METRICS, LOG_SLOTS = 0, 1, 2, 14, 15, 20
+
 MAX_LAYERS = 8
 
 
@@ -122,6 +126,12 @@ class GanStepT(ctypes.Structure):
                 ("d_lstm", LstmStackT)]
 
 
+class EpochLogT(ctypes.Structure):
+    _fields_ = [("kind", ctypes.c_int), ("n_static", ctypes.c_int),
+                ("static_cols", ctypes.c_int * MAX_COLS),
+                ("cols", DistortionColsT)]
+
+
 OPT_ADAGRAD, OPT_ADAM = 0, 1
 
 _lib = None
@@ -155,6 +165,10 @@ SIGNATURES = {
     "gantts_distortions_workspace_bytes": (_sz, []),
     "gantts_distortions": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp,
                                 ctypes.POINTER(DistortionColsT), _vp, _vp, _sz, _vp]),
+    "gantts_epoch_log_workspace_bytes": (_sz, [ctypes.POINTER(EpochLogT)]),
+    "gantts_epoch_log_reset": (_i, [_vp, _vp]),
+    "gantts_epoch_log_add": (_i, [ctypes.POINTER(EpochLogT), _i, _vp, _vp, _vp, _i64, _i64, _i, _vp, _i64, _i64, _vp,
+                                  _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "gantts_masked_bce_fwd": (_i, [_vp, _vp, _i64, _i, _vp, _vp, _sz, _vp]),
     "gantts_masked_bce_bwd": (_i, [_vp, _vp, _i64, _i, _vp, _vp, _vp]),
     "gantts_linear_workspace_bytes": (_sz, [_i64, _i, _i, _i]),

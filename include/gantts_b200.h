@@ -574,6 +574,66 @@ int gantts_distortions(const float* y, int64_t y_bstride, int64_t y_tstride, con
                        const float* mean_dev, const float* std_dev, const gantts_distortion_cols_t* cols,
                        float* out8_dev, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Epoch log of the training loop (reference train.py:531-595 per batch, :597-637 per phase): gantts_epoch_log_add,
+ * called once after each step, folds that step's results into a per-phase record of GANTTS_LOG_SLOTS doubles in device
+ * memory.  Nothing is read back; the caller reads the record once at the end of the phase.  Enqueue-only: no allocation,
+ * no host synchronisation, every argument checked before the first launch.
+ *
+ * Record (fp64, like train.py's Python-float sums of fp32 .item() values):
+ *   [GANTTS_LOG_N]        batches added                                       (train.py:490, N)
+ *   [GANTTS_LOG_FRAMES]   sum of lengths_dev over the batches                 (:532, total_num_frames)
+ *   [GANTTS_LOG_LOSSES+i] sum of losses_dev[i], the 12 scalars of gantts_gan_step (loss_d, loss_fake_d, loss_real_d,
+ *                         loss_mse, loss_mge, loss_adv, loss_g, real_correct, fake_correct, frames, d_grad_norm,
+ *                         g_grad_norm): D's (0-2, 7, 8, 10) under LOG_UPDATE_D (:562-571), G's (3-6, 11) under
+ *                         LOG_UPDATE_G (:574-585), frames (9) always
+ *   [GANTTS_LOG_SPOOFED]  sum of spoof_dev[0] under LOG_SPOOF                 (:549-558, regard_fake_as_natural)
+ *   [GANTTS_LOG_METRICS+k] under LOG_UPDATE_G the batch's distortions (:587-595): k = 0 mcd, 1 bap_mcd, 2 f0_rmse,
+ *                         3 vuv_err, 4 dur_rmse; the metric kind says which are written
+ * The batch's distortions are those of compute_distortions (:399-432) with gantts_b200/metrics.py's formulas in fp64 on
+ * the eight sums of gantts_distortions (same pass, same reduction): mcd = 10/ln10 sqrt2 s0/frames, bap_mcd = the same of
+ * s1 / 10, f0_rmse = sqrt(s2/s3) or NaN when no frame is voiced in both (the reference maps ZeroDivisionError to NaN and
+ * the NaN stays in the epoch sum), vuv_err = s4/frames, dur_rmse = sqrt(s6/frames).
+ *
+ * The target is read from the step's input y [B][T][y_cols] (static + dynamic columns) through static_cols, the
+ * static-column map of gantts_gan_step_t (multistream.static_feature_columns), so y_static is never built; y_hat_static
+ * [B][T][n_static] is read with its own strides.  mean_dev / std_dev: float32[n_static], the de-normalisation of each
+ * static column (train.py:358-380 indexes the static+dynamic-domain statistics: Y_data_mean[static_cols]).
+ * Workspace: gantts_epoch_log_workspace_bytes(cfg) (0 = the config is rejected; the message names the rule).
+ * gantts_epoch_log_reset zeroes a record on the stream.  y, y_hat_static, mean_dev and std_dev are only read under
+ * LOG_UPDATE_G and may be NULL otherwise; spoof_dev only under LOG_SPOOF.
+ */
+#define GANTTS_METRIC_ACOUSTIC 0 /* hp.name "acoustic": mcd, bap_mcd, f0_rmse, vuv_err */
+#define GANTTS_METRIC_DURATION 1 /* "duration": dur_rmse */
+#define GANTTS_METRIC_VC 2       /* "vc": mcd */
+
+#define GANTTS_LOG_UPDATE_D 1
+#define GANTTS_LOG_UPDATE_G 2
+#define GANTTS_LOG_SPOOF 4
+
+#define GANTTS_LOG_NUM_LOSSES 12
+#define GANTTS_LOG_N 0
+#define GANTTS_LOG_FRAMES 1
+#define GANTTS_LOG_LOSSES 2
+#define GANTTS_LOG_SPOOFED 14
+#define GANTTS_LOG_METRICS 15
+#define GANTTS_LOG_SLOTS 20
+
+typedef struct {
+  int kind;                             /* GANTTS_METRIC_* */
+  int n_static;                         /* columns of y_hat_static */
+  int static_cols[GANTTS_MAX_COLS];     /* y column of each static column */
+  gantts_distortion_cols_t cols;        /* column groups, in static columns (train.py:383-396, 412-428) */
+} gantts_epoch_log_t;
+
+size_t gantts_epoch_log_workspace_bytes(const gantts_epoch_log_t* cfg);
+int gantts_epoch_log_reset(double* record_dev, void* stream);
+int gantts_epoch_log_add(const gantts_epoch_log_t* cfg, int flags, const float* losses_dev, const float* spoof_dev,
+                         const float* y, int64_t y_bstride, int64_t y_tstride, int y_cols, const float* y_hat_static,
+                         int64_t yh_bstride, int64_t yh_tstride, const int64_t* lengths_dev, int B, int T,
+                         const float* mean_dev, const float* std_dev, double* record_dev, void* workspace,
+                         size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
