@@ -128,33 +128,59 @@ def in2out_highway_forward(x, R, gate, layers, static_dim, dropout_p=0.0, traini
     return h, x_static + Tx * Gx
 
 
-def in2out_rnn_highway_forward(x, R, lengths, gate, lstm, hidden2out, static_dim):
-    """reference gantts/models.py:92-118 -- pack -> nn.LSTM -> pad -> hidden2out -> MLPG; returns
+def lstm_stack(x, lengths, layers, masks=None):
+    """pack -> nn.LSTM -> pad (reference gantts/models.py:100-108,182-187,205-210) through a torch ``nn.LSTM``, or
+    through each nn.LSTM of the list ``layers`` in turn, padded back to x's length (``lengths=None``: unpacked, as the
+    reference runs it).  The oracle for the recurrent kernels is torch's own CPU LSTM, as in the reference;
+    ``GeneratorOracle`` and ``DiscriminatorOracle`` run it one layer at a time so that ``masks[k]`` ([B * T][ndir H]
+    multipliers, the product's own inter-layer dropout decisions) can scale the output of layer k < len(layers) - 1.
+    Without masks, single-layer LSTMs in turn give on CPU exactly the bits of one multi-layer nn.LSTM without
+    dropout."""
+    if isinstance(layers, torch.nn.LSTM):
+        layers = [layers]
+    h = x
+    for k, lstm in enumerate(layers):
+        if lengths is None:
+            h, _ = lstm(h)
+        else:
+            out, _ = lstm(torch.nn.utils.rnn.pack_padded_sequence(h, [int(l) for l in lengths], batch_first=True))
+            h, _ = torch.nn.utils.rnn.pad_packed_sequence(out, batch_first=True, total_length=x.size(1))
+        if masks is not None and k + 1 < len(layers):
+            h = h * masks[k].view_as(h)
+    return h
+
+
+def in2out_rnn_highway_forward(x, R, lengths, gate, lstm, hidden2out, static_dim, masks=None):
+    """reference gantts/models.py:92-118 -- ``lstm_stack`` -> hidden2out -> MLPG; returns
     ``(x, x_static + sigmoid(T x_static) * Gx)``: the FIRST output is the input itself (``:118``)."""
     x = x.unsqueeze(0) if x.dim() == 2 else x
     x_static = x[:, :, :static_dim]
     Tx = torch.sigmoid(F.linear(x_static, gate[0], gate[1]))
-    if lengths is not None:
-        packed = torch.nn.utils.rnn.pack_padded_sequence(x, [int(l) for l in lengths], batch_first=True)
-        out, _ = lstm(packed)
-        out, _ = torch.nn.utils.rnn.pad_packed_sequence(out, batch_first=True)
-    else:
-        out, _ = lstm(x)
-    out = F.linear(out, hidden2out[0], hidden2out[1])
+    out = F.linear(lstm_stack(x, lengths, lstm, masks), hidden2out[0], hidden2out[1])
     Gx = nn_port.unit_variance_mlpg(R, out)
     return x, x_static + Tx * Gx
 
 
-def lstm_forward(x, lengths, lstm, hidden2out, last_sigmoid=False):
+def lstm_forward(x, lengths, lstm, hidden2out, last_sigmoid=False, masks=None):
     """reference gantts/models.py:204-213 (LSTMRNN) / :181-190 (GRURNN, also an nn.LSTM):
-    pack -> nn.LSTM -> pad -> Linear (-> sigmoid).  ``lstm`` is a torch ``nn.LSTM`` (the oracle
-    for the recurrent kernel is torch's own CPU LSTM, as in the reference)."""
-    lengths = [int(l) for l in lengths]
-    packed = torch.nn.utils.rnn.pack_padded_sequence(x, lengths, batch_first=True)
-    out, _ = lstm(packed)
-    out, _ = torch.nn.utils.rnn.pad_packed_sequence(out, batch_first=True)
-    out = F.linear(out, hidden2out[0], hidden2out[1])
+    ``lstm_stack`` -> Linear (-> sigmoid).  ``lstm``: a torch ``nn.LSTM`` or a list of them (see ``lstm_stack``)."""
+    out = F.linear(lstm_stack(x, lengths, lstm, masks), hidden2out[0], hidden2out[1])
     return torch.sigmoid(out) if last_sigmoid else out
+
+
+def sru_forward(x, layers, hidden2out, bidirectional, activation_type, masks=None):
+    """SRURNN (reference gantts/models.py:144-167): ``sru_layer_forward`` per layer, then hidden2out.  ``layers`` holds
+    each layer's (weight, bias) as the model stores them, the bias [f-bias | r-bias] over both directions;
+    ``activation_type`` 0 / 1 / 2 is identity / tanh / ReLU.  ``masks`` = [(mask_x, mask_h or None)] per layer."""
+    dirs = 2 if bidirectional else 1
+    h = x
+    for i, (W, b) in enumerate(layers):
+        nc = b.numel() // 2
+        bport = torch.stack([b[:nc].view(dirs, nc // dirs), b[nc:].view(dirs, nc // dirs)], 1).reshape(-1)
+        mx, mh = masks[i] if masks is not None else (None, None)
+        h = sru_layer_forward(h.transpose(0, 1), W, bport, bidirectional=bidirectional, use_tanh=activation_type == 1,
+                              use_relu=activation_type == 2, mask_x=mx, mask_h=mh).transpose(0, 1)
+    return F.linear(h, hidden2out[0], hidden2out[1])
 
 
 # ------------------------------------------------------------------- train.py step functions
@@ -251,43 +277,49 @@ def apply_generator(model_out, x, R, hp, include_parameter_generation=False):
     return y_hat, multi_stream_mlpg(y_hat, R, hp["stream_sizes"], hp["has_dynamic_features"])
 
 
-def gan_step(g_forward, g_params, g_sum, d_layers, d_sum, x, y, lengths, R, hp, w_d=1.0, mse_w=0.0,
+def gan_step(g_forward, g_params, g_sum, d, d_sum, x, y, lengths, R, hp, w_d=1.0, mse_w=0.0,
              mge_w=1.0, adv_w=1.0, dropout_d=0.0, training=True, lr=0.01, weight_decay=1e-7, update=True,
-             d_masks=None, d_opt=None, g_opt=None):
+             update_g=True, d_masks=None, d_opt=None, g_opt=None):
     """One mini-batch of the reference train_loop body (train.py:528-580) for ANY generator:
     ``g_forward()`` -> ``(y_hat, y_hat_static)`` is the result of ``apply_generator`` (train.py:336-355)
-    with autograd history on ``g_params``; ``d_layers`` is the MLP discriminator ``[(W, b), ...]`` or
-    None.  ``d_masks`` = {"real": [...], "fake": [...], "adv": [...]} injects dropout multipliers into
-    the three discriminator forwards (see ``mlp_forward``).
+    with autograd history on ``g_params``; ``d`` is a ``DiscriminatorOracle``, the MLP discriminator
+    ``[(W, b), ...]`` or None.  ``d_masks`` = {"real": [...], "fake": [...], "adv": [...]} injects dropout
+    multipliers into the three discriminator forwards (see ``DiscriminatorOracle.forward``).
 
     Order of operations and quirks preserved (SURVEY.md section 3.2): single zero_grad at the
     top; y_hat_static is NOT detached in the discriminator update, so ``loss_d.backward`` also
     deposits the fake-term gradient on the generator; the discriminator steps before the third
     D forward used by the adversarial loss; gradients of both backwards accumulate on G before
     its clip + Adagrad step.  ``training=False`` with ``update=False`` is the "test" phase of
-    train.py:481-486 (forwards and losses only).  Returns a dict of python floats and the
-    generator outputs."""
+    train.py:481-486 (forwards and losses only).  ``update_g=False`` is the discriminator warm-up step
+    (train.py --discriminator-warmup, :696): the generator runs without a graph and update_generator is not
+    called, so the step reports loss_adv = 0, g_grad_norm = 0 and loss_g = mse_w loss_mse + mge_w loss_mge.
+    The discriminator steps in place with Adagrad (state ``d_sum``) or the stepper ``d_opt``, the generator
+    with ``g_sum`` or ``g_opt``.  Returns a dict of python floats and the generator outputs."""
+    if isinstance(d, list):
+        d = DiscriminatorOracle.of_layers(d)
     nw = hp["num_windows"]
     y_static = get_static_features(y, nw, hp["stream_sizes"], hp["has_dynamic_features"])   # :528-529
     mask = sequence_mask(lengths, x.size(1)).unsqueeze(-1)                                   # :535
-    d_params = [t for pair in d_layers for t in pair] if d_layers is not None else []
+    d_params = d.params() if d is not None else []
     for p in list(g_params) + d_params:                                                      # :538-539
         p.grad = None
-    y_hat, y_hat_static = g_forward()                                                        # :542
+    with torch.set_grad_enabled(torch.is_grad_enabled() and update_g):
+        y_hat, y_hat_static = g_forward()                                                    # :542
     out = {}
     T = mask.sum().item()
     cond = hp.get("discriminator_linguistic_condition", False)
     dm = d_masks or {}
-    if w_d > 0 and d_layers is not None:
+    if w_d > 0 and d is not None:
         # update_discriminator, train.py:245-279
         real_in = get_selected_static_stream(y_static, hp)
         fake_in = get_selected_static_stream(y_hat_static, hp)
         if cond:
             real_in = torch.cat((x, real_in), -1)
             fake_in = torch.cat((x, fake_in), -1)
-        D_real = mlp_forward(real_in, d_layers, dropout_d, training, last_sigmoid=True, masks=dm.get("real"))
+        D_real = d.forward(real_in, lengths, dm.get("real"), dropout_d, training)
         out["real_correct"] = ((D_real > 0.5).float() * mask).sum().item()
-        D_fake = mlp_forward(fake_in, d_layers, dropout_d, training, last_sigmoid=True, masks=dm.get("fake"))
+        D_fake = d.forward(fake_in, lengths, dm.get("fake"), dropout_d, training)
         out["fake_correct"] = ((D_fake < 0.5).float() * mask).sum().item()
         loss_real = bce_real(D_real, mask, T)
         loss_fake = bce_fake(D_fake, mask, T)
@@ -304,17 +336,17 @@ def gan_step(g_forward, g_params, g_sum, d_layers, d_sum, x, y, lengths, R, hp, 
     # update_generator, train.py:282-320
     loss_mge = masked_mse(y_hat_static, y_static, mask=mask)
     loss_mse = masked_mse(y_hat, y, mask=mask)
-    if adv_w > 0 and w_d > 0 and d_layers is not None:
+    if adv_w > 0 and w_d > 0 and d is not None and update_g:
         fake_in = get_selected_static_stream(y_hat_static, hp)
         if cond:
             fake_in = torch.cat((x, fake_in), -1)
-        D_adv = mlp_forward(fake_in, d_layers, dropout_d, training, last_sigmoid=True, masks=dm.get("adv"))
+        D_adv = d.forward(fake_in, lengths, dm.get("adv"), dropout_d, training)
         loss_adv = bce_real(D_adv, mask, T)
     else:
         loss_adv = y.new_zeros(1)
         adv_w = 0.0
     loss_g = (mse_w * loss_mse + mge_w * loss_mge) + adv_w * loss_adv
-    if update:
+    if update and update_g:
         loss_g.backward()
         g_params = list(g_params)
         gg = [p.grad if p.grad is not None else torch.zeros_like(p) for p in g_params]
@@ -323,8 +355,10 @@ def gan_step(g_forward, g_params, g_sum, d_layers, d_sum, x, y, lengths, R, hp, 
             g_opt(g_params, gg)
         else:
             adagrad_step(g_params, gg, g_sum, lr, weight_decay)
+    elif update:
+        out["g_grad_norm"] = 0.0
     out.update(loss_mse=loss_mse.item(), loss_mge=loss_mge.item(), loss_adv=float(loss_adv.detach()),
-               loss_g=float(loss_g.detach()))
+               loss_g=float(loss_g.detach()), frames=T)
     return out, y_hat.detach(), y_hat_static.detach()
 
 
@@ -346,39 +380,70 @@ def gan_step_mlp(state, x, y, lengths, R, hp, w_d=1.0, mse_w=0.0, mge_w=1.0, adv
                     d_opt=d_opt, g_opt=g_opt)
 
 
+def _pair(sd, k, named):
+    """(``k``.weight, ``k``.bias) of a reference state_dict as leaf tensors (requires_grad), recorded in ``named``."""
+    pair = tuple(torch.as_tensor(np.asarray(sd[k + s])).clone().float().requires_grad_(True)
+                 for s in (".weight", ".bias"))
+    named[k + ".weight"], named[k + ".bias"] = pair
+    return pair
+
+
+def _count(sd, pre):
+    return len([k for k in sd if k.startswith(pre) and k.endswith(".weight")])
+
+
+def _linear_layers(sd, pre, named):
+    """[(W, b), ...] of the ``pre``.i layers then last_linear of a reference state_dict, recorded in ``named``."""
+    return [_pair(sd, k, named) for k in ["%s.%d" % (pre, i) for i in range(_count(sd, pre + "."))] + ["last_linear"]]
+
+
+def _lstm_layers(sd, prefix, num_layers, hidden, bidirectional, named):
+    """One single-layer torch nn.LSTM per layer of the nn.LSTM stored under ``prefix`` in a reference state_dict (see
+    ``lstm_stack``); their parameters are recorded in ``named`` under the stack's names, in its parameters() order."""
+    layers = []
+    for k in range(num_layers):
+        n_in = np.asarray(sd["%s.weight_ih_l%d" % (prefix, k)]).shape[1]
+        lstm = torch.nn.LSTM(n_in, hidden, 1, batch_first=True, bidirectional=bidirectional)
+        with torch.no_grad():
+            for s in ("", "_reverse")[:2 if bidirectional else 1]:
+                for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"):
+                    p = getattr(lstm, "%s_l0%s" % (n, s))
+                    p.copy_(torch.as_tensor(np.asarray(sd["%s.%s_l%d%s" % (prefix, n, k, s)])))
+                    named["%s.%s_l%d%s" % (prefix, n, k, s)] = p
+        layers.append(lstm)
+    return layers
+
+
 class GeneratorOracle(object):
     """CPU generator + Adagrad state for ``gan_step`` built from a reference ``state_dict`` (same key
-    names as the reference classes, models.py:40-48,84-86,128-131,198-200).  ``kind``:
+    names as the reference classes, models.py:40-48,84-86,128-131,153-158,198-200).  ``kind``:
     "mlp" (MLP), "highway" (In2OutHighwayNet), "rnn_highway" (In2OutRNNHighwayNet), "lstm" (LSTMRNN;
-    GRURNN with ``rnn_attr="gru"``).  Recurrent kinds run torch's own CPU ``nn.LSTM`` on packed
-    sequences exactly like the reference."""
+    GRURNN with ``rnn_attr="gru"``), "sru" (SRURNN, with ``bidirectional`` and the cells' ``activation_type``;
+    parity unpinned, see ``sru_layer_forward``).  Recurrent LSTM kinds run torch's own CPU ``nn.LSTM`` on
+    packed sequences like the reference (``lstm_stack``).  ``named`` / ``params()`` / ``sums`` follow the
+    model's parameters() order.
+
+    ``forward``'s ``masks`` injects the product's dropout decisions: the hidden-layer multipliers of "mlp" /
+    "highway" (see ``mlp_forward``), the inter-layer multipliers of "rnn_highway" / "lstm" (see ``lstm_stack``)
+    and [(mask_x, mask_h or None)] per layer of "sru" (see ``sru_layer_forward``).  ``dropout_p`` / ``training``
+    apply to "mlp" / "highway" without masks; the recurrent kinds drop out nothing of their own."""
 
     def __init__(self, kind, sd, static_dim=None, num_hidden=None, hidden_dim=None, bidirectional=False,
-                 rnn_attr="lstm"):
+                 rnn_attr="lstm", activation_type=2):
         self.kind, self.static_dim = kind, static_dim
-        t = lambda k: torch.as_tensor(np.asarray(sd[k])).clone().float().requires_grad_(True)
+        self.bidirectional, self.activation_type = bidirectional, activation_type
         self.named = {}
-        if kind in ("mlp", "highway"):
-            pre = "layers" if kind == "mlp" else "H"
-            n = len([k for k in sd if k.startswith(pre + ".") and k.endswith(".weight")])
-            self.layers = [(t("%s.%d.weight" % (pre, i)), t("%s.%d.bias" % (pre, i))) for i in range(n)]
-            self.layers.append((t("last_linear.weight"), t("last_linear.bias")))
-            for i in range(n):
-                self.named["%s.%d.weight" % (pre, i)], self.named["%s.%d.bias" % (pre, i)] = self.layers[i]
-            self.named["last_linear.weight"], self.named["last_linear.bias"] = self.layers[-1]
-        else:
-            in_dim = np.asarray(sd[rnn_attr + ".weight_ih_l0"]).shape[1]
-            self.lstm = torch.nn.LSTM(in_dim, hidden_dim, num_hidden, batch_first=True, bidirectional=bidirectional)
-            self.lstm.load_state_dict({k[len(rnn_attr) + 1:]: torch.as_tensor(np.asarray(v)).float()
-                                       for k, v in sd.items() if k.startswith(rnn_attr + ".")})
-            self.lstm.train()
-            for k, p in self.lstm.named_parameters():
-                self.named[rnn_attr + "." + k] = p
-            self.h2o = (t("hidden2out.weight"), t("hidden2out.bias"))
-            self.named["hidden2out.weight"], self.named["hidden2out.bias"] = self.h2o
         if kind in ("highway", "rnn_highway"):
-            self.gate = (t("T.weight"), t("T.bias"))
-            self.named["T.weight"], self.named["T.bias"] = self.gate
+            self.gate = _pair(sd, "T", self.named)
+        if kind in ("mlp", "highway"):
+            self.layers = _linear_layers(sd, "layers" if kind == "mlp" else "H", self.named)
+        else:
+            if kind == "sru":
+                n = _count(sd, "gru.rnn_lst.")
+                self.layers = [_pair(sd, "gru.rnn_lst.%d" % i, self.named) for i in range(n)]
+            else:
+                self.layers = _lstm_layers(sd, rnn_attr, num_hidden, hidden_dim, bidirectional, self.named)
+            self.h2o = _pair(sd, "hidden2out", self.named)
         self.sums = [torch.zeros_like(p) for p in self.params()]
 
     def params(self):
@@ -394,18 +459,68 @@ class GeneratorOracle(object):
         elif self.kind == "highway":
             out = in2out_highway_forward(x, R, self.gate, self.layers, self.static_dim, dropout_p, training, masks)
         elif self.kind == "rnn_highway":
-            out = in2out_rnn_highway_forward(x, R, lengths, self.gate, self.lstm, self.h2o, self.static_dim)
+            out = in2out_rnn_highway_forward(x, R, lengths, self.gate, self.layers, self.h2o, self.static_dim, masks)
+        elif self.kind == "sru":
+            out = sru_forward(x, self.layers, self.h2o, self.bidirectional, self.activation_type, masks)
         else:
-            out = lstm_forward(x, lengths, self.lstm, self.h2o)
+            out = lstm_forward(x, lengths, self.layers, self.h2o, masks=masks)
         return apply_generator(out, x, R, hp, self.include_parameter_generation())
 
 
 def discriminator_layers(sd):
     """[(W, b), ...] (requires_grad) of a reference ``MLP`` state_dict (``layers.i``, ``last_linear``)."""
-    t = lambda k: torch.as_tensor(np.asarray(sd[k])).clone().float().requires_grad_(True)
-    n = len([k for k in sd if k.startswith("layers.") and k.endswith(".weight")])
-    return [(t("layers.%d.weight" % i), t("layers.%d.bias" % i)) for i in range(n)] + \
-           [(t("last_linear.weight"), t("last_linear.bias"))]
+    return _linear_layers(sd, "layers", {})
+
+
+class DiscriminatorOracle(object):
+    """CPU discriminator for ``gan_step`` and the spoofing-rate count, built from a reference ``state_dict`` whose keys
+    give its kind and whose tensors give its shape: ``MLP`` (``layers.i.*``, ``last_linear.*``; models.py:121-141) or
+    ``LSTMRNN`` / ``GRURNN`` (an nn.LSTM under ``lstm.`` or ``gru.``, then ``hidden2out.*``; models.py:170-213), with
+    last_sigmoid=True as train.py:774 builds it.  ``named`` / ``params()`` follow the state_dict.  A recurrent one
+    runs ``lstm_stack`` and drops out nothing but the injected masks."""
+
+    def __init__(self, sd):
+        self.named = {}
+        if "last_linear.weight" in sd:
+            self.mlp = _linear_layers(sd, "layers", self.named)
+            return
+        self.mlp = None
+        pre = "lstm" if "lstm.weight_ih_l0" in sd else "gru"
+        n = len([k for k in sd if k.startswith(pre + ".weight_ih_l") and not k.endswith("_reverse")])
+        hidden = np.asarray(sd[pre + ".weight_hh_l0"]).shape[1]
+        self.layers = _lstm_layers(sd, pre, n, hidden, pre + ".weight_ih_l0_reverse" in sd, self.named)
+        self.h2o = _pair(sd, "hidden2out", self.named)
+
+    @classmethod
+    def of_layers(cls, layers):
+        """The MLP discriminator ``[(W, b), ...]`` itself (stepped in place), as ``discriminator_layers`` gives it."""
+        d = cls.__new__(cls)
+        d.mlp = layers
+        names = ["layers.%d" % i for i in range(len(layers) - 1)] + ["last_linear"]
+        d.named = {k + s: t for k, pair in zip(names, layers) for s, t in zip((".weight", ".bias"), pair)}
+        return d
+
+    def params(self):
+        return list(self.named.values())
+
+    def forward(self, x, lengths, masks=None, dropout_p=0.0, training=False):
+        """D(x) in (0, 1); ``masks`` as ``mlp_forward`` / ``lstm_stack`` take them.  ``dropout_p`` / ``training``
+        apply to an MLP without masks; an MLP ignores ``lengths``."""
+        if self.mlp is not None:
+            return mlp_forward(x, self.mlp, dropout_p, training, last_sigmoid=True, masks=masks)
+        return lstm_forward(x, lengths, self.layers, self.h2o, last_sigmoid=True, masks=masks)
+
+
+def reference_output(ref_d, y_hat_static, lengths, hp):
+    """The reference discriminator's output on the adversarial columns of y_hat_static (train.py:549-558): dropout off
+    (D_ref in eval mode, :445), no linguistic conditioning (:554-555).  ``ref_d`` is a ``DiscriminatorOracle``."""
+    with torch.no_grad():
+        return ref_d.forward(get_selected_static_stream(y_hat_static, hp), lengths)
+
+
+def spoof_count(ref_d, y_hat_static, lengths, mask, hp):
+    """``((D_ref(get_selected_static_stream(y_hat_static), lengths) > 0.5).float() * mask).sum()`` (train.py:549-558)."""
+    return ((reference_output(ref_d, y_hat_static, lengths, hp) > 0.5).float() * mask).sum().item()
 
 
 # ------------------------------------------------------------------------------ SRU (unpinned)

@@ -1,14 +1,17 @@
-"""Helpers shared by the fused-generator test modules (test_gpu_fused_highway.py, test_gpu_fused_sru.py,
-test_gpu_fused_rnn_highway.py): batches, the step's discriminator masks, the oracle's re-sync between steps, the
-comparisons, and host-only gantts_gan_step_t configurations for the configuration-rule tests."""
+"""Helpers shared by the fused-step test modules: the product's models and their oracles, batches, the step's own dropout
+masks regenerated from its seeds, the oracle's re-sync between steps, the comparisons, and host-only gantts_gan_step_t
+configurations for the configuration-rule tests.  The mask helpers call the product's gantts_dropout, so they live here
+and not in the oracle package."""
 import numpy as np
 import pytest
 import torch
 
-from conftest import WINDOWS
+from conftest import TTS_HP, WINDOWS
 from oracle import gantts_port as gp
 
 FAKE = 1 << 20          # placeholder device pointer: the configuration check and the workspace layout never dereference it
+ADAM = dict(lr=1e-3, betas=(0.5, 0.9), weight_decay=0.0, eps=1e-8)
+TTS_STREAMS = [(0, 60, 1, 0), (180, 1, 1, 60), (183, 1, 0, 61), (184, 1, 1, 62)]
 
 
 @pytest.fixture(scope="module")
@@ -51,8 +54,126 @@ def sd_numpy(m):
     return {k: v.detach().cpu().numpy() for k, v in m.state_dict().items()}
 
 
+def snapshot(*tensors):
+    return [t.detach().clone() for t in tensors]
+
+
+def assert_equal_lists(a, b, what):
+    assert len(a) == len(b)
+    for i, (u, v) in enumerate(zip(a, b)):
+        assert torch.equal(u, v), (what, i)
+
+
+# ---- the product's models and their oracles
+def vc_ohp(width, cond=False):
+    return dict(stream_sizes=[width], has_dynamic_features=[True], adversarial_streams=[True],
+                mask_nth_mgc_for_adv_loss=0, num_windows=3, discriminator_linguistic_condition=cond)
+
+
+def tts_ohp(cond=False):
+    return dict(TTS_HP, discriminator_linguistic_condition=cond)
+
+
+def sru_models(seed, in_dim, out_dim, layers, hidden, bidir, relu, p, rnn_p, d_hidden, d_layers, d_p, n_adv):
+    import gantts_b200
+    torch.manual_seed(seed)
+    mg = gantts_b200.models.SRURNN(in_dim=in_dim, out_dim=out_dim, num_hidden=layers, hidden_dim=hidden,
+                                   bidirectional=bidir, dropout=p, use_relu=int(relu), rnn_dropout=rnn_p)
+    for cell in mg.gru.rnn_lst:                        # non-zero forget / reset biases
+        cell.bias.data.uniform_(-0.5, 0.5)
+    md = gantts_b200.models.MLP(in_dim + n_adv, 1, d_layers, d_hidden, dropout=d_p, last_sigmoid=True)
+    return mg, md
+
+
+def rhw_models(seed, S, layers, hidden, bidir, p, d_hidden, d_layers, p_d, cond=False):
+    import gantts_b200
+    torch.manual_seed(seed)
+    mg = gantts_b200.models.In2OutRNNHighwayNet(in_dim=3 * S, out_dim=3 * S, static_dim=S, num_hidden=layers,
+                                                hidden_dim=hidden, bidirectional=bidir, dropout=p)
+    md = gantts_b200.models.MLP(S + (3 * S if cond else 0), 1, d_layers, d_hidden, dropout=p_d, last_sigmoid=True)
+    return mg, md
+
+
+def build(kind, seed):
+    """(model_g, model_d, oracle hparams, d_in, d_out, G hidden widths (MLP / highway), D hidden width, D dropout) with
+    an MLP discriminator."""
+    import gantts_b200
+    M = gantts_b200.models
+    torch.manual_seed(seed)
+    if kind == "mlp":
+        mg = M.MLP(20, 187, 2, 32, dropout=0.5, last_sigmoid=False)
+        md = M.MLP(58, 1, 2, 16, dropout=0.5, last_sigmoid=True)
+        return mg, md, TTS_HP, 20, 187, [32, 32], 16, 0.5
+    if kind == "highway":
+        mg = M.In2OutHighwayNet(in_dim=27, out_dim=27, static_dim=9, num_hidden=2, hidden_dim=24, dropout=0.5)
+        md = M.MLP(9, 1, 2, 16, dropout=0.5, last_sigmoid=True)
+        return mg, md, vc_ohp(27), 27, 27, [24, 24], 16, 0.5
+    if kind == "vc_full":
+        mg = M.In2OutHighwayNet(in_dim=177, out_dim=177, static_dim=59, num_hidden=3, hidden_dim=512, dropout=0.5)
+        md = M.MLP(59, 1, 2, 256, dropout=0.5, last_sigmoid=True)
+        return mg, md, vc_ohp(177), 177, 177, [512] * 3, 256, 0.5
+    if kind == "sru":
+        mg, md = sru_models(seed, 20, 187, 2, 16, True, True, 0.2, 0.2, 32, 2, 0.5, 58)
+        return mg, md, tts_ohp(True), 20, 187, None, 32, 0.5
+    mg, md = rhw_models(seed, 8, 2, 12, True, 0.3, 32, 2, 0.5)
+    return mg, md, vc_ohp(24), 24, 24, None, 32, 0.5
+
+
+def make_models(kind, seed, cond, d_layers=2, d_hidden=12, bidir=True, p_d=0.5, gru=False, full=False):
+    """(generator, recurrent discriminator, ohp, generator input width) with every generator dropout 0; the
+    discriminator is an LSTMRNN (GRURNN with gru=True) with LSTM dropout p_d."""
+    import gantts_b200
+    M = gantts_b200.models
+    torch.manual_seed(seed)
+    if kind == "mlp":
+        ohp, d_in = tts_ohp(cond), 20
+        mg = M.MLP(d_in, 187, 2, 24, dropout=0.0, last_sigmoid=False)
+    elif kind == "highway":
+        S = 59 if full else 8
+        ohp, d_in = vc_ohp(3 * S, cond), 3 * S
+        mg = M.In2OutHighwayNet(in_dim=d_in, out_dim=d_in, static_dim=S, num_hidden=3 if full else 2,
+                                hidden_dim=512 if full else 24, dropout=0.0)
+    elif kind == "rnn_highway":
+        ohp, d_in = vc_ohp(24, cond), 24
+        mg = M.In2OutRNNHighwayNet(in_dim=24, out_dim=24, static_dim=8, num_hidden=2, hidden_dim=12, bidirectional=True,
+                                   dropout=0.0)
+    else:
+        ohp, d_in = tts_ohp(cond), 425 if full else 20
+        mg = M.SRURNN(in_dim=d_in, out_dim=187, num_hidden=6 if full else 2, hidden_dim=512 if full else 16,
+                      bidirectional=True, dropout=0.0, use_relu=1, rnn_dropout=0.0)
+        for cell in mg.gru.rnn_lst:
+            cell.bias.data.uniform_(-0.5, 0.5)
+    n_adv = 58 if ohp["stream_sizes"] == TTS_HP["stream_sizes"] else d_in // 3
+    cls = M.GRURNN if gru else M.LSTMRNN
+    md = cls(in_dim=n_adv + (d_in if cond else 0), out_dim=1, num_hidden=d_layers, hidden_dim=d_hidden,
+             bidirectional=bidir, dropout=p_d, last_sigmoid=True)
+    return mg, md, ohp, d_in
+
+
+def generator_oracle(mg):
+    """gp.GeneratorOracle of the product's generator mg (MLP, In2OutHighwayNet, In2OutRNNHighwayNet or SRURNN)."""
+    sd, name = sd_numpy(mg), type(mg).__name__
+    if name == "MLP":
+        return gp.GeneratorOracle("mlp", sd)
+    if name == "In2OutHighwayNet":
+        return gp.GeneratorOracle("highway", sd, static_dim=mg.static_dim)
+    if name == "SRURNN":
+        cell = mg.gru.rnn_lst[0]
+        return gp.GeneratorOracle("sru", sd, bidirectional=cell.bidirectional, activation_type=cell.activation_type)
+    lm = mg.lstm
+    return gp.GeneratorOracle("rnn_highway", sd, static_dim=mg.static_dim, num_hidden=lm.num_layers,
+                              hidden_dim=lm.hidden_size, bidirectional=lm.bidirectional)
+
+
+def fused(mg, md, hp, B, T, optimizer="Adagrad", **kw):
+    from gantts_b200 import fused as F
+    return F.FusedGanStep(mg, md, step_hp(hp), B, T, weight_decay=0.0, optimizer=optimizer,
+                          optimizer_params=ADAM if optimizer == "Adam" else None, **kw)
+
+
+# ---- the dropout masks of the product's last training step, regenerated from its seeds
 def d_masks(fs, M, d_hidden, p, dev):
-    """The discriminator's keep masks of the last training step (gantts_gan_step_seed: 1 = stacked real|fake, 2 = adv)."""
+    """The MLP discriminator's keep masks (gantts_gan_step_seed: 1 = stacked real|fake, 2 = adv)."""
     from gantts_b200 import ops, _lib
     lib = _lib.load()
     s = fs.last_seed
@@ -61,20 +182,66 @@ def d_masks(fs, M, d_hidden, p, dev):
             "adv": [m.cpu() for m in ops.mlp_dropout_masks(M, d_hidden, p, lib.gantts_gan_step_seed(s, 2), dev)]}
 
 
-def adv_loss_with(md, x, ys_ref, lens, ohp, adv_masks):
-    """loss_adv of the oracle's y_hat_static through the PRODUCT's updated discriminator.  The adversarial forward runs
-    after the discriminator's first Adagrad / Adam step, which moves every weight by about lr * sign(g): a weight whose
-    gradient is within rounding of zero lands 2 lr apart in the two implementations, and at the conditioned D's 483
-    inputs those few weights move loss_adv by a few 1e-4.  With the product's D on both sides the comparison isolates
-    the generator's output and the loss arithmetic."""
-    ps = list(md.parameters())
-    layers = [(w.detach().cpu(), b.detach().cpu()) for w, b in zip(ps[0::2], ps[1::2])]
+def d_lstm_masks(fs, md, M, dev):
+    """The recurrent discriminator's inter-layer masks (gantts_d_lstm_mask_seed: 1 = stacked real|fake, 2 = adv)."""
+    from gantts_b200 import ops, _lib
+    lib = _lib.load()
+    lstm = getattr(md, md._rnn_attr)
+    nh = lstm.hidden_size * (2 if lstm.bidirectional else 1)
+    mk = lambda rows, which: [ops.dropout_mask(rows, nh, lstm.dropout, lib.gantts_d_lstm_mask_seed(fs.last_seed, which, k),
+                                               dev).cpu() for k in range(lstm.num_layers - 1)]
+    stacked = mk(2 * M, 1)
+    return {"real": [m[:M] for m in stacked], "fake": [m[M:] for m in stacked], "adv": mk(M, 2)}
+
+
+def sru_masks(fs, mg, B, dev):
+    """The SRURNN generator's masks: [(mask_x, mask_h or None)] per layer (gantts_sru_mask_seed)."""
+    from gantts_b200 import ops, _lib
+    lib = _lib.load()
+    cells = list(mg.gru.rnn_lst)
+    out = []
+    for i, cell in enumerate(cells):
+        nc = cell.n_out * (2 if cell.bidirectional else 1)
+        mx = ops.dropout_mask(B, cell.n_in, cell.rnn_dropout, lib.gantts_sru_mask_seed(fs.last_seed, i, 0), dev).cpu()
+        mh = ops.dropout_mask(B, nc, cell.dropout, lib.gantts_sru_mask_seed(fs.last_seed, i, 1), dev).cpu() \
+            if i + 1 < len(cells) else None
+        out.append((mx, mh))
+    return out
+
+
+def lstm_masks(fs, mg, B, T, dev):
+    """The In2OutRNNHighwayNet generator's inter-layer masks (gantts_lstm_mask_seed)."""
+    from gantts_b200 import ops, _lib
+    lib = _lib.load()
+    lm = mg.lstm
+    nh = lm.hidden_size * (2 if lm.bidirectional else 1)
+    return [ops.dropout_mask(B * T, nh, lm.dropout, lib.gantts_lstm_mask_seed(fs.last_seed, k), dev).cpu()
+            for k in range(lm.num_layers - 1)]
+
+
+def g_masks(kind, fs, mg, B, T, g_hidden, dev):
+    """The generator's keep masks of a `build(kind, ...)` generator."""
+    from gantts_b200 import ops, _lib
+    if kind == "sru":
+        return sru_masks(fs, mg, B, dev)
+    if kind == "rnn_highway":
+        return lstm_masks(fs, mg, B, T, dev)
+    seed = _lib.load().gantts_gan_step_seed(fs.last_seed, 0)
+    return [m.cpu() for m in ops.mlp_dropout_masks(B * T, g_hidden, mg.dropout_p, seed, dev)]
+
+
+def adv_loss_with(d, x, ys_ref, lens, ohp, adv_masks):
+    """loss_adv of the oracle's y_hat_static through `d`, the gp.DiscriminatorOracle of the PRODUCT's updated
+    discriminator.  The adversarial forward runs after the discriminator's first Adagrad / Adam step, which moves every
+    weight by about lr * sign(g): a weight whose gradient is within rounding of zero lands 2 lr apart in the two
+    implementations, and at the conditioned D's 483 inputs those few weights move loss_adv by a few 1e-4.  With the
+    product's D on both sides the comparison isolates the generator's output and the loss arithmetic."""
     fake_in = gp.get_selected_static_stream(ys_ref, ohp)
     if ohp["discriminator_linguistic_condition"]:
         fake_in = torch.cat((x, fake_in), -1)
     mask = gp.sequence_mask(lens, x.size(1)).unsqueeze(-1)
-    D = gp.mlp_forward(fake_in, layers, last_sigmoid=True, masks=adv_masks)
-    return float(gp.bce_real(D, mask, mask.sum().item()))
+    with torch.no_grad():
+        return float(gp.bce_real(d.forward(fake_in, lens, adv_masks), mask, mask.sum().item()))
 
 
 def loss_errors(got, ref, keys):
@@ -155,6 +322,56 @@ def use_adam(c, missing=()):
             tab.state2[i] = FAKE
     for i in missing:
         c.g_tensors.state2[i] = None
+
+
+def _vc_step_config():
+    """A valid In2OutHighwayNet configuration of gantts_gan_step_t: G 177 -> 64 -> 3 S with the gate (S = 59), D S -> 32
+    -> 1 (host pointers are placeholders: only the configuration check and the workspace layout run)."""
+    S = 59
+    c = step_config((177, 64, 3 * S), (S, 32, 1), [(0, S, True, 0)], range(S), range(S))
+    c.highway.static_dim = S
+    return fill_tables(c, 2 + 2 * 2)
+
+
+def _sru_step_config():
+    """A valid SRURNN configuration of gantts_gan_step_t on the tts_acoustic layout with a conditioned D: 3 bidirectional
+    layers of 16 over in_dim 40, hidden2out 32 -> 187, D 40 + 58 -> 32 -> 1 (host pointers are placeholders: only the
+    configuration check and the workspace layout run)."""
+    from gantts_b200 import multistream, step as gstep
+    in_dim, hidden, nl = 40, 16, 3
+    hp = gstep.TTS_ACOUSTIC
+    entries, n_static = multistream.mlpg_stream_entries(hp.stream_sizes, hp.has_dynamic_features, [True] * 4, 3)
+    c = step_config((2 * hidden, 187), (in_dim + 58, 32, 1), entries, range(n_static), range(2, 60), conditioned=True)
+    s = c.sru
+    s.num_layers, s.in_dim, s.hidden, s.bidirectional, s.act = nl, in_dim, hidden, 1, 2
+    s.dropout, s.rnn_dropout = 0.2, 0.2
+    return fill_tables(c, 2 * nl + 2)
+
+
+def _rhw_step_config():
+    """A valid In2OutRNNHighwayNet configuration of gantts_gan_step_t on the cfg3 layout: the gate (S = 59), 3
+    bidirectional LSTM layers of 16 over 3 S, hidden2out 32 -> 3 S, D S -> 32 -> 1 (host pointers are placeholders: only
+    the configuration check and the workspace layout run)."""
+    S, H, nl = 59, 16, 3
+    c = step_config((2 * H, 3 * S), (S, 32, 1), [(0, S, True, 0)], range(S), range(S))
+    c.highway.static_dim = S
+    ls = c.lstm
+    ls.num_layers, ls.in_dim, ls.hidden, ls.bidirectional, ls.dropout = nl, 3 * S, H, 1, 0.5
+    return fill_tables(c, 2 + 8 * nl + 2)
+
+
+def _rnn_d_config(bidir=1, layers=2, hidden=16, cond=False):
+    """An MLP generator 20 -> 24 -> 27 on one dynamic stream of 9 static columns, and an LSTMRNN D over those 9 columns
+    (plus the 20 conditioning columns when cond): `layers` LSTM layers of `hidden` units, then hidden2out -> 1."""
+    nh = hidden * (2 if bidir else 1)
+    c = step_config((20, 24, 27), (nh, 1), [(0, 9, True, 0)], range(9), range(9), conditioned=cond)
+    dl = c.d_lstm
+    dl.num_layers, dl.in_dim, dl.hidden, dl.bidirectional, dl.dropout = layers, 9 + (20 if cond else 0), hidden, bidir, 0.5
+    fill_tables(c, 4)
+    c.d_tensors.n = 4 * layers * (2 if bidir else 1) + 2
+    for i in range(c.d_tensors.n):
+        c.d_tensors.param[i] = c.d_tensors.state[i] = c.g_tensors.param[0]
+    return c
 
 
 def config_checker():

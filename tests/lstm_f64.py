@@ -1,10 +1,12 @@
 """Plain float64 restatement of one LSTM layer at the contract of gantts_lstm_layer_fwd / _bwd and gantts_lstm_hprev
-(include/gantts_b200.h), and a mirror of which recurrence kernel csrc/lstm.cu launches for a shape.
+(include/gantts_b200.h), a mirror of which recurrence kernel csrc/lstm.cu launches for a shape, and the case
+matrix tests/test_gpu_lstm_kernels.py runs.
 
 The layer: xproj [B][T][ndir*4H] (x W_ih^T + b_ih + b_hh, direction-major columns), W_hh [ndir][4H][H], lengths [B].
 Sequence b runs for t < lengths[b]; direction 1 starts at t = lengths[b] - 1 (pack_padded_sequence semantics).  There is
 no hand-written backward here: dxproj is torch.autograd through the float64 loop.
 """
+import numpy as np
 import torch
 
 # csrc/lstm.cu
@@ -119,3 +121,38 @@ def first_untrainable(ndir, sms, reg=True):
         H += 4
         assert H <= 4096
     return H
+
+
+H_LIST = (4, 12, 256, 260, 512, 516, 528)
+
+
+def case_lengths(kind, B, T, seed):
+    if kind in ("full", "T=1"):
+        return [T] * B
+    if kind == "desc":
+        return [max(1, T - (b * T) // B) for b in range(B)]
+    # unsorted ragged: the full length, two sequences of length 1, the rest anywhere in [1, T]
+    rng = np.random.RandomState(seed)
+    lens = [T, 1, 1] + [int(v) for v in rng.randint(1, T + 1, max(B - 3, 0))]
+    lens = lens[:B]
+    rng.shuffle(lens)
+    return lens
+
+
+def _cases():
+    """(id, B, T, H, ndir, lengths) of the GPU case matrix (tests/test_gpu_lstm_kernels.py)"""
+    cases = []
+    for H in H_LIST:
+        T = 23 if H < 256 else 7          # the float64 loop runs on the CPU: short where H is large
+        for ndir in (1, 2):
+            shapes = [(1, T, "full"), (17, T, "desc"), (33, T, "unsorted"), (16, 1, "T=1")]
+            if H in (12, 260, 528):
+                shapes.append((128, T, "unsorted"))
+            for B, Tc, kind in shapes:
+                cases.append(("H%d-%s-B%d-T%d-%s" % (H, "bi" if ndir == 2 else "uni", B, Tc, kind), B, Tc, H, ndir, kind))
+    cases.append(("spoof-count-max-B128-T64-H256-bi", 128, 64, 256, 2, "unsorted"))
+    cases.append(("cfg3-width-B16-T200-H512-bi", 16, 200, 512, 2, "desc"))
+    return [(cid, B, T, H, ndir, case_lengths(kind, B, T, i)) for i, (cid, B, T, H, ndir, kind) in enumerate(cases)]
+
+
+CASES = _cases()

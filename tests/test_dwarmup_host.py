@@ -1,6 +1,6 @@
 """CPU-only tests of the discriminator warm-up step (update_g = False) and of the spoofing-rate count:
 
-* the CPU restatement (tests/dwarmup_oracle.py) pinned to tests/golden/dwarmup.npz (written by
+* the oracle's gan_step(update_g=False) and spoof_count pinned to tests/golden/dwarmup.npz (written by
   tests/golden/make_golden_dwarmup.py), the vectors of the UNMODIFIED
   reference's apply_generator + update_discriminator (train.py:336-355, 245-279; update_generator not called, :696) and
   of its spoofing-rate block (train.py:549-558) -- losses, counts, post-step discriminator weights and optimiser state,
@@ -17,7 +17,6 @@ import torch
 
 from conftest import GOLDEN, TTS_HP, WINDOWS, rel_err
 from fused_step_helpers import FAKE, config_checker, fill_tables, step_config
-import dwarmup_oracle as dwo
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
 
@@ -46,15 +45,15 @@ def test_d_only_step_and_spoof_count_match_reference(golden, case, opt):
     d_params = [t for pair in d_layers for t in pair]
     d_sum = [torch.zeros_like(t) for t in d_params]
     d_opt = gp.AdamStepper(d_params, lr=1e-3, betas=(0.5, 0.9), eps=1e-8, weight_decay=0.0) if opt == "adam" else None
-    ref_layers = [(W.detach(), b.detach()) for W, b in gp.discriminator_layers(sub(g, tag + "ref_"))]
+    ref_d = gp.DiscriminatorOracle(sub(g, tag + "ref_"))
     g0 = [p.detach().clone() for p in gen.params()]
     for it in range(2):
         p = "%sit%d_" % (tag, it)
         x, y = torch.from_numpy(g[p + "x"]), torch.from_numpy(g[p + "y"])
         lens = [int(v) for v in g[p + "lengths"]]
         R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, x.size(1)))
-        out, y_hat, y_hat_static = dwo.d_only_step(lambda: gen.forward(x, R, lens, hp, training=True), d_layers, d_sum,
-                                                   x, y, lens, hp, d_opt=d_opt)
+        out, y_hat, y_hat_static = gp.gan_step(lambda: gen.forward(x, R, lens, hp, training=True), gen.params(), None,
+                                               d_layers, d_sum, x, y, lens, R, hp, update_g=False, d_opt=d_opt)
         assert rel_err(y_hat.numpy(), g[p + "y_hat"]) < F32_TOL
         assert rel_err(y_hat_static.numpy(), g[p + "y_hat_static"]) < F32_TOL
         for k, v in zip(LOSS_KEYS, g[p + "losses"]):
@@ -65,7 +64,7 @@ def test_d_only_step_and_spoof_count_match_reference(golden, case, opt):
         assert out["loss_adv"] == 0.0 and out["g_grad_norm"] == 0.0
         assert out["loss_g"] == pytest.approx(out["loss_mge"], rel=1e-7)          # mse_w = 0, mge_w = 1
         mask = gp.sequence_mask(lens, x.size(1)).unsqueeze(-1)
-        assert dwo.spoof_count(ref_layers, y_hat_static, mask, hp) == float(g[p + "spoof"])
+        assert gp.spoof_count(ref_d, y_hat_static, lens, mask, hp) == float(g[p + "spoof"])
         gold_d = sub(g, p + "d_")
         names = ["layers.%d" % i for i in range(len(d_layers) - 1)] + ["last_linear"]
         for n, (W, b) in zip(names, d_layers):

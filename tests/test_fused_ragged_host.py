@@ -6,9 +6,7 @@ import ctypes
 import pytest
 
 from conftest import WINDOWS
-from fused_step_helpers import FAKE, config_checker, fill_tables, step_config
-
-TTS_STREAMS = [(0, 60, 1, 0), (180, 1, 1, 60), (183, 1, 0, 61), (184, 1, 1, 62)]
+from fused_step_helpers import FAKE, TTS_STREAMS, config_checker, fill_tables, step_config
 
 
 @pytest.fixture(scope="module")

@@ -2,106 +2,23 @@
 (train.py:549-558) on the GPU: FusedGanStep(update_g=False) / GANTTS_STEP_D_ONLY, gantts_spoof_count, and the same two
 features of GanTrainer.
 
-Checkers: the full fused step from the same weights and seed (bit for bit), and the CPU restatement tests/dwarmup_oracle.py
-(pinned to the reference by test_dwarmup_host.py) with the step's own dropout masks injected.  Tolerances as in the
-fused-generator modules: losses, gradient norm and y_hat_static 2e-4 relative; post-step weights median |delta| < 5e-6
-and max <= 0.0201 (a first Adagrad / Adam step moves a weight by lr * sign(g)).
+Checkers: the full fused step from the same weights and seed (bit for bit), and the oracle's gan_step(update_g=False)
+and spoof_count (pinned to the reference by test_dwarmup_host.py) with the step's own dropout masks injected.
+Tolerances as in the fused-generator modules: losses, gradient norm and y_hat_static 2e-4 relative; post-step weights
+median |delta| < 5e-6 and max <= 0.0201 (a first Adagrad / Adam step moves a weight by lr * sign(g)).
 """
 import numpy as np
 import pytest
 import torch
 
 from conftest import TTS_HP, WINDOWS, rel_err
-from fused_step_helpers import (check_weights, d_masks, dev, make_batch, npy, ragged_lengths, sd_numpy,  # noqa: F401
-                                step_hp)
-import dwarmup_oracle as dwo
+from fused_step_helpers import (ADAM, assert_equal_lists, build, check_weights, d_masks, dev, fused,  # noqa: F401
+                                g_masks, generator_oracle, make_batch, npy, ragged_lengths, sd_numpy, snapshot, step_hp)
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
 
 TOL = 2e-4
-ADAM = dict(lr=1e-3, betas=(0.5, 0.9), weight_decay=0.0, eps=1e-8)
 D_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mse", "loss_mge", "d_grad_norm")
-
-
-def vc_ohp(width):
-    return dict(stream_sizes=[width], has_dynamic_features=[True], adversarial_streams=[True],
-                mask_nth_mgc_for_adv_loss=0, num_windows=3, discriminator_linguistic_condition=False)
-
-
-ACOUSTIC_COND = dict(TTS_HP, discriminator_linguistic_condition=True)
-
-
-def build(kind, seed):
-    """(model_g, model_d, oracle hparams, d_in, d_out, G hidden widths (MLP / highway), D hidden width, D dropout)."""
-    import gantts_b200
-    M = gantts_b200.models
-    torch.manual_seed(seed)
-    if kind == "mlp":
-        mg = M.MLP(20, 187, 2, 32, dropout=0.5, last_sigmoid=False)
-        md = M.MLP(58, 1, 2, 16, dropout=0.5, last_sigmoid=True)
-        return mg, md, TTS_HP, 20, 187, [32, 32], 16, 0.5
-    if kind == "highway":
-        mg = M.In2OutHighwayNet(in_dim=27, out_dim=27, static_dim=9, num_hidden=2, hidden_dim=24, dropout=0.5)
-        md = M.MLP(9, 1, 2, 16, dropout=0.5, last_sigmoid=True)
-        return mg, md, vc_ohp(27), 27, 27, [24, 24], 16, 0.5
-    if kind == "vc_full":
-        mg = M.In2OutHighwayNet(in_dim=177, out_dim=177, static_dim=59, num_hidden=3, hidden_dim=512, dropout=0.5)
-        md = M.MLP(59, 1, 2, 256, dropout=0.5, last_sigmoid=True)
-        return mg, md, vc_ohp(177), 177, 177, [512] * 3, 256, 0.5
-    if kind == "sru":
-        from test_gpu_fused_sru import sru_models
-        mg, md = sru_models(seed, 20, 187, 2, 16, True, True, 0.2, 0.2, 32, 2, 0.5, 58)
-        return mg, md, ACOUSTIC_COND, 20, 187, None, 32, 0.5
-    from test_gpu_fused_rnn_highway import rhw_models
-    mg, md = rhw_models(seed, 8, 2, 12, True, 0.3, 32, 2, 0.5)
-    return mg, md, vc_ohp(24), 24, 24, None, 32, 0.5
-
-
-def gen_oracle(kind, mg):
-    """(oracle generator, forward(x, R, lens, masks)) of the product's generator."""
-    if kind == "sru":
-        from test_gpu_fused_sru import SruOracle
-        gen = SruOracle(sd_numpy(mg), mg.gru.rnn_lst[0].bidirectional, mg.gru.rnn_lst[0].activation_type)
-        return gen, lambda x, R, lens, hp, m: gen.forward(x, R, hp, m)
-    if kind == "rnn_highway":
-        from test_gpu_fused_rnn_highway import RnnHighwayOracle
-        lm = mg.lstm
-        gen = RnnHighwayOracle(sd_numpy(mg), lm.num_layers, lm.hidden_size, lm.bidirectional, mg.static_dim)
-        return gen, lambda x, R, lens, hp, m: gen.forward(x, R, lens, m)
-    if kind == "mlp":
-        gen = gp.GeneratorOracle("mlp", sd_numpy(mg))
-    else:
-        gen = gp.GeneratorOracle("highway", sd_numpy(mg), static_dim=mg.static_dim)
-    return gen, lambda x, R, lens, hp, m: gen.forward(x, R, lens, hp, mg.dropout_p, True, m)
-
-
-def g_masks(kind, fs, mg, B, T, g_hidden, dev):
-    """The generator's keep masks of the last training step."""
-    from gantts_b200 import ops, _lib
-    if kind == "sru":
-        from test_gpu_fused_sru import sru_masks
-        return sru_masks(fs, mg, B, dev)
-    if kind == "rnn_highway":
-        from test_gpu_fused_rnn_highway import lstm_masks
-        return lstm_masks(fs, mg, B, T, dev)
-    seed = _lib.load().gantts_gan_step_seed(fs.last_seed, 0)
-    return [m.cpu() for m in ops.mlp_dropout_masks(B * T, g_hidden, mg.dropout_p, seed, dev)]
-
-
-def snapshot(*tensors):
-    return [t.detach().clone() for t in tensors]
-
-
-def assert_equal_lists(a, b, what):
-    assert len(a) == len(b)
-    for i, (u, v) in enumerate(zip(a, b)):
-        assert torch.equal(u, v), (what, i)
-
-
-def fused(mg, md, hp, B, T, optimizer="Adagrad", **kw):
-    from gantts_b200 import fused as F
-    return F.FusedGanStep(mg, md, step_hp(hp), B, T, weight_decay=0.0, optimizer=optimizer,
-                          optimizer_params=ADAM if optimizer == "Adam" else None, **kw)
 
 
 @pytest.mark.gpu
@@ -148,7 +65,7 @@ def test_d_only_step_vs_oracle(dev, kind, optimizer):
     D's post-step weights; G bit-unchanged.  The oracle's next step starts from the product's D and optimiser state."""
     B, T = (4, 100) if kind == "vc_full" else (3, 40)
     mg, md, hp, d_in, d_out, g_hidden, d_hidden, p_d = build(kind, 20)
-    gen, g_fwd = gen_oracle(kind, mg)
+    gen = generator_oracle(mg)
     d_layers = gp.discriminator_layers(sd_numpy(md))
     d_params = [t for pair in d_layers for t in pair]
     d_sum = [torch.zeros_like(t) for t in d_params]
@@ -164,8 +81,9 @@ def test_d_only_step_vs_oracle(dev, kind, optimizer):
         got = fs.loss_dict()
         gm = g_masks(kind, fs, mg, B, T, g_hidden, dev)
         dm = d_masks(fs, B * T, [d_hidden] * (len(d_layers) - 1), p_d, dev)
-        ref, _, ys_ref = dwo.d_only_step(lambda: g_fwd(x, R, lens, hp, gm), d_layers, d_sum, x, y, lens, hp, mse_w=0.5,
-                                         dropout_d=p_d, weight_decay=0.0, d_masks=dm, d_opt=d_opt)
+        ref, _, ys_ref = gp.gan_step(lambda: gen.forward(x, R, lens, hp, masks=gm), gen.params(), None, d_layers,
+                                     d_sum, x, y, lens, R, hp, mse_w=0.5, dropout_d=p_d, weight_decay=0.0,
+                                     update_g=False, d_masks=dm, d_opt=d_opt)
         errs = {k: abs(got[k] - ref[k]) / max(abs(ref[k]), 1e-12) for k in D_KEYS + ("loss_g",)}
         errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), ys_ref.numpy())
         assert max(errs.values()) < TOL, (kind, it, errs)
@@ -215,7 +133,7 @@ def test_adam_step_counts_per_model_and_resume(dev):
     FusedGanStep resumed from it takes the next step bit-identically."""
     B, T = 3, 40
     mg, md, hp, d_in, d_out, g_hidden, d_hidden, p_d = build("mlp", 40)
-    gen, g_fwd = gen_oracle("mlp", mg)
+    gen = generator_oracle(mg)
     d_layers = gp.discriminator_layers(sd_numpy(md))
     d_params = [t for pair in d_layers for t in pair]
     g_opt, d_opt = gp.AdamStepper(gen.params(), **ADAM), gp.AdamStepper(d_params, **ADAM)
@@ -231,13 +149,9 @@ def test_adam_step_counts_per_model_and_resume(dev):
         fs.step(x.to(dev), y.to(dev), torch.LongTensor(lens).to(dev), update_g=update_g)
         gm = g_masks("mlp", fs, mg, B, T, g_hidden, dev)
         dm = d_masks(fs, B * T, [d_hidden] * (len(d_layers) - 1), p_d, dev)
-        if update_g:
-            gp.gan_step(lambda: g_fwd(x, R, lens, hp, gm), gen.params(), None, d_layers, None, x, y, lens, R, hp,
-                        w_d=1.0, mse_w=0.0, mge_w=1.0, adv_w=1.0, dropout_d=p_d, training=True, weight_decay=0.0,
-                        d_masks=dm, d_opt=d_opt, g_opt=g_opt)
-        else:
-            dwo.d_only_step(lambda: g_fwd(x, R, lens, hp, gm), d_layers, None, x, y, lens, hp, dropout_d=p_d,
-                            weight_decay=0.0, d_masks=dm, d_opt=d_opt)
+        gp.gan_step(lambda: gen.forward(x, R, lens, hp, masks=gm), gen.params(), None, d_layers, None,
+                    x, y, lens, R, hp, w_d=1.0, mse_w=0.0, mge_w=1.0, adv_w=1.0, dropout_d=p_d, training=True,
+                    weight_decay=0.0, update_g=update_g, d_masks=dm, d_opt=d_opt, g_opt=g_opt)
         for q, r in zip(md.parameters(), d_params):
             dd = np.abs(npy(q) - r.detach().numpy())
             assert np.median(dd) < 5e-6 and dd.max() <= 0.0201, (it, np.median(dd), dd.max())
@@ -287,11 +201,11 @@ def test_gan_trainer_d_only_matches_oracle_and_fused_step(dev):
         return (gantts_b200.models.MLP(20, 187, 2, 32, dropout=0.0, last_sigmoid=False).to(dev).train(),
                 gantts_b200.models.MLP(58, 1, 2, 16, dropout=0.0, last_sigmoid=True).to(dev).train())
     mg, md = models()
-    gen, g_fwd = gen_oracle("mlp", mg)
+    gen = generator_oracle(mg)
     d_layers = gp.discriminator_layers(sd_numpy(md))
     d_sum = [torch.zeros_like(t) for pair in d_layers for t in pair]
-    ref, _, ys_ref = dwo.d_only_step(lambda: g_fwd(x, R, lens, TTS_HP, None), d_layers, d_sum, x, y, lens, TTS_HP,
-                                     mse_w=0.5, weight_decay=0.0)
+    ref, _, ys_ref = gp.gan_step(lambda: gen.forward(x, R, lens, TTS_HP, mg.dropout_p, True), gen.params(), None,
+                                 d_layers, d_sum, x, y, lens, R, TTS_HP, mse_w=0.5, weight_decay=0.0, update_g=False)
     g0 = snapshot(*mg.parameters())
     tr = gstep.GanTrainer(mg, md, gstep.TTS_ACOUSTIC, w_d=1.0, mse_w=0.5, weight_decay=0.0)
     out, _, ys = tr.step(xd, yd, lens, R.to(dev), update_g=False)
@@ -326,17 +240,16 @@ def centre(ref_d, ys, hp):
     with torch.no_grad():
         ref_d.last_linear.weight.mul_(10.0)
         ref_d.last_linear.bias.zero_()
-        layers = gp.discriminator_layers(sd_numpy(ref_d))
-        z = torch.logit(dwo.reference_output([(W.detach(), b.detach()) for W, b in layers], ys, hp))
+        z = torch.logit(gp.reference_output(gp.DiscriminatorOracle(sd_numpy(ref_d)), ys, None, hp))
         ref_d.last_linear.bias.fill_(-float(z.median()))
 
 
 def check_count(got, ref_d, ys, lens, hp):
     """got == the oracle's count on ys, up to the frames where the CPU's |D_ref - 0.5| < 1e-5."""
-    layers = [(W.detach(), b.detach()) for W, b in gp.discriminator_layers(sd_numpy(ref_d))]
+    d = gp.DiscriminatorOracle(sd_numpy(ref_d))
     mask = gp.sequence_mask(lens, ys.size(1)).unsqueeze(-1)
-    want = dwo.spoof_count(layers, ys, mask, hp)
-    close = float(((dwo.reference_output(layers, ys, hp) - 0.5).abs() < 1e-5).float().mul(mask).sum())
+    want = gp.spoof_count(d, ys, lens, mask, hp)
+    close = float(((gp.reference_output(d, ys, lens, hp) - 0.5).abs() < 1e-5).float().mul(mask).sum())
     assert abs(float(got) - want) <= close, (float(got), want, close)
     return want
 

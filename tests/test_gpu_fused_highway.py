@@ -11,8 +11,8 @@ import pytest
 import torch
 
 from conftest import WINDOWS, rel_err
-from fused_step_helpers import (FAKE, check_weights, config_checker, dev, fill_tables, loss_errors, make_batch, npy,  # noqa: F401
-                                ragged_lengths, resync_oracle, sd_numpy, step_config)
+from fused_step_helpers import (FAKE, _vc_step_config, check_weights, config_checker, dev, loss_errors,  # noqa: F401
+                                make_batch, npy, ragged_lengths, resync_oracle, sd_numpy)
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
 
@@ -269,15 +269,6 @@ def test_fused_highway_phase_split_is_bitwise_equal(dev):
                     + [s.clone() for s in fs._sums])
     for a, b in zip(*runs):
         assert torch.equal(a, b)
-
-
-def _vc_step_config():
-    """A valid In2OutHighwayNet configuration of gantts_gan_step_t: G 177 -> 64 -> 3 S with the gate (S = 59), D S -> 32
-    -> 1 (host pointers are placeholders: only the configuration check and the workspace layout run)."""
-    S = 59
-    c = step_config((177, 64, 3 * S), (S, 32, 1), [(0, S, True, 0)], range(S), range(S))
-    c.highway.static_dim = S
-    return fill_tables(c, 2 + 2 * 2)
 
 
 def test_highway_step_config_rules_on_tensor_tables():

@@ -10,10 +10,9 @@ import pytest
 import torch
 
 from conftest import TTS_HP, WINDOWS, rel_err
-from fused_step_helpers import dev, make_batch, npy, ragged_lengths, step_hp  # noqa: F401
+from fused_step_helpers import build, dev, fused, make_batch, npy, ragged_lengths, step_hp  # noqa: F401
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
-from test_gpu_dwarmup_spoof import build, fused
 
 TOL = 2e-4
 B, T = 3, 40

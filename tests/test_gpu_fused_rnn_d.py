@@ -1,113 +1,31 @@
 """The fused GAN step (gantts_gan_step / FusedGanStep) with a recurrent discriminator: LSTMRNN, or GRURNN (also an
 nn.LSTM), with last_sigmoid=True, as train.py:774 builds it from hp.discriminator.  Every generator the fused step runs,
-conditioned and unconditioned, Adagrad and Adam, against the CPU restatement tests/rnn_d_oracle.py with the step's own
-inter-layer masks injected (each is gantts_dropout(ones[rows][ndir H], p, gantts_d_lstm_mask_seed(seed, which, layer)),
-rows = 2 B T on the stacked forward, B T on the adversarial one).  Tolerances are those of test_gpu_fused_rnn_highway.py:
-losses, gradient norms and y_hat_static 2e-4 relative, post-step weights median |delta| < 5e-6 and max <= 0.0201.  The
-phase split, D-only and eval steps, shaped calls, GRURNN vs LSTMRNN and resume are compared bit for bit.
+conditioned and unconditioned, Adagrad and Adam, against the oracle's gan_step with a DiscriminatorOracle and the step's
+own inter-layer masks injected (each is gantts_dropout(ones[rows][ndir H], p, gantts_d_lstm_mask_seed(seed, which,
+layer)), rows = 2 B T on the stacked forward, B T on the adversarial one).  Tolerances are those of
+test_gpu_fused_rnn_highway.py: losses, gradient norms and y_hat_static 2e-4 relative, post-step weights median |delta| <
+5e-6 and max <= 0.0201.  The phase split, D-only and eval steps, shaped calls, GRURNN vs LSTMRNN and resume are compared
+bit for bit.
 """
 import numpy as np
 import pytest
 import torch
 
-from conftest import TTS_HP, WINDOWS, rel_err
-from fused_step_helpers import (check_weights, dev, loss_errors, make_batch, npy, ragged_lengths,  # noqa: F401
-                                resync_oracle, sd_numpy, step_hp)
+from conftest import WINDOWS, rel_err
+from fused_step_helpers import (ADAM, adv_loss_with, check_weights, d_lstm_masks, dev, generator_oracle,  # noqa: F401
+                                loss_errors, make_batch, make_models, npy, ragged_lengths, resync_oracle, sd_numpy,
+                                step_hp)
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
-from rnn_d_oracle import RnnDiscriminator, gan_step
-from test_gpu_fused_sru import SruOracle
 
 LOSS_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mge", "loss_mse", "loss_adv", "loss_g")
 TOL = 2e-4
-ADAM = dict(lr=1e-3, betas=(0.5, 0.9), weight_decay=0.0, eps=1e-8)
-
-
-def vc_ohp(width, cond=False):
-    return dict(stream_sizes=[width], has_dynamic_features=[True], adversarial_streams=[True],
-                mask_nth_mgc_for_adv_loss=0, num_windows=3, discriminator_linguistic_condition=cond)
-
-
-def tts_ohp(cond=False):
-    return dict(TTS_HP, discriminator_linguistic_condition=cond)
-
-
-def make_models(kind, seed, cond, d_layers=2, d_hidden=12, bidir=True, p_d=0.5, gru=False, full=False):
-    """(generator, discriminator, ohp, generator input width) with every generator dropout 0 (the restatement runs the
-    generator without masks); the discriminator's LSTM dropout p_d."""
-    import gantts_b200
-    M = gantts_b200.models
-    torch.manual_seed(seed)
-    if kind == "mlp":
-        ohp, d_in = tts_ohp(cond), 20
-        mg = M.MLP(d_in, 187, 2, 24, dropout=0.0, last_sigmoid=False)
-    elif kind == "highway":
-        S = 59 if full else 8
-        ohp, d_in = vc_ohp(3 * S, cond), 3 * S
-        mg = M.In2OutHighwayNet(in_dim=d_in, out_dim=d_in, static_dim=S, num_hidden=3 if full else 2,
-                                hidden_dim=512 if full else 24, dropout=0.0)
-    elif kind == "rnn_highway":
-        ohp, d_in = vc_ohp(24, cond), 24
-        mg = M.In2OutRNNHighwayNet(in_dim=24, out_dim=24, static_dim=8, num_hidden=2, hidden_dim=12, bidirectional=True,
-                                   dropout=0.0)
-    else:
-        ohp, d_in = tts_ohp(cond), 425 if full else 20
-        mg = M.SRURNN(in_dim=d_in, out_dim=187, num_hidden=6 if full else 2, hidden_dim=512 if full else 16,
-                      bidirectional=True, dropout=0.0, use_relu=1, rnn_dropout=0.0)
-        for cell in mg.gru.rnn_lst:
-            cell.bias.data.uniform_(-0.5, 0.5)
-    n_adv = 58 if ohp is not None and ohp["stream_sizes"] == TTS_HP["stream_sizes"] else d_in // 3
-    cls = M.GRURNN if gru else M.LSTMRNN
-    md = cls(in_dim=n_adv + (d_in if cond else 0), out_dim=1, num_hidden=d_layers, hidden_dim=d_hidden,
-             bidirectional=bidir, dropout=p_d, last_sigmoid=True)
-    return mg, md, ohp, d_in
-
-
-def gen_oracle(kind, mg):
-    """(oracle generator with .named / .sums / .params(), forward(x, R, lengths, ohp))."""
-    sd = sd_numpy(mg)
-    if kind == "sru":
-        gen = SruOracle(sd, True, 2)
-        return gen, lambda x, R, lens, ohp: gen.forward(x, R, ohp)
-    if kind == "rnn_highway":
-        gen = gp.GeneratorOracle(kind, sd, static_dim=8, num_hidden=2, hidden_dim=12, bidirectional=True)
-    else:
-        gen = gp.GeneratorOracle(kind, sd, static_dim=getattr(mg, "static_dim", None))
-    return gen, lambda x, R, lens, ohp: gen.forward(x, R, lens, ohp)
-
-
-def d_oracle(md):
-    lstm = getattr(md, md._rnn_attr)
-    return RnnDiscriminator(sd_numpy(md), md._rnn_attr, lstm.num_layers, lstm.hidden_size, lstm.bidirectional)
-
-
-def d_lstm_masks(fs, md, M, dev):
-    """The discriminator's inter-layer masks of the last training step of `fs`."""
-    from gantts_b200 import ops, _lib
-    lib = _lib.load()
-    lstm = getattr(md, md._rnn_attr)
-    nh = lstm.hidden_size * (2 if lstm.bidirectional else 1)
-    mk = lambda rows, which: [ops.dropout_mask(rows, nh, lstm.dropout, lib.gantts_d_lstm_mask_seed(fs.last_seed, which, k),
-                                               dev).cpu() for k in range(lstm.num_layers - 1)]
-    stacked = mk(2 * M, 1)
-    return {"real": [m[:M] for m in stacked], "fake": [m[M:] for m in stacked], "adv": mk(M, 2)}
-
-
-def adv_loss_with(md, x, ys_ref, lens, ohp, adv_masks):
-    """loss_adv of the restatement's y_hat_static through the PRODUCT's updated discriminator (see
-    fused_step_helpers.adv_loss_with: a first optimiser step lands weights with near-zero gradients 2 lr apart)."""
-    fake_in = gp.get_selected_static_stream(ys_ref, ohp)
-    if ohp["discriminator_linguistic_condition"]:
-        fake_in = torch.cat((x, fake_in), -1)
-    mask = gp.sequence_mask(lens, x.size(1)).unsqueeze(-1)
-    with torch.no_grad():
-        return float(gp.bce_real(d_oracle(md).forward(fake_in, lens, adv_masks), mask, mask.sum().item()))
 
 
 def run_vs_restatement(dev, kind, mg, md, ohp, d_in, B, T, steps, seed, optimizer="Adagrad", mse_w=0.0):
     from gantts_b200 import fused
-    gen, g_fwd = gen_oracle(kind, mg)
-    d = d_oracle(md)
+    gen = generator_oracle(mg)
+    d = gp.DiscriminatorOracle(sd_numpy(md))
     d_sum = [torch.zeros_like(t) for t in d.params()]
     okw = ADAM if optimizer == "Adam" else None
     g_opt = gp.AdamStepper(gen.params(), **okw) if okw else None
@@ -125,9 +43,10 @@ def run_vs_restatement(dev, kind, mg, md, ohp, d_in, B, T, steps, seed, optimize
         fs.step(x.to(dev), y.to(dev), torch.LongTensor(lens).to(dev), frames=sum(lens))
         got = fs.loss_dict()
         dm = d_lstm_masks(fs, md, B * T, dev)
-        ref, yh_ref, ys_ref = gan_step(lambda: g_fwd(x, R, lens, ohp), gen.params(), gen.sums, d, d_sum, x, y, lens, R,
-                                       ohp, mse_w=mse_w, weight_decay=0.0, d_masks=dm, d_opt=d_opt, g_opt=g_opt)
-        ref = dict(ref, loss_adv=adv_loss_with(md, x, ys_ref, lens, ohp, dm["adv"]))
+        ref, yh_ref, ys_ref = gp.gan_step(lambda: gen.forward(x, R, lens, ohp), gen.params(), gen.sums, d, d_sum, x, y,
+                                          lens, R, ohp, mse_w=mse_w, weight_decay=0.0, d_masks=dm, d_opt=d_opt,
+                                          g_opt=g_opt)
+        ref = dict(ref, loss_adv=adv_loss_with(gp.DiscriminatorOracle(sd_numpy(md)), x, ys_ref, lens, ohp, dm["adv"]))
         errs = loss_errors(got, ref, LOSS_KEYS + ("d_grad_norm", "g_grad_norm"))
         errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), ys_ref.numpy())
         assert max(errs.values()) < TOL, (kind, it, errs)
@@ -335,8 +254,8 @@ def test_gan_trainer_rnn_d_vs_restatement_and_fused(dev, cond):
         with torch.no_grad():
             for a, b in zip(list(mg.parameters()) + list(md.parameters()), list(tg.parameters()) + list(td.parameters())):
                 b.copy_(a)
-        gen, g_fwd = gen_oracle("highway", tg)
-        d = d_oracle(td)
+        gen = generator_oracle(tg)
+        d = gp.DiscriminatorOracle(sd_numpy(td))
         if not train:
             for m in (mg, md, tg, td):
                 m.eval()
@@ -345,18 +264,18 @@ def test_gan_trainer_rnn_d_vs_restatement_and_fused(dev, cond):
         out, yh, ys = tr.step(x.to(dev), y.to(dev), lens, R.to(dev), train=train)
         fs.step(x.to(dev), y.to(dev), torch.LongTensor(lens).to(dev))
         got = fs.loss_dict()
-        ref, _, ys_ref = gan_step(lambda: g_fwd(x, R, lens, ohp), gen.params(), gen.sums, d,
-                                  [torch.zeros_like(t) for t in d.params()], x, y, lens, R, ohp, weight_decay=0.0,
-                                  training=train, update=train)
+        ref, _, ys_ref = gp.gan_step(lambda: gen.forward(x, R, lens, ohp), gen.params(), gen.sums, d,
+                                     [torch.zeros_like(t) for t in d.params()], x, y, lens, R, ohp, weight_decay=0.0,
+                                     training=train, update=train)
         trained = {k: float(out[k]) for k in LOSS_KEYS}
         # loss_adv (and loss_g = loss_mge + loss_adv) through each side's own updated D on the other side's y_hat_static
         # (see adv_loss_with); from the second step on the optimiser states of the two sides differ as well
-        ref["loss_adv"] = adv_loss_with(td, x, ys_ref, lens, ohp, None)
+        ref["loss_adv"] = adv_loss_with(gp.DiscriminatorOracle(sd_numpy(td)), x, ys_ref, lens, ohp, None)
         ref["loss_g"] = ref["loss_mge"] + ref["loss_adv"]
         errs = loss_errors(trained, ref, LOSS_KEYS)
         errs["y_hat_static"] = rel_err(npy(ys), ys_ref.numpy())
         assert max(errs.values()) < TOL, ("GanTrainer vs restatement", it, errs)
-        trained["loss_adv"] = adv_loss_with(md, x, ys.detach().cpu(), lens, ohp, None)
+        trained["loss_adv"] = adv_loss_with(gp.DiscriminatorOracle(sd_numpy(md)), x, ys.detach().cpu(), lens, ohp, None)
         trained["loss_g"] = trained["loss_mge"] + trained["loss_adv"]
         errs = loss_errors(got, trained, LOSS_KEYS)
         errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), npy(ys))

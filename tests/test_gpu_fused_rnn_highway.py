@@ -2,21 +2,22 @@
 gantts/models.py:72-118; bench.py cfg3): the sigmoid gate on x_static, the packed-sequence LSTM stack, hidden2out and the
 highway combine around the MLPG, their backward and their optimiser step inside the one-call step.
 
-The checker composes one-layer CPU torch nn.LSTMs on packed sequences and injects the step's own inter-layer dropout masks
-between them (every mask is gantts_dropout(ones[B * T][ndir * H], p, gantts_lstm_mask_seed(seed, layer))); with all-ones
-masks it equals the oracle port's In2OutRNNHighwayNet.  The discriminator's masks come from gantts_gan_step_seed as in
-test_gpu_fused_highway.py.  Tolerances: losses, gradient norms and y_hat_static 2e-4 relative (the cfg3 bound of
-test_gpu_train_mode.py); y_hat is the input, bit for bit; post-step weights median |delta| < 5e-6 and max <= 0.0201 (a
-first Adagrad / Adam step moves a weight by lr * sign(g)).  The configuration-rule test is host-only (no mark).
+The checker, GeneratorOracle("rnn_highway"), composes one-layer CPU torch nn.LSTMs on packed sequences and injects the
+step's own inter-layer dropout masks between them (every mask is gantts_dropout(ones[B * T][ndir * H], p,
+gantts_lstm_mask_seed(seed, layer))); with all-ones masks it equals the reference's one multi-layer nn.LSTM.  The
+discriminator's masks come from gantts_gan_step_seed as in test_gpu_fused_highway.py.  Tolerances: losses, gradient norms
+and y_hat_static 2e-4 relative (the cfg3 bound of test_gpu_train_mode.py); y_hat is the input, bit for bit; post-step
+weights median |delta| < 5e-6 and max <= 0.0201 (a first Adagrad / Adam step moves a weight by lr * sign(g)).  The
+configuration-rule test is host-only (no mark).
 """
 import numpy as np
 import pytest
 import torch
 
 from conftest import WINDOWS, rel_err
-from fused_step_helpers import (adv_loss_with, check_weights, config_checker, d_masks, dev, fill_tables,  # noqa: F401
-                                loss_errors, make_batch, npy, ragged_lengths, resync_oracle, sd_numpy, step_config,
-                                step_hp, use_adam)
+from fused_step_helpers import (_rhw_step_config, adv_loss_with, check_weights, config_checker, d_masks,  # noqa: F401
+                                dev, generator_oracle, loss_errors, lstm_masks, make_batch, npy, ragged_lengths,
+                                resync_oracle, rhw_models, sd_numpy, step_hp, use_adam, vc_ohp)
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
 
@@ -24,81 +25,14 @@ LOSS_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mge", "loss_mse", "lo
 GOLD_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mse", "loss_mge", "loss_adv", "loss_g",
              "real_correct", "fake_correct")
 TOL = 2e-4
-KINDS = ("weight_ih", "weight_hh", "bias_ih", "bias_hh")
-
-
-def vc_ohp(width, cond=False):
-    return dict(stream_sizes=[width], has_dynamic_features=[True], adversarial_streams=[True],
-                mask_nth_mgc_for_adv_loss=0, num_windows=3, discriminator_linguistic_condition=cond)
-
-
-def rhw_models(seed, S, layers, hidden, bidir, p, d_hidden, d_layers, p_d, cond=False):
-    import gantts_b200
-    torch.manual_seed(seed)
-    mg = gantts_b200.models.In2OutRNNHighwayNet(in_dim=3 * S, out_dim=3 * S, static_dim=S, num_hidden=layers,
-                                                hidden_dim=hidden, bidirectional=bidir, dropout=p)
-    md = gantts_b200.models.MLP(S + (3 * S if cond else 0), 1, d_layers, d_hidden, dropout=p_d, last_sigmoid=True)
-    return mg, md
-
-
-class RnnHighwayOracle(object):
-    """CPU In2OutRNNHighwayNet for gp.gan_step: one single-layer torch nn.LSTM per layer on packed sequences, with the
-    inter-layer dropout multipliers injected between them.  ``named`` maps the model's state_dict keys to the leaf
-    tensors; ``sums`` is the Adagrad state in the same order."""
-
-    def __init__(self, sd, num_layers, hidden, bidir, static_dim):
-        t = lambda k: torch.as_tensor(np.asarray(sd[k])).clone().float().requires_grad_(True)
-        self.S, self.sfx = static_dim, ["", "_reverse"][:2 if bidir else 1]
-        self.named = {"T.weight": t("T.weight"), "T.bias": t("T.bias")}
-        self.layers = []
-        for k in range(num_layers):
-            n_in = np.asarray(sd["lstm.weight_ih_l%d" % k]).shape[1]
-            m = torch.nn.LSTM(n_in, hidden, 1, batch_first=True, bidirectional=bidir)
-            with torch.no_grad():
-                for s in self.sfx:
-                    for n in KINDS:
-                        getattr(m, "%s_l0%s" % (n, s)).copy_(torch.as_tensor(np.asarray(sd["lstm.%s_l%d%s" % (n, k, s)])))
-                        self.named["lstm.%s_l%d%s" % (n, k, s)] = getattr(m, "%s_l0%s" % (n, s))
-            self.layers.append(m)
-        self.named["hidden2out.weight"], self.named["hidden2out.bias"] = t("hidden2out.weight"), t("hidden2out.bias")
-        self.sums = [torch.zeros_like(q) for q in self.params()]
-
-    def params(self):
-        return list(self.named.values())
-
-    def forward(self, x, R, lengths, masks=None):
-        """(y_hat, y_hat_static) = (x, x_s + sigmoid(T x_s) * MLPG(hidden2out(LSTM(x)))); masks[k] multiplies the output
-        of layer k < num_layers - 1, or None."""
-        xs = x[:, :, :self.S]
-        Tx = torch.sigmoid(torch.nn.functional.linear(xs, self.named["T.weight"], self.named["T.bias"]))
-        h = x
-        for k, m in enumerate(self.layers):
-            packed = torch.nn.utils.rnn.pack_padded_sequence(h, [int(v) for v in lengths], batch_first=True)
-            out, _ = m(packed)
-            h, _ = torch.nn.utils.rnn.pad_packed_sequence(out, batch_first=True, total_length=x.size(1))
-            if masks is not None and k + 1 < len(self.layers):
-                h = h * masks[k].view_as(h)
-        out = torch.nn.functional.linear(h, self.named["hidden2out.weight"], self.named["hidden2out.bias"])
-        return x, xs + Tx * nnp.unit_variance_mlpg(R, out)
-
-
-def lstm_masks(fs, mg, B, T, dev):
-    """The inter-layer masks the last training step of `fs` drew."""
-    from gantts_b200 import ops, _lib
-    lib = _lib.load()
-    lm = mg.lstm
-    nh = lm.hidden_size * (2 if lm.bidirectional else 1)
-    return [ops.dropout_mask(B * T, nh, lm.dropout, lib.gantts_lstm_mask_seed(fs.last_seed, k), dev).cpu()
-            for k in range(lm.num_layers - 1)]
 
 
 def run_vs_oracle(dev, mg, md, ohp, B, T, steps, mse_w, p_d, d_hidden, seed, tag, optimizer="Adagrad"):
     """`steps` training steps of FusedGanStep, each against the oracle started from the product's weights and optimiser
     state, with the step's own masks injected."""
     from gantts_b200 import fused
-    lm = mg.lstm
     S = mg.static_dim
-    gen = RnnHighwayOracle(sd_numpy(mg), lm.num_layers, lm.hidden_size, lm.bidirectional, S)
+    gen = generator_oracle(mg)
     d_layers = gp.discriminator_layers(sd_numpy(md))
     d_params = [t for pair in d_layers for t in pair]
     d_sum = [torch.zeros_like(t) for t in d_params]
@@ -118,10 +52,11 @@ def run_vs_oracle(dev, mg, md, ohp, B, T, steps, mse_w, p_d, d_hidden, seed, tag
         got = fs.loss_dict()
         gm = lstm_masks(fs, mg, B, T, dev)
         dm = d_masks(fs, B * T, [d_hidden] * (len(d_layers) - 1), p_d, dev)
-        ref, yh_ref, ys_ref = gp.gan_step(lambda: gen.forward(x, R, lens, gm), gen.params(), gen.sums, d_layers, d_sum,
-                                          x, y, lens, R, ohp, w_d=1.0, mse_w=mse_w, mge_w=1.0, adv_w=1.0, dropout_d=p_d,
-                                          training=True, weight_decay=0.0, d_masks=dm, d_opt=d_opt, g_opt=g_opt)
-        ref = dict(ref, loss_adv=adv_loss_with(md, x, ys_ref, lens, ohp, dm["adv"]))
+        ref, yh_ref, ys_ref = gp.gan_step(lambda: gen.forward(x, R, lens, ohp, masks=gm), gen.params(), gen.sums,
+                                          d_layers, d_sum, x, y, lens, R, ohp, w_d=1.0, mse_w=mse_w, mge_w=1.0,
+                                          adv_w=1.0, dropout_d=p_d, training=True, weight_decay=0.0, d_masks=dm,
+                                          d_opt=d_opt, g_opt=g_opt)
+        ref = dict(ref, loss_adv=adv_loss_with(gp.DiscriminatorOracle(sd_numpy(md)), x, ys_ref, lens, ohp, dm["adv"]))
         errs = loss_errors(got, ref, LOSS_KEYS + ("d_grad_norm", "g_grad_norm"))
         errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), ys_ref.numpy())
         assert max(errs.values()) < TOL, (tag, it, errs)
@@ -178,18 +113,18 @@ def test_fused_rnn_highway_cfg3_widths_train_mode(dev):
     256 -> 1 with dropout 0.5, B = 4 x T = 300 ragged (max length T), train mode, Adagrad: one step against the oracle
     with the step's own masks -- the losses, both gradient norms, y_hat_static, and every post-step generator tensor
     (weight_ih, weight_hh and both biases of every layer and direction).  With all-ones masks the oracle equals the
-    oracle port's In2OutRNNHighwayNet."""
+    oracle port's In2OutRNNHighwayNet on the reference's one multi-layer nn.LSTM."""
     B, T = 4, 300
     mg, md = rhw_models(5, 59, 3, 512, True, 0.5, 256, 2, 0.5)
     lens = ragged_lengths(B, T, 7)
     x, _ = make_batch(B, T, 177, 177, lens, 8)
     R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, T))
-    sd = sd_numpy(mg)
-    port = gp.GeneratorOracle("rnn_highway", sd, static_dim=59, num_hidden=3, hidden_dim=512, bidirectional=True)
-    mine = RnnHighwayOracle(sd, 3, 512, True, 59)
+    gen = generator_oracle(mg)
+    lstm = torch.nn.LSTM(177, 512, 3, batch_first=True, bidirectional=True)
+    lstm.load_state_dict({k[5:]: torch.from_numpy(v) for k, v in sd_numpy(mg).items() if k.startswith("lstm.")})
     with torch.no_grad():
-        _, a = port.forward(x, R, lens, vc_ohp(177))
-        _, b = mine.forward(x, R, lens, None)
+        _, a = gp.in2out_rnn_highway_forward(x, R, lens, gen.gate, lstm, gen.h2o, 59)
+        _, b = gen.forward(x, R, lens, vc_ohp(177), masks=[torch.ones(B * T, 1024)] * 2)
     assert rel_err(b.numpy(), a.numpy()) < 1e-5
     run_vs_oracle(dev, mg, md, vc_ohp(177), B, T, 1, 0.0, 0.5, 256, 300, "cfg3")
 
@@ -367,18 +302,6 @@ def test_fused_step_still_rejects_grurnn_and_unsupported_lstms(dev):
         mg.hidden2out = torch.nn.Linear((4 if "proj_size" in kw else 16) * 2, 24)
         with pytest.raises(RuntimeError, match="GanTrainer"):
             fused.FusedGanStep(mg.to(dev), md, hp, 2, 10)
-
-
-def _rhw_step_config():
-    """A valid In2OutRNNHighwayNet configuration of gantts_gan_step_t on the cfg3 layout: the gate (S = 59), 3
-    bidirectional LSTM layers of 16 over 3 S, hidden2out 32 -> 3 S, D S -> 32 -> 1 (host pointers are placeholders: only
-    the configuration check and the workspace layout run)."""
-    S, H, nl = 59, 16, 3
-    c = step_config((2 * H, 3 * S), (S, 32, 1), [(0, S, True, 0)], range(S), range(S))
-    c.highway.static_dim = S
-    ls = c.lstm
-    ls.num_layers, ls.in_dim, ls.hidden, ls.bidirectional, ls.dropout = nl, 3 * S, H, 1, 0.5
-    return fill_tables(c, 2 + 8 * nl + 2)
 
 
 def lstm_tensor(layer, direction, kind):

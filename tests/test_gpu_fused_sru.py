@@ -3,20 +3,21 @@
 step inside the one-call step.
 
 The checker is the CPU restatement of the SRU recurrence in oracle/gantts_port.py (sru_layer_forward) composed into an
-SRURNN below; SRU parity with the upstream `cuda_functional` package stays unpinned (it is not vendored).  Train-mode
-parity injects the step's own masks: every SRU mask is gantts_dropout(ones, p, gantts_sru_mask_seed(seed, layer, which)),
-the discriminator's masks come from gantts_gan_step_seed as in test_gpu_fused_highway.py.  Tolerances: losses, outputs
-and gradient norms 2e-4 relative; post-step weights median |delta| < 5e-6 and max <= 0.0201 (a first Adagrad / Adam
-step moves a weight by lr * sign(g)).  The configuration-rule test is host-only (no mark).
+SRURNN by GeneratorOracle("sru"); SRU parity with the upstream `cuda_functional` package stays unpinned (it is not
+vendored).  Train-mode parity injects the step's own masks: every SRU mask is gantts_dropout(ones, p,
+gantts_sru_mask_seed(seed, layer, which)), the discriminator's masks come from gantts_gan_step_seed as in
+test_gpu_fused_highway.py.  Tolerances: losses, outputs and gradient norms 2e-4 relative; post-step weights median
+|delta| < 5e-6 and max <= 0.0201 (a first Adagrad / Adam step moves a weight by lr * sign(g)).  The configuration-rule
+test is host-only (no mark).
 """
 import numpy as np
 import pytest
 import torch
 
 from conftest import WINDOWS, TTS_HP, rel_err
-from fused_step_helpers import (adv_loss_with, check_weights, config_checker, d_masks, dev, fill_tables,  # noqa: F401
-                                loss_errors, make_batch, npy, ragged_lengths, resync_oracle, sd_numpy, step_config,
-                                step_hp, use_adam)
+from fused_step_helpers import (_sru_step_config, adv_loss_with, check_weights, config_checker, d_masks,  # noqa: F401
+                                dev, generator_oracle, loss_errors, make_batch, npy, ragged_lengths, resync_oracle,
+                                sd_numpy, sru_masks, sru_models, step_hp, use_adam)
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
 
@@ -27,72 +28,11 @@ LOSS_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mge", "loss_mse", "lo
 TOL = 2e-4
 
 
-def sru_models(seed, in_dim, out_dim, layers, hidden, bidir, relu, p, rnn_p, d_hidden, d_layers, d_p, n_adv):
-    import gantts_b200
-    torch.manual_seed(seed)
-    mg = gantts_b200.models.SRURNN(in_dim=in_dim, out_dim=out_dim, num_hidden=layers, hidden_dim=hidden,
-                                   bidirectional=bidir, dropout=p, use_relu=int(relu), rnn_dropout=rnn_p)
-    for cell in mg.gru.rnn_lst:                        # non-zero forget / reset biases
-        cell.bias.data.uniform_(-0.5, 0.5)
-    md = gantts_b200.models.MLP(in_dim + n_adv, 1, d_layers, d_hidden, dropout=d_p, last_sigmoid=True)
-    return mg, md
-
-
-class SruOracle(object):
-    """CPU SRURNN for gp.gan_step built from the model's state_dict (gru.rnn_lst.{i}.weight / .bias, hidden2out.*):
-    gp.sru_layer_forward per layer with injected masks, then hidden2out.  ``named`` / ``params()`` follow
-    model_g.parameters() order; ``sums`` is the Adagrad state."""
-
-    def __init__(self, sd, bidirectional, act):
-        t = lambda k: torch.as_tensor(np.asarray(sd[k])).clone().float().requires_grad_(True)
-        n = len([k for k in sd if k.startswith("gru.rnn_lst.") and k.endswith(".weight")])
-        self.named = {}
-        for i in range(n):
-            for s in ("weight", "bias"):
-                self.named["gru.rnn_lst.%d.%s" % (i, s)] = t("gru.rnn_lst.%d.%s" % (i, s))
-        self.named["hidden2out.weight"], self.named["hidden2out.bias"] = t("hidden2out.weight"), t("hidden2out.bias")
-        self.n, self.bidir, self.act = n, bidirectional, act
-        self.sums = [torch.zeros_like(p) for p in self.params()]
-
-    def params(self):
-        return list(self.named.values())
-
-    def forward(self, x, R, hp, masks=None):
-        """(y_hat, y_hat_static); masks = [(mask_x [B][n_in], mask_h [B][ncols] or None)] per layer, or None."""
-        dirs = 2 if self.bidir else 1
-        h = x
-        for i in range(self.n):
-            W, b = self.named["gru.rnn_lst.%d.weight" % i], self.named["gru.rnn_lst.%d.bias" % i]
-            nc = b.numel() // 2
-            bport = torch.stack([b[:nc].view(dirs, nc // dirs), b[nc:].view(dirs, nc // dirs)], 1).reshape(-1)
-            mx, mh = masks[i] if masks is not None else (None, None)
-            h = gp.sru_layer_forward(h.transpose(0, 1), W, bport, bidirectional=self.bidir, use_tanh=self.act == 1,
-                                     use_relu=self.act == 2, mask_x=mx, mask_h=mh).transpose(0, 1)
-        y_hat = torch.nn.functional.linear(h, self.named["hidden2out.weight"], self.named["hidden2out.bias"])
-        return gp.apply_generator(y_hat, x, R, hp)
-
-
-def sru_masks(fs, mg, B, dev):
-    """The SRU masks the last training step of `fs` drew."""
-    from gantts_b200 import ops, _lib
-    lib = _lib.load()
-    cells = list(mg.gru.rnn_lst)
-    out = []
-    for i, cell in enumerate(cells):
-        nc = cell.n_out * (2 if cell.bidirectional else 1)
-        mx = ops.dropout_mask(B, cell.n_in, cell.rnn_dropout, lib.gantts_sru_mask_seed(fs.last_seed, i, 0), dev).cpu()
-        mh = ops.dropout_mask(B, nc, cell.dropout, lib.gantts_sru_mask_seed(fs.last_seed, i, 1), dev).cpu() \
-            if i + 1 < len(cells) else None
-        out.append((mx, mh))
-    return out
-
-
 def run_vs_oracle(dev, mg, md, ohp, B, T, steps, mse_w, p_d, d_hidden, seed, tag, with_outputs=True):
     from gantts_b200 import fused
     in_dim = mg.gru.rnn_lst[0].n_in
     out_dim = mg.hidden2out.weight.shape[0]
-    relu = mg.gru.rnn_lst[0].activation_type
-    gen = SruOracle(sd_numpy(mg), mg.gru.rnn_lst[0].bidirectional, relu)
+    gen = generator_oracle(mg)
     d_layers = gp.discriminator_layers(sd_numpy(md))
     d_sum = [torch.zeros_like(t) for pair in d_layers for t in pair]
     mg.to(dev).train(), md.to(dev).train()
@@ -104,10 +44,10 @@ def run_vs_oracle(dev, mg, md, ohp, B, T, steps, mse_w, p_d, d_hidden, seed, tag
         fs.step(x.to(dev), y.to(dev), torch.LongTensor(lens).to(dev), frames=sum(lens))
         got = fs.loss_dict()
         gm, dm = sru_masks(fs, mg, B, dev), d_masks(fs, B * T, [d_hidden] * (len(d_layers) - 1), p_d, dev)
-        ref, yh_ref, ys_ref = gp.gan_step(lambda: gen.forward(x, R, ohp, gm), gen.params(), gen.sums, d_layers, d_sum,
-                                          x, y, lens, R, ohp, w_d=1.0, mse_w=mse_w, mge_w=1.0, adv_w=1.0, dropout_d=p_d,
-                                          training=True, weight_decay=0.0, d_masks=dm)
-        ref = dict(ref, loss_adv=adv_loss_with(md, x, ys_ref, lens, ohp, dm["adv"]))
+        ref, yh_ref, ys_ref = gp.gan_step(lambda: gen.forward(x, R, lens, ohp, masks=gm), gen.params(), gen.sums,
+                                          d_layers, d_sum, x, y, lens, R, ohp, w_d=1.0, mse_w=mse_w, mge_w=1.0,
+                                          adv_w=1.0, dropout_d=p_d, training=True, weight_decay=0.0, d_masks=dm)
+        ref = dict(ref, loss_adv=adv_loss_with(gp.DiscriminatorOracle(sd_numpy(md)), x, ys_ref, lens, ohp, dm["adv"]))
         errs = loss_errors(got, ref, LOSS_KEYS + ("d_grad_norm", "g_grad_norm"))
         if with_outputs:
             errs["y_hat"] = rel_err(npy(fs.y_hat), yh_ref.numpy())
@@ -156,7 +96,7 @@ def test_fused_sru_tts_duration_adam_and_resume(dev):
     def build():
         return sru_models(11, 416, 5, 6, 512, True, True, p, p, 256, 3, pd, 5)
     mg, md = build()
-    gen = SruOracle(sd_numpy(mg), True, 2)
+    gen = generator_oracle(mg)
     d_layers = gp.discriminator_layers(sd_numpy(md))
     d_params = [t for pair in d_layers for t in pair]
     g_opt, d_opt = gp.AdamStepper(gen.params(), **okw), gp.AdamStepper(d_params, **okw)
@@ -170,10 +110,11 @@ def test_fused_sru_tts_duration_adam_and_resume(dev):
         fs.step(x.to(dev), y.to(dev), torch.LongTensor(lens).to(dev), frames=sum(lens))
         got = fs.loss_dict()
         gm, dm = sru_masks(fs, mg, B, dev), d_masks(fs, B * T, [256] * 3, pd, dev)
-        ref, yh_ref, ys_ref = gp.gan_step(lambda: gen.forward(x, None, DURATION_HP, gm), gen.params(), None, d_layers,
-                                          None, x, y, lens, None, DURATION_HP, w_d=1.0, mse_w=1.0, mge_w=0.0, adv_w=1.0,
-                                          dropout_d=pd, training=True, d_masks=dm, d_opt=d_opt, g_opt=g_opt)
-        ref = dict(ref, loss_adv=adv_loss_with(md, x, ys_ref, lens, DURATION_HP, dm["adv"]))
+        ref, yh_ref, ys_ref = gp.gan_step(lambda: gen.forward(x, None, lens, DURATION_HP, masks=gm), gen.params(), None,
+                                          d_layers, None, x, y, lens, None, DURATION_HP, w_d=1.0, mse_w=1.0, mge_w=0.0,
+                                          adv_w=1.0, dropout_d=pd, training=True, d_masks=dm, d_opt=d_opt, g_opt=g_opt)
+        ref = dict(ref, loss_adv=adv_loss_with(gp.DiscriminatorOracle(sd_numpy(md)), x, ys_ref, lens, DURATION_HP,
+                                               dm["adv"]))
         errs = loss_errors(got, ref, ("loss_d", "loss_mse", "loss_adv", "loss_g", "d_grad_norm", "g_grad_norm"))
         errs["y_hat"] = rel_err(npy(fs.y_hat), yh_ref.numpy())
         errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), ys_ref.numpy())
@@ -307,21 +248,6 @@ def test_fused_sru_rejects_sigmoid_output(dev):
     md = gantts_b200.models.MLP(58, 1, 2, 16, dropout=0.0, last_sigmoid=True).to(dev)
     with pytest.raises(RuntimeError, match="linear-output"):
         fused.FusedGanStep(mg, md, step_hp(TTS_HP), 2, 10)
-
-
-def _sru_step_config():
-    """A valid SRURNN configuration of gantts_gan_step_t on the tts_acoustic layout with a conditioned D: 3 bidirectional
-    layers of 16 over in_dim 40, hidden2out 32 -> 187, D 40 + 58 -> 32 -> 1 (host pointers are placeholders: only the
-    configuration check and the workspace layout run)."""
-    from gantts_b200 import multistream, step as gstep
-    in_dim, hidden, nl = 40, 16, 3
-    hp = gstep.TTS_ACOUSTIC
-    entries, n_static = multistream.mlpg_stream_entries(hp.stream_sizes, hp.has_dynamic_features, [True] * 4, 3)
-    c = step_config((2 * hidden, 187), (in_dim + 58, 32, 1), entries, range(n_static), range(2, 60), conditioned=True)
-    s = c.sru
-    s.num_layers, s.in_dim, s.hidden, s.bidirectional, s.act = nl, in_dim, hidden, 1, 2
-    s.dropout, s.rnn_dropout = 0.2, 0.2
-    return fill_tables(c, 2 * nl + 2)
 
 
 def test_sru_step_config_rules_on_tensor_tables():

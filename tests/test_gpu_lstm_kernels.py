@@ -18,48 +18,15 @@ import subprocess
 import sys
 import tempfile
 
-import numpy as np
 import pytest
 import torch
 
 import lstm_f64 as ref
+from lstm_f64 import CASES
 
 pytestmark = pytest.mark.gpu
 
 TOL = {"h": 5e-6, "gates": 5e-6, "cells": 5e-6, "dxproj": 5e-6}
-H_LIST = (4, 12, 256, 260, 512, 516, 528)
-
-
-def _lengths(kind, B, T, seed):
-    if kind in ("full", "T=1"):
-        return [T] * B
-    if kind == "desc":
-        return [max(1, T - (b * T) // B) for b in range(B)]
-    # unsorted ragged: the full length, two sequences of length 1, the rest anywhere in [1, T]
-    rng = np.random.RandomState(seed)
-    lens = [T, 1, 1] + [int(v) for v in rng.randint(1, T + 1, max(B - 3, 0))]
-    lens = lens[:B]
-    rng.shuffle(lens)
-    return lens
-
-
-def _cases():
-    """(id, B, T, H, ndir, lengths)"""
-    cases = []
-    for H in H_LIST:
-        T = 23 if H < 256 else 7          # the float64 loop runs on the CPU: short where H is large
-        for ndir in (1, 2):
-            shapes = [(1, T, "full"), (17, T, "desc"), (33, T, "unsorted"), (16, 1, "T=1")]
-            if H in (12, 260, 528):
-                shapes.append((128, T, "unsorted"))
-            for B, Tc, kind in shapes:
-                cases.append(("H%d-%s-B%d-T%d-%s" % (H, "bi" if ndir == 2 else "uni", B, Tc, kind), B, Tc, H, ndir, kind))
-    cases.append(("spoof-count-max-B128-T64-H256-bi", 128, 64, 256, 2, "unsorted"))
-    cases.append(("cfg3-width-B16-T200-H512-bi", 16, 200, 512, 2, "desc"))
-    return [(cid, B, T, H, ndir, _lengths(kind, B, T, i)) for i, (cid, B, T, H, ndir, kind) in enumerate(cases)]
-
-
-CASES = _cases()
 
 
 def _lib():
@@ -288,7 +255,7 @@ def test_repeated_calls_are_bit_identical():
     L = _lib()
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     for H, ndir, B in ((12, 2, 33), (260, 1, 17), (516, 1, 17), (528, 2, 20)):
-        T, lengths = 6, _lengths("unsorted", B, 6, 7)
+        T, lengths = 6, ref.case_lengths("unsorted", B, 6, 7)
         xproj, W_hh, dh = _inputs(B, T, H, ndir, 77)
         layer = Layer(L, xproj, W_hh, lengths)
         runs = []

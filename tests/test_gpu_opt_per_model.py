@@ -1,8 +1,8 @@
 """One optimiser per model (reference train.py:796-799: optimizer_g and optimizer_d from their own hparams) in
 FusedGanStep and GanTrainer, on the GPU.
 
-Checkers: the oracle's gan_step / the D-only restatement with a stepper per model and the step's own dropout masks
-injected (tolerances of the fused-generator modules: losses 2e-4 relative, weights through check_weights); the
+Checkers: the oracle's gan_step (update_g=False for the D-only step) with a stepper per model and the step's own
+dropout masks injected (tolerances of the fused-generator modules: losses 2e-4 relative, weights through check_weights); the
 reference's per-batch logic (tests/trainpy_mirror.py) with torch.optim.Adam for G and torch.optim.Adagrad for D; and bit
 for bit against the same step built another way (optimizer_d=None, the former two-call sequence, the data-parallel phase
 calls, a step built with the decayed lr, a resumed step).
@@ -14,15 +14,13 @@ import pytest
 import torch
 
 from conftest import ROOT, WINDOWS, rel_err
-from fused_step_helpers import (check_weights, d_masks, dev, make_batch, npy, ragged_lengths, resync_oracle,  # noqa: F401
-                                sd_numpy, step_hp)
-import dwarmup_oracle as dwo
+from fused_step_helpers import (ADAM, assert_equal_lists, build, check_weights, d_masks, dev, g_masks,  # noqa: F401
+                                generator_oracle, make_batch, npy, ragged_lengths, resync_oracle, sd_numpy, snapshot,
+                                step_hp)
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
-from test_gpu_dwarmup_spoof import assert_equal_lists, build, g_masks, gen_oracle, snapshot
 
 TOL = 2e-4
-ADAM = dict(lr=1e-3, betas=(0.5, 0.9), weight_decay=0.0, eps=1e-8)
 # (G kind, G params, D kind, D params): Adam G with an Adagrad D of its own lr, and Adagrad on both with different lrs
 SETTINGS = {"adam_g_adagrad_d": ("Adam", ADAM, "Adagrad", dict(lr=1e-3, weight_decay=0.0)),
             "adagrad_two_lrs": ("Adagrad", dict(lr=0.01, weight_decay=0.0), "Adagrad", dict(lr=0.003, weight_decay=0.0))}
@@ -90,7 +88,7 @@ def test_fused_step_with_an_optimiser_per_model_vs_oracle(dev, kind, setting):
     B, T = 3, 40
     kg, pg, kd, pd = SETTINGS[setting]
     mg, md, hp, d_in, d_out, g_hidden, d_hidden, p_d = build(kind, 80)
-    gen, g_fwd = gen_oracle(kind, mg)
+    gen = generator_oracle(mg)
     d_layers = gp.discriminator_layers(sd_numpy(md))
     d_params = [t for pair in d_layers for t in pair]
     d_sum = [torch.zeros_like(t) for t in d_params]
@@ -105,13 +103,10 @@ def test_fused_step_with_an_optimiser_per_model_vs_oracle(dev, kind, setting):
         got = fs.loss_dict()
         gm = g_masks(kind, fs, mg, B, T, g_hidden, dev)
         dm = d_masks(fs, B * T, [d_hidden] * (len(d_layers) - 1), p_d, dev)
-        if update_g:
-            ref, _, ys_ref = gp.gan_step(lambda: g_fwd(x, R, lens, hp, gm), gen.params(), gen.sums, d_layers, d_sum, x, y,
-                                         lens, R, hp, w_d=1.0, mse_w=0.0, mge_w=1.0, adv_w=1.0, dropout_d=p_d,
-                                         training=True, weight_decay=0.0, d_masks=dm, d_opt=d_opt, g_opt=g_opt)
-        else:
-            ref, _, ys_ref = dwo.d_only_step(lambda: g_fwd(x, R, lens, hp, gm), d_layers, d_sum, x, y, lens, hp,
-                                             dropout_d=p_d, weight_decay=0.0, d_masks=dm, d_opt=d_opt)
+        ref, _, ys_ref = gp.gan_step(lambda: gen.forward(x, R, lens, hp, masks=gm), gen.params(), gen.sums, d_layers,
+                                     d_sum, x, y, lens, R, hp, w_d=1.0, mse_w=0.0, mge_w=1.0, adv_w=1.0, dropout_d=p_d,
+                                     training=True, weight_decay=0.0, update_g=update_g, d_masks=dm, d_opt=d_opt,
+                                     g_opt=g_opt)
         errs = {k: abs(got[k] - ref[k]) / max(abs(ref[k]), 1e-12) for k in PRE_UPDATE_KEYS}
         errs["y_hat_static"] = rel_err(npy(fs.y_hat_static), ys_ref.numpy())
         assert max(errs.values()) < TOL, (kind, setting, it, errs)

@@ -2,7 +2,7 @@
 GanTrainer with reference_discriminator = LSTMRNN / GRURNN (train.py:779-781 builds it from hp.discriminator like D), run by
 gantts_spoof_count_lstm.
 
-Checker: the CPU restatement tests/spoof_rnn_oracle.py (pinned to the reference by test_spoof_rnn_host.py) on the
+Checker: the oracle's spoof_count on a DiscriminatorOracle (pinned to the reference by test_spoof_rnn_host.py) on the
 product's own pre-update y_hat_static.  The count is an integer, but a frame whose D_ref lies within rounding of 0.5 may
 fall on either side: the counts may differ by at most the number of valid frames whose CPU |D_ref - 0.5| is below
 TIE_BAND.  The band is 1e-5: on an NVIDIA H100 80GB HBM3 (700 W) the count's own D_ref output, read back from its
@@ -15,11 +15,10 @@ import pytest
 import torch
 
 from conftest import WINDOWS
-from fused_step_helpers import dev, make_batch, ragged_lengths, sd_numpy, step_hp  # noqa: F401
+from fused_step_helpers import (assert_equal_lists, dev, make_batch, make_models, ragged_lengths, sd_numpy,  # noqa: F401
+                                snapshot, step_hp)
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
-import spoof_rnn_oracle as sro
-from test_gpu_fused_rnn_d import make_models
 
 TIE_BAND = 1e-5
 
@@ -32,45 +31,30 @@ def ref_discriminator(n_adv, layers, hidden, bidir, dev, seed, gru=False):
     return cls(n_adv, 1, layers, hidden, bidirectional=bidir, dropout=0.5, last_sigmoid=True).to(dev).train()
 
 
-def oracle_of(ref_d):
-    rnn = getattr(ref_d, ref_d._rnn_attr)
-    return sro.reference_d(sd_numpy(ref_d), ref_d._rnn_attr, rnn.num_layers, rnn.hidden_size, rnn.bidirectional)
-
-
 def centre(ref_d, ys, lens, ohp):
     """Scale and shift ref_d's hidden2out so that its outputs on ys fall on both sides of 0.5."""
     with torch.no_grad():
         ref_d.hidden2out.weight.mul_(10.0)
         ref_d.hidden2out.bias.zero_()
-        z = torch.logit(sro.reference_output_rnn(oracle_of(ref_d), ys, lens, ohp))
+        z = torch.logit(gp.reference_output(gp.DiscriminatorOracle(sd_numpy(ref_d)), ys, lens, ohp))
         mask = gp.sequence_mask(lens, ys.size(1)).unsqueeze(-1)
         ref_d.hidden2out.bias.fill_(-float(z[mask > 0].median()))
 
 
 def check_count(got, ref_d, ys, lens, ohp, what):
     """got == the restatement's count on ys, up to the valid frames whose CPU |D_ref - 0.5| < TIE_BAND."""
-    o = oracle_of(ref_d)
+    o = gp.DiscriminatorOracle(sd_numpy(ref_d))
     mask = gp.sequence_mask(lens, ys.size(1)).unsqueeze(-1)
-    want = sro.spoof_count_rnn(o, ys, lens, mask, ohp)
-    close = float(((sro.reference_output_rnn(o, ys, lens, ohp) - 0.5).abs() < TIE_BAND).float().mul(mask).sum())
+    want = gp.spoof_count(o, ys, lens, mask, ohp)
+    close = float(((gp.reference_output(o, ys, lens, ohp) - 0.5).abs() < TIE_BAND).float().mul(mask).sum())
     print("spoof count %s: got %g, restatement %g, %g frame(s) within %g of 0.5" % (what, float(got), want, close,
                                                                                    TIE_BAND))
     assert abs(float(got) - want) <= close, (what, float(got), want, close)
     return want
 
 
-def snapshot(*tensors):
-    return [t.detach().clone() for t in tensors]
-
-
-def assert_equal_lists(a, b, what):
-    assert len(a) == len(b)
-    for i, (u, v) in enumerate(zip(a, b)):
-        assert torch.equal(u, v), (what, i)
-
-
 def models(kind, seed, d_kind):
-    """(generator, discriminator, ohp, d_in, d_out, n_adv): the generator of test_gpu_fused_rnn_d.make_models with its
+    """(generator, discriminator, ohp, d_in, d_out, n_adv): the generator of fused_step_helpers.make_models with its
     LSTMRNN D (d_kind "lstm": 2 x 12 bidirectional, dropout 0.5), or an MLP D (d_kind "mlp": 2 x 16, dropout 0.5)."""
     import gantts_b200
     mg, md, ohp, d_in = make_models(kind, seed, False)

@@ -8,7 +8,7 @@ import torch
 from torch.nn.utils.rnn import pack_padded_sequence, pad_packed_sequence
 
 import lstm_f64 as ref
-from test_gpu_lstm_kernels import CASES
+from lstm_f64 import CASES
 
 TOL = 1e-12
 

@@ -17,7 +17,8 @@ import pytest
 import torch
 
 from conftest import ROOT
-from fused_step_helpers import FAKE, config_checker, fill_tables, step_config, use_adam
+from fused_step_helpers import (FAKE, TTS_STREAMS, _rhw_step_config, _rnn_d_config, _sru_step_config, _vc_step_config,
+                                config_checker, fill_tables, step_config, use_adam)
 
 # gantts_gan_step_workspace_bytes of these configurations before gantts_gan_step_t had the d_opt block (every one
 # accepted; the same with Adagrad and with Adam on both models)
@@ -25,16 +26,11 @@ PARENT_WORKSPACE = {"mlp": 1495552, "highway": 1860352, "sru": 1831168, "rnn_hig
 
 
 def _mlp_config():
-    from test_fused_ragged_host import TTS_STREAMS
     c = step_config([20, 32, 187], [58, 16, 1], TTS_STREAMS, list(range(60)) + [180, 183, 184], list(range(2, 60)))
     return fill_tables(c, 4)
 
 
 def _configs():
-    from test_gpu_fused_highway import _vc_step_config
-    from test_gpu_fused_rnn_highway import _rhw_step_config
-    from test_gpu_fused_sru import _sru_step_config
-    from test_rnn_d_host import _rnn_d_config
     return {"mlp": _mlp_config, "highway": _vc_step_config, "sru": _sru_step_config, "rnn_highway": _rhw_step_config,
             "rnn_d": _rnn_d_config}
 

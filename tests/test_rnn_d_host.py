@@ -1,7 +1,8 @@
 """CPU-only tests of the recurrent discriminator (LSTMRNN / GRURNN) of the fused GAN step:
 
-* the CPU restatement tests/rnn_d_oracle.py pinned to tests/golden/rnn_d.npz (written by tests/golden/make_golden_rnn_d.py
-  from the unmodified reference) -- losses, counts, y_hat_static, post-step weights of both models, optimiser state;
+* the oracle's gan_step with a DiscriminatorOracle pinned to tests/golden/rnn_d.npz (written by
+  tests/golden/make_golden_rnn_d.py from the unmodified reference) -- losses, counts, y_hat_static, post-step weights
+  of both models, optimiser state;
 * the host-only rules of gantts_gan_step_t.d_lstm that gantts_gan_step_workspace_bytes applies, the workspace of a
   zero-filled block, the mask-seed stream and the ctypes binding (placeholder device pointers: only the configuration
   check and the workspace layout run)."""
@@ -13,25 +14,11 @@ import pytest
 import torch
 
 from conftest import GOLDEN, TTS_HP, WINDOWS, rel_err
-from fused_step_helpers import config_checker, fill_tables, step_config, use_adam
+from fused_step_helpers import _rnn_d_config, config_checker, use_adam
 
 F32_TOL = 1e-6
 VC_TOY_HP = dict(stream_sizes=[27], has_dynamic_features=[True], adversarial_streams=[True],
                  mask_nth_mgc_for_adv_loss=0, num_windows=3, discriminator_linguistic_condition=False)
-
-
-def _rnn_d_config(bidir=1, layers=2, hidden=16, cond=False):
-    """An MLP generator 20 -> 24 -> 27 on one dynamic stream of 9 static columns, and an LSTMRNN D over those 9 columns
-    (plus the 20 conditioning columns when cond): `layers` LSTM layers of `hidden` units, then hidden2out -> 1."""
-    nh = hidden * (2 if bidir else 1)
-    c = step_config((20, 24, 27), (nh, 1), [(0, 9, True, 0)], range(9), range(9), conditioned=cond)
-    dl = c.d_lstm
-    dl.num_layers, dl.in_dim, dl.hidden, dl.bidirectional, dl.dropout = layers, 9 + (20 if cond else 0), hidden, bidir, 0.5
-    fill_tables(c, 4)
-    c.d_tensors.n = 4 * layers * (2 if bidir else 1) + 2
-    for i in range(c.d_tensors.n):
-        c.d_tensors.param[i] = c.d_tensors.state[i] = c.g_tensors.param[0]
-    return c
 
 
 def test_rnn_d_config_rules():
@@ -102,8 +89,8 @@ def test_d_lstm_ctypes_binding():
     assert names[-2:] == ["opt_step", "d_lstm"] and _lib.GanStepT.d_lstm.offset >= _lib.GanStepT.opt_step.offset + 8
 
 
-# ---- the CPU restatement (tests/rnn_d_oracle.py) pinned to tests/golden/rnn_d.npz (tests/golden/make_golden_rnn_d.py: the
-# unmodified reference's apply_generator / update_discriminator / update_generator with a recurrent discriminator)
+# ---- the oracle's gan_step with a DiscriminatorOracle pinned to tests/golden/rnn_d.npz (tests/golden/make_golden_rnn_d.py:
+# the unmodified reference's apply_generator / update_discriminator / update_generator with a recurrent discriminator)
 GOLD_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mse", "loss_mge", "loss_adv", "loss_g",
              "real_correct", "fake_correct")
 GOLD_CASES = {  # tag: (hparams set, D state_dict prefix, bidirectional, conditioned, update_g)
@@ -127,7 +114,6 @@ def test_restatement_matches_reference(golden, case, opt):
     weights of both models and the discriminator optimiser's state."""
     from oracle import gantts_port as gp
     from oracle import nnmnkwii_port as nnp
-    import rnn_d_oracle as rdo
     g = golden
     hp_name, prefix, bidir, cond, update_g = GOLD_CASES[case]
     tag = "%s_%s_" % (case, opt)
@@ -135,7 +121,9 @@ def test_restatement_matches_reference(golden, case, opt):
     hp = dict(VC_TOY_HP if hp_name == "vc" else TTS_HP, discriminator_linguistic_condition=cond)
     kind = "highway" if hp_name == "vc" else "mlp"
     gen = gp.GeneratorOracle(kind, sub(hp_name + "_g0_"), static_dim=9 if kind == "highway" else None)
-    d = rdo.RnnDiscriminator(sub(tag + "d0_"), prefix, 2, 4, bidir)
+    d = gp.DiscriminatorOracle(sub(tag + "d0_"))
+    assert (d.layers[0].hidden_size, len(d.layers), d.layers[0].bidirectional) == (4, 2, bidir)
+    assert list(d.named)[0].startswith(prefix + ".")
     d_sum = [torch.zeros_like(t) for t in d.params()]
     akw = dict(lr=1e-3, betas=(0.5, 0.9), eps=1e-8, weight_decay=0.0)
     g_opt = gp.AdamStepper(gen.params(), **akw) if opt == "adam" else None
@@ -146,8 +134,8 @@ def test_restatement_matches_reference(golden, case, opt):
         x, y = torch.from_numpy(g[p + "x"]), torch.from_numpy(g[p + "y"])
         lens = [int(v) for v in g[p + "lengths"]]
         R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, x.size(1)))
-        out, _, y_hat_static = rdo.gan_step(lambda: gen.forward(x, R, lens, hp, training=True), gen.params(), gen.sums,
-                                            d, d_sum, x, y, lens, R, hp, update_g=update_g, d_opt=d_opt, g_opt=g_opt)
+        out, _, y_hat_static = gp.gan_step(lambda: gen.forward(x, R, lens, hp, training=True), gen.params(), gen.sums,
+                                           d, d_sum, x, y, lens, R, hp, update_g=update_g, d_opt=d_opt, g_opt=g_opt)
         for k, v in zip(GOLD_KEYS, g["%sit%d_losses" % (tag, it)]):
             if np.isnan(v):
                 continue

@@ -1,6 +1,6 @@
 """CPU-only tests of the spoofing-rate count with a recurrent reference discriminator (LSTMRNN / GRURNN):
 
-* the CPU restatement (tests/spoof_rnn_oracle.py) pinned to tests/golden/spoof_rnn.npz (written by
+* the oracle's spoof_count on a DiscriminatorOracle pinned to tests/golden/spoof_rnn.npz (written by
   tests/golden/make_golden_spoof_rnn.py from the UNMODIFIED reference's spoof block, train.py:549-558) -- the generator
   output it counts on, the reference discriminator's output and the count, exactly;
 * the host-only configuration rules of gantts_spoof_count_lstm_workspace_bytes / gantts_spoof_count_lstm through the C ABI
@@ -16,7 +16,6 @@ import torch
 
 from conftest import GOLDEN, TTS_HP, WINDOWS, rel_err
 from fused_step_helpers import FAKE, config_checker
-import spoof_rnn_oracle as sro
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
 
@@ -34,13 +33,6 @@ def sub(g, pre):
     return {k[len(pre):]: g[k] for k in g.files if k.startswith(pre)}
 
 
-def ref_from_state(sd, prefix):
-    """RnnDiscriminator of a reference LSTMRNN / GRURNN state_dict (its shape read off the tensors)."""
-    layers = len([k for k in sd if k.startswith(prefix + ".weight_ih_l") and not k.endswith("_reverse")])
-    bidir = (prefix + ".weight_ih_l0_reverse") in sd
-    return sro.reference_d(sd, prefix, layers, sd[prefix + ".weight_hh_l0"].shape[1], bidir)
-
-
 @pytest.mark.parametrize("ref_cls", ["lstmrnn", "grurnn"])
 @pytest.mark.parametrize("case", ["vc", "tts"])
 def test_spoof_count_rnn_matches_reference(golden, case, ref_cls):
@@ -48,7 +40,8 @@ def test_spoof_count_rnn_matches_reference(golden, case, ref_cls):
     count equal the reference's; the count is exact (it is an integer)."""
     g, hp, tag = golden, CASES[case], "%s_%s_" % (case, ref_cls)
     gen = gp.GeneratorOracle("mlp", sub(g, tag + "g0_"))
-    ref_d = ref_from_state(sub(g, tag + "ref_"), "lstm" if ref_cls == "lstmrnn" else "gru")
+    ref_d = gp.DiscriminatorOracle(sub(g, tag + "ref_"))
+    assert list(ref_d.named)[0].startswith("lstm." if ref_cls == "lstmrnn" else "gru.")
     for it in range(2):
         p = "%sit%d_" % (tag, it)
         x = torch.from_numpy(g[p + "x"])
@@ -58,12 +51,12 @@ def test_spoof_count_rnn_matches_reference(golden, case, ref_cls):
             _, y_hat_static = gen.forward(x, R, lens, hp, training=True)
         assert rel_err(y_hat_static.numpy(), g[p + "y_hat_static"]) < 1e-6, (it, "y_hat_static")
         ys = torch.from_numpy(g[p + "y_hat_static"])
-        target = sro.reference_output_rnn(ref_d, ys, lens, hp)
+        target = gp.reference_output(ref_d, ys, lens, hp)
         assert rel_err(target.numpy(), g[p + "target"]) < 1e-6, (it, "target")
         mask = gp.sequence_mask(lens, x.size(1)).unsqueeze(-1)
         want = float(g[p + "spoof"])
-        assert sro.spoof_count_rnn(ref_d, ys, lens, mask, hp) == want, it
-        assert sro.spoof_count_rnn(ref_d, y_hat_static, lens, mask, hp) == want, it
+        assert gp.spoof_count(ref_d, ys, lens, mask, hp) == want, it
+        assert gp.spoof_count(ref_d, y_hat_static, lens, mask, hp) == want, it
         if it == 0:
             assert 0 < want < sum(lens)                    # the reference D's outputs straddle 0.5
 
