@@ -3,11 +3,12 @@
 // memory, so a phase ends with one read instead of ~10 host reads per batch plus two (B, T, D) copies for
 // compute_distortions.
 //
-// The distortion pass is distortions_partial_kernel's (one warp per frame, same fmaf order, same grid and the same
-// two-stage reduction, so a batch's eight sums are bitwise those of gantts_distortions), except that the target is read
-// from the step's input y (static + dynamic columns) through the static-column map: the fused step never materialises
-// y_static (get_static_features, train.py:528), and the map keeps it that way.  The fold kernel turns the sums into the
-// batch's metrics with the formulas of gantts_b200/metrics.py in fp64 and adds them, with the flagged losses, to the record.
+// The distortion pass is metrics.cu's distortions_partial_kernel on the same grid, and the fold kernel finishes its sums
+// with the same distortions_totals, so a batch's eight sums are bitwise those of gantts_distortions.  The kernel reads the
+// target from the step's input y (static + dynamic columns) through the static-column map: the fused step never
+// materialises y_static (get_static_features, train.py:528), and the map keeps it that way.  The fold kernel turns the
+// sums into the batch's metrics with the formulas of gantts_b200/metrics.py in fp64 and adds them, with the flagged
+// losses, to the record.
 #include "common.cuh"
 
 namespace gantts {
@@ -16,104 +17,15 @@ constexpr int ELOG_FLAGS = GANTTS_LOG_UPDATE_D | GANTTS_LOG_UPDATE_G | GANTTS_LO
 // 10 / ln(10) * sqrt(2) rounded to double: nnmnkwii.metrics.melcd's constant, as gantts_b200/metrics.py computes it
 constexpr double ELOG_LOGDB = 6.141851463713754;
 
-__global__ void __launch_bounds__(MET_THREADS)
-epoch_log_distortions_kernel(const float* __restrict__ y, int64_t y_bs, int64_t y_ts, const float* __restrict__ yh,
-                             int64_t yh_bs, int64_t yh_ts, const int64_t* __restrict__ lengths, int B, int T,
-                             const float* __restrict__ mean, const float* __restrict__ stdv,
-                             const __grid_constant__ gantts_epoch_log_t cfg, MetWs* ws) {
-  __shared__ float sm[4 * 32];
-  __shared__ int ycol[GANTTS_MAX_COLS];
-  for (int i = threadIdx.x; i < cfg.n_static; i += MET_THREADS) ycol[i] = cfg.static_cols[i];
-  __syncthreads();
-  const gantts_distortion_cols_t& c = cfg.cols;
-  float v[MET_NV] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * MET_THREADS + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * MET_THREADS) >> 5;
-  const int64_t frames = (int64_t)B * T;
-  for (int64_t f = warp; f < frames; f += nwarps) {
-    const int b = (int)(f / T), t = (int)(f - (int64_t)b * T);
-    if ((int64_t)t >= lengths[b]) continue;
-    const float* a = y + b * y_bs + t * y_ts;
-    const float* h = yh + b * yh_bs + t * yh_ts;
-    float s0 = 0.f, s1 = 0.f, s2 = 0.f;
-    for (int d = c.mcd_start + lane; d < c.mcd_start + c.mcd_count; d += 32) {
-      const float z = (a[ycol[d]] * stdv[d] + mean[d]) - (h[d] * stdv[d] + mean[d]);
-      s0 = fmaf(z, z, s0);
-    }
-    for (int d = c.bap_start + lane; d < c.bap_start + c.bap_count; d += 32) {
-      const float z = (a[ycol[d]] * stdv[d] + mean[d]) - (h[d] * stdv[d] + mean[d]);
-      s1 = fmaf(z, z, s1);
-    }
-    for (int d = c.mse_start + lane; d < c.mse_start + c.mse_count; d += 32) {
-      const float z = (a[ycol[d]] * stdv[d] + mean[d]) - (h[d] * stdv[d] + mean[d]);
-      s2 = fmaf(z, z, s2);
-    }
-    s0 = warp_sum(s0);
-    s1 = warp_sum(s1);
-    s2 = warp_sum(s2);
-    if (lane == 0) {
-      if (c.mcd_count > 0) v[0] += sqrtf(s0);
-      if (c.bap_count > 0) v[1] += sqrtf(s1);
-      v[6] += s2;
-      v[5] += 1.f;
-      if (c.vuv_col >= 0) {
-        const int k = c.vuv_col;
-        const bool va = a[ycol[k]] * stdv[k] + mean[k] > 0.5f, vh = h[k] * stdv[k] + mean[k] > 0.5f;
-        if (va != vh) v[4] += 1.f;
-        if (va && vh && c.lf0_col >= 0) {
-          const int l = c.lf0_col;
-          float fa = a[ycol[l]] * stdv[l] + mean[l], fh = h[l] * stdv[l] + mean[l];
-          if (c.lf0_linear) {
-            fa = expf(fa);
-            fh = expf(fh);
-          }
-          const float z = fa - fh;
-          v[2] = fmaf(z, z, v[2]);
-          v[3] += 1.f;
-        }
-      }
-    }
-  }
-  float lo4[4] = {v[0], v[1], v[2], v[3]}, hi4[4] = {v[4], v[5], v[6], v[7]};
-  block_sum<4>(lo4, sm);
-  __syncthreads();
-  block_sum<4>(hi4, sm);
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      ws->partial[blockIdx.x][k] = lo4[k];
-      ws->partial[blockIdx.x][4 + k] = hi4[k];
-    }
-  }
-}
-
-// One block: the batch's eight sums (distortions_finish_kernel's reduction, rounded to fp32 like its output), the
+// One block: the batch's eight sums (distortions_totals, rounded to fp32 like distortions_finish_kernel's output), the
 // batch's metrics, and the fold into the record.  nblocks = 0 when the batch logs no distortions.
 __global__ void __launch_bounds__(MET_THREADS)
 epoch_log_fold_kernel(const MetWs* ws, int nblocks, int kind, int flags, const float* __restrict__ losses,
                       const float* __restrict__ spoof, const int64_t* __restrict__ lengths, int B, double* rec) {
-  __shared__ double sm[MET_THREADS / 32][MET_NV];
-  double v[MET_NV] = {0, 0, 0, 0, 0, 0, 0, 0};
-  for (int i = threadIdx.x; i < nblocks; i += MET_THREADS) {
-#pragma unroll
-    for (int k = 0; k < MET_NV; ++k) v[k] += (double)ws->partial[i][k];
-  }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < MET_NV; ++k) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-    if (lane == 0) sm[warp][k] = v[k];
-  }
-  __syncthreads();
+  const double* tot = distortions_totals(ws, nblocks);
   if (threadIdx.x != 0) return;
   double s[MET_NV];
-  for (int k = 0; k < MET_NV; ++k) {
-    double x = 0;
-    for (int w = 0; w < MET_THREADS / 32; ++w) x += sm[w][k];
-    s[k] = (double)(float)x;
-  }
+  for (int k = 0; k < MET_NV; ++k) s[k] = (double)(float)tot[k];
   int64_t frames = 0;
   for (int b = 0; b < B; ++b) frames += lengths[b];
   rec[GANTTS_LOG_N] += 1.0;
@@ -217,11 +129,13 @@ extern "C" int gantts_epoch_log_add(const gantts_epoch_log_t* cfg, int flags, co
   cudaStream_t st = as_stream(stream);
   int nb = 0;
   if (dist) {
-    nb = grid_for((int64_t)B * T * 32, MET_THREADS);
-    if (nb > MET_MAX_BLOCKS) nb = MET_MAX_BLOCKS;
-    epoch_log_distortions_kernel<<<nb, MET_THREADS, 0, st>>>(y, y_bstride, y_tstride, y_hat_static, yh_bstride,
-                                                             yh_tstride, lengths_dev, B, T, mean_dev, std_dev, e, ws);
-    GANTTS_LAUNCH_CHECK("epoch_log_distortions_kernel");
+    ColList ymap;
+    ymap.n = e.n_static;
+    for (int i = 0; i < e.n_static; ++i) ymap.c[i] = e.static_cols[i];
+    nb = distortions_blocks(B, T);
+    distortions_partial_kernel<<<nb, MET_THREADS, 0, st>>>(y, y_bstride, y_tstride, y_hat_static, yh_bstride, yh_tstride,
+                                                           lengths_dev, B, T, mean_dev, std_dev, e.cols, ymap, ws);
+    GANTTS_LAUNCH_CHECK("distortions_partial_kernel");
   }
   epoch_log_fold_kernel<<<1, MET_THREADS, 0, st>>>(ws, nb, e.kind, flags, losses_dev, spoof_dev, lengths_dev, B,
                                                    record_dev);

@@ -40,11 +40,6 @@ enum ScalarSlot {
   S_COUNT = 32
 };
 
-struct ColList {
-  int n;
-  int c[GANTTS_MAX_COLS];
-};
-
 __global__ void gather_cols_list_kernel(const float* __restrict__ in, int64_t in_rs, float* __restrict__ out,
                                         int64_t out_rs, ColList cols, int64_t rows) {
   __shared__ int sc[GANTTS_MAX_COLS];
@@ -146,142 +141,6 @@ enum RedSlot { R_REAL = 0, R_FAKE = 1, R_ADV = 2, R_MGE = 3, R_MSE = 4, R_COUNT 
 struct RedCounts {
   int n[R_COUNT];      // blocks that wrote partials into slot i (0 = slot unused this step)
 };
-
-// Adversarial BCE terms of train.py:262-270,307-308 for one or two halves of a stacked discriminator output, forward
-// sums AND the gradient w.r.t. D in one pass: half 0 = rows [0, M) with kind0, half 1 = rows [M, 2M) with kind1
-// (kind 0: -log(D + eps) * m, correct = D > 0.5; kind 1: -log(1 - D + eps) * m, correct = D < 0.5).  mask is [M] for
-// both halves.  Blocks [0, nbh) serve half 0 and write ws0, blocks [nbh, 2 nbh) serve half 1 and write ws1.
-__global__ void __launch_bounds__(RED_THREADS)
-bce_fwd_bwd_kernel(const float* __restrict__ Dv, const float* __restrict__ mask, int64_t M, int kind0, int kind1,
-                   int nbh, const float* __restrict__ scale, float* __restrict__ gD, RedWs* ws0, RedWs* ws1) {
-  pdl_entry();
-  __shared__ float sm[RED_NV * 32];
-  const int half = blockIdx.x >= nbh ? 1 : 0;
-  const int kind = half ? kind1 : kind0;
-  const int blk = blockIdx.x - half * nbh;
-  const float* d = Dv + (int64_t)half * M;
-  float* g = gD ? gD + (int64_t)half * M : nullptr;
-  const float s = scale[0];
-  float v[RED_NV] = {0.f, 0.f, 0.f, 0.f};
-  for (int64_t i = (int64_t)blk * RED_THREADS + threadIdx.x; i < M; i += (int64_t)nbh * RED_THREADS) {
-    const float dv = d[i], m = mask[i];
-    const float arg = kind == 0 ? (dv + 1e-20f) : (1.f - dv + 1e-20f);
-    v[0] -= logf(arg) * m;
-    const bool hit = kind == 0 ? (dv > 0.5f) : (dv < 0.5f);
-    v[1] += hit ? m : 0.f;
-    v[2] += m;
-    if (g) g[i] = kind == 0 ? (-s * m / (dv + 1e-20f)) : (s * m / (1.f - dv + 1e-20f));
-  }
-  block_sum<RED_NV>(v, sm);
-  if (threadIdx.x == 0) {
-    RedWs* ws = half ? ws1 : ws0;
-#pragma unroll
-    for (int k = 0; k < RED_NV; ++k) ws->partial[blk][k] = v[k];
-  }
-}
-
-// MaskedMSELoss forward sums (gantts/seqloss.py:41-43) AND its gradient 2 * scale * (a m - b m) * m in one pass
-// (ga == nullptr: forward only).  The gradient is STORED (not accumulated): this launch initialises the buffer.
-// bmap.n > 0: column d of the target is column bmap.c[d] of `b` (the static features are read straight out of y:
-// get_static_features of multistream.py:56-79 without materialising y_static).
-__global__ void __launch_bounds__(RED_THREADS)
-sse_fwd_bwd_kernel(const float* __restrict__ a, int64_t a_rs, const float* __restrict__ b, int64_t b_rs,
-                   const float* __restrict__ mask, int64_t rows, int D, const float* __restrict__ scale,
-                   float* __restrict__ ga, int64_t ga_rs, RedWs* ws, ColList bmap) {
-  pdl_entry();
-  __shared__ float sm[RED_NV * 32];
-  __shared__ int sc[GANTTS_MAX_COLS];
-  for (int i = threadIdx.x; i < bmap.n; i += RED_THREADS) sc[i] = bmap.c[i];
-  __syncthreads();
-  const bool mapped = bmap.n > 0;
-  float v[RED_NV] = {0.f, 0.f, 0.f, 0.f};
-  const float s2 = ga ? 2.f * scale[0] : 0.f;
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * RED_THREADS + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * RED_THREADS) >> 5;
-  for (int64_t r = warp; r < rows; r += nwarps) {
-    const float m = mask[r];
-    const float* ar = a + r * a_rs;
-    const float* br = b + r * b_rs;
-#pragma unroll 4
-    for (int d = lane; d < D; d += 32) {
-      const float x = ar[d] * m - br[mapped ? sc[d] : d] * m;
-      v[0] = fmaf(x, x, v[0]);
-      if (ga) ga[r * ga_rs + d] = s2 * x * m;
-    }
-    if (lane == 0) v[1] += m;
-  }
-  block_sum<RED_NV>(v, sm);
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int k = 0; k < RED_NV; ++k) ws->partial[blockIdx.x][k] = v[k];
-  }
-}
-
-// clip_grad_norm_'s coefficient min(1, max_norm / (norm + 1e-6)) with the sum of squares taken from the per-block partials
-// of sumsq_partial_kernel: every block re-reduces the (<= 592) partials itself in the same fixed order, which removes the
-// finish launch; block 0 stores the sum of squares.
-__device__ __forceinline__ float clip_coef(const float* __restrict__ partial, int npartial, float* __restrict__ sumsq_out,
-                                           float max_norm) {
-  __shared__ float sm[32];
-  __shared__ float total_s;
-  float v[1] = {0.f};
-  for (int i = threadIdx.x; i < npartial; i += OPT_THREADS) v[0] += partial[i];
-  block_sum<1>(v, sm);
-  if (threadIdx.x == 0) {
-    total_s = v[0];
-    if (blockIdx.x == 0) sumsq_out[0] = v[0];
-  }
-  __syncthreads();
-  const float total_norm = sqrtf(total_s);
-  const float coef = max_norm / (total_norm + 1e-6f);
-  return coef < 1.f ? coef : 1.f;
-}
-
-// clip_grad_norm_ + Adagrad
-__global__ void __launch_bounds__(OPT_THREADS)
-clip_adagrad_partials_kernel(TensorList tl, const float* __restrict__ partial, int npartial, float* __restrict__ sumsq_out,
-                             float max_norm, float lr, float wd, float eps) {
-  pdl_entry();
-  const float coef = clip_coef(partial, npartial, sumsq_out, max_norm);
-  const int64_t total = tl.off[tl.n];
-  for (int64_t i = (int64_t)blockIdx.x * OPT_THREADS + threadIdx.x; i < total;
-       i += (int64_t)gridDim.x * OPT_THREADS) {
-    int k = find_tensor(tl, i);
-    int64_t j = i - tl.off[k];
-    float g = tl.g[k][j] * coef;
-    tl.g[k][j] = g;
-    float p = tl.p[k][j];
-    g = fmaf(wd, p, g);
-    float s = fmaf(g, g, tl.s[k][j]);
-    tl.s[k][j] = s;
-    tl.p[k][j] = p - lr * g / (sqrtf(s) + eps);
-  }
-}
-
-// The same with torch.optim.Adam (amsgrad off; reference hparams.py:125-130): tl.s = exp_avg, tl.s2 = exp_avg_sq;
-// step_size = lr / (1 - beta1^t), inv_sqrt_bc2 = 1 / sqrt(1 - beta2^t) come from the host.
-__global__ void __launch_bounds__(OPT_THREADS)
-clip_adam_partials_kernel(TensorList tl, const float* __restrict__ partial, int npartial, float* __restrict__ sumsq_out,
-                          float max_norm, float b1, float b2, float wd, float eps, float step_size, float inv_sqrt_bc2) {
-  pdl_entry();
-  const float coef = clip_coef(partial, npartial, sumsq_out, max_norm);
-  const int64_t total = tl.off[tl.n];
-  for (int64_t i = (int64_t)blockIdx.x * OPT_THREADS + threadIdx.x; i < total;
-       i += (int64_t)gridDim.x * OPT_THREADS) {
-    int k = find_tensor(tl, i);
-    int64_t j = i - tl.off[k];
-    float g = tl.g[k][j] * coef;
-    tl.g[k][j] = g;
-    const float p = tl.p[k][j];
-    g = fmaf(wd, p, g);
-    const float m = b1 * tl.s[k][j] + (1.f - b1) * g;
-    const float q = b2 * tl.s2[k][j] + (1.f - b2) * g * g;
-    tl.s[k][j] = m;
-    tl.s2[k][j] = q;
-    tl.p[k][j] = p - step_size * m / (sqrtf(q) * inv_sqrt_bc2 + eps);
-  }
-}
 
 // losses[0..11] = loss_d, loss_fake_d, loss_real_d, loss_mse, loss_mge, loss_adv, loss_g,
 //                 real_correct, fake_correct, frames(local sum of mask), d_grad_norm, g_grad_norm
@@ -534,29 +393,6 @@ static int64_t g_param_count(const gantts_gan_step_t* c) {
   return pl.total;
 }
 
-static inline int bce_blocks(int64_t rows) { return grid_for(rows, RED_THREADS); }
-static inline int sse_blocks(int64_t rows, int D) { return grid_for(rows * D, RED_THREADS * 4); }
-
-// BCE of a stacked discriminator output: halves = 2 -> rows [0,M) kind0 into slot0 and rows [M,2M) kind1 into slot1
-static int launch_bce(const float* Dv, const float* mask, int64_t M, int halves, int kind0, int kind1, const float* scale,
-                      float* gD, RedWs* ws0, RedWs* ws1, cudaStream_t st) {
-  const int nbh = bce_blocks(M);
-  GANTTS_PDL_LAUNCH((bce_fwd_bwd_kernel), nbh * halves, RED_THREADS, 0, st, Dv, mask, M, kind0, kind1, nbh, scale, gD, ws0, ws1);
-  GANTTS_LAUNCH_CHECK("bce_fwd_bwd_kernel");
-  return GANTTS_OK;
-}
-
-static int launch_sse(const float* a, int64_t a_rs, const float* b, int64_t b_rs, const float* mask, int64_t rows, int D,
-                      const float* scale, float* ga, int64_t ga_rs, RedWs* ws, cudaStream_t st,
-                      const ColList* bmap = nullptr) {
-  ColList none;
-  none.n = 0;
-  GANTTS_PDL_LAUNCH((sse_fwd_bwd_kernel), sse_blocks(rows, D), RED_THREADS, 0, st, a, a_rs, b, b_rs, mask, rows, D, scale, ga, ga_rs, ws,
-                                                                 bmap ? *bmap : none);
-  GANTTS_LAUNCH_CHECK("sse_fwd_bwd_kernel");
-  return GANTTS_OK;
-}
-
 // One model's optimiser: the step's top-level fields for the generator, d_opt for the discriminator when it has its own
 struct OptSpec {
   int kind;
@@ -581,11 +417,9 @@ static int clip_opt_model(const gantts_gan_step_t* c, const OptSpec& o, const Pa
   GANTTS_LAUNCH_CHECK("sumsq_partial_kernel");
   if (adam) {
     GANTTS_CHECK_ARG(o.step >= 1, "gan_step: Adam needs opt_step >= 1 (the number of the step being taken)");
-    const double t = (double)o.step;
-    const float step_size = (float)((double)lr / (1.0 - pow((double)o.beta1, t)));
-    const float inv_sqrt_bc2 = (float)(1.0 / sqrt(1.0 - pow((double)o.beta2, t)));
+    const AdamScales a = adam_scales(lr, o.beta1, o.beta2, o.step);
     GANTTS_PDL_LAUNCH((clip_adam_partials_kernel), nb, OPT_THREADS, 0, st, tl, partial, nb, sumsq_out, c->max_norm, o.beta1, o.beta2,
-                      wd, o.eps, step_size, inv_sqrt_bc2);
+                      wd, o.eps, a.step_size, a.inv_sqrt_bc2);
     GANTTS_LAUNCH_CHECK("clip_adam_partials_kernel");
   } else {
     GANTTS_PDL_LAUNCH((clip_adagrad_partials_kernel), nb, OPT_THREADS, 0, st, tl, partial, nb, sumsq_out, c->max_norm, lr, wd, o.eps);
@@ -1683,6 +1517,39 @@ static int check_spoof_d(const gantts_mlp_t* d, int64_t rows) {
   return GANTTS_OK;
 }
 
+// The adversarial columns of y_hat_static the reference discriminator reads: n_adv of them, as many as its input width
+static int spoof_cols(const char* who, const int* adv_cols, int n_adv, int n_static, int d_width, ColList* cols) {
+  GANTTS_CHECK_ARG(n_adv >= 1 && n_adv <= GANTTS_MAX_COLS && n_adv == d_width,
+                   "%s: %d adversarial columns != reference discriminator input width %d (it gets no "
+                   "linguistic conditioning, train.py:554-555)", who, n_adv, d_width);
+  GANTTS_CHECK_ARG(n_static >= 1, "%s: bad n_static", who);
+  cols->n = n_adv;
+  for (int i = 0; i < n_adv; ++i) {
+    GANTTS_CHECK_ARG(adv_cols[i] >= 0 && adv_cols[i] < n_static, "%s: adversarial column %d out of range", who,
+                     adv_cols[i]);
+    cols->c[i] = adv_cols[i];
+  }
+  return GANTTS_OK;
+}
+
+// those columns of y_hat_static's `rows` frames into the operand planes of the discriminator's first layer
+static int spoof_gather(const float* y_hat_static, int n_static, const ColList& cols, int64_t rows, const Planes& in,
+                        cudaStream_t st) {
+  ColList none;
+  none.n = 0;
+  GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(rows * cols.n, 1024), 256, 0, st, y_hat_static, (int64_t)n_static, cols,
+                    rows, nullptr, 0, none, 0, in.hi, in.lo, in.pitch);
+  GANTTS_LAUNCH_CHECK("gather_planes_kernel(spoof)");
+  return GANTTS_OK;
+}
+
+// the threshold count over the discriminator's output dout [B * T]
+static int spoof_threshold(const float* dout, const int64_t* lengths_dev, int B, int T, float* count_dev, cudaStream_t st) {
+  GANTTS_PDL_LAUNCH((spoof_count_kernel), 1, RED_THREADS, 0, st, dout, lengths_dev, B, T, count_dev);
+  GANTTS_LAUNCH_CHECK("spoof_count_kernel");
+  return GANTTS_OK;
+}
+
 extern "C" size_t gantts_spoof_count_workspace_bytes(const gantts_mlp_t* d, int64_t rows) {
   if (check_spoof_d(d, rows)) return 0;
   return al256(gantts_mlp_tape_bytes(d, rows)) + al256((size_t)rows * sizeof(float)) + 256;
@@ -1696,17 +1563,8 @@ extern "C" int gantts_spoof_count(const gantts_mlp_t* d, const float* y_hat_stat
   int rc = check_spoof_d(d, rows);
   if (rc) return rc;
   GANTTS_CHECK_ARG(y_hat_static && adv_cols && lengths_dev && count_dev, "spoof_count: null pointer");
-  GANTTS_CHECK_ARG(n_adv >= 1 && n_adv <= GANTTS_MAX_COLS && n_adv == d->dims[0],
-                   "spoof_count: %d adversarial columns != reference discriminator input width %d (it gets no "
-                   "linguistic conditioning, train.py:554-555)", n_adv, d->dims[0]);
-  GANTTS_CHECK_ARG(n_static >= 1, "spoof_count: bad n_static");
   ColList cols;
-  cols.n = n_adv;
-  for (int i = 0; i < n_adv; ++i) {
-    GANTTS_CHECK_ARG(adv_cols[i] >= 0 && adv_cols[i] < n_static, "spoof_count: adversarial column %d out of range",
-                     adv_cols[i]);
-    cols.c[i] = adv_cols[i];
-  }
+  if ((rc = spoof_cols("spoof_count", adv_cols, n_adv, n_static, d->dims[0], &cols))) return rc;
   const size_t need = gantts_spoof_count_workspace_bytes(d, rows);
   if (!ws || ws_bytes < need) {
     set_error("spoof_count: workspace too small (%zu < %zu)", ws_bytes, need);
@@ -1721,15 +1579,9 @@ extern "C" int gantts_spoof_count(const gantts_mlp_t* d, const float* y_hat_stat
   const cudaStream_t st = as_stream(stream);
   Planes din;
   if ((rc = mlp_tape_input_planes(&m, rows, tape, tape_bytes, &din))) return rc;
-  ColList none;
-  none.n = 0;
-  GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(rows * n_adv, 1024), 256, 0, st, y_hat_static, (int64_t)n_static, cols,
-                    rows, nullptr, 0, none, 0, din.hi, din.lo, din.pitch);
-  GANTTS_LAUNCH_CHECK("gather_planes_kernel(spoof)");
+  if ((rc = spoof_gather(y_hat_static, n_static, cols, rows, din, st))) return rc;
   if ((rc = mlp_fwd_impl(&m, nullptr, 0, rows, dout, 1, tape, tape_bytes, stream, true))) return rc;
-  GANTTS_PDL_LAUNCH((spoof_count_kernel), 1, RED_THREADS, 0, st, dout, lengths_dev, B, T, count_dev);
-  GANTTS_LAUNCH_CHECK("spoof_count_kernel");
-  return GANTTS_OK;
+  return spoof_threshold(dout, lengths_dev, B, T, count_dev, st);
 }
 
 // ---- the same count with a recurrent reference discriminator (LSTMRNN / GRURNN with last_sigmoid, train.py:779-781
@@ -1799,17 +1651,8 @@ extern "C" int gantts_spoof_count_lstm(const gantts_lstm_stack_t* ls, const floa
                    "spoof_count_lstm: %d LSTM tensors, the stack has %d (W_ih, W_hh, b_ih, b_hh per layer and direction)",
                    n_tensors, want);
   for (int i = 0; i < n_tensors; ++i) GANTTS_CHECK_ARG(lstm_tensors[i], "spoof_count_lstm: null pointer (LSTM tensor %d)", i);
-  GANTTS_CHECK_ARG(n_adv >= 1 && n_adv <= GANTTS_MAX_COLS && n_adv == ls->in_dim,
-                   "spoof_count_lstm: %d adversarial columns != reference discriminator input width %d (it gets no "
-                   "linguistic conditioning, train.py:554-555)", n_adv, ls->in_dim);
-  GANTTS_CHECK_ARG(n_static >= 1, "spoof_count_lstm: bad n_static");
   ColList cols;
-  cols.n = n_adv;
-  for (int i = 0; i < n_adv; ++i) {
-    GANTTS_CHECK_ARG(adv_cols[i] >= 0 && adv_cols[i] < n_static, "spoof_count_lstm: adversarial column %d out of range",
-                     adv_cols[i]);
-    cols.c[i] = adv_cols[i];
-  }
+  if ((rc = spoof_cols("spoof_count_lstm", adv_cols, n_adv, n_static, ls->in_dim, &cols))) return rc;
   const size_t need = gantts_spoof_count_lstm_workspace_bytes(ls, head, B, T);
   if (!ws || ws_bytes < need) {
     set_error("spoof_count_lstm: workspace too small (%zu < %zu)", ws_bytes, need);
@@ -1830,17 +1673,10 @@ extern "C" int gantts_spoof_count_lstm(const gantts_lstm_stack_t* ls, const floa
   gantts_mlp_t m = *head;
   m.dropout_p = 0.f;
   const cudaStream_t st = as_stream(stream);
-  const Planes in0 = lstm_in_planes(k, 0, rows);
-  ColList none;
-  none.n = 0;
-  GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(rows * n_adv, 1024), 256, 0, st, y_hat_static, (int64_t)n_static, cols,
-                    rows, nullptr, 0, none, 0, in0.hi, in0.lo, in0.pitch);
-  GANTTS_LAUNCH_CHECK("gather_planes_kernel(spoof lstm)");
+  if ((rc = spoof_gather(y_hat_static, n_static, cols, rows, lstm_in_planes(k, 0, rows), st))) return rc;
   Planes top;
   if ((rc = mlp_tape_input_planes(&m, rows, L.tape, L.tape_bytes, &top))) return rc;
   if ((rc = lstm_stack_fwd(k, nullptr, 0, top, lengths_dev, B, T, 0, false, st))) return rc;
   if ((rc = mlp_fwd_impl(&m, nullptr, 0, rows, L.dout, 1, L.tape, L.tape_bytes, stream, true))) return rc;
-  GANTTS_PDL_LAUNCH((spoof_count_kernel), 1, RED_THREADS, 0, st, L.dout, lengths_dev, B, T, count_dev);
-  GANTTS_LAUNCH_CHECK("spoof_count_kernel");
-  return GANTTS_OK;
+  return spoof_threshold(L.dout, lengths_dev, B, T, count_dev, st);
 }

@@ -1,7 +1,10 @@
 // Sequence mask, masked MSE, masked adversarial BCE and stream column gathers.
 // HBM-bound streaming kernels: one pass over the operands, deterministic two-stage reductions
 // (per-block partials in the caller's workspace, then a single-block finish), grid sized to a
-// multiple of the SM count.
+// multiple of the SM count.  sse_fwd_bwd_kernel and bce_fwd_bwd_kernel are the one MaskedMSE and BCE forward of the
+// library: the modular ops launch them for the sums alone and finish with reduce_finish_kernel; the fused step
+// (gan_step.cu) launches them through launch_sse / launch_bce for the sums and the gradient, and reduces the partials
+// in its finalize kernel.
 #include "common.cuh"
 
 namespace gantts {
@@ -23,15 +26,30 @@ __global__ void sequence_mask_kernel(const int64_t* __restrict__ lengths, float*
   mask[i] = (int64_t)t < lengths[b] ? 1.f : 0.f;
 }
 
-// reference gantts/seqloss.py:41-43: criterion(input * mask_, target * mask_) summed, / mask.sum().
-// (a*m - b*m)^2 is evaluated exactly like that (two products, one subtraction, one square).
+// Column map of a stream: up to GANTTS_MAX_COLS column indices passed by value (n = 0: no map).
+struct ColList {
+  int n;
+  int c[GANTTS_MAX_COLS];
+};
+
+// MaskedMSELoss forward sums (reference gantts/seqloss.py:41-43: criterion(input * mask_, target * mask_) summed,
+// / mask.sum()) AND its gradient 2 * scale * (a m - b m) * m in one pass; (a*m - b*m)^2 is evaluated exactly like that
+// (two products, one subtraction, one square).  ga == nullptr: sums only, scale is not read.  The gradient is STORED (not
+// accumulated): this launch initialises the buffer.  bmap.n > 0: column d of the target is column bmap.c[d] of `b` (the
+// fused step reads the static features straight out of y: get_static_features of multistream.py:56-79 without
+// materialising y_static).  One warp per row (lanes stride over the columns: coalesced, no integer division).
 __global__ void __launch_bounds__(RED_THREADS)
-masked_sse_partial_kernel(const float* __restrict__ a, int64_t a_rs, const float* __restrict__ b,
-                          int64_t b_rs, const float* __restrict__ mask, int64_t rows, int D,
-                          RedWs* ws) {
+sse_fwd_bwd_kernel(const float* __restrict__ a, int64_t a_rs, const float* __restrict__ b, int64_t b_rs,
+                   const float* __restrict__ mask, int64_t rows, int D, const float* __restrict__ scale,
+                   float* __restrict__ ga, int64_t ga_rs, RedWs* ws, ColList bmap) {
+  pdl_entry();
   __shared__ float sm[RED_NV * 32];
+  __shared__ int sc[GANTTS_MAX_COLS];
+  for (int i = threadIdx.x; i < bmap.n; i += RED_THREADS) sc[i] = bmap.c[i];
+  __syncthreads();
+  const bool mapped = bmap.n > 0;
   float v[RED_NV] = {0.f, 0.f, 0.f, 0.f};
-  // one warp per row (lanes stride over the columns: coalesced, no integer division)
+  const float s2 = ga ? 2.f * scale[0] : 0.f;
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * RED_THREADS + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * RED_THREADS) >> 5;
@@ -41,8 +59,9 @@ masked_sse_partial_kernel(const float* __restrict__ a, int64_t a_rs, const float
     const float* br = b + r * b_rs;
 #pragma unroll 4
     for (int d = lane; d < D; d += 32) {
-      const float x = ar[d] * m - br[d] * m;
+      const float x = ar[d] * m - br[mapped ? sc[d] : d] * m;
       v[0] = fmaf(x, x, v[0]);
+      if (ga) ga[r * ga_rs + d] = s2 * x * m;
     }
     if (lane == 0) v[1] += m;
   }
@@ -88,25 +107,37 @@ masked_sse_bwd_kernel(const float* __restrict__ a, int64_t a_rs, const float* __
   }
 }
 
-// reference train.py:262,266,269-270,307-308.  logf (not __logf) to stay within 1e-6 of torch.
+// Adversarial BCE terms of reference train.py:262-270,307-308 for one or two halves of a stacked discriminator output,
+// forward sums AND the gradient w.r.t. D in one pass: half 0 = rows [0, M) with kind0, half 1 = rows [M, 2M) with kind1
+// (kind 0: -log(D + eps) * m, correct = D > 0.5; kind 1: -log(1 - D + eps) * m, correct = D < 0.5).  mask is [M] for
+// both halves.  Blocks [0, nbh) serve half 0 and write ws0, blocks [nbh, 2 nbh) serve half 1 and write ws1.
+// gD == nullptr: sums only, scale is not read.  logf (not __logf) to stay within 1e-6 of torch.
 __global__ void __launch_bounds__(RED_THREADS)
-masked_bce_partial_kernel(const float* __restrict__ Dv, const float* __restrict__ mask, int64_t rows,
-                          int kind, RedWs* ws) {
+bce_fwd_bwd_kernel(const float* __restrict__ Dv, const float* __restrict__ mask, int64_t M, int kind0, int kind1,
+                   int nbh, const float* __restrict__ scale, float* __restrict__ gD, RedWs* ws0, RedWs* ws1) {
+  pdl_entry();
   __shared__ float sm[RED_NV * 32];
+  const int half = blockIdx.x >= nbh ? 1 : 0;
+  const int kind = half ? kind1 : kind0;
+  const int blk = blockIdx.x - half * nbh;
+  const float* d = Dv + (int64_t)half * M;
+  float* g = gD ? gD + (int64_t)half * M : nullptr;
+  const float s = g ? scale[0] : 0.f;
   float v[RED_NV] = {0.f, 0.f, 0.f, 0.f};
-  for (int64_t i = (int64_t)blockIdx.x * RED_THREADS + threadIdx.x; i < rows;
-       i += (int64_t)gridDim.x * RED_THREADS) {
-    float d = Dv[i], m = mask[i];
-    float arg = kind == 0 ? (d + 1e-20f) : (1.f - d + 1e-20f);
+  for (int64_t i = (int64_t)blk * RED_THREADS + threadIdx.x; i < M; i += (int64_t)nbh * RED_THREADS) {
+    const float dv = d[i], m = mask[i];
+    const float arg = kind == 0 ? (dv + 1e-20f) : (1.f - dv + 1e-20f);
     v[0] -= logf(arg) * m;
-    bool hit = kind == 0 ? (d > 0.5f) : (d < 0.5f);
+    const bool hit = kind == 0 ? (dv > 0.5f) : (dv < 0.5f);
     v[1] += hit ? m : 0.f;
     v[2] += m;
+    if (g) g[i] = kind == 0 ? (-s * m / (dv + 1e-20f)) : (s * m / (1.f - dv + 1e-20f));
   }
   block_sum<RED_NV>(v, sm);
   if (threadIdx.x == 0) {
+    RedWs* ws = half ? ws1 : ws0;
 #pragma unroll
-    for (int k = 0; k < RED_NV; ++k) ws->partial[blockIdx.x][k] = v[k];
+    for (int k = 0; k < RED_NV; ++k) ws->partial[blk][k] = v[k];
   }
 }
 
@@ -147,6 +178,30 @@ static inline int grid_for(int64_t work, int threads) {
   return (int)b;
 }
 
+static inline int bce_blocks(int64_t rows) { return grid_for(rows, RED_THREADS); }
+static inline int sse_blocks(int64_t rows, int D) { return grid_for(rows * D, RED_THREADS * 4); }
+
+// The fused step's launches.  BCE of a stacked discriminator output: halves = 2 -> rows [0,M) kind0 into slot0 and rows
+// [M,2M) kind1 into slot1
+static int launch_bce(const float* Dv, const float* mask, int64_t M, int halves, int kind0, int kind1, const float* scale,
+                      float* gD, RedWs* ws0, RedWs* ws1, cudaStream_t st) {
+  const int nbh = bce_blocks(M);
+  GANTTS_PDL_LAUNCH((bce_fwd_bwd_kernel), nbh * halves, RED_THREADS, 0, st, Dv, mask, M, kind0, kind1, nbh, scale, gD, ws0, ws1);
+  GANTTS_LAUNCH_CHECK("bce_fwd_bwd_kernel");
+  return GANTTS_OK;
+}
+
+static int launch_sse(const float* a, int64_t a_rs, const float* b, int64_t b_rs, const float* mask, int64_t rows, int D,
+                      const float* scale, float* ga, int64_t ga_rs, RedWs* ws, cudaStream_t st,
+                      const ColList* bmap = nullptr) {
+  ColList none;
+  none.n = 0;
+  GANTTS_PDL_LAUNCH((sse_fwd_bwd_kernel), sse_blocks(rows, D), RED_THREADS, 0, st, a, a_rs, b, b_rs, mask, rows, D, scale, ga, ga_rs, ws,
+                                                                 bmap ? *bmap : none);
+  GANTTS_LAUNCH_CHECK("sse_fwd_bwd_kernel");
+  return GANTTS_OK;
+}
+
 }  // namespace gantts
 
 using namespace gantts;
@@ -169,10 +224,13 @@ extern "C" int gantts_masked_sse_fwd(const float* a, int64_t a_rs, const float* 
     set_error("masked_sse_fwd: workspace too small (%zu < %zu)", workspace_bytes, sizeof(RedWs));
     return GANTTS_E_WORKSPACE;
   }
-  int nb = grid_for(rows * D, RED_THREADS * 4);
+  const int nb = sse_blocks(rows, D);
   RedWs* ws = static_cast<RedWs*>(workspace);
-  masked_sse_partial_kernel<<<nb, RED_THREADS, 0, as_stream(stream)>>>(a, a_rs, b, b_rs, mask, rows, D, ws);
-  GANTTS_LAUNCH_CHECK("masked_sse_partial_kernel");
+  ColList none;
+  none.n = 0;
+  sse_fwd_bwd_kernel<<<nb, RED_THREADS, 0, as_stream(stream)>>>(a, a_rs, b, b_rs, mask, rows, D, nullptr, nullptr, 0, ws,
+                                                                none);
+  GANTTS_LAUNCH_CHECK("sse_fwd_bwd_kernel");
   reduce_finish_kernel<<<1, RED_THREADS, 0, as_stream(stream)>>>(ws, nb, sums_dev, 2);
   GANTTS_LAUNCH_CHECK("reduce_finish_kernel");
   return GANTTS_OK;
@@ -199,10 +257,11 @@ extern "C" int gantts_masked_bce_fwd(const float* D, const float* mask, int64_t 
     set_error("masked_bce_fwd: workspace too small");
     return GANTTS_E_WORKSPACE;
   }
-  int nb = grid_for(rows, RED_THREADS);
+  const int nb = bce_blocks(rows);
   RedWs* ws = static_cast<RedWs*>(workspace);
-  masked_bce_partial_kernel<<<nb, RED_THREADS, 0, as_stream(stream)>>>(D, mask, rows, kind, ws);
-  GANTTS_LAUNCH_CHECK("masked_bce_partial_kernel");
+  bce_fwd_bwd_kernel<<<nb, RED_THREADS, 0, as_stream(stream)>>>(D, mask, rows, kind, kind, nb, nullptr, nullptr, ws,
+                                                                nullptr);
+  GANTTS_LAUNCH_CHECK("bce_fwd_bwd_kernel");
   reduce_finish_kernel<<<1, RED_THREADS, 0, as_stream(stream)>>>(ws, nb, out_dev, 3);
   GANTTS_LAUNCH_CHECK("reduce_finish_kernel");
   return GANTTS_OK;
