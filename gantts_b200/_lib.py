@@ -133,6 +133,7 @@ class EpochLogT(ctypes.Structure):
 
 
 OPT_ADAGRAD, OPT_ADAM = 0, 1
+GANTTS_E_BADARG = 1
 
 _lib = None
 
@@ -162,6 +163,9 @@ SIGNATURES = {
     "gantts_mlpg_var_workspace_bytes": (_sz, [ctypes.POINTER(WindowsT), _i, _i, _i]),
     "gantts_mlpg_var": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i64, ctypes.POINTER(WindowsT),
                              _i, _i, _i, _vp, _sz, _vp]),
+    "gantts_mlpg_ragged_workspace_bytes": (_sz, [ctypes.POINTER(StreamsT), ctypes.POINTER(WindowsT), _vp, _i, _i]),
+    "gantts_mlpg_ragged": (_i, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, ctypes.POINTER(StreamsT),
+                                ctypes.POINTER(WindowsT), _vp, _i, _i, _vp, _sz, _vp]),
     "gantts_distortions_workspace_bytes": (_sz, []),
     "gantts_distortions": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp,
                                 ctypes.POINTER(DistortionColsT), _vp, _vp, _sz, _vp]),
@@ -201,6 +205,7 @@ SIGNATURES = {
     "gantts_dropout": (_i, [_vp, _vp, _i64, _i, _f, _u64, _vp]),
     "gantts_sru_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "gantts_sru_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "gantts_sru_fwd_lengths": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "gantts_optim_workspace_bytes": (_sz, []),
     "gantts_grad_sumsq": (_i, [_vp, _vp, _i, _vp, _vp, _sz, _vp]),
     "gantts_clip_adagrad_step": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _f, _f, _f, _f, _vp]),

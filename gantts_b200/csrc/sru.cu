@@ -21,6 +21,7 @@ struct SruParams {
   float* du;            // bwd [B][T][ncols*k]
   float* dx;            // bwd [B][T][ncols] (+=) when k == 3
   float* dbias_part;    // bwd [B][2*ncols]
+  const int64_t* lengths;  // fwd with lengths [B]
   int B, T, d, k, bidir, act;   // act: 0 identity, 1 tanh, 2 relu
 };
 
@@ -35,8 +36,12 @@ __device__ __forceinline__ float sru_dact(float c, float val, int act) {
 // steps are processed in chunks of SRU_UNR: all loads of a chunk are issued first (independent, SRU_UNR deep
 // per thread), then the recurrence runs on registers.
 constexpr int SRU_UNR = 8;
+constexpr int SRU_MAX_T = 1 << 24;   // of gantts_sru_fwd_lengths
 
-template <int K>
+// LEN = false: gantts_sru_fwd, every sequence runs over the padded T (the reverse direction starts at T - 1) and the
+// cell states are saved.  LEN = true: gantts_sru_fwd_lengths, sequence b runs over its own L = lengths[b] frames (the
+// reverse direction starts at L - 1 with a zero cell), h is 0 at and beyond L, and no cell state is kept.
+template <int K, bool LEN>
 __global__ void __launch_bounds__(128) sru_fwd_kernel(const SruParams p) {
   const int ncols = p.d * (p.bidir ? 2 : 1);
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -44,17 +49,23 @@ __global__ void __launch_bounds__(128) sru_fwd_kernel(const SruParams p) {
   const int b = idx / ncols, col = idx - b * ncols;
   const bool rev = p.bidir && col >= p.d;
   const float bf = p.bias[col], br = p.bias[col + ncols];
-  const float m = p.mask_h ? p.mask_h[idx] : 1.f;
+  const float m = (!LEN && p.mask_h) ? p.mask_h[idx] : 1.f;    // eval mode: no mask
+  int L = p.T;
   const int64_t base = (int64_t)b * p.T * ncols + col;       // element (b, t = 0, col)
+  if (LEN) {
+    const int64_t l = p.lengths[b];
+    L = l < 0 ? 0 : (l > p.T ? p.T : (int)l);
+    for (int t = L; t < p.T; ++t) p.h[base + (int64_t)t * ncols] = 0.f;
+  }
   const int64_t tstep = rev ? -(int64_t)ncols : (int64_t)ncols;
-  const int64_t first = rev ? base + (int64_t)(p.T - 1) * ncols : base;
+  const int64_t first = rev ? base + (int64_t)(L - 1) * ncols : base;
   float c = 0.f;
-  for (int s0 = 0; s0 < p.T; s0 += SRU_UNR) {
+  for (int s0 = 0; s0 < L; s0 += SRU_UNR) {
     float u0[SRU_UNR], u1[SRU_UNR], u2[SRU_UNR], xp[SRU_UNR];
 #pragma unroll
     for (int j = 0; j < SRU_UNR; ++j) {
       u0[j] = u1[j] = u2[j] = xp[j] = 0.f;
-      if (s0 + j < p.T) {
+      if (s0 + j < L) {
         const int64_t e = first + (int64_t)(s0 + j) * tstep;
         if (K == 4) {
           const float4 v = __ldg(reinterpret_cast<const float4*>(p.u + e * 4));
@@ -68,12 +79,12 @@ __global__ void __launch_bounds__(128) sru_fwd_kernel(const SruParams p) {
     }
 #pragma unroll
     for (int j = 0; j < SRU_UNR; ++j) {
-      if (s0 + j < p.T) {
+      if (s0 + j < L) {
         const int64_t e = first + (int64_t)(s0 + j) * tstep;
         const float g1 = 1.f / (1.f + expf(-(u1[j] + bf)));
         const float g2 = 1.f / (1.f + expf(-(u2[j] + br)));
         c = (c - u0[j]) * g1 + u0[j];
-        p.c[e] = c;
+        if (!LEN) p.c[e] = c;
         const float val = sru_act(c, p.act);
         p.h[e] = (val * m - xp[j]) * g2 + xp[j];
       }
@@ -407,9 +418,28 @@ extern "C" int gantts_sru_fwd(const float* u, const float* x, const float* bias,
   if (rc) return rc;
   GANTTS_CHECK_ARG(h && c, "sru_fwd: null output");
   const int n = B * d * (bidir ? 2 : 1);
-  if (k == 4) sru_fwd_kernel<4><<<(n + 127) / 128, 128, 0, as_stream(stream)>>>(p);
-  else sru_fwd_kernel<3><<<(n + 127) / 128, 128, 0, as_stream(stream)>>>(p);
+  if (k == 4) sru_fwd_kernel<4, false><<<(n + 127) / 128, 128, 0, as_stream(stream)>>>(p);
+  else sru_fwd_kernel<3, false><<<(n + 127) / 128, 128, 0, as_stream(stream)>>>(p);
   GANTTS_LAUNCH_CHECK("sru_fwd_kernel");
+  return GANTTS_OK;
+}
+
+extern "C" int gantts_sru_fwd_lengths(const float* u, const float* x, const float* bias, const int64_t* lengths_dev,
+                                      float* h, int B, int T, int d, int k, int bidir, int act, void* stream) {
+  SruParams p{};
+  p.u = u; p.x = x; p.bias = bias; p.h = h; p.lengths = lengths_dev;
+  p.B = B; p.T = T; p.d = d; p.k = k; p.bidir = bidir ? 1 : 0; p.act = act;
+  GANTTS_CHECK_ARG(lengths_dev, "sru_fwd_lengths: null lengths: sequence b runs over its own lengths_dev[b] frames");
+  GANTTS_CHECK_ARG(T >= 1 && T <= SRU_MAX_T, "sru_fwd_lengths: padded length T = %d must be in [1, %d]", T, SRU_MAX_T);
+  GANTTS_CHECK_ARG(B >= 1 && d >= 1 && (int64_t)B * d * (bidir ? 2 : 1) <= ((int64_t)1 << 30),
+                   "sru_fwd_lengths: B = %d and d = %d must be >= 1 with B * columns <= 2^30", B, d);
+  int rc = sru_check(p);
+  if (rc) return rc;
+  GANTTS_CHECK_ARG(h, "sru_fwd_lengths: null output");
+  const int n = B * d * (bidir ? 2 : 1);
+  if (k == 4) sru_fwd_kernel<4, true><<<(n + 127) / 128, 128, 0, as_stream(stream)>>>(p);
+  else sru_fwd_kernel<3, true><<<(n + 127) / 128, 128, 0, as_stream(stream)>>>(p);
+  GANTTS_LAUNCH_CHECK("sru_fwd_lengths_kernel");
   return GANTTS_OK;
 }
 

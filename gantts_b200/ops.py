@@ -238,6 +238,50 @@ def mlpg_var(mean, variance, windows):
     return out.squeeze(0) if squeeze else out
 
 
+def _column_vector(v, n, device, what):
+    """None, or `v` as a contiguous float32 CUDA vector of n values."""
+    if v is None:
+        return None
+    v = torch.as_tensor(v, dtype=torch.float32, device=device).reshape(-1).contiguous()
+    if v.numel() != n:
+        raise RuntimeError("gantts_b200: %s has %d values, expected %d" % (what, v.numel(), n))
+    return v
+
+
+def mlpg_ragged(x, lengths, windows, stream_entries, ncols_out, var=None, in_affine=None, out_affine=None):
+    """Length-exact multi-stream MLPG of generation (gantts_mlpg_ragged): row b of the padded batch x (B, T, D) CUDA
+    float32 is solved over its own lengths[b] frames (int64 CUDA (B,)), as the evaluation scripts solve each utterance
+    alone; frames at or beyond lengths[b] are 0.  stream_entries: [(in_start, sd, dyn, out_start)], static-only streams
+    pass through.  var: (D,) time-invariant variances or None (unit).  in_affine / out_affine: (scale, shift) over the
+    input columns (applied before the solve) / the ncols_out output columns (after it), or None.  No host sync."""
+    require_cuda(x)
+    lib = _lib.load()
+    if not (torch.is_tensor(lengths) and lengths.is_cuda and lengths.dtype == torch.int64):
+        raise RuntimeError("gantts_b200: mlpg_ragged needs int64 CUDA lengths")
+    B, T, D = x.shape
+    if x.stride(2) != 1:
+        x = x.contiguous()
+    lengths = lengths.contiguous()
+    dev = x.device
+    var = _column_vector(var, D, dev, "var")
+    isc, ish = (None, None) if in_affine is None else (_column_vector(in_affine[0], D, dev, "input scale"),
+                                                      _column_vector(in_affine[1], D, dev, "input shift"))
+    osc, osh = (None, None) if out_affine is None else (_column_vector(out_affine[0], ncols_out, dev, "output scale"),
+                                                       _column_vector(out_affine[1], ncols_out, dev, "output shift"))
+    s, w = _lib.make_streams(stream_entries), _lib.make_windows(windows)
+    nbytes = lib.gantts_mlpg_ragged_workspace_bytes(ctypes.byref(s), ctypes.byref(w), lengths.data_ptr(), B, T)
+    if nbytes == 0:
+        _lib.check(_lib.GANTTS_E_BADARG)
+    ws = workspace(nbytes, dev, "mlpg_ragged")
+    out = torch.empty(B, T, ncols_out, dtype=torch.float32, device=dev)
+    ptr = lambda t: t.data_ptr() if t is not None else None
+    _lib.check(lib.gantts_mlpg_ragged(x.data_ptr(), x.stride(0), x.stride(1), ptr(var), ptr(isc), ptr(ish),
+                                      out.data_ptr(), out.stride(0), out.stride(1), ptr(osc), ptr(osh),
+                                      ctypes.byref(s), ctypes.byref(w), lengths.data_ptr(), B, T, ws.data_ptr(),
+                                      ws.numel(), _stream()))
+    return out
+
+
 def distortion_sums(y, y_hat, lengths, mean, std, mcd=(0, 0), bap=(0, 0), lf0_col=-1, vuv_col=-1,
                     lf0_linear=True, mse=(0, 0)):
     """Eight sums behind the objective metrics of reference train.py:399-432 (see include/gantts_b200.h,

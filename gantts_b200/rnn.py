@@ -201,10 +201,14 @@ class SRUCell(torch.nn.Module):
         val_range = (3.0 / n_in) ** 0.5
         torch.nn.init.uniform_(self.weight, -val_range, val_range)
 
-    def forward(self, x, engine=None):
-        """x: (B, T, n_in) -> (B, T, dirs*n_out)."""
+    def forward(self, x, engine=None, lengths=None):
+        """x: (B, T, n_in) -> (B, T, dirs*n_out).  lengths: None (every sequence runs over the padded T, like the
+        upstream SRU), or int64 CUDA (B,) in eval mode: sequence b runs over its own lengths[b] frames, its reverse
+        direction starts at lengths[b] - 1, and h is 0 beyond (gantts_sru_fwd_lengths; forward only)."""
         B, T, _ = x.shape
         ncols = self.n_out * (2 if self.bidirectional else 1)
+        if lengths is not None:
+            return self._forward_lengths(x, lengths, engine)
         # upstream cuda_functional.SRUCell.forward: only the GEMM input is masked (u = (input * mask_x) @ W); the
         # highway term (1 - r) * x of SRU_Compute receives the UNMASKED input.
         x_in = x
@@ -220,6 +224,25 @@ class SRUCell(torch.nn.Module):
                               self.activation_type)
 
 
+    def _forward_lengths(self, x, lengths, engine):
+        if self.training or torch.is_grad_enabled() and (x.requires_grad or self.weight.requires_grad):
+            raise RuntimeError("gantts_b200: the SRU forward with lengths is eval-only and has no backward: call it in "
+                               "eval mode under torch.no_grad()")
+        if not (torch.is_tensor(lengths) and lengths.is_cuda and lengths.dtype == torch.int64):
+            raise RuntimeError("gantts_b200: the SRU forward with lengths needs int64 CUDA lengths")
+        lib = _lib.load()
+        B, T, _ = x.shape
+        ncols = self.n_out * (2 if self.bidirectional else 1)
+        u = ops.linear_act(x, self.weight.t().contiguous(), None, _lib.ACT_NONE, engine=engine).contiguous()
+        xh = x.contiguous() if self.k == 3 else None
+        h = torch.empty(B, T, ncols, dtype=torch.float32, device=x.device)
+        _lib.check(lib.gantts_sru_fwd_lengths(u.data_ptr(), xh.data_ptr() if xh is not None else None,
+                                              self.bias.data_ptr(), lengths.contiguous().data_ptr(), h.data_ptr(),
+                                              B, T, self.n_out, self.k, int(self.bidirectional),
+                                              self.activation_type, ops._stream()))
+        return h
+
+
 class SRU(torch.nn.Module):
     """Stack of SRU layers (``rnn_lst``) like upstream ``cuda_functional.SRU``; batch-first here."""
 
@@ -233,7 +256,8 @@ class SRU(torch.nn.Module):
                                         dropout=dropout if i + 1 != num_layers else 0.0, rnn_dropout=rnn_dropout,
                                         bidirectional=bidirectional, use_tanh=use_tanh, use_relu=use_relu))
 
-    def forward(self, x, engine=None):
+    def forward(self, x, engine=None, lengths=None):
+        """lengths: see SRUCell.forward (None: the padded semantics of the reference's SRURNN, used in training)."""
         for cell in self.rnn_lst:
-            x = cell(x, engine=engine)
+            x = cell(x, engine=engine, lengths=lengths)
         return x

@@ -299,6 +299,15 @@ int gantts_sru_fwd(const float* u, const float* x, const float* bias, const floa
 int gantts_sru_bwd(const float* u, const float* x, const float* bias, const float* mask_h, const float* c,
                    const float* dh, float* du, float* dx, float* dbias_part, int B, int T, int d, int k,
                    int bidir, int act, void* stream);
+/* Length-exact SRU forward of generation (replaces the SRU stack of reference gantts/models.py:162-165 SRURNN.forward as
+ * evaluation_tts.py:167,221 run it: one utterance at B = 1 and T = its own length).  gantts_sru_fwd in eval mode (no
+ * dropout mask, no cell states kept) except that sequence b runs over its own L = lengths_dev[b] frames (int64[B], clamped
+ * to [0, T]): the reverse direction starts at frame L - 1 with a zero cell, and h is 0 at and beyond L.  So each row
+ * equals gantts_sru_fwd of that sequence alone at T = L, and nothing in it depends on the padding.  With every length
+ * equal to T the output is bit for bit gantts_sru_fwd's h.  gantts_sru_fwd keeps the reference's padded semantics
+ * (training).  Rules, checked before any device work: lengths_dev non-null, 1 <= T <= 2^24, B, d >= 1. */
+int gantts_sru_fwd_lengths(const float* u, const float* x, const float* bias, const int64_t* lengths_dev, float* h,
+                           int B, int T, int d, int k, int bidir, int act, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Fused GAN training step: one call enqueues the whole mini-batch of reference train.py:528-580
@@ -544,6 +553,31 @@ int gantts_mlpg_var(const float* mean, int64_t m_bstride, int64_t m_tstride, con
                     int64_t v_bstride, int64_t v_tstride, float* out, int64_t o_bstride, int64_t o_tstride,
                     const gantts_windows_t* windows, int B, int T, int sd, void* workspace,
                     size_t workspace_bytes, void* stream);
+
+/* Length-exact multi-stream MLPG of generation (replaces, per utterance, the parameter generation of reference
+ * evaluation_vc.py:70,74-89 -- unit_variance_mlpg_matrix(hp.windows, T) with multi_stream_mlpg, then inv_scale -- and
+ * evaluation_tts.py:62-98 gen_parameters, both branches).  Row b is solved over its own L = lengths_dev[b] frames
+ * (int64[B], clamped to [0, T]) by the banded Cholesky of gantts_mlpg_var: W^T P W has its end boundary at L, so the row
+ * equals the evaluation scripts' solve of that utterance alone at T = L.  Frames at or beyond L are written as 0.
+ *   in  float32 [B][T][*], element strides (in_bstride, in_tstride); the stream table gives the columns as for
+ *       gantts_mlpg_fwd.  Dynamic streams are solved; static-only streams (dyn = 0, e.g. vuv) are passed through.
+ *   var [input columns]: time-invariant variance per input column (evaluation_tts.py:95-98 Y_var = Y_std**2), or NULL for
+ *       unit variance (:71-74, evaluation_vc.py:70).
+ *   in_scale / in_shift [input columns], or both NULL: x * in_scale + in_shift as each mean is read, BEFORE the solve
+ *       (the non-MGE branch's inv_scale, evaluation_tts.py:86).
+ *   out_scale / out_shift [output columns], or both NULL: y * out_scale + out_shift as each frame is stored, AFTER the
+ *       solve (the MGE branch's inv_scale, evaluation_tts.py:77-83; evaluation_vc.py:88-89).
+ *   out float32 [B][T][*], strides (out_bstride, out_tstride): stream s's static part in [out_start, out_start + sd).
+ * The affine maps and the solve run in double.  Workspace: gantts_mlpg_ragged_workspace_bytes (0 = rejected, the error
+ * string names the rule): lengths_dev non-null, B >= 1, 1 <= T <= 2^24, 1..GANTTS_MAX_STREAMS streams of static width
+ * sd in [1, GANTTS_MAX_COLS], 1..GANTTS_MAX_WINDOWS windows of at most GANTTS_MAX_WINDOW_TAPS taps. */
+size_t gantts_mlpg_ragged_workspace_bytes(const gantts_streams_t* streams, const gantts_windows_t* windows,
+                                          const int64_t* lengths_dev, int B, int T);
+int gantts_mlpg_ragged(const float* in, int64_t in_bstride, int64_t in_tstride, const float* var, const float* in_scale,
+                       const float* in_shift, float* out, int64_t out_bstride, int64_t out_tstride,
+                       const float* out_scale, const float* out_shift, const gantts_streams_t* streams,
+                       const gantts_windows_t* windows, const int64_t* lengths_dev, int B, int T, void* workspace,
+                       size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Objective distortions of the training loop (reference train.py:399-432 compute_distortions, :383-396
