@@ -133,6 +133,7 @@ class EpochLogT(ctypes.Structure):
 
 
 OPT_ADAGRAD, OPT_ADAM = 0, 1
+MCEP_R0, MCEP_SP = 0, 1     # GANTTS_MCEP_*: merlin_post_filter's energy operator, mc2sp's
 GANTTS_E_BADARG = 1
 
 _lib = None
@@ -166,6 +167,9 @@ SIGNATURES = {
     "gantts_mlpg_ragged_workspace_bytes": (_sz, [ctypes.POINTER(StreamsT), ctypes.POINTER(WindowsT), _vp, _i, _i]),
     "gantts_mlpg_ragged": (_i, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, ctypes.POINTER(StreamsT),
                                 ctypes.POINTER(WindowsT), _vp, _i, _i, _vp, _sz, _vp]),
+    "gantts_mcep_operator": (_i, [ctypes.c_double, _i, _i, _i, _vp]),
+    "gantts_mcep_postfilter": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, ctypes.c_double, _vp, _i, _i, _i, _i, _vp]),
+    "gantts_mcep_to_sp": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _i, _i, _i, _i, _vp]),
     "gantts_distortions_workspace_bytes": (_sz, []),
     "gantts_distortions": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp,
                                 ctypes.POINTER(DistortionColsT), _vp, _vp, _sz, _vp]),

@@ -9,13 +9,18 @@ options:
     --batch-size=<N>            Utterances per batch (default: hp.batch_size).
     --no-mge                    tts_acoustic: the generator was trained without MGE (de-normalise, then MLPG with the
                                 variances of the statistics).
+    --fs=<fs>                   Sampling frequency [default: 16000].
+    --post-filter               tts_acoustic: apply Merlin's post filter to spectral features.
+    --spectrogram               tts_acoustic: also write the power spectral envelope "sp" (mc2sp of mgc).
     -h, --help                  Show this help message and exit
 """
 # The parameter generation of the reference's evaluation scripts (evaluation_vc.py:40-91, evaluation_tts.py:50-176) for a
 # padded batch of any lengths: each utterance gets exactly what those scripts compute for it alone at B = 1 and T = its own
 # length.  The length-exact pieces are the device kernels gantts_mlpg_ragged (MLPG over each row's own frames) and
 # gantts_sru_fwd_lengths (SRU whose reverse direction starts at each row's last frame); the LSTM stacks already run on
-# lengths and the MLP layers frame by frame.  The command writes <dst_dir>/{eval,test}/<name>.npz, no audio.
+# lengths and the MLP layers frame by frame.  Under tts_acoustic, gen_waveform's spectral steps (evaluation_tts.py:112-115:
+# merlin_post_filter, mc2sp) run on the device too (gantts_mcep_postfilter, gantts_mcep_to_sp).  The command writes
+# <dst_dir>/{eval,test}/<name>.npz, no audio: WORLD synthesis and decode_aperiodicity are not done here.
 import os
 import sys
 from os.path import abspath, basename, join, splitext
@@ -32,6 +37,9 @@ from . import train
 LSTM_MAX_B = 128            # sequences per call of the LSTM recurrence kernels (csrc/lstm.cu LSTM_MAX_B)
 HIGHWAY_GENERATORS = ("In2OutHighwayNet", "In2OutRNNHighwayNet")
 OUTPUT_NAMES = {"vc": ("mc",), "acoustic": ("mgc", "lf0", "vuv", "bap", "f0"), "duration": ("duration",)}
+SPECTROGRAM_NAME = "sp"     # the extra acoustic output of spectrogram=True, after OUTPUT_NAMES["acoustic"]
+POSTFILTER_COEF = 1.4       # gen_waveform's coef (evaluation_tts.py:103)
+MAX_FFTLEN = 4096           # gantts_mcep_to_sp's largest FFT
 
 
 # ---- statistics and input normalisation (evaluation_vc.py:61,142-144; evaluation_tts.py:153-156,210-212) ----
@@ -80,7 +88,26 @@ def derive_dims(hp, stats):
         train.derive_tts_dims(hp, stats["X_min"].shape[-1], stats["Y_mean"].shape[-1])
 
 
-def check_hparams(hp, mge_training=True):
+def mcep_alpha(fs):
+    """pysptk.util.mcepalpha(fs) (evaluation_tts.py:105): the all-pass constant in arange(0, 1, 0.001) whose warped
+    frequency axis is closest, in mean squared distance over 1000 points, to the mel scale on [0, fs/2)."""
+    n = 1000
+    mel = np.log1p((fs / 2.0) / n * np.arange(n) / 1000.0) * (1000.0 / np.log(2.0))
+    mel /= mel[-1]
+    alphas = np.arange(0.0, 1.0, 0.001)[:, None]
+    omega = np.pi / n * np.arange(n)[None, :]
+    warp = np.arctan((1 - alphas * alphas) * np.sin(omega) / ((1 + alphas * alphas) * np.cos(omega) - 2 * alphas))
+    warp = np.where(warp < 0, warp + np.pi, warp)
+    warp /= warp[:, -1:]
+    return float(alphas[int(np.argmin(np.sum((mel - warp) ** 2, axis=1) / n)), 0])
+
+
+def cheaptrick_fft_size(fs):
+    """pyworld.get_cheaptrick_fft_size(fs) (evaluation_tts.py:106) at its default F0 floor of 71 Hz."""
+    return 2 ** (1 + int(np.floor(np.log2(3.0 * fs / 71.0 + 1.0))))
+
+
+def check_hparams(hp, mge_training=True, post_filter=False, spectrogram=False, fs=16000):
     """The configurations the evaluation scripts can run; raises ValueError naming the rule otherwise."""
     if hp.name not in OUTPUT_NAMES:
         raise ValueError("hp.name must be vc, acoustic or duration (got %r)" % (hp.name,))
@@ -91,6 +118,15 @@ def check_hparams(hp, mge_training=True):
                          "(evaluation_tts.py calls the generator as model(x, lengths))" % hp.generator)
     if not mge_training and hp.name != "acoustic":
         raise ValueError("--no-mge applies to tts_acoustic only")
+    for on, flag in ((post_filter, "--post-filter"), (spectrogram, "--spectrogram")):
+        if on and hp.name != "acoustic":
+            raise ValueError("%s applies to tts_acoustic only: it works on the generated mgc, which vc and duration "
+                             "models do not produce" % flag)
+    if fs <= 0:
+        raise ValueError("--fs must be > 0 (got %d)" % fs)
+    if spectrogram and cheaptrick_fft_size(fs) > MAX_FFTLEN:
+        raise ValueError("--fs=%d needs a %d-point FFT; at most %d points are supported"
+                         % (fs, cheaptrick_fft_size(fs), MAX_FFTLEN))
 
 
 def plan_batches(lengths, batch_size, max_b=LSTM_MAX_B):
@@ -105,11 +141,16 @@ def plan_batches(lengths, batch_size, max_b=LSTM_MAX_B):
 class ParameterGenerator(object):
     """A trained generator in eval mode and the parameter generation of the evaluation scripts after it, on a padded
     device batch.  ``stats`` as ``load_stats`` returns them; ``mge_training`` picks gen_parameters' branch for
-    tts_acoustic (evaluation_tts.py:64-98)."""
+    tts_acoustic (evaluation_tts.py:64-98).  tts_acoustic only: ``post_filter`` replaces mgc with Merlin's post filter of
+    it and ``spectrogram`` adds its power spectral envelope "sp", at the all-pass constant and FFT size of ``fs``
+    (gen_waveform, evaluation_tts.py:103-115)."""
 
-    def __init__(self, model_g, hp, stats, mge_training=True):
-        check_hparams(hp, mge_training)
+    def __init__(self, model_g, hp, stats, mge_training=True, post_filter=False, spectrogram=False, fs=16000):
+        check_hparams(hp, mge_training, post_filter, spectrogram, fs)
         self.model, self.hp, self.stats, self.kind = model_g.eval(), hp, stats, hp.name
+        self.post_filter, self.spectrogram = bool(post_filter), bool(spectrogram)
+        if self.post_filter or self.spectrogram:
+            self.alpha, self.fftlen = mcep_alpha(fs), cheaptrick_fft_size(fs)
         self.device = next(model_g.parameters()).device
         if self.device.type != "cuda":
             raise RuntimeError("gantts_b200: ParameterGenerator needs the generator on a CUDA device")
@@ -164,7 +205,8 @@ class ParameterGenerator(object):
     def generate(self, x, lengths):
         """x: (B, T, D) normalised inputs (normalize_input), zero-padded, CUDA float32; lengths: int64 CUDA (B,).
         Returns {name: CUDA float32 tensor (B, T, ...)} with the names of OUTPUT_NAMES[hp.name] -- vc "mc"; acoustic
-        "mgc", "lf0", "vuv" (B, T), "bap", "f0"; duration "duration" -- de-normalised.  Frame t of row b is what the
+        "mgc", "lf0", "vuv" (B, T), "bap", "f0", with spectrogram also "sp" (B, T, fftlen/2 + 1); duration "duration" --
+        de-normalised (mgc post-filtered under post_filter).  Frame t of row b is what the
         evaluation scripts compute for that utterance alone for t < lengths[b]; later frames are not part of the result.
         No host synchronisation."""
         ops.require_cuda(x)
@@ -188,15 +230,19 @@ class ParameterGenerator(object):
             # frame whose lf0 is exactly 0 stays 0)
             voiced = ~(vuv < 0.5).unsqueeze(-1) & (lf0 != 0)
             f0 = torch.where(voiced, torch.exp(lf0), torch.zeros_like(lf0))
-            return {"mgc": mgc, "lf0": lf0, "vuv": vuv, "bap": bap, "f0": f0}
+            if self.post_filter:                                # evaluation_tts.py:112-113
+                mgc = ops.mcep_postfilter(mgc, lengths, self.alpha, POSTFILTER_COEF)
+            out = {"mgc": mgc, "lf0": lf0, "vuv": vuv, "bap": bap, "f0": f0}
+            if self.spectrogram:                                # :115
+                out[SPECTROGRAM_NAME] = ops.mc2sp(mgc, lengths, self.alpha, self.fftlen)
+            return out
 
     def generate_utterances(self, arrays, batch_size):
         """Un-normalised input feature arrays (T_i, D) -> one dict of float32 numpy arrays of T_i frames per utterance,
-        in input order.  The utterances are sorted by length and batched (plan_batches); each batch makes one
-        host-to-device and one device-to-host copy."""
+        in input order, with the keys ``generate`` returns.  The utterances are sorted by length and batched
+        (plan_batches); each batch makes one host-to-device and one device-to-host copy."""
         arrays = [normalize_input(a, self.hp, self.stats) for a in arrays]
         results = [None] * len(arrays)
-        names = OUTPUT_NAMES[self.kind]
         for idx in plan_batches([len(a) for a in arrays], batch_size):
             lens = [len(arrays[i]) for i in idx]
             T = max(lens)
@@ -206,6 +252,7 @@ class ParameterGenerator(object):
             x = torch.from_numpy(xb).to(self.device)
             lengths = torch.tensor(lens, dtype=torch.int64).to(self.device)
             out = self.generate(x, lengths)
+            names = list(out)
             widths = [1 if out[k].dim() == 2 else out[k].shape[-1] for k in names]
             host = torch.cat([out[k].reshape(len(idx), T, -1) for k in names], -1).cpu().numpy()
             for j, i in enumerate(idx):
@@ -241,8 +288,13 @@ def main(argv=None, hp=None):
     hp.parse(args["--hparams"])
     mge_training = not args["--no-mge"]
     batch_size = int(args["--batch-size"]) if args["--batch-size"] is not None else int(hp.batch_size)
+    post_filter, spectrogram = bool(args["--post-filter"]), bool(args["--spectrogram"])
     try:
-        check_hparams(hp, mge_training)
+        fs = int(args["--fs"])
+    except ValueError:
+        raise SystemExit("gantts_b200.generate: --fs must be an integer sampling frequency (got %r)" % args["--fs"])
+    try:
+        check_hparams(hp, mge_training, post_filter, spectrogram, fs)
         if batch_size < 1:
             raise ValueError("--batch-size must be >= 1 (got %d)" % batch_size)
     except ValueError as e:
@@ -256,7 +308,7 @@ def main(argv=None, hp=None):
     derive_dims(hp, stats)
     model_g = getattr(models, hp.generator)(**hp.generator_params)
     train.load_checkpoint(model_g, checkpoint_path)
-    gen = ParameterGenerator(model_g.to(device), hp, stats, mge_training)
+    gen = ParameterGenerator(model_g.to(device), hp, stats, mge_training, post_filter, spectrogram, fs)
 
     for sub, files in utterance_files(inputs_dir):
         out_dir = join(dst_dir, sub)

@@ -282,6 +282,70 @@ def mlpg_ragged(x, lengths, windows, stream_entries, ncols_out, var=None, in_aff
     return out
 
 
+# ----------------------------------------------------------------- mel-cepstrum post-processing
+POSTFILTER_FFTLEN = 1024    # merlin_post_filter's defaults: fftlen 1024, minimum-phase order 511 (evaluation_tts.py:113)
+_mcep_op_cache = {}
+
+
+def mcep_operator_host(alpha, order, fftlen, kind):
+    """The (fftlen/2 + 1, order + 1) float64 matrix of gantts_mcep_operator: row k maps a mel-cepstrum to its log power at
+    bin k, for merlin_post_filter's energy (kind _lib.MCEP_R0) or for mc2sp (_lib.MCEP_SP).  Host computation."""
+    lib = _lib.load()
+    op = np.zeros((int(fftlen) // 2 + 1, int(order) + 1), dtype=np.float64)
+    _lib.check(lib.gantts_mcep_operator(float(alpha), int(order), int(fftlen), int(kind), op.ctypes.data))
+    return op
+
+
+def _mcep_operator(alpha, order, fftlen, kind, device):
+    key = (float(alpha), int(order), int(fftlen), int(kind), device.index)
+    op = _mcep_op_cache.get(key)
+    if op is None:
+        op = torch.from_numpy(mcep_operator_host(alpha, order, fftlen, kind)).to(device)
+        _mcep_op_cache[key] = op
+    return op
+
+
+def _mcep_args(mc, lengths, what):
+    require_cuda(mc)
+    if not (torch.is_tensor(lengths) and lengths.is_cuda and lengths.dtype == torch.int64):
+        raise RuntimeError("gantts_b200: %s needs int64 CUDA lengths" % what)
+    if mc.dim() != 3:
+        raise RuntimeError("gantts_b200: %s needs mc (B, T, M+1)" % what)
+    if mc.stride(2) != 1:
+        mc = mc.contiguous()
+    return mc, lengths.contiguous()
+
+
+def mcep_postfilter(mc, lengths, alpha, coef=1.4):
+    """nnmnkwii.postfilters.merlin_post_filter(mc, alpha, coef=coef) on every frame t < lengths[b] of row b
+    (gantts_mcep_postfilter): mc (B, T, M+1) CUDA float32, lengths int64 CUDA (B,).  Returns (B, T, M+1) float32 with 0
+    beyond each length.  The operator is built once per (alpha, order, device) and cached.  No host sync."""
+    mc, lengths = _mcep_args(mc, lengths, "mcep_postfilter")
+    lib = _lib.load()
+    B, T, M1 = mc.shape
+    op = _mcep_operator(alpha, M1 - 1, POSTFILTER_FFTLEN, _lib.MCEP_R0, mc.device)
+    out = torch.empty(B, T, M1, dtype=torch.float32, device=mc.device)
+    _lib.check(lib.gantts_mcep_postfilter(mc.data_ptr(), mc.stride(0), mc.stride(1), out.data_ptr(), out.stride(0),
+                                          out.stride(1), op.data_ptr(), float(coef), lengths.data_ptr(), B, T, M1 - 1,
+                                          op.shape[0], _stream()))
+    return out
+
+
+def mc2sp(mc, lengths, alpha, fftlen):
+    """pysptk.mc2sp(mc, alpha, fftlen) on every frame t < lengths[b] of row b (gantts_mcep_to_sp): the power spectral
+    envelope (B, T, fftlen/2 + 1) float32, 0 beyond each length.  The operator is cached per (alpha, order, fftlen,
+    device).  No host sync."""
+    mc, lengths = _mcep_args(mc, lengths, "mc2sp")
+    lib = _lib.load()
+    B, T, M1 = mc.shape
+    op = _mcep_operator(alpha, M1 - 1, fftlen, _lib.MCEP_SP, mc.device)
+    sp = torch.empty(B, T, op.shape[0], dtype=torch.float32, device=mc.device)
+    _lib.check(lib.gantts_mcep_to_sp(mc.data_ptr(), mc.stride(0), mc.stride(1), sp.data_ptr(), sp.stride(0),
+                                     sp.stride(1), op.data_ptr(), lengths.data_ptr(), B, T, M1 - 1, op.shape[0],
+                                     _stream()))
+    return sp
+
+
 def distortion_sums(y, y_hat, lengths, mean, std, mcd=(0, 0), bap=(0, 0), lf0_col=-1, vuv_col=-1,
                     lf0_linear=True, mse=(0, 0)):
     """Eight sums behind the objective metrics of reference train.py:399-432 (see include/gantts_b200.h,

@@ -579,6 +579,39 @@ int gantts_mlpg_ragged(const float* in, int64_t in_bstride, int64_t in_tstride, 
                        const gantts_windows_t* windows, const int64_t* lengths_dev, int B, int T, void* workspace,
                        size_t workspace_bytes, void* stream);
 
+/* Spectral post-processing of generated mel-cepstra (replaces, per utterance, reference evaluation_tts.py:112-115:
+ * nnmnkwii.postfilters.merlin_post_filter(mgc, alpha, coef=coef) and pysptk.mc2sp(mgc, fftlen, alpha)).  Up to the final
+ * exp both are linear in the frame, so each is one K x (M+1) fp64 matrix (K = fftlen/2 + 1 bins, M the order) whose row k
+ * maps a frame to its log power at bin k:
+ *   GANTTS_MCEP_R0  cosine transform of freqt(., fftlen/2 - 1, -alpha): the merlin_post_filter energy r0 =
+ *                   c2acr(freqt(mc, 511, -alpha), 0, 1024) = sum_k w_k exp(row_k . mc) / fftlen, w = 1, 2, ..., 2, 1;
+ *   GANTTS_MCEP_SP  cosine transform of freqt(., fftlen/2, -alpha) with c0 doubled and the Nyquist term counted once:
+ *                   mc2sp(mc)[k] = exp(row_k . mc).
+ * gantts_mcep_operator builds either matrix on the host in double by running SPTK's freqt recursion on unit vectors; it
+ * writes out[k * (M+1) + m].  Rules: |alpha| < 1, 1 <= M+1 <= 128, fftlen a power of two in [64, 4096], kind 0 or 1,
+ * out non-null.  No device work. */
+#define GANTTS_MCEP_R0 0
+#define GANTTS_MCEP_SP 1
+int gantts_mcep_operator(double alpha, int order, int fftlen, int kind, double* out);
+/* Merlin's post filter on every valid frame of a padded batch: mc float32 [B][T][M+1] (element strides mc_bstride,
+ * mc_tstride; unit column stride), op_r the GANTTS_MCEP_R0 matrix on the device at fftlen = 2 (K - 1) (the reference's
+ * defaults are fftlen 1024, minimum-phase order 511).  Writes w*mc with c0 shifted by log(r0(mc) / r0(w*mc)) / 2,
+ * w = coef except w[0] = w[1] = 1: what mc2b(w*mc), b[0] += that shift, b2mc computes in closed form.  out [B][T][M+1]
+ * (strides out_bstride, out_tstride). */
+int gantts_mcep_postfilter(const float* mc, int64_t mc_bstride, int64_t mc_tstride, float* out, int64_t out_bstride,
+                           int64_t out_tstride, const double* op_r, double coef, const int64_t* lengths_dev, int B,
+                           int T, int M, int K, void* stream);
+/* pysptk.mc2sp on every valid frame of a padded batch: sp float32 [B][T][K] (strides sp_bstride, sp_tstride; unit bin
+ * stride) = exp(op_s . mc), op_s the GANTTS_MCEP_SP matrix on the device.
+ * Both kernels: row b is processed over its own L = lengths_dev[b] frames (int64[B], clamped to [0, T]); frames at or
+ * beyond L are written as 0, and a row equals that utterance alone at B = 1, T = L, bit for bit.  They compute in double
+ * and store float32.  Rules, checked before any device work (the error string names the one that failed): lengths_dev
+ * non-null, 1 <= B <= 65535, 1 <= T <= 2^24, 1 <= M+1 <= 128, fftlen = 2 (K - 1) a power of two in [64, 4096], non-null
+ * buffers, and for the post filter a finite coef. */
+int gantts_mcep_to_sp(const float* mc, int64_t mc_bstride, int64_t mc_tstride, float* sp, int64_t sp_bstride,
+                      int64_t sp_tstride, const double* op_s, const int64_t* lengths_dev, int B, int T, int M, int K,
+                      void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Objective distortions of the training loop (reference train.py:399-432 compute_distortions, :383-396
  * split_streams, :358-380 inv_scale; nnmnkwii.metrics.{melcd, lf0_mean_squared_error, vuv_error,
