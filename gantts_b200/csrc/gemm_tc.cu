@@ -12,8 +12,9 @@
 // (SWIZZLE_128B, full/empty mbarriers per stage) across all of the CTA's tiles; warpgroups 1-2: every tile together,
 // warpgroup w issuing one wgmma.m64n{BN}k16 per product for rows 64w .. 64w + 63.  Each warpgroup stages its
 // accumulators through its warps' shared-memory buffers so that each epilogue thread owns 16 consecutive columns of one
-// row (bias / LeakyReLU / dropout / sigmoid, 16-byte stores); that epilogue runs while the producer refills the ring
-// for the CTA's next tile.
+// row (bias / LeakyReLU / dropout / sigmoid; fp32 outputs leave as 16-byte stores, bf16 hi/lo planes are restaged in
+// the same buffer and leave as TMA stores that drain while the warps go on); that epilogue runs while the producer
+// refills the ring for the CTA's next tile.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -62,8 +63,7 @@ struct GemmParams {
   int vec_ok;           // C 16-byte aligned, ldc % 4 == 0, no accumulate: float4 stores from registers;
                         // 0 = through the warp's buffer as a transpose scratch (epilogue_f32_smem)
   int accumulate;
-  // planes output (EPI_PLANES_*)
-  __nv_bfloat16 *out_hi, *out_lo;
+  // planes output (EPI_PLANES_*): written through the tmOh / tmOl tensor maps, [rows_a][out_pitch] bf16
   int64_t out_pitch;
   // activation-derivative code plane: 2 bits per element (bit0 = zero/dropped, bit1 = negative), one
   // uint32 per (row, 16 columns).  Written by EPI_PLANES_FWD, read by EPI_PLANES_BWD.
@@ -98,22 +98,31 @@ __device__ __forceinline__ void split8(const float* v, uint32_t* h, uint32_t* l)
   }
 }
 
-// 16 fp32 values of one row -> hi/lo planes: two 16-byte stores per plane (a full 32 B sector); `pitch` is a
-// multiple of 16 elements and col a multiple of 16, so the address is 32-byte aligned.  Tail: 16-byte stores up
-// to the pitch.
-__device__ __forceinline__ void store_planes16(const float* v, __nv_bfloat16* hi, __nv_bfloat16* lo, int col,
-                                               int64_t pitch) {
-  uint32_t h[8], l[8];
-  split8(v, h, l);
-  split8(v + 8, h + 4, l + 4);
-  if (col + 16 <= pitch) {
-    reinterpret_cast<uint4*>(hi)[0] = make_uint4(h[0], h[1], h[2], h[3]);
-    reinterpret_cast<uint4*>(hi)[1] = make_uint4(h[4], h[5], h[6], h[7]);
-    reinterpret_cast<uint4*>(lo)[0] = make_uint4(l[0], l[1], l[2], l[3]);
-    reinterpret_cast<uint4*>(lo)[1] = make_uint4(l[4], l[5], l[6], l[7]);
-  } else if (col + 8 <= pitch) {
-    *reinterpret_cast<uint4*>(hi) = make_uint4(h[0], h[1], h[2], h[3]);
-    *reinterpret_cast<uint4*>(lo) = make_uint4(l[0], l[1], l[2], l[3]);
+// One pass of a warp's planes epilogue out to global memory: lane l's 16 split values (row l % 16 of the warp's 16,
+// columns 16 (l / 16) .. + 15 of the pass) go to the warp's buffer as a dense [16][32] bf16 box per plane (hi at byte
+// 0, lo at 1024), and lane 0 hands both boxes to the TMA unit as one bulk group.  The caller has read the buffer out
+// (the __syncwarp below orders that) and waits with bulk_wait_read before writing it again; so does this function,
+// for the store it issued last.  TMA clips the box at
+// rows_a and at the pitch: every 16-column chunk that starts below cols_b is written whole, the pad columns up to the
+// pitch holding the epilogue of zero-padded operands.
+__device__ __forceinline__ void store_planes_pass(const CUtensorMap* mh, const CUtensorMap* ml, float* buf,
+                                                  const uint32_t (&h)[8], const uint32_t (&l)[8], int lane, int col,
+                                                  int64_t row0, const GemmParams& p) {
+  if (lane == 0) ptx::bulk_wait_read<0>();
+  __syncwarp();
+  uint4* sh = reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(buf) + (lane & 15) * 64 + (lane >> 4) * 32);
+  uint4* sl = sh + 1024 / 16;
+  sh[0] = make_uint4(h[0], h[1], h[2], h[3]);
+  sh[1] = make_uint4(h[4], h[5], h[6], h[7]);
+  sl[0] = make_uint4(l[0], l[1], l[2], l[3]);
+  sl[1] = make_uint4(l[4], l[5], l[6], l[7]);
+  ptx::fence_proxy_async();
+  __syncwarp();
+  if (lane == 0 && row0 < p.rows_a && col < p.out_pitch) {
+    const uint32_t s = ptx::smem_u32(buf);
+    ptx::tma_store_2d(mh, s, col, (int32_t)row0);
+    ptx::tma_store_2d(ml, s + 1024, col, (int32_t)row0);
+    ptx::bulk_commit();
   }
 }
 
@@ -204,12 +213,13 @@ __device__ __forceinline__ void epilogue_f32_smem(const GemmParams& p, const uin
   __syncwarp();
 }
 
-// One 16-column chunk of one output row: registers (fp32 accumulators) -> global.
-// Returns the derivative code word of the chunk (EPI_PLANES_FWD); `code_in` is the saved word (BWD).
+// One 16-column chunk of one output row: registers (fp32 accumulators) -> global (EPI_F32) or -> the split hi / lo
+// words `h`, `l` (EPI_PLANES_*).  Returns the derivative code word of the chunk (EPI_PLANES_FWD); `code_in` is the
+// saved word (BWD).
 template <int EPI>
 __device__ __forceinline__ uint32_t epilogue_chunk16(const GemmParams& p, const uint32_t (&r)[16], int64_t row,
                                                      int col, int z, const float* __restrict__ bias_s,
-                                                     uint32_t code_in) {
+                                                     uint32_t code_in, uint32_t (&h)[8], uint32_t (&l)[8]) {
   uint32_t code = 0;
   float v[16];
 #pragma unroll
@@ -290,9 +300,8 @@ __device__ __forceinline__ uint32_t epilogue_chunk16(const GemmParams& p, const 
         if (neg) code |= 2u << (2 * j);
       }
     }
-    __nv_bfloat16* oh = p.out_hi + row * p.out_pitch + col;
-    __nv_bfloat16* ol = p.out_lo + row * p.out_pitch + col;
-    store_planes16(v, oh, ol, col, p.out_pitch);
+    split8(v, h, l);
+    split8(v + 8, h + 4, l + 4);
   } else {  // EPI_PLANES_BWD: gz = g * act'(h), derivative class from the saved 2-bit code
     const float dpos = p.keep_scale, dneg = p.slope * p.keep_scale;
     const float dzero = p.thresh ? 0.f : p.slope;
@@ -301,9 +310,8 @@ __device__ __forceinline__ uint32_t epilogue_chunk16(const GemmParams& p, const 
       const uint32_t cj = (code_in >> (2 * j)) & 3u;
       v[j] *= (cj & 1u) ? dzero : ((cj & 2u) ? dneg : dpos);
     }
-    __nv_bfloat16* oh = p.out_hi + row * p.out_pitch + col;
-    __nv_bfloat16* ol = p.out_lo + row * p.out_pitch + col;
-    store_planes16(v, oh, ol, col, p.out_pitch);
+    split8(v, h, l);
+    split8(v + 8, h + 4, l + 4);
   }
   return code;
 }
@@ -377,8 +385,10 @@ template <bool MN, int EPI, int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                    const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
+                   const __grid_constant__ CUtensorMap tmOh, const __grid_constant__ CUtensorMap tmOl,
                    const GemmParams p) {
   constexpr int BK = MN ? TC_MN_BK : TC_KK_BK;
+  constexpr bool PLANES = EPI != EPI_F32;   // output planes leave through TMA stores (tmOh / tmOl)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = ptx::smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -403,6 +413,10 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
     ptx::prefetch_tensormap(&tmAl);
     ptx::prefetch_tensormap(&tmBh);
     ptx::prefetch_tensormap(&tmBl);
+    if (PLANES) {
+      ptx::prefetch_tensormap(&tmOh);
+      ptx::prefetch_tensormap(&tmOl);
+    }
   }
   // PDL: let the next kernel of the stream set itself up while this one drains; nothing produced by the
   // previous kernel is read before the dependency wait.
@@ -475,6 +489,19 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
     const int nk = k_blocks(z);
     const int ta = rem / p.num_b, tb = rem % p.num_b;
     const int a0 = ta * TC_BM, b0 = tb * BN;
+    const int64_t row0 = (int64_t)a0 + 64 * wg + 16 * q;   // first row of this warp in the tile
+    const int64_t row = row0 + (lane & 15);                // the lane's row in the epilogue
+    const bool row_ok = row < p.rows_a;
+    // derivative code words of the lane's chunk in each pass (chunk 2k + lane / 16 of the tile), loaded before the
+    // mainloop so that they arrive under the MMAs
+    constexpr int PASSES = BN / 32;
+    uint32_t codes[PASSES];
+#pragma unroll
+    for (int k = 0; k < PASSES; ++k) {
+      const int c = b0 + 16 * (2 * k + (lane >> 4));
+      codes[k] = 0u;
+      if (EPI == EPI_PLANES_BWD && row_ok && c < p.cols_b) codes[k] = __ldg(p.code + row * p.code_pitch + (c >> 4));
+    }
     float acc[BN / 2];
     float accdb[4] = {0.f, 0.f, 0.f, 0.f};
     const bool do_db = MN && p.db != nullptr && tb == 0;
@@ -482,7 +509,6 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
       mma_tile<MN, BN, MN>(p, acc, accdb, base, full0, empty0, d_ones, nk, s, ph, lane, wg);
     else
       mma_tile<MN, BN, false>(p, acc, accdb, base, full0, empty0, d_ones, nk, s, ph, lane, wg);
-    const int64_t row0 = (int64_t)a0 + 64 * wg + 16 * q;   // first row of this warp in the tile
     if (do_db && (lane & 3) == 0) {
       // m64n8 layout: lane holds rows lane/4 and lane/4 + 8 of its warp's 16, columns 0-1 (all columns are equal)
       const int64_t r = row0 + (lane >> 2);
@@ -492,21 +518,15 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
     // ------------------------------------------------------------ epilogue.  Warp q holds rows 16q .. 16q + 15 of its
     // warpgroup's 64-row block; per pass of two 16-column chunks its fragments go through the warp's own shared-memory
     // buffer [32][TC_WARP_PITCH] so that lane l owns 16 consecutive columns of one row: row row0 + (l % 16), chunk
-    // l / 16 of the pass.
-    const int64_t row = row0 + (lane & 15);
-    const bool row_ok = row < p.rows_a;
-    // derivative code words of the lane's chunk in each pass: chunk 2k + lane / 16 of the tile
-    constexpr int PASSES = BN / 32;
-    uint32_t codes[PASSES];
+    // l / 16 of the pass.  Planes: pass k's split values wait in registers (hw, lw) until pass k + 1's fragments have
+    // been read out of the buffer; the buffer then stages them for a TMA store, which reads it while pass k + 1's
+    // arithmetic runs.  The last pass's store drains under the next tile's mainloop.
     uint32_t code_out[PASSES];
+    uint32_t hw[8], lw[8];
 #pragma unroll
     for (int k = 0; k < PASSES; ++k) {
-      const int c = b0 + 16 * (2 * k + (lane >> 4));
-      codes[k] = code_out[k] = 0u;
-      if (EPI == EPI_PLANES_BWD && row_ok && c < p.cols_b) codes[k] = __ldg(p.code + row * p.code_pitch + (c >> 4));
-    }
-#pragma unroll
-    for (int k = 0; k < PASSES; ++k) {
+      code_out[k] = 0u;
+      if (PLANES && lane == 0) ptx::bulk_wait_read<0>(); // the buffer's last TMA store has read it
       __syncwarp();                                      // the previous pass has been read out of the buffer
       // m64nN layout: register 4j + 2g + e is row 16q + lane / 4 + 8g, column 8j + 2 (lane % 4) + e.  Slots 16h ..
       // 16h + 15 take the warp's rows of chunk 2k + h.
@@ -533,10 +553,14 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
       if (EPI == EPI_F32 && !p.vec_ok) {                 // whole warp takes part; rows beyond rows_a masked at the store
         __syncwarp();                                    // the buffer becomes the transpose scratch
         if (col < p.cols_b) epilogue_f32_smem(p, rr, row0, lane, col, z, bias_s, wbuf);
-      } else if (row_ok && lcol < p.cols_b) {
-        code_out[k] = epilogue_chunk16<EPI>(p, rr, row, lcol, z, bias_s, codes[k]);
+      } else if (EPI == EPI_F32) {
+        if (row_ok && lcol < p.cols_b) epilogue_chunk16<EPI>(p, rr, row, lcol, z, bias_s, 0u, hw, lw);
+      } else {                                           // whole warp: the TMA store clips rows and columns
+        if (k > 0) store_planes_pass(&tmOh, &tmOl, wbuf, hw, lw, lane, col - 32, row0, p);
+        code_out[k] = epilogue_chunk16<EPI>(p, rr, row, lcol, z, bias_s, codes[k], hw, lw);
       }
     }
+    if (PLANES) store_planes_pass(&tmOh, &tmOl, wbuf, hw, lw, lane, b0 + 32 * (PASSES - 1), row0, p);
     if (EPI == EPI_PLANES_FWD && p.code != nullptr && row_ok) {
       uint32_t* cpp = p.code + row * p.code_pitch + (b0 >> 4);
 #pragma unroll
@@ -546,6 +570,7 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
       }
     }
   }
+  if (PLANES && lane == 0) ptx::bulk_wait<0>();          // the last stores are complete before the CTA exits
 }
 
 // ---------------------------------------------------------------------------- operand planes
@@ -604,9 +629,11 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-// 2D bf16 tensor [rows][cols] with row pitch `pitch` elements; box = {64 columns (one 128-byte swizzled row),
-// box_rows}.  Out-of-range box elements are filled with zeros.
-static int make_map(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols, int64_t pitch, int box_rows) {
+// 2D bf16 tensor [rows][cols] with row pitch `pitch` elements; box = {box_cols, box_rows}, by default 64 columns (one
+// 128-byte swizzled row) for the operand loads.  Out-of-range box elements are filled with zeros by loads and skipped
+// by stores.
+static int make_map(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols, int64_t pitch, int box_rows,
+                    int box_cols = 64, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn enc = get_encode();
   if (!enc) {
     set_error("tc: cuTensorMapEncodeTiled entry point unavailable");
@@ -614,10 +641,10 @@ static int make_map(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols,
   }
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)pitch * 2};
-  cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
+  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -712,8 +739,6 @@ static void fill_epilogue(GemmParams& p, const EpiArgs& e) {
   p.ldc = e.ldc;
   p.accumulate = e.accumulate;
   p.vec_ok = (!e.accumulate && e.C && (e.ldc & 3) == 0 && (reinterpret_cast<uintptr_t>(e.C) & 15) == 0) ? 1 : 0;
-  p.out_hi = e.out_hi;
-  p.out_lo = e.out_lo;
   p.out_pitch = e.out_pitch;
   p.code = e.code;
   p.code_pitch = e.code_pitch;
@@ -740,9 +765,11 @@ static size_t plan_smem(GemmParams& p, const EpiArgs& e) {
   return (size_t)p.bar_off + 256 + 1024;
 }
 
+// mOh / mOl: the output planes of EPI_PLANES_* (any initialised map otherwise: the kernel does not read them).
 template <bool MN, int EPI, int BN>
 static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const CUtensorMap& mBh,
-                         const CUtensorMap& mBl, const GemmParams& p, size_t smem, cudaStream_t st) {
+                         const CUtensorMap& mBl, const CUtensorMap& mOh, const CUtensorMap& mOl, const GemmParams& p,
+                         size_t smem, cudaStream_t st) {
   if (smem > TC_SMEM_MAX) {
     set_error("gemm: shared-memory plan of %zu bytes exceeds %u", smem, TC_SMEM_MAX);
     return GANTTS_E_UNSUPPORTED;
@@ -763,7 +790,8 @@ static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const C
   const int tiles = p.num_a * p.num_b * p.num_z;
   const int grid = tiles < num_sms() ? tiles : num_sms();
   prof_begin(MN ? PROF_GEMM_MN : PROF_GEMM_KK, 2.0 * (double)p.rows_a * p.cols_b * (double)p.red, st);
-  GANTTS_PDL_LAUNCH((gemm_bf16x3_kernel<MN, EPI, BN>), (unsigned)grid, TC_THREADS, smem, st, mAh, mAl, mBh, mBl, p);
+  GANTTS_PDL_LAUNCH((gemm_bf16x3_kernel<MN, EPI, BN>), (unsigned)grid, TC_THREADS, smem, st, mAh, mAl, mBh, mBl, mOh,
+                    mOl, p);
   prof_end(st);
   GANTTS_LAUNCH_CHECK("gemm_bf16x3_kernel");
   return GANTTS_OK;
@@ -771,9 +799,10 @@ static int launch_kernel(const CUtensorMap& mAh, const CUtensorMap& mAl, const C
 
 template <bool MN, int EPI>
 static int launch_bn(const CUtensorMap& mAh, const CUtensorMap& mAl, const CUtensorMap& mBh, const CUtensorMap& mBl,
-                     const GemmParams& p, size_t smem, cudaStream_t st) {
-  if (p.bn == 64) return launch_kernel<MN, EPI, 64>(mAh, mAl, mBh, mBl, p, smem, st);
-  return launch_kernel<MN, EPI, 128>(mAh, mAl, mBh, mBl, p, smem, st);
+                     const CUtensorMap& mOh, const CUtensorMap& mOl, const GemmParams& p, size_t smem,
+                     cudaStream_t st) {
+  if (p.bn == 64) return launch_kernel<MN, EPI, 64>(mAh, mAl, mBh, mBl, mOh, mOl, p, smem, st);
+  return launch_kernel<MN, EPI, 128>(mAh, mAl, mBh, mBl, mOh, mOl, p, smem, st);
 }
 
 // out[rows_a][cols_b] = epi(A * B^T)   (K-major planes A [rows_a][red], B [cols_b][red]).
@@ -804,10 +833,14 @@ static int launch_gemm_kk(const Planes& A, const Planes& B, const EpiArgs& e, cu
   if ((rc = make_map(&mAl, A.lo, A.rows, A.cols, A.pitch, TC_BM))) return rc;
   if ((rc = make_map(&mBh, B.hi, B.rows, B.cols, B.pitch, p.bn))) return rc;
   if ((rc = make_map(&mBl, B.lo, B.rows, B.cols, B.pitch, p.bn))) return rc;
+  if (e.epi == EPI_F32) return launch_bn<false, EPI_F32>(mAh, mAl, mBh, mBl, mAh, mAl, p, smem, st);
+  // output planes [rows_a][pitch]: one warp's pass is a 16-row x 32-column box per plane, written up to the pitch
+  CUtensorMap mOh, mOl;
+  if ((rc = make_map(&mOh, e.out_hi, p.rows_a, e.out_pitch, e.out_pitch, 16, 32, CU_TENSOR_MAP_SWIZZLE_NONE))) return rc;
+  if ((rc = make_map(&mOl, e.out_lo, p.rows_a, e.out_pitch, e.out_pitch, 16, 32, CU_TENSOR_MAP_SWIZZLE_NONE))) return rc;
   switch (e.epi) {
-    case EPI_F32: return launch_bn<false, EPI_F32>(mAh, mAl, mBh, mBl, p, smem, st);
-    case EPI_PLANES_FWD: return launch_bn<false, EPI_PLANES_FWD>(mAh, mAl, mBh, mBl, p, smem, st);
-    case EPI_PLANES_BWD: return launch_bn<false, EPI_PLANES_BWD>(mAh, mAl, mBh, mBl, p, smem, st);
+    case EPI_PLANES_FWD: return launch_bn<false, EPI_PLANES_FWD>(mAh, mAl, mBh, mBl, mOh, mOl, p, smem, st);
+    case EPI_PLANES_BWD: return launch_bn<false, EPI_PLANES_BWD>(mAh, mAl, mBh, mBl, mOh, mOl, p, smem, st);
   }
   set_error("gemm_kk: bad epilogue %d", e.epi);
   return GANTTS_E_BADARG;
@@ -973,7 +1006,7 @@ static int launch_gemm_mn(const Planes& A, const Planes& B, float* C, float* gb,
   if ((rc = make_map(&mAl, A.lo, A.rows, A.cols, A.pitch, TC_MN_BK))) return rc;
   if ((rc = make_map(&mBh, B.hi, B.rows, B.cols, B.pitch, TC_MN_BK))) return rc;
   if ((rc = make_map(&mBl, B.lo, B.rows, B.cols, B.pitch, TC_MN_BK))) return rc;
-  if ((rc = launch_bn<true, EPI_F32>(mAh, mAl, mBh, mBl, p, smem, st))) return rc;
+  if ((rc = launch_bn<true, EPI_F32>(mAh, mAl, mBh, mBl, mAh, mAl, p, smem, st))) return rc;
   if (!direct) {
     if (defer && defer->n + 2 <= REDUCE_MAX_JOBS) {
       int j = defer->n++;

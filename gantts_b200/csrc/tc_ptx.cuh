@@ -1,4 +1,5 @@
-// Thin inline-PTX wrappers for the Hopper (sm_90a) tensor path: mbarrier, TMA (cp.async.bulk.tensor), programmatic
+// Thin inline-PTX wrappers for the Hopper (sm_90a) tensor path: mbarrier, TMA (cp.async.bulk.tensor loads and stores,
+// bulk async-groups), programmatic
 // dependent launch, and warpgroup MMA (wgmma) with its shared-memory matrix descriptors.
 #pragma once
 #include <cuda.h>
@@ -62,6 +63,20 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
+// 2D tile store shared -> global into the issuing thread's current bulk async-group; box elements outside the tensor
+// are not written.  The shared-memory writes it reads must be ordered before it by fence_proxy_async.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int32_t c0, int32_t c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// Wait until at most N of the thread's committed bulk groups are still reading their shared-memory source.
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// Wait until at most N of the thread's committed bulk groups are incomplete (their global writes done).
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ------------------------------------------------------------------ programmatic dependent launch
 // launch_dependents: the next kernel in the stream (if it was launched with programmatic stream
