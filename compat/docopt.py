@@ -1,5 +1,6 @@
-"""Minimal docopt (reference train.py:24): supports the ``usage: prog [options] <a> <b>`` pattern with
-an ``options:`` section of ``--name=<v>  text [default: x]`` / ``--flag`` / ``-h, --help`` lines."""
+"""Minimal docopt (reference train.py:24): supports the ``usage: prog [options] <a> <b>`` pattern, whose last
+positional may repeat (``<c>...``: one or more, returned as a list), with an ``options:`` section of
+``--name=<v>  text [default: x]`` / ``--flag`` / ``-h, --help`` lines."""
 import re
 import sys
 
@@ -8,6 +9,7 @@ def docopt(doc, argv=None):
     argv = list(sys.argv[1:] if argv is None else argv)
     usage = re.search(r"usage:\s*\S+(.*)", doc, re.I).group(1)
     positional = re.findall(r"<([^>]+)>", usage)
+    repeats = bool(re.search(r">\.\.\.", usage))
     opts, takes_value = {}, {}
     in_opts = False
     for line in doc.splitlines():
@@ -46,8 +48,10 @@ def docopt(doc, argv=None):
         else:
             pos.append(a)
         i += 1
-    if len(pos) != len(positional):
+    if len(pos) != len(positional) and not (repeats and len(pos) > len(positional)):
         raise SystemExit(doc)
     for n, v in zip(positional, pos):
         args["<%s>" % n] = v
+    if repeats:
+        args["<%s>" % positional[-1]] = pos[len(positional) - 1:]
     return args

@@ -170,6 +170,8 @@ SIGNATURES = {
     "gantts_mcep_operator": (_i, [ctypes.c_double, _i, _i, _i, _vp]),
     "gantts_mcep_postfilter": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, ctypes.c_double, _vp, _i, _i, _i, _i, _vp]),
     "gantts_mcep_to_sp": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "gantts_modspec": (_i, [_vp, _i64, _i64, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "gantts_global_variance": (_i, [_vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp]),
     "gantts_distortions_workspace_bytes": (_sz, []),
     "gantts_distortions": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp,
                                 ctypes.POINTER(DistortionColsT), _vp, _vp, _sz, _vp]),

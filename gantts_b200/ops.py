@@ -346,6 +346,49 @@ def mc2sp(mc, lengths, alpha, fftlen):
     return sp
 
 
+# ------------------------------------------------------------- global variance and modulation spectrum
+def _feature_args(x, lengths, what):
+    require_cuda(x)
+    if not (torch.is_tensor(lengths) and lengths.is_cuda and lengths.dtype == torch.int64):
+        raise RuntimeError("gantts_b200: %s needs int64 CUDA lengths" % what)
+    if x.dim() != 3 or lengths.dim() != 1 or lengths.numel() != x.shape[0]:
+        raise RuntimeError("gantts_b200: %s needs x (B, T, D) and lengths (B,)" % what)
+    if x.stride(2) != 1:
+        x = x.contiguous()
+    return x, lengths.contiguous()
+
+
+def modspec(x, lengths, n, out_sum=None):
+    """np.log(nnmnkwii.preprocessing.modspec(x[b, :lengths[b]], n)) of every row b (gantts_modspec): x (B, T, D) CUDA
+    float32, any batch and time strides (a column slice is read in place), lengths int64 CUDA (B,).  Returns the
+    (B, n/2 + 1, D) float64 log power.  out_sum: None, or a (n/2 + 1, D) float64 CUDA tensor to which the rows are added
+    one at a time in row order.  No host sync."""
+    x, lengths = _feature_args(x, lengths, "modspec")
+    lib = _lib.load()
+    B, T, D = x.shape
+    K = int(n) // 2 + 1
+    if out_sum is not None and not (out_sum.is_cuda and out_sum.dtype == torch.float64 and out_sum.device == x.device
+                                    and tuple(out_sum.shape) == (K, D) and out_sum.is_contiguous()):
+        raise RuntimeError("gantts_b200: modspec's out_sum must be a contiguous float64 (%d, %d) tensor on %s"
+                           % (K, D, x.device))
+    out = torch.empty(B, K, D, dtype=torch.float64, device=x.device)
+    _lib.check(lib.gantts_modspec(x.data_ptr(), x.stride(0), x.stride(1), lengths.data_ptr(), B, T, D, int(n),
+                                  out.data_ptr(), None if out_sum is None else out_sum.data_ptr(), _stream()))
+    return out
+
+
+def global_variance(x, lengths):
+    """np.var(x[b, :lengths[b]].astype(np.float64), axis=0) of every row b (gantts_global_variance): x (B, T, D) CUDA
+    float32, lengths int64 CUDA (B,).  Returns (B, D) float64.  No host sync."""
+    x, lengths = _feature_args(x, lengths, "global_variance")
+    lib = _lib.load()
+    B, T, D = x.shape
+    out = torch.empty(B, D, dtype=torch.float64, device=x.device)
+    _lib.check(lib.gantts_global_variance(x.data_ptr(), x.stride(0), x.stride(1), lengths.data_ptr(), B, T, D,
+                                          out.data_ptr(), _stream()))
+    return out
+
+
 def distortion_sums(y, y_hat, lengths, mean, std, mcd=(0, 0), bap=(0, 0), lf0_col=-1, vuv_col=-1,
                     lf0_linear=True, mse=(0, 0)):
     """Eight sums behind the objective metrics of reference train.py:399-432 (see include/gantts_b200.h,

@@ -612,6 +612,24 @@ int gantts_mcep_to_sp(const float* mc, int64_t mc_bstride, int64_t mc_tstride, f
                       int64_t sp_tstride, const double* op_s, const int64_t* lengths_dev, int B, int T, int M, int K,
                       void* stream);
 
+/* Objective measures of generated features (the reference notebooks' vis_gv and mean_modspec), per feature column of
+ * every row of a padded batch x float32 [B][T][D] (element strides x_bstride, x_tstride; unit column stride), over
+ * the row's own L = lengths_dev[b] frames (int64[B], clamped to [0, T]).  Frames at or beyond L are never read.
+ * gantts_modspec: out[b][k][d] = log(|rfft(x[b, :L, d], n)[k]|^2) in fp64, k = 0 .. n/2 (nnmnkwii.preprocessing.modspec
+ *   followed by np.log; frames beyond n are cropped, shorter columns zero-padded, a zero power gives -inf).  out is
+ *   contiguous fp64 [B][n/2+1][D].  sum_dev: NULL, or a contiguous fp64 [n/2+1][D] to which out[0], out[1], ... are
+ *   added in that order after the spectra are written.
+ * gantts_global_variance: out[b][d] = np.var(x[b, :L, d]) in fp64 (two passes, ddof 0; L = 0 gives NaN); out is
+ *   contiguous fp64 [B][D].
+ * Both compute in fp64, and a column's result depends on nothing but its valid frames: the same bits at any batch
+ * position, padded length or padding contents, whatever the other columns hold.  Rules, checked before any device work
+ * (the error string names the one that failed): lengths_dev non-null, 1 <= B <= 65535, 1 <= T <= 2^24,
+ * 1 <= D <= 65535, strides >= 0, non-null x and out, and for gantts_modspec n a power of two in [64, 8192]. */
+int gantts_modspec(const float* x, int64_t x_bstride, int64_t x_tstride, const int64_t* lengths_dev, int B, int T,
+                   int D, int n, double* out, double* sum_dev, void* stream);
+int gantts_global_variance(const float* x, int64_t x_bstride, int64_t x_tstride, const int64_t* lengths_dev, int B,
+                           int T, int D, double* out, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Objective distortions of the training loop (reference train.py:399-432 compute_distortions, :383-396
  * split_streams, :358-380 inv_scale; nnmnkwii.metrics.{melcd, lf0_mean_squared_error, vuv_error,
