@@ -134,6 +134,9 @@ class EpochLogT(ctypes.Structure):
 
 OPT_ADAGRAD, OPT_ADAM = 0, 1
 MCEP_R0, MCEP_SP = 0, 1     # GANTTS_MCEP_*: merlin_post_filter's energy operator, mc2sp's
+SUBPHONE_FEATURES = 9       # GANTTS_SUBPHONE_FEATURES: Merlin's "full" frame-position columns
+FRAMES_BAD_DURATION, FRAMES_TOO_LONG = 1, 2     # GANTTS_FRAMES_*: gantts_state_frame_offsets' status bits
+MAX_FRAMES = 1 << 24        # per state duration and per row
 GANTTS_E_BADARG = 1
 
 _lib = None
@@ -172,6 +175,9 @@ SIGNATURES = {
     "gantts_mcep_to_sp": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _i, _i, _i, _i, _vp]),
     "gantts_modspec": (_i, [_vp, _i64, _i64, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "gantts_global_variance": (_i, [_vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp]),
+    "gantts_state_frame_offsets": (_i, [_vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "gantts_expand_state_frames": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp,
+                                        _vp]),
     "gantts_distortions_workspace_bytes": (_sz, []),
     "gantts_distortions": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp,
                                 ctypes.POINTER(DistortionColsT), _vp, _vp, _sz, _vp]),

@@ -389,6 +389,72 @@ def global_variance(x, lengths):
     return out
 
 
+# ------------------------------------------------------------- phone rows and state durations to frames
+def _durations(dur, what):
+    require_cuda(dur)
+    if dur.dim() != 3:
+        raise RuntimeError("gantts_b200: %s needs durations (B, P, S)" % what)
+    return dur if dur.stride(2) == 1 else dur.contiguous()
+
+
+def state_frame_offsets(dur, phone_lengths):
+    """Each phone's first frame (gantts_state_frame_offsets): dur (B, P, S) CUDA float32 state durations, any batch and
+    phone strides; phone_lengths int64 CUDA (B,).  Returns (offsets int64 CUDA (B, P+1), frame_lengths int64 CUDA (B,),
+    frame_lengths as a host numpy array).  Makes the one host synchronisation of the duration-to-frames chain: a single
+    device-to-host copy of the frame lengths and the status word, because the frame count sizes the acoustic batch.
+    Raises RuntimeError naming the rule when a duration is not a finite integer in [1, 2^24] or a row is too long."""
+    dur = _durations(dur, "state_frame_offsets")
+    if not (torch.is_tensor(phone_lengths) and phone_lengths.is_cuda and phone_lengths.dtype == torch.int64):
+        raise RuntimeError("gantts_b200: state_frame_offsets needs int64 CUDA phone lengths")
+    lib = _lib.load()
+    B, P, S = dur.shape
+    phone_lengths = phone_lengths.contiguous()
+    offsets = torch.empty(B, P + 1, dtype=torch.int64, device=dur.device)
+    buf = torch.empty(B + 1, dtype=torch.int64, device=dur.device)     # frame lengths, then the status word
+    _lib.check(lib.gantts_state_frame_offsets(dur.data_ptr(), dur.stride(0), dur.stride(1), phone_lengths.data_ptr(),
+                                              B, P, S, offsets.data_ptr(), buf.data_ptr(), buf[B:].data_ptr(),
+                                              _stream()))
+    host = buf.cpu().numpy()
+    status = int(host[B])
+    if status & _lib.FRAMES_BAD_DURATION:
+        raise RuntimeError("gantts_b200: state_frame_offsets: a state duration is not a finite integer in [1, %d]"
+                           % _lib.MAX_FRAMES)
+    if status & _lib.FRAMES_TOO_LONG:
+        raise RuntimeError("gantts_b200: state_frame_offsets: a row has more than %d frames (max %d)"
+                           % (_lib.MAX_FRAMES, int(host[:B].max())))
+    return offsets, buf[:B], host[:B].copy()
+
+
+def expand_state_frames(phone_x, dur, offsets, frame_lengths, scale, min_, T):
+    """The acoustic model's inputs (gantts_expand_state_frames): every phone's row of phone_x (B, P, L) CUDA float32
+    repeated over its frames and followed by Merlin's nine "full" subphone features of its durations dur (B, P, S), then
+    fl(fl(v * scale) + min_) per column in float32 (generate.normalize_input's arithmetic; scale 1 and min_ 0 give the raw
+    features).  offsets, frame_lengths: state_frame_offsets' device tensors; scale, min_: (L+9,) float32.  Returns
+    (B, T, L+9) float32, 0 at and beyond each row's frame length.  No host sync."""
+    require_cuda(phone_x)
+    dur = _durations(dur, "expand_state_frames")
+    if phone_x.dim() != 3 or phone_x.shape[:2] != dur.shape[:2]:
+        raise RuntimeError("gantts_b200: expand_state_frames needs phone_x (B, P, L) and dur (B, P, S)")
+    if phone_x.stride(2) != 1:
+        phone_x = phone_x.contiguous()
+    B, P, L = phone_x.shape
+    S = dur.shape[2]
+    W = L + _lib.SUBPHONE_FEATURES
+    for t, shape in ((offsets, (B, P + 1)), (frame_lengths, (B,))):
+        if not (t.is_cuda and t.dtype == torch.int64 and tuple(t.shape) == shape and t.is_contiguous()):
+            raise RuntimeError("gantts_b200: expand_state_frames needs state_frame_offsets' contiguous int64 offsets "
+                               "(B, P+1) and frame lengths (B,)")
+    dev = phone_x.device
+    scale, min_ = _column_vector(scale, W, dev, "scale"), _column_vector(min_, W, dev, "min")
+    lib = _lib.load()
+    out = torch.empty(B, int(T), W, dtype=torch.float32, device=dev)
+    _lib.check(lib.gantts_expand_state_frames(phone_x.data_ptr(), phone_x.stride(0), phone_x.stride(1), dur.data_ptr(),
+                                              dur.stride(0), dur.stride(1), offsets.data_ptr(), frame_lengths.data_ptr(),
+                                              scale.data_ptr(), min_.data_ptr(), B, P, L, S, int(T), out.data_ptr(),
+                                              _stream()))
+    return out
+
+
 def distortion_sums(y, y_hat, lengths, mean, std, mcd=(0, 0), bap=(0, 0), lf0_col=-1, vuv_col=-1,
                     lf0_linear=True, mse=(0, 0)):
     """Eight sums behind the objective metrics of reference train.py:399-432 (see include/gantts_b200.h,

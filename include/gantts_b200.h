@@ -630,6 +630,39 @@ int gantts_modspec(const float* x, int64_t x_bstride, int64_t x_tstride, const i
 int gantts_global_variance(const float* x, int64_t x_bstride, int64_t x_tstride, const int64_t* lengths_dev, int B,
                            int T, int D, double* out, void* stream);
 
+/* Acoustic-model inputs from phone-level rows and predicted state durations (replaces, per utterance, the frame
+ * expansion of reference evaluation_tts.py:200-212: fe.linguistic_features(labels with the durations set,
+ * add_frame_features=True, subphone_features="full"), silence frames removed, P.minmax_scale).  Phone p of row b has
+ * state durations d_1..d_S (dur float32 [B][P][S], element strides dur_bstride, dur_pstride, unit state stride),
+ * N = sum d_s frames and base_s = sum_{r<s} d_r.  Frame i (0-based) of state s (1-based) is the phone's L linguistic
+ * columns followed by GANTTS_SUBPHONE_FEATURES columns (Merlin's "full" block):
+ *   L+0 (i+1)/d_s   L+1 (d_s-i)/d_s   L+2 d_s   L+3 s   L+4 S+1-s   L+5 N   L+6 d_s/N   L+7 (N-i-base_s)/N
+ *   L+8 (base_s+i+1)/N
+ * each computed in double and rounded to float.
+ * gantts_state_frame_offsets: offsets int64 [B][P+1], offsets[b][p] the first frame of phone p (an exact prefix sum of
+ *   the phones' N; phones at or beyond the row's length phone_lengths_dev[b] (int64[B], clamped to [0, P]) count 0
+ *   frames and are never read), frame_lengths int64 [B] = offsets[b][P].  *status_dev (int64) is zeroed and then gets
+ *   GANTTS_FRAMES_BAD_DURATION when a duration read is not a finite integer in [1, 2^24] (it is counted as 1) and
+ *   GANTTS_FRAMES_TOO_LONG when a row has more than 2^24 frames.  No host synchronisation: the caller reads the status.
+ * gantts_expand_state_frames: out contiguous float32 [B][T][L+9], frame t of row b = fl(fl(v * scale_dev[c]) +
+ *   min_dev[c]) per column c (two float32 roundings, no FMA: generate.normalize_input's arithmetic on float32
+ *   statistics; scale 1 and min 0 give the raw features), v the raw value.  phone_x float32 [B][P][L] (element strides
+ *   x_bstride, x_pstride, unit column stride); offsets and frame_lengths as gantts_state_frame_offsets wrote them.
+ *   Frames at and beyond min(frame_lengths[b], T) are written as 0, frames >= T never.  A row's bits depend only on
+ *   its own valid phones and durations.
+ * Rules, checked before any device work (the error string names the one that failed): non-null pointers,
+ * 1 <= B <= 65535, P >= 1, 1 <= S <= 16, strides >= 0, and for the expansion 1 <= L <= 65535, 1 <= T <= 2^24. */
+#define GANTTS_SUBPHONE_FEATURES 9
+#define GANTTS_FRAMES_BAD_DURATION 1
+#define GANTTS_FRAMES_TOO_LONG 2
+int gantts_state_frame_offsets(const float* dur, int64_t dur_bstride, int64_t dur_pstride,
+                               const int64_t* phone_lengths_dev, int B, int P, int S, int64_t* offsets,
+                               int64_t* frame_lengths, int64_t* status_dev, void* stream);
+int gantts_expand_state_frames(const float* phone_x, int64_t x_bstride, int64_t x_pstride, const float* dur,
+                               int64_t dur_bstride, int64_t dur_pstride, const int64_t* offsets,
+                               const int64_t* frame_lengths, const float* scale_dev, const float* min_dev, int B,
+                               int P, int L, int S, int T, float* out, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Objective distortions of the training loop (reference train.py:399-432 compute_distortions, :383-396
  * split_streams, :358-380 inv_scale; nnmnkwii.metrics.{melcd, lf0_mean_squared_error, vuv_error,
