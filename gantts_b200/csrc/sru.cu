@@ -400,6 +400,9 @@ static int launch_sru_step_bwd(const SruStepBwd& p, int k, cudaStream_t st) {
 static int sru_check(const SruParams& p) {
   GANTTS_CHECK_ARG(p.B >= 1 && p.T >= 1 && p.d >= 1 && (p.k == 3 || p.k == 4), "sru: bad shape (B=%d T=%d d=%d k=%d)",
                    p.B, p.T, p.d, p.k);
+  // one thread per (batch row, column): the launches count B * columns in int
+  GANTTS_CHECK_ARG((int64_t)p.B * p.d * (p.bidir ? 2 : 1) <= ((int64_t)1 << 30),
+                   "sru: B = %d and d = %d must be >= 1 with B * columns <= 2^30", p.B, p.d);
   GANTTS_CHECK_ARG(p.act >= 0 && p.act <= 2, "sru: bad activation %d", p.act);
   GANTTS_CHECK_ARG(p.u && p.bias && (p.k == 4 || p.x), "sru: null pointer");
   return GANTTS_OK;

@@ -292,7 +292,8 @@ int gantts_dropout(const float* x, float* y, int64_t rows, int cols, float p, ui
  * x [B][T][ncols] is the highway input when k == 3; bias [2*ncols] = forget | reset; mask_h [B][ncols]
  * optional (already scaled) output dropout mask shared over time; act: 0 identity, 1 tanh, 2 relu.
  * Outputs h, c [B][T][ncols].  Backward: du [B][T][ncols*k], dx += (k == 3), dbias_part [B][2*ncols]
- * (sum over B gives the bias gradient).
+ * (sum over B gives the bias gradient).  Rules, checked before any device work: B, T, d >= 1, k = 3 or 4,
+ * B * ncols <= 2^30.
  */
 int gantts_sru_fwd(const float* u, const float* x, const float* bias, const float* mask_h, float* h, float* c,
                    int B, int T, int d, int k, int bidir, int act, void* stream);
