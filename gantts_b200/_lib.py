@@ -137,6 +137,7 @@ MCEP_R0, MCEP_SP = 0, 1     # GANTTS_MCEP_*: merlin_post_filter's energy operato
 SUBPHONE_FEATURES = 9       # GANTTS_SUBPHONE_FEATURES: Merlin's "full" frame-position columns
 FRAMES_BAD_DURATION, FRAMES_TOO_LONG = 1, 2     # GANTTS_FRAMES_*: gantts_state_frame_offsets' status bits
 MAX_FRAMES = 1 << 24        # per state duration and per row
+CORPUS_BAD_ROW = 1          # GANTTS_CORPUS_BAD_ROW: gantts_corpus_gather's status bit
 GANTTS_E_BADARG = 1
 
 _lib = None
@@ -178,6 +179,7 @@ SIGNATURES = {
     "gantts_state_frame_offsets": (_i, [_vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "gantts_expand_state_frames": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp,
                                         _vp]),
+    "gantts_corpus_gather": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "gantts_distortions_workspace_bytes": (_sz, []),
     "gantts_distortions": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp,
                                 ctypes.POINTER(DistortionColsT), _vp, _vp, _sz, _vp]),

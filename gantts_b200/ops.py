@@ -455,6 +455,39 @@ def expand_state_frames(phone_x, dur, offsets, frame_lengths, scale, min_, T):
     return out
 
 
+# ------------------------------------------------------------- mini-batches from a corpus on the device
+def corpus_gather(X, Y, offsets, lengths, t, x_out=None, y_out=None, status=None):
+    """One padded mini-batch from a packed corpus on the device (gantts_corpus_gather): X (N, Dx), Y (N, Dy) contiguous
+    CUDA float32, the utterances' frames one after another; offsets, lengths contiguous int64 CUDA (b,), row r the
+    utterance at frames [offsets[r], offsets[r] + lengths[r]).  Returns (x (b, t, Dx), y (b, t, Dy)) float32, 0 at and
+    beyond each row's length, written into x_out / y_out when given (contiguous, of those shapes).  status: None, or an
+    int64 CUDA scalar into which GANTTS_CORPUS_BAD_ROW is OR-ed when a row lies outside the corpus or is longer than t
+    (that row is written as 0).  One launch, no host sync."""
+    require_cuda(X, Y, x_out, y_out)
+    if X.dim() != 2 or Y.dim() != 2 or X.shape[0] != Y.shape[0] or not (X.is_contiguous() and Y.is_contiguous()):
+        raise RuntimeError("gantts_b200: corpus_gather needs contiguous X (N, Dx) and Y (N, Dy) of the same N")
+    for v in (offsets, lengths):
+        if not (torch.is_tensor(v) and v.is_cuda and v.dtype == torch.int64 and v.dim() == 1 and v.is_contiguous()):
+            raise RuntimeError("gantts_b200: corpus_gather needs contiguous int64 CUDA offsets and lengths (b,)")
+    if offsets.numel() != lengths.numel():
+        raise RuntimeError("gantts_b200: corpus_gather: offsets and lengths differ in length")
+    if status is not None and not (status.is_cuda and status.dtype == torch.int64 and status.numel() == 1):
+        raise RuntimeError("gantts_b200: corpus_gather's status must be an int64 CUDA scalar")
+    b, t, dev = offsets.numel(), int(t), X.device
+    out = []
+    for given, D in ((x_out, X.shape[1]), (y_out, Y.shape[1])):
+        if given is None:
+            given = torch.empty(b, t, D, dtype=torch.float32, device=dev)
+        elif tuple(given.shape) != (b, t, D) or not given.is_contiguous():
+            raise RuntimeError("gantts_b200: corpus_gather's outputs must be contiguous (%d, %d, %d)" % (b, t, D))
+        out.append(given)
+    lib = _lib.load()
+    _lib.check(lib.gantts_corpus_gather(X.data_ptr(), Y.data_ptr(), X.shape[0], X.shape[1], Y.shape[1],
+                                        offsets.data_ptr(), lengths.data_ptr(), b, t, out[0].data_ptr(),
+                                        out[1].data_ptr(), None if status is None else status.data_ptr(), _stream()))
+    return out[0], out[1]
+
+
 def distortion_sums(y, y_hat, lengths, mean, std, mcd=(0, 0), bap=(0, 0), lf0_col=-1, vuv_col=-1,
                     lf0_linear=True, mse=(0, 0)):
     """Eight sums behind the objective metrics of reference train.py:399-432 (see include/gantts_b200.h,

@@ -24,7 +24,8 @@ options:
 # The usage above is the reference train.py's, so each `python train.py ...` line of train_gan.sh runs as
 # `python -m gantts_b200.train ...`.  The step is FusedGanStep (one native call per mini-batch) whenever it takes the
 # models, else GanTrainer; each phase's logged values accumulate on the device (epochlog.EpochLog) and are read once
-# per phase.  --disable-slack is accepted and does nothing.
+# per phase.  Each split's normalised features stay on the device when they fit (DeviceBatches), so a mini-batch is
+# one gather kernel rather than a host collate and copy.  --disable-slack is accepted and does nothing.
 import json
 import os
 import sys
@@ -38,6 +39,7 @@ from torch.utils import data as data_utils
 
 from . import models
 from . import multistream
+from . import ops
 from .epochlog import EpochLog
 from .fused import LOSS_NAMES, FusedGanStep
 from .step import GanTrainer
@@ -164,9 +166,91 @@ def sort_batch(x, y, lengths):
     return x[indices], y[indices], sorted_lengths.long()
 
 
+def _indices(batch):
+    return np.asarray(batch, dtype=np.int64)
+
+
+def pack_corpus(dataset):
+    """Every utterance of `dataset` (pairs of frame arrays) as collate_fn casts it, float32, packed frame after frame:
+    (X (N, Dx), Y (N, Dy), lengths int64 per utterance)."""
+    xs, ys = [], []
+    for i in range(len(dataset)):
+        x, y = dataset[i]
+        xs.append(np.asarray(x, dtype=np.float32))
+        ys.append(np.asarray(y, dtype=np.float32))
+    lengths = np.array([len(x) for x in xs], dtype=np.int64)
+    return np.concatenate(xs), np.concatenate(ys), lengths
+
+
+class BatchPlan(object):
+    """The host side of DeviceBatches: which utterances make each mini-batch, in which row order.  The batches and the
+    draws from the global torch RNG are those of a DataLoader over the dataset with the same batch_size and shuffle,
+    because a DataLoader over the indices alone makes them; each batch's rows are sorted by sort_batch's torch.sort."""
+
+    def __init__(self, lengths, batch_size, shuffle):
+        self.lengths = np.asarray(lengths, dtype=np.int64)
+        self.starts = np.concatenate([[0], np.cumsum(self.lengths)[:-1]]).astype(np.int64)
+        self.index_loader = data_utils.DataLoader(range(len(self.lengths)), batch_size=batch_size, shuffle=shuffle,
+                                                  collate_fn=_indices)
+
+    def __len__(self):
+        return len(self.index_loader)
+
+    def epoch(self):
+        """One epoch: (plan int64 (2, rows), bounds).  plan[0] holds each row's first frame in the pack and plan[1]
+        its length, batch after batch; batch j is rows bounds[j]:bounds[j + 1]."""
+        rows, bounds = [], [0]
+        for idx in self.index_loader:
+            _, order = torch.sort(torch.from_numpy(self.lengths[idx]), dim=0, descending=True)
+            rows.append(idx[order.numpy()])
+            bounds.append(bounds[-1] + len(idx))
+        rows = np.concatenate(rows) if rows else np.zeros(0, dtype=np.int64)
+        return np.stack([self.starts[rows], self.lengths[rows]]), bounds
+
+
+class DeviceBatches(object):
+    """One split's normalised features resident on the device, batched as a DataLoader over `dataset` with collate_fn,
+    then sort_batch, batches them, bit for bit and with the same draws from the global torch RNG.  Each utterance is
+    normalised once, here, by the dataset's own __getitem__.  Iterating yields (x, y, lengths, host lengths) per batch:
+    x, y padded on the device by one gantts_corpus_gather launch, lengths a slice of the epoch's plan, which is copied to
+    the device once per epoch.  Nothing is copied per batch and nothing waits for the device."""
+
+    def __init__(self, dataset, batch_size, shuffle, device):
+        X, Y, lengths = pack_corpus(dataset)
+        self.plan = BatchPlan(lengths, batch_size, shuffle)
+        self.X = torch.from_numpy(X).to(device)
+        self.Y = torch.from_numpy(Y).to(device)
+        self.device = device
+
+    def __len__(self):
+        return len(self.plan)
+
+    def __iter__(self):
+        plan, bounds = self.plan.epoch()
+        # A fresh pinned buffer per epoch: the host allocator does not hand it out again before the copy has read it.
+        staged = torch.empty(plan.shape, dtype=torch.int64, pin_memory=True)
+        staged.numpy()[...] = plan
+        dev = staged.to(self.device, non_blocking=True)
+        for j in range(len(bounds) - 1):
+            s, e = bounds[j], bounds[j + 1]
+            lengths = dev[1, s:e]
+            x, y = ops.corpus_gather(self.X, self.Y, dev[0, s:e], lengths, int(plan[1, s]))
+            yield x, y, lengths, plan[1, s:e].tolist()
+
+
+def device_corpus_budget():
+    """Bytes the resident corpus may take on the current CUDA device: half of its free memory (0 without CUDA)."""
+    if not torch.cuda.is_available():
+        return 0
+    return torch.cuda.mem_get_info()[0] // 2
+
+
 def load_data(hp, inputs_dir, outputs_dir, max_files):
     """Datasets, statistics (saved to data_dir under the reference's names), derived dims and the two loaders
-    (train.py:701-770).  Returns (loaders, Y_data_mean, Y_data_std, longest utterance of either split)."""
+    (train.py:701-770).  Returns (loaders, Y_data_mean, Y_data_std, longest utterance of either split).
+
+    The loaders are DeviceBatches when both splits fit in device_corpus_budget() and every utterance has a frame, else
+    train.py's DataLoaders; both give the same batches from the same RNG draws."""
     data_dir = abspath(join(inputs_dir, os.pardir))
     assert data_dir == abspath(join(outputs_dir, os.pardir))
     X, Y, utt_lengths = {}, {}, {}
@@ -204,9 +288,26 @@ def load_data(hp, inputs_dir, outputs_dir, max_files):
         derive_tts_dims(hp, X_data_min.shape[-1], Y_data_mean.shape[-1])
         make = lambda p: TTSDataset(X[p], Y[p], X_data_min, X_data_max, Y_data_mean, Y_data_std, hp)
         Y_mean, Y_std = Y_data_mean, Y_data_std
-    loaders = {p: data_utils.DataLoader(make(p), batch_size=hp.batch_size, num_workers=hp.num_workers,
-                                        pin_memory=hp.pin_memory, shuffle=(p == "train"), collate_fn=collate_fn)
-               for p in ("train", "test")}
+    frames = sum(int(v.sum()) for v in utt_lengths.values())
+    widths = [(X[p][0].shape[-1], Y[p][0].shape[-1]) for p in ("train", "test") if len(X[p])][0]
+    corpus_mb = frames * sum(widths) * 4 / 2**20
+    # A batch whose utterances all have 0 frames pads to t = 0, which collate_fn returns and the gather refuses.
+    empty = any(len(v) and v.min() < 1 for v in utt_lengths.values())
+    budget = 0 if empty else device_corpus_budget()
+    if all(len(X[p]) for p in ("train", "test")) and frames * sum(widths) * 4 <= budget:
+        device = torch.device("cuda", torch.cuda.current_device())
+        loaders = {p: DeviceBatches(make(p), hp.batch_size, p == "train", device) for p in ("train", "test")}
+        print("Data loader: device corpus on {}, {} frames x ({} + {}) float32 columns = {:.1f} MB".format(
+            device, frames, widths[0], widths[1], corpus_mb))
+    else:
+        loaders = {p: data_utils.DataLoader(make(p), batch_size=hp.batch_size, num_workers=hp.num_workers,
+                                            pin_memory=hp.pin_memory, shuffle=(p == "train"), collate_fn=collate_fn)
+                   for p in ("train", "test")}
+        if empty:
+            print("Data loader: host DataLoader (an utterance has no frames)")
+        else:
+            print("Data loader: host DataLoader, corpus {:.1f} MB, device budget {:.1f} MB".format(corpus_mb,
+                                                                                                budget / 2**20))
     return loaders, Y_mean, Y_std, longest
 
 
@@ -307,17 +408,22 @@ def make_path(model_g, model_d, hp, B, T, w_d, mse_w, mge_w, reference_discrimin
 
 # ---- the loop (train.py:435-648) ----
 
-def run_phase(path, loader, log, phase, adv_w, update_d, update_g, device):
-    """One phase: every batch sorted on the host, copied without blocking, stepped and folded into `log` on the device.
-    Nothing here waits for the GPU; the caller reads `log` once."""
-    log.reset()
-    train = phase == "train"
+def host_batches(loader, device):
+    """The batches of a host DataLoader as DeviceBatches yields them: sorted on the host, copied without blocking."""
     for x, y, lengths in loader:
         x, y, lengths = sort_batch(x, y, lengths)
         cpu_lengths = lengths.tolist()
-        x = x.to(device, non_blocking=True)
-        y = y.to(device, non_blocking=True)
-        lengths = lengths.to(device, non_blocking=True)
+        yield (x.to(device, non_blocking=True), y.to(device, non_blocking=True),
+               lengths.to(device, non_blocking=True), cpu_lengths)
+
+
+def run_phase(path, loader, log, phase, adv_w, update_d, update_g, device):
+    """One phase: every batch (DeviceBatches, or a host DataLoader's through host_batches) stepped and folded into `log`
+    on the device.  Nothing here waits for the GPU; the caller reads `log` once."""
+    log.reset()
+    train = phase == "train"
+    batches = loader if isinstance(loader, DeviceBatches) else host_batches(loader, device)
+    for x, y, lengths, cpu_lengths in batches:
         losses, y_hat_static, spoof = path.step(x, y, lengths, cpu_lengths, adv_w, train, update_g)
         log.add(losses, y, y_hat_static, lengths, update_d, update_g, spoof)
 

@@ -664,6 +664,23 @@ int gantts_expand_state_frames(const float* phone_x, int64_t x_bstride, int64_t 
                                const int64_t* frame_lengths, const float* scale_dev, const float* min_dev, int B,
                                int P, int L, int S, int T, float* out, void* stream);
 
+/* Mini-batches of the training loop gathered from a split held on the device (replaces, per batch, reference
+ * train.py:145-159 collate_fn and the sort of :494-501 on the host, and the batch's host-to-device copy).  The split's
+ * normalised utterances are packed frame after frame: X float32 [N][Dx] and Y float32 [N][Dy], contiguous.  Row r of
+ * the batch is the utterance at frames [offsets_dev[r], offsets_dev[r] + lengths_dev[r]) of the pack (int64[b] each,
+ * on the device; the caller lists the rows in sorted order).  Outputs, contiguous float32: x_out [b][t][Dx] and
+ * y_out [b][t][Dy], where row r's first lengths_dev[r] frames are the utterance's frames and frames at or beyond its
+ * length are written as 0.  One launch writes both outputs; it only copies, so a row's bits are its utterance's bits
+ * and depend on nothing else.  A row with offsets_dev[r] < 0, lengths_dev[r] < 0, lengths_dev[r] > t or
+ * offsets_dev[r] + lengths_dev[r] > N is written as all 0 and, when status_dev is non-null, GANTTS_CORPUS_BAD_ROW is
+ * OR-ed into *status_dev (never cleared here: the caller zeroes it and reads it when it chooses).  No host
+ * synchronisation.  Rules, checked before any device work (the error string names the one that failed): non-null
+ * X, Y, offsets_dev, lengths_dev, x_out and y_out, N >= 1, 1 <= Dx, Dy <= 65535, 1 <= b <= 65535, 1 <= t <= 2^24. */
+#define GANTTS_CORPUS_BAD_ROW 1
+int gantts_corpus_gather(const float* X, const float* Y, int64_t N, int Dx, int Dy, const int64_t* offsets_dev,
+                         const int64_t* lengths_dev, int b, int t, float* x_out, float* y_out, int64_t* status_dev,
+                         void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Objective distortions of the training loop (reference train.py:399-432 compute_distortions, :383-396
  * split_streams, :358-380 inv_scale; nnmnkwii.metrics.{melcd, lf0_mean_squared_error, vuv_error,
