@@ -138,6 +138,7 @@ SUBPHONE_FEATURES = 9       # GANTTS_SUBPHONE_FEATURES: Merlin's "full" frame-po
 FRAMES_BAD_DURATION, FRAMES_TOO_LONG = 1, 2     # GANTTS_FRAMES_*: gantts_state_frame_offsets' status bits
 MAX_FRAMES = 1 << 24        # per state duration and per row
 CORPUS_BAD_ROW = 1          # GANTTS_CORPUS_BAD_ROW: gantts_corpus_gather's status bit
+WORLD_BAD_F0, WORLD_SHORT = 1, 2    # GANTTS_WORLD_*: gantts_world_time_base's status bits
 GANTTS_E_BADARG = 1
 
 _lib = None
@@ -180,6 +181,16 @@ SIGNATURES = {
     "gantts_expand_state_frames": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp,
                                         _vp]),
     "gantts_corpus_gather": (_i, [_vp, _vp, _i64, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
+    "gantts_world_band_count": (_i, [_i]),
+    "gantts_world_y_length": (_i64, [_i64, _i, ctypes.c_double]),
+    "gantts_world_decode_aperiodicity": (_i, [_vp, _i64, _i64, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "gantts_world_time_base": (_i, [_vp, _i64, _i64, _vp, _i, _i, _i, ctypes.c_double, _i, _i, _vp, _vp, _vp, _vp,
+                                    _vp]),
+    "gantts_world_randn_workspace_bytes": (_sz, [_i64]),
+    "gantts_world_randn": (_i, [_i64, _vp, _vp, _sz, _vp]),
+    "gantts_world_synthesize_workspace_bytes": (_sz, [_i, _i, _i64]),
+    "gantts_world_synthesize": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i, _i64, _vp, _i, _i,
+                                     _i, ctypes.c_double, _i, _i, _vp, _vp, _sz, _vp]),
     "gantts_distortions_workspace_bytes": (_sz, []),
     "gantts_distortions": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp,
                                 ctypes.POINTER(DistortionColsT), _vp, _vp, _sz, _vp]),

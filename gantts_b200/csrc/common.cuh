@@ -39,7 +39,7 @@ int cuda_fail(cudaError_t e, const char* what);
 // (gantts_profile_*): event pairs are recorded on the launching stream around each profiled launch.
 void count_launch();
 enum ProfKind { PROF_GEMM_KK = 0, PROF_GEMM_MN = 1, PROF_MLPG_FWD = 2, PROF_MLPG_BWD = 3, PROF_LSTM_FWD = 4,
-                PROF_LSTM_BWD = 5, PROF_KINDS = 8 };
+                PROF_LSTM_BWD = 5, PROF_WORLD_RESPONSE = 6, PROF_WORLD_OLA = 7, PROF_KINDS = 8 };
 void prof_begin(int kind, double work, cudaStream_t st);   // work: algorithmic flops or bytes
 void prof_end(cudaStream_t st);
 
@@ -103,6 +103,35 @@ __device__ __forceinline__ void block_sum(float (&v)[NV], float* smem) {
       v[i] = warp_sum(x);
     }
   }
+}
+
+// In-place radix-2 decimation-in-time FFT of N = n/2 complex points in shared memory, by the whole block: z holds the
+// input in bit-reversed order, w[j] = exp(-2 pi i j / n) for j < N; butterflies of span h use the twiddle
+// exp(-2 pi i pos / 2h) = w[pos * N / h].  Ends with a barrier.  (modspec.cu, world.cu)
+__device__ __forceinline__ void fft_radix2_stages(double2* z, const double2* w, int N) {
+  for (int h = 1; h < N; h <<= 1) {
+    const int step = N / h;
+    for (int i = threadIdx.x; i < N / 2; i += blockDim.x) {
+      const int pos = i & (h - 1), i0 = ((i - pos) << 1) + pos, i1 = i0 + h;
+      const double2 tw = w[pos * step], a = z[i0], v = z[i1];
+      const double tr = tw.x * v.x - tw.y * v.y, ti = tw.x * v.y + tw.y * v.x;
+      z[i0] = make_double2(a.x + tr, a.y + ti);
+      z[i1] = make_double2(a.x - tr, a.y - ti);
+    }
+    __syncthreads();
+  }
+}
+
+// Bin k (0 <= k <= N) of the n-point real FFT X of x from Z, the N-point FFT of x[2j] + i x[2j+1]:
+// X[k] = E[k] + w^k O[k], E = (Z[k] + conj Z[N-k]) / 2, O = (Z[k] - conj Z[N-k]) / 2i.
+__device__ __forceinline__ double2 rfft_split(const double2* z, const double2* w, int k, int N) {
+  if (k == 0 || k == N)                                  // E[0] = Re Z[0], O[0] = Im Z[0], w^N = -1
+    return make_double2(k == 0 ? z[0].x + z[0].y : z[0].x - z[0].y, 0.0);
+  const double2 a = z[k], c = z[N - k];
+  const double er = 0.5 * (a.x + c.x), ei = 0.5 * (a.y - c.y);
+  const double orr = 0.5 * (a.y + c.y), oi = -0.5 * (a.x - c.x);
+  const double2 tw = w[k];
+  return make_double2(er + (tw.x * orr - tw.y * oi), ei + (tw.x * oi + tw.y * orr));
 }
 
 // Counter-based keep decision for dropout: one 32-bit mixing chain per FOUR adjacent columns

@@ -52,33 +52,12 @@ __global__ void __launch_bounds__(MS_THREADS) modspec_kernel(const FeatureParams
     z[__brev((unsigned)j) >> (32 - logN)] = make_double2(re, im);
   }
   __syncthreads();
-  for (int h = 1; h < N; h <<= 1) {                      // butterflies of span h: twiddle exp(-2 pi i pos / 2h)
-    const int step = N / h;
-    for (int i = threadIdx.x; i < N / 2; i += blockDim.x) {
-      const int pos = i & (h - 1), i0 = ((i - pos) << 1) + pos, i1 = i0 + h;
-      const double2 tw = w[pos * step], a = z[i0], v = z[i1];
-      const double tr = tw.x * v.x - tw.y * v.y, ti = tw.x * v.y + tw.y * v.x;
-      z[i0] = make_double2(a.x + tr, a.y + ti);
-      z[i1] = make_double2(a.x - tr, a.y - ti);
-    }
-    __syncthreads();
-  }
+  fft_radix2_stages(z, w, N);
   const int K = N + 1;
   double* o = out + (int64_t)b * K * p.D + d;
   for (int k = threadIdx.x; k < K; k += blockDim.x) {
-    double re, im;
-    if (k == 0 || k == N) {                              // E[0] = Re Z[0], O[0] = Im Z[0], w^N = -1
-      re = k == 0 ? z[0].x + z[0].y : z[0].x - z[0].y;
-      im = 0.0;
-    } else {
-      const double2 a = z[k], c = z[N - k];
-      const double er = 0.5 * (a.x + c.x), ei = 0.5 * (a.y - c.y);
-      const double orr = 0.5 * (a.y + c.y), oi = -0.5 * (a.x - c.x);
-      const double2 tw = w[k];
-      re = er + (tw.x * orr - tw.y * oi);
-      im = ei + (tw.x * oi + tw.y * orr);
-    }
-    o[(int64_t)k * p.D] = log(re * re + im * im);
+    const double2 X = rfft_split(z, w, k, N);
+    o[(int64_t)k * p.D] = log(X.x * X.x + X.y * X.y);
   }
 }
 

@@ -455,6 +455,126 @@ def expand_state_frames(phone_x, dur, offsets, frame_lengths, scale, min_, T):
     return out
 
 
+# ------------------------------------------------------------- WORLD waveform synthesis
+WORLD_CHUNK_BYTES = 256 << 20   # per-pulse response buffer of world_synthesize: pulses beyond it run in further chunks
+
+
+def world_band_count(fs):
+    """WORLD's number of coded aperiodicity bands at fs: floor(min(15000, fs/2 - 3000) / 3000), 0 below 12 kHz."""
+    return int(_lib.load().gantts_world_band_count(int(fs)))
+
+
+def world_y_length(frames, fs, frame_period):
+    """int(frames * frame_period * fs / 1000): the samples pyworld.synthesize makes of `frames` frames."""
+    return int(_lib.load().gantts_world_y_length(int(frames), int(fs), float(frame_period)))
+
+
+def _world_rows(x, lengths, what, width=None):
+    """x (B, T) or (B, T, width) CUDA float32 -> (x, lengths) with a unit last stride."""
+    require_cuda(x)
+    if not (torch.is_tensor(lengths) and lengths.is_cuda and lengths.dtype == torch.int64):
+        raise RuntimeError("gantts_b200: %s needs int64 CUDA lengths" % what)
+    if x.dim() != 3 or (width is not None and x.shape[2] != width) or lengths.dim() != 1 \
+            or lengths.numel() != x.shape[0]:
+        raise RuntimeError("gantts_b200: %s needs x (B, T, %s) and lengths (B,)" % (what, width or "K"))
+    return (x if x.stride(2) == 1 else x.contiguous()), lengths.contiguous()
+
+
+def world_decode_aperiodicity(bap, lengths, fs, fftlen):
+    """pyworld.decode_aperiodicity(bap[b, :lengths[b]], fs, fftlen) of every row b (gantts_world_decode_aperiodicity):
+    bap (B, T, nb) CUDA float32 with nb = world_band_count(fs), lengths int64 CUDA (B,).  Returns (B, T, fftlen/2 + 1)
+    float64, 0 beyond each length.  No host sync."""
+    bap, lengths = _world_rows(bap, lengths, "world_decode_aperiodicity")
+    B, T, nb = bap.shape
+    ap = torch.empty(B, T, int(fftlen) // 2 + 1, dtype=torch.float64, device=bap.device)
+    _lib.check(_lib.load().gantts_world_decode_aperiodicity(bap.data_ptr(), bap.stride(0), bap.stride(1),
+                                                            lengths.data_ptr(), B, T, nb, int(fs), int(fftlen),
+                                                            ap.data_ptr(), _stream()))
+    return ap
+
+
+def world_time_base(f0, lengths, fs, frame_period, fftlen):
+    """WORLD's pulse locations of every row (gantts_world_time_base): f0 (B, T) or (B, T, 1) CUDA float32 in Hz, lengths
+    int64 CUDA (B,).  Returns a dict: "index" int32, "shift" float64 (seconds), "vuv" uint8, each (B, cap) CUDA with the
+    pulses of row b in its first counts[b] entries, and "counts", "y_lengths" as host int64 arrays.  Makes one host
+    synchronisation, the read of the counts, the y_lengths and the status word; raises RuntimeError naming the rule when
+    a valid f0 is not finite or a row has fewer than 2 frames."""
+    if f0.dim() == 2:
+        f0 = f0.unsqueeze(-1)
+    f0, lengths = _world_rows(f0, lengths, "world_time_base", 1)
+    B, T, _ = f0.shape
+    lib = _lib.load()
+    cap = world_y_length(T, fs, frame_period)
+    dev = f0.device
+    index = torch.empty(B, max(cap, 1), dtype=torch.int32, device=dev)
+    shift = torch.empty(B, max(cap, 1), dtype=torch.float64, device=dev)
+    vuv = torch.empty(B, max(cap, 1), dtype=torch.uint8, device=dev)
+    info = torch.empty(2 * B + 1, dtype=torch.int64, device=dev)
+    _lib.check(lib.gantts_world_time_base(f0.data_ptr(), f0.stride(0), f0.stride(1), lengths.data_ptr(), B, T, int(fs),
+                                          float(frame_period), int(fftlen), cap, index.data_ptr(), shift.data_ptr(),
+                                          vuv.data_ptr(), info.data_ptr(), _stream()))
+    host = info.cpu().numpy()
+    status = int(host[2 * B])
+    if status & _lib.WORLD_BAD_F0:
+        raise RuntimeError("gantts_b200: world_time_base: an f0 value within a row's length is not finite")
+    if status & _lib.WORLD_SHORT:
+        raise RuntimeError("gantts_b200: world_time_base: a row has fewer than 2 frames (WORLD synthesis needs 2)")
+    return {"index": index, "shift": shift, "vuv": vuv, "info": info, "cap": cap,
+            "counts": host[:B].copy(), "y_lengths": host[B:2 * B].copy()}
+
+
+def world_randn(count, device):
+    """Draws 0 .. count-1 of WORLD's randn after randn_reseed, float64 CUDA (count,), bit for bit (gantts_world_randn).
+    No host sync."""
+    lib = _lib.load()
+    out = torch.empty(int(count), dtype=torch.float64, device=device)
+    nbytes = lib.gantts_world_randn_workspace_bytes(int(count))
+    ws = workspace(nbytes, device, "world_randn")
+    _lib.check(lib.gantts_world_randn(int(count), out.data_ptr(), ws.data_ptr(), nbytes, _stream()))
+    return out
+
+
+def world_synthesize(f0, sp, ap, lengths, fs, frame_period, pulses=None, noise=None):
+    """pyworld.synthesize(f0[b, :F], sp[b, :F], ap[b, :F], fs, frame_period) of every row b, F = lengths[b]
+    (gantts_world_time_base, gantts_world_randn, gantts_world_synthesize): f0 (B, T) or (B, T, 1) CUDA float32 in Hz, sp
+    (B, T, fftlen/2 + 1) CUDA float32, ap the same shape in float64 (world_decode_aperiodicity), lengths int64 CUDA (B,).
+    Returns (y (B, Ymax) float64 CUDA with 0 beyond each row's y_length, y_lengths as a host int64 array).  The time
+    base's read of the pulse counts is the one host synchronisation; pulses: that time base, when already made.
+    noise: world_randn of at least Ymax draws, when already made (the stream is the same for every call)."""
+    sp, lengths = _world_rows(sp, lengths, "world_synthesize")
+    B, T, K = sp.shape
+    if not (torch.is_tensor(ap) and ap.is_cuda and ap.dtype == torch.float64 and tuple(ap.shape) == (B, T, K)):
+        raise RuntimeError("gantts_b200: world_synthesize needs ap (B, T, K) float64 CUDA, the shape of sp")
+    if ap.stride(2) != 1:
+        ap = ap.contiguous()
+    n = 2 * (K - 1)
+    if pulses is None:
+        pulses = world_time_base(f0, lengths, fs, frame_period, n)
+    lib = _lib.load()
+    y_lengths = pulses["y_lengths"]
+    y_max = max(int(y_lengths.max()), 1)
+    total = int(pulses["counts"].sum())
+    if noise is None:
+        noise = world_randn(y_max, sp.device)
+    elif not (noise.is_cuda and noise.dtype == torch.float64 and noise.dim() == 1 and noise.numel() >= y_max
+              and noise.is_contiguous()):
+        raise RuntimeError("gantts_b200: world_synthesize's noise must be world_randn's contiguous float64 CUDA draws, "
+                           "at least %d of them" % y_max)
+    chunk = max(1, min(total, WORLD_CHUNK_BYTES // (8 * n)))
+    nbytes = lib.gantts_world_synthesize_workspace_bytes(B, n, chunk)
+    if nbytes == 0:
+        raise RuntimeError("gantts_b200: world_synthesize: fftlen = %d must be a power of two in [64, 4096]" % n)
+    ws = workspace(nbytes, sp.device, "world_synthesize")
+    y = torch.empty(B, y_max, dtype=torch.float64, device=sp.device)
+    _lib.check(lib.gantts_world_synthesize(sp.data_ptr(), sp.stride(0), sp.stride(1), ap.data_ptr(), ap.stride(0),
+                                           ap.stride(1), lengths.data_ptr(), pulses["index"].data_ptr(),
+                                           pulses["shift"].data_ptr(), pulses["vuv"].data_ptr(),
+                                           pulses["info"].data_ptr(), pulses["cap"], total, noise.data_ptr(), B, T,
+                                           int(fs), float(frame_period), n, y_max, y.data_ptr(), ws.data_ptr(), nbytes,
+                                           _stream()))
+    return y, y_lengths
+
+
 # ------------------------------------------------------------- mini-batches from a corpus on the device
 def corpus_gather(X, Y, offsets, lengths, t, x_out=None, y_out=None, status=None):
     """One padded mini-batch from a packed corpus on the device (gantts_corpus_gather): X (N, Dx), Y (N, Dy) contiguous

@@ -42,10 +42,11 @@ const char* gantts_last_error_string(void);     /* thread-local, never NULL */
 int gantts_device_supported(void);
 /* Number of kernels this library has launched in this process (bench.py's gpu_launches). */
 long long gantts_launch_count(void);
-/* Measurement hooks: when enabled, the tensor-core GEMM and MLPG launches are bracketed by CUDA
+/* Measurement hooks: when enabled, the tensor-core GEMM, MLPG, LSTM and WORLD synthesis launches are bracketed by CUDA
  * events on the launching stream.  gantts_profile_collect synchronises those events and ADDS, per
- * kind (0 = GEMM K-major, 1 = GEMM MN-major, 2 = MLPG fwd, 3 = MLPG bwd), the elapsed milliseconds,
- * the algorithmic work (flops for GEMMs, bytes for MLPG) and the launch count into arrays of 8. */
+ * kind (0 = GEMM K-major, 1 = GEMM MN-major, 2 = MLPG fwd, 3 = MLPG bwd, 4 / 5 = LSTM fwd / bwd, 6 = WORLD pulse
+ * responses, 7 = WORLD overlap-add), the elapsed milliseconds, the work (flops for GEMMs, bytes for MLPG, pulses for
+ * kind 6, output samples for kind 7) and the launch count into arrays of 8. */
 int gantts_profile_enable(int on);
 int gantts_profile_collect(double* ms, double* work, long long* launches);
 
@@ -680,6 +681,58 @@ int gantts_expand_state_frames(const float* phone_x, int64_t x_bstride, int64_t 
 int gantts_corpus_gather(const float* X, const float* Y, int64_t N, int Dx, int Dy, const int64_t* offsets_dev,
                          const int64_t* lengths_dev, int b, int t, float* x_out, float* y_out, int64_t* status_dev,
                          void* stream);
+
+/* Waveforms from generated TTS features: WORLD's decode_aperiodicity and Synthesis (replaces, per utterance, reference
+ * evaluation_tts.py:116-122: pyworld.decode_aperiodicity(bap, fs, fftlen) and pyworld.synthesize(f0, sp, ap, fs,
+ * frame_period)), in fp64.  Row b is processed over its own F = lengths_dev[b] frames (int64[B], clamped to [0, T]), and
+ * its results depend only on that row: the same bits at any batch position, padded length or padding contents.
+ * gantts_world_band_count: WORLD's number of coded aperiodicity bands, floor(min(15000, fs/2 - 3000) / 3000) (0 below
+ *   fs = 12000).  gantts_world_y_length: int(frames * frame_period * fs / 1000), the samples pyworld.synthesize makes.
+ * gantts_world_decode_aperiodicity: bap float32 [B][T][nb] (element strides bap_bstride, bap_tstride) -> ap contiguous
+ *   fp64 [B][T][fftlen/2 + 1].  A frame whose mean coded value is above -0.5 is 1 - 1e-12 in every bin; any other
+ *   interpolates linearly in dB over bin frequency k fs / fftlen through (0 Hz, -60), (3000 j Hz, bap[j-1]) for
+ *   j = 1..nb and (fs/2, -1e-12), then ap = 10^(dB/20).  Frames at or beyond F are written as 0.
+ * gantts_world_time_base: f0 float32 [B][T] (strides f0_bstride, f0_tstride) -> the pulses of each row: pulse_index int32
+ *   [B][cap] (the sample of each pulse, ascending), pulse_shift fp64 [B][cap] (its fractional shift in seconds),
+ *   pulse_vuv uint8 [B][cap] (the interpolated V/UV at its sample), and info_dev int64 [2B + 1]: the pulse count of each
+ *   row, its y_length, then a status word, zeroed here, that gets GANTTS_WORLD_BAD_F0 when a valid frame's f0 is not
+ *   finite and GANTTS_WORLD_SHORT when a row has fewer than 2 frames (its count is 0).  cap >= gantts_world_y_length(T).
+ *   The accumulated phase is one sequential fp64 chain in sample order per row, as WORLD's loop runs it, and the time
+ *   base is computed without FMA contraction, so the pulses are those of the C loop.  No host synchronisation: the caller
+ *   reads info_dev to size gantts_world_synthesize.
+ * gantts_world_randn: out fp64 [count] = draws 0 .. count-1 of WORLD's randn after randn_reseed (xorshift128 seeded
+ *   123456789, 362436069, 521288629, 88675123; a draw is the uint32 sum of w >> 4 over 12 outputs, / 2^28 - 6), bit for
+ *   bit, made in parallel by GF(2) jump-ahead.  Workspace: gantts_world_randn_workspace_bytes(count).
+ * gantts_world_synthesize: y contiguous fp64 [B][y_max], row b WORLD's Synthesis of its F frames of f0 (through the pulses
+ *   of gantts_world_time_base and its info_dev), sp float32 [B][T][fftlen/2 + 1] and ap fp64 [B][T][fftlen/2 + 1]
+ *   (element strides given, unit bin stride), with 0 beyond its y_length.  noise: gantts_world_randn of at least y_max
+ *   draws (Synthesis reseeds per utterance, so every row reads the same stream from draw 0).  total_pulses = the sum of the
+ *   pulse counts.  Each pulse's response is computed on its own; y[s] then adds the responses covering s in ascending
+ *   pulse order (no atomics), in chunks of as many pulses as the workspace holds, processed in order:
+ *   gantts_world_synthesize_workspace_bytes(B, fftlen, chunk_pulses) holds chunk_pulses.  A pulse whose noise segment is
+ *   longer than fftlen keeps its first fftlen zero-mean samples (WORLD writes past its FFT buffer there).
+ * Rules, checked before any device work (the error string names the one that failed): non-null pointers,
+ * 1 <= B <= 65535, 1 <= T <= 2^24, fs >= 1, frame_period finite and > 0, fftlen a power of two in [64, 4096],
+ * 1 <= gantts_world_y_length(T) <= 2^31 - 1, strides >= 0, cap >= gantts_world_y_length(T), 1 <= y_max <= that, and for
+ * the decoder nb == gantts_world_band_count(fs) >= 1. */
+#define GANTTS_WORLD_BAD_F0 1
+#define GANTTS_WORLD_SHORT 2
+int gantts_world_band_count(int fs);
+int64_t gantts_world_y_length(int64_t frames, int fs, double frame_period);
+int gantts_world_decode_aperiodicity(const float* bap, int64_t bap_bstride, int64_t bap_tstride,
+                                     const int64_t* lengths_dev, int B, int T, int nb, int fs, int fftlen, double* ap,
+                                     void* stream);
+int gantts_world_time_base(const float* f0, int64_t f0_bstride, int64_t f0_tstride, const int64_t* lengths_dev, int B,
+                           int T, int fs, double frame_period, int fftlen, int cap, int32_t* pulse_index,
+                           double* pulse_shift, uint8_t* pulse_vuv, int64_t* info_dev, void* stream);
+size_t gantts_world_randn_workspace_bytes(int64_t count);
+int gantts_world_randn(int64_t count, double* out, void* workspace, size_t workspace_bytes, void* stream);
+size_t gantts_world_synthesize_workspace_bytes(int B, int fftlen, int64_t chunk_pulses);
+int gantts_world_synthesize(const float* sp, int64_t sp_bstride, int64_t sp_tstride, const double* ap,
+                            int64_t ap_bstride, int64_t ap_tstride, const int64_t* lengths_dev, const int32_t* pulse_index,
+                            const double* pulse_shift, const uint8_t* pulse_vuv, const int64_t* info_dev, int cap,
+                            int64_t total_pulses, const double* noise, int B, int T, int fs, double frame_period,
+                            int fftlen, int y_max, double* y, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Objective distortions of the training loop (reference train.py:399-432 compute_distortions, :383-396
