@@ -560,20 +560,12 @@ static int lstm_pick_hs(int H, int ndir, int* slices) {
   return 0;
 }
 
-static int lstm_use_reg() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("GANTTS_B200_LSTM_REG");
-    v = e ? atoi(e) : 1;
-  }
-  return v;
-}
-
-// The kernel lstm_run launches for one layer: HS hidden units per CTA, `slices` CTAs per direction, register-resident
-// (HS = 8, H <= 512, unless GANTTS_B200_LSTM_REG=0) or shared-memory kernels, and its dynamic shared memory.
+// The kernel lstm_run launches for one layer: HS hidden units per CTA, `slices` CTAs per direction, the register-resident
+// kernels when HS = 8 and H <= 512 (64 weights per thread), the shared-memory kernels otherwise, and its dynamic shared
+// memory.
 struct LstmPlan {
   int hs, slices;
-  bool reg;
+  const void* fn;
   size_t smem;
 };
 
@@ -585,14 +577,20 @@ static int lstm_plan(bool bwd, int H, int ndir, LstmPlan* pl) {
     return GANTTS_E_UNSUPPORTED;
   }
   const size_t HS = pl->hs;
-  pl->reg = HS == 8 && H <= 512 && lstm_use_reg();
-  if (pl->reg) {
+  if (HS == 8 && H <= 512) {
     const size_t KR = H <= 256 ? 32 : 64, RPT = 4 * H <= 4 * LSTM_THREADS ? 4 : 8;
-    pl->smem = (!bwd ? LSTM_BC * 8 * KR + 8 * LSTM_BC * 32 + LSTM_MAX_B * 8
-                     : LSTM_BC * RPT * LSTM_THREADS + 8 * 64 + 2 * LSTM_MAX_B * 8) * sizeof(float);
+    if (!bwd) {
+      pl->fn = KR == 32 ? (const void*)lstm_fwd_reg_kernel<32> : (const void*)lstm_fwd_reg_kernel<64>;
+      pl->smem = (LSTM_BC * 8 * KR + 8 * LSTM_BC * 32 + LSTM_MAX_B * 8) * sizeof(float);
+    } else {
+      pl->fn = RPT == 4 ? (const void*)lstm_bwd_reg_kernel<4> : (const void*)lstm_bwd_reg_kernel<8>;
+      pl->smem = (LSTM_BC * RPT * LSTM_THREADS + 8 * 64 + 2 * LSTM_MAX_B * 8) * sizeof(float);
+    }
   } else if (!bwd) {
+    pl->fn = HS == 8 ? (const void*)lstm_fwd_kernel<8> : (const void*)lstm_fwd_kernel<16>;
     pl->smem = (4 * HS * (H + 4) + (size_t)LSTM_BC * H + LSTM_BC * 4 * HS + LSTM_MAX_B * HS) * sizeof(float);
   } else {
+    pl->fn = HS == 8 ? (const void*)lstm_bwd_kernel<8> : (const void*)lstm_bwd_kernel<16>;
     pl->smem = (HS * (4 * H + 4) + (size_t)LSTM_BC * (4 * H + 4) + LSTM_THREADS + 2 * LSTM_MAX_B * HS) * sizeof(float);
   }
   if (pl->smem > 227 * 1024) {
@@ -603,52 +601,25 @@ static int lstm_plan(bool bwd, int H, int ndir, LstmPlan* pl) {
   return GANTTS_OK;
 }
 
-template <int HS>
-static int lstm_launch(bool bwd, LstmParams& p, size_t smem, cudaStream_t st) {
-  const int H = p.H;
-  void* fn = bwd ? (void*)lstm_bwd_kernel<HS> : (void*)lstm_fwd_kernel<HS>;
-  GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  GANTTS_CUDA(cudaMemsetAsync(p.bar, 0, 4 * sizeof(unsigned int), st));
-  void* args[] = {&p};
-  dim3 grid(p.slices * p.ndir), block(LSTM_THREADS);
-  // work = recurrent-matmul flops: 2 * B * T * dirs * 4H * H forward, twice that backward (dh and the gate chain)
-  prof_begin(bwd ? PROF_LSTM_BWD : PROF_LSTM_FWD, (bwd ? 2.0 : 1.0) * 8.0 * p.B * (double)p.T * p.ndir * (double)H * H, st);
-  cudaError_t e = cudaLaunchCooperativeKernel(fn, grid, block, args, smem, st);
-  prof_end(st);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchCooperativeKernel(lstm)");
-  count_launch();
-  return GANTTS_OK;
-}
-
-// Register-resident kernels: HS = 8 and H <= 512 (64 weights per thread).
-static int lstm_launch_reg(bool bwd, LstmParams& p, size_t smem, cudaStream_t st) {
-  const int H = p.H;
-  void* fn;
-  if (!bwd)
-    fn = H <= 256 ? (void*)lstm_fwd_reg_kernel<32> : (void*)lstm_fwd_reg_kernel<64>;
-  else
-    fn = 4 * H <= 4 * LSTM_THREADS ? (void*)lstm_bwd_reg_kernel<4> : (void*)lstm_bwd_reg_kernel<8>;
-  GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  GANTTS_CUDA(cudaMemsetAsync(p.bar, 0, 4 * sizeof(unsigned int), st));
-  void* args[] = {&p};
-  dim3 grid(p.slices * p.ndir), block(LSTM_THREADS);
-  prof_begin(bwd ? PROF_LSTM_BWD : PROF_LSTM_FWD, (bwd ? 2.0 : 1.0) * 8.0 * p.B * (double)p.T * p.ndir * (double)H * H, st);
-  cudaError_t e = cudaLaunchCooperativeKernel(fn, grid, block, args, smem, st);
-  prof_end(st);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchCooperativeKernel(lstm reg)");
-  count_launch();
-  return GANTTS_OK;
-}
-
-// One layer's recurrence (forward or backward) in one cooperative launch; p.slices is chosen here.  The barrier
-// counters at p.bar are zeroed on the stream before the launch.
+// One layer's recurrence (forward or backward) in one cooperative launch of the planned kernel; p.slices is chosen here.
+// The barrier counters at p.bar are zeroed on the stream before the launch.
 static int lstm_run(bool bwd, LstmParams& p, cudaStream_t st) {
   LstmPlan pl;
   const int rc = lstm_plan(bwd, p.H, p.ndir, &pl);
   if (rc) return rc;
   p.slices = pl.slices;
-  if (pl.reg) return lstm_launch_reg(bwd, p, pl.smem, st);
-  return pl.hs == 8 ? lstm_launch<8>(bwd, p, pl.smem, st) : lstm_launch<16>(bwd, p, pl.smem, st);
+  GANTTS_CUDA(cudaFuncSetAttribute(pl.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem));
+  GANTTS_CUDA(cudaMemsetAsync(p.bar, 0, 4 * sizeof(unsigned int), st));
+  void* args[] = {&p};
+  dim3 grid(p.slices * p.ndir), block(LSTM_THREADS);
+  // work = recurrent-matmul flops: 2 * B * T * dirs * 4H * H forward, twice that backward (dh and the gate chain)
+  const double H = p.H;
+  prof_begin(bwd ? PROF_LSTM_BWD : PROF_LSTM_FWD, (bwd ? 2.0 : 1.0) * 8.0 * p.B * (double)p.T * p.ndir * H * H, st);
+  cudaError_t e = cudaLaunchCooperativeKernel(pl.fn, grid, block, args, pl.smem, st);
+  prof_end(st);
+  if (e != cudaSuccess) return cuda_fail(e, "cudaLaunchCooperativeKernel(lstm)");
+  count_launch();
+  return GANTTS_OK;
 }
 
 // A layer that trains needs both launches; the backward is the larger one, but check both.

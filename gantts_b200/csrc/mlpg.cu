@@ -676,9 +676,9 @@ static SolveGrid solve_grid(int B, int T, int ncols) {
   return g;
 }
 
-// which: 1 = forward, 2 = backward.  GANTTS_B200_MLPG_SOLVE is a bit mask of the directions that use the substitution
-// kernels (default 3: both directions use them; the FIR kernels remain for windows wider than +-2 frames).
-static bool solve_taps(const gantts_windows_t* win, SolveTaps* tp, int which) {
+// True when the windows admit the substitution kernels: half bandwidth l + u <= 2 for every window, so that the Cholesky
+// factor has the two sub-diagonals the table holds.  Wider windows take the FIR kernels.
+static bool solve_taps(const gantts_windows_t* win, SolveTaps* tp) {
   int hb = 0;
   tp->nw = win->n;
   for (int w = 0; w < GANTTS_MAX_WINDOWS; ++w)
@@ -696,12 +696,53 @@ static bool solve_taps(const gantts_windows_t* win, SolveTaps* tp, int which) {
     if (w == 1) std3 = std3 && tp->c[1][2] == 0.f;
   }
   tp->std3 = std3 ? 1 : 0;
-  const char* e = getenv("GANTTS_B200_MLPG_SOLVE");
-  const int use = e ? atoi(e) : 3;
-  return (use & which) && hb <= 2;
+  return hb <= 2;
 }
 
 static bool fits_i32(int64_t v) { return v >= 0 && v < ((int64_t)1 << 31); }
+
+// mlpg_solve_{fwd,bwd}_kernel<STD3, HW> for the windows' sparsity pattern and the highway combine
+template <bool BWD>
+static auto solve_kernel(bool std3, bool hw) {
+  if constexpr (BWD)
+    return hw ? (std3 ? mlpg_solve_bwd_kernel<true, true> : mlpg_solve_bwd_kernel<false, true>)
+              : (std3 ? mlpg_solve_bwd_kernel<true, false> : mlpg_solve_bwd_kernel<false, false>);
+  else
+    return hw ? (std3 ? mlpg_solve_fwd_kernel<true, true> : mlpg_solve_fwd_kernel<false, true>)
+              : (std3 ? mlpg_solve_fwd_kernel<true, false> : mlpg_solve_fwd_kernel<false, false>);
+}
+
+// Algorithmic bytes of one MLPG pass, either direction: every input column read and every output column written once.
+static double mlpg_bytes(const gantts_streams_t* st, const gantts_windows_t* win, int B, int T, int ncols) {
+  int in_cols = 0;
+  for (int s = 0; s < st->n; ++s) in_cols += st->sd[s] * (st->dyn[s] ? win->n : 1);
+  return 4.0 * (double)B * T * (in_cols + ncols);
+}
+
+// One substitution-kernel launch: the forward (src = in, dst = out) or, with BWD, the adjoint (src = go, dst = gi; `tail`
+// is the adjoint kernel's accumulate flag and output planes).  Returns GANTTS_E_UNSUPPORTED, having launched nothing,
+// when the windows are wider than solve_taps admits or a row offset does not fit in int32: those shapes take the FIR
+// kernels.
+template <bool BWD, typename... Tail>
+static int launch_solve(const float* src, int64_t src_bs, int64_t src_ts, float* dst, int64_t dst_bs, int64_t dst_ts,
+                        const float* table, const gantts_streams_t* st, const gantts_windows_t* win, int B, int T,
+                        int ncols, void* stream, const HighwayArgs* hw, Tail... tail) {
+  SolveTaps tp;
+  if (!solve_taps(win, &tp) || !fits_i32((int64_t)T * src_ts) || !fits_i32((int64_t)T * dst_ts))
+    return GANTTS_E_UNSUPPORTED;
+  const SolveGrid g = solve_grid(B, T, ncols);
+  const auto fn = solve_kernel<BWD>(tp.std3, hw != nullptr);
+  GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
+  // 50 KB per block: the full shared-memory carve-out lets 4 blocks (16 warps) share an SM
+  GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+  const cudaStream_t cs = as_stream(stream);
+  prof_begin(BWD ? PROF_MLPG_BWD : PROF_MLPG_FWD, mlpg_bytes(st, win, B, T, ncols), cs);
+  GANTTS_PDL_LAUNCH((fn), g.blocks, 32 * SOLVE_WARPS, g.smem, cs, src, src_bs, (int)src_ts, dst, dst_bs, (int)dst_ts,
+                    table, *st, tp, B, T, ncols, g.ncg, g.bpc, tail..., hw ? *hw : HighwayArgs{});
+  prof_end(cs);
+  GANTTS_LAUNCH_CHECK("mlpg_solve_{fwd,bwd}_kernel");
+  return GANTTS_OK;
+}
 
 static int check_layout(const gantts_streams_t* st, const gantts_windows_t* win, int* ncols) {
   GANTTS_CHECK_ARG(st && win, "mlpg: null stream/window table");
@@ -989,26 +1030,8 @@ static int gantts::mlpg_fwd_impl(const float* in, int64_t in_bs, int64_t in_ts, 
   if (rc) return rc;
   GANTTS_CHECK_ARG(in && out && table_dev && B >= 1 && T >= 1, "mlpg_fwd: bad arguments");
   if ((rc = check_highway(hw, ncols, out_bs, out_ts, T))) return rc;
-  {
-    SolveTaps tp;
-    if (solve_taps(win, &tp, 1) && fits_i32((int64_t)T * in_ts) && fits_i32((int64_t)T * out_ts)) {
-      const SolveGrid g = solve_grid(B, T, ncols);
-      auto fn = hw ? (tp.std3 ? mlpg_solve_fwd_kernel<true, true> : mlpg_solve_fwd_kernel<false, true>)
-                   : (tp.std3 ? mlpg_solve_fwd_kernel<true, false> : mlpg_solve_fwd_kernel<false, false>);
-      GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
-      // 50 KB per block: the full shared-memory carve-out lets 4 blocks (16 warps) share an SM
-      GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-      int in_cols = 0;
-      for (int s = 0; s < st->n; ++s) in_cols += st->sd[s] * (st->dyn[s] ? win->n : 1);
-      prof_begin(PROF_MLPG_FWD, 4.0 * (double)B * T * (in_cols + ncols), as_stream(stream));
-      HighwayArgs none{};
-      GANTTS_PDL_LAUNCH((fn), g.blocks, 32 * SOLVE_WARPS, g.smem, as_stream(stream), in, in_bs, (int)in_ts, out, out_bs, (int)out_ts, table_dev, *st,
-                                                                  tp, B, T, ncols, g.ncg, g.bpc, hw ? *hw : none);
-      prof_end(as_stream(stream));
-      GANTTS_LAUNCH_CHECK("mlpg_solve_fwd_kernel");
-      return GANTTS_OK;
-    }
-  }
+  rc = launch_solve<false>(in, in_bs, in_ts, out, out_bs, out_ts, table_dev, st, win, B, T, ncols, stream, hw);
+  if (rc != GANTTS_E_UNSUPPORTED) return rc;
   if (hw) {
     // FIR family: MLPG into Gx, then the combine as one elementwise pass
     if ((rc = mlpg_fwd_impl(in, in_bs, in_ts, hw->gx, (int64_t)T * hw->S, hw->S, table_dev, st, win, B, T, stream,
@@ -1032,11 +1055,7 @@ static int gantts::mlpg_fwd_impl(const float* in, int64_t in_bs, int64_t in_ts, 
     GANTTS_CUDA(cudaFuncSetAttribute(mlpg_fwd_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
   }
   dim3 grid((ncols + TC - 1) / TC, (T + TT - 1) / TT, B);
-  {
-    int in_cols = 0;
-    for (int s = 0; s < st->n; ++s) in_cols += st->sd[s] * (st->dyn[s] ? win->n : 1);
-    prof_begin(PROF_MLPG_FWD, 4.0 * (double)B * T * (in_cols + ncols), as_stream(stream));
-  }
+  prof_begin(PROF_MLPG_FWD, mlpg_bytes(st, win, B, T, ncols), as_stream(stream));
   mlpg_fwd_kernel<<<grid, MLPG_THREADS, smem, as_stream(stream)>>>(in, in_bs, in_ts, out, out_bs, out_ts,
                                                                   table_dev, *st, *win, T, ncols);
   prof_end(as_stream(stream));
@@ -1056,22 +1075,9 @@ static int mlpg_bwd_planes(const float* go, int64_t go_bs, int64_t go_ts, __nv_b
   int rc = check_layout(st, win, &ncols);
   if (rc) return rc;
   if ((rc = check_highway(hw, ncols, go_bs, go_ts, T))) return rc;
-  SolveTaps tp;
-  if (!solve_taps(win, &tp, 2) || !fits_i32((int64_t)T * go_ts) || !fits_i32((int64_t)B * T * ppitch)) return GANTTS_E_UNSUPPORTED;
-  const SolveGrid g = solve_grid(B, T, ncols);
-  auto fn = hw ? (tp.std3 ? mlpg_solve_bwd_kernel<true, true> : mlpg_solve_bwd_kernel<false, true>)
-               : (tp.std3 ? mlpg_solve_bwd_kernel<true, false> : mlpg_solve_bwd_kernel<false, false>);
-  GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
-  GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-  int in_cols = 0;
-  for (int s = 0; s < st->n; ++s) in_cols += st->sd[s] * (st->dyn[s] ? win->n : 1);
-  prof_begin(PROF_MLPG_BWD, 4.0 * (double)B * T * (in_cols + ncols), as_stream(stream));
-  HighwayArgs none{};
-  GANTTS_PDL_LAUNCH((fn), g.blocks, 32 * SOLVE_WARPS, g.smem, as_stream(stream), go, go_bs, (int)go_ts, nullptr, 0, 0, table_dev, *st, tp, B, T, ncols,
-                                                              g.ncg, g.bpc, 0, phi, plo, (int)ppitch, hw ? *hw : none);
-  prof_end(as_stream(stream));
-  GANTTS_LAUNCH_CHECK("mlpg_solve_bwd_kernel(planes)");
-  return GANTTS_OK;
+  if (!fits_i32((int64_t)B * T * ppitch)) return GANTTS_E_UNSUPPORTED;
+  return launch_solve<true>(go, go_bs, go_ts, nullptr, 0, 0, table_dev, st, win, B, T, ncols, stream, hw, 0, phi, plo,
+                            (int)ppitch);
 }
 
 // With hw and the FIR family, go is scaled by Tx in place before the unchanged adjoint runs on it.
@@ -1095,25 +1101,9 @@ static int gantts::mlpg_bwd_impl(const float* go, int64_t go_bs, int64_t go_ts, 
   if (rc) return rc;
   GANTTS_CHECK_ARG(go && gi && table_dev && B >= 1 && T >= 1, "mlpg_bwd: bad arguments");
   if ((rc = check_highway(hw, ncols, go_bs, go_ts, T))) return rc;
-  {
-    SolveTaps tp;
-    if (solve_taps(win, &tp, 2) && fits_i32((int64_t)T * go_ts) && fits_i32((int64_t)T * gi_ts)) {
-      const SolveGrid g = solve_grid(B, T, ncols);
-      auto fn = hw ? (tp.std3 ? mlpg_solve_bwd_kernel<true, true> : mlpg_solve_bwd_kernel<false, true>)
-                   : (tp.std3 ? mlpg_solve_bwd_kernel<true, false> : mlpg_solve_bwd_kernel<false, false>);
-      GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
-      GANTTS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-      int in_cols = 0;
-      for (int s = 0; s < st->n; ++s) in_cols += st->sd[s] * (st->dyn[s] ? win->n : 1);
-      prof_begin(PROF_MLPG_BWD, 4.0 * (double)B * T * (in_cols + ncols), as_stream(stream));
-      HighwayArgs none{};
-      GANTTS_PDL_LAUNCH((fn), g.blocks, 32 * SOLVE_WARPS, g.smem, as_stream(stream), go, go_bs, (int)go_ts, gi, gi_bs, (int)gi_ts, table_dev, *st, tp, B, T,
-                                                                  ncols, g.ncg, g.bpc, accumulate, nullptr, nullptr, 0, hw ? *hw : none);
-      prof_end(as_stream(stream));
-      GANTTS_LAUNCH_CHECK("mlpg_solve_bwd_kernel");
-      return GANTTS_OK;
-    }
-  }
+  rc = launch_solve<true>(go, go_bs, go_ts, gi, gi_bs, gi_ts, table_dev, st, win, B, T, ncols, stream, hw, accumulate,
+                          nullptr, nullptr, 0);
+  if (rc != GANTTS_E_UNSUPPORTED) return rc;
   if (hw) {
     const int64_t rows = (int64_t)B * T;
     GANTTS_PDL_LAUNCH((highway_bwd_prep_kernel), elementwise_blocks(rows * hw->S), 256, 0, as_stream(stream), *hw,
@@ -1131,11 +1121,7 @@ static int gantts::mlpg_bwd_impl(const float* go, int64_t go_bs, int64_t go_ts, 
     GANTTS_CUDA(cudaFuncSetAttribute(mlpg_bwd_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
   }
   dim3 grid((ncols + TC - 1) / TC, (T + TT - 1) / TT, B);
-  {
-    int in_cols = 0;
-    for (int s = 0; s < st->n; ++s) in_cols += st->sd[s] * (st->dyn[s] ? win->n : 1);
-    prof_begin(PROF_MLPG_BWD, 4.0 * (double)B * T * (in_cols + ncols), as_stream(stream));
-  }
+  prof_begin(PROF_MLPG_BWD, mlpg_bytes(st, win, B, T, ncols), as_stream(stream));
   mlpg_bwd_kernel<<<grid, MLPG_THREADS, smem, as_stream(stream)>>>(go, go_bs, go_ts, gi, gi_bs, gi_ts,
                                                                   table_dev, *st, *win, T, ncols, accumulate);
   prof_end(as_stream(stream));

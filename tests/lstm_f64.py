@@ -81,13 +81,12 @@ def pick_hs(H, ndir, sms):
     return 0, 0
 
 
-def plan(H, ndir, sms, bwd, reg=True):
-    """lstm_plan / lstm_run: (kernel name, dynamic shared memory in bytes, refusal or None).  reg=False is
-    GANTTS_B200_LSTM_REG=0."""
+def plan(H, ndir, sms, bwd):
+    """lstm_plan / lstm_run: (kernel name, dynamic shared memory in bytes, refusal or None)."""
     hs, _ = pick_hs(H, ndir, sms)
     if hs == 0:
         return None, 0, "one wave"
-    if hs == 8 and H <= 512 and reg:
+    if hs == 8 and H <= 512:
         if not bwd:
             KR = 32 if H <= 256 else 64
             return "lstm_fwd_reg_kernel<%d>" % KR, (LSTM_BC * 8 * KR + 8 * LSTM_BC * 32 + LSTM_MAX_B * 8) * F32, None
@@ -101,23 +100,23 @@ def plan(H, ndir, sms, bwd, reg=True):
     return name, smem, ("shared memory" if smem > SMEM_LIMIT else None)
 
 
-def variant(H, ndir, sms, reg=True):
+def variant(H, ndir, sms):
     """'forward kernel / backward kernel' of a layer; a refused launch reads 'refused (<kernel>: <limit>)'."""
     out = []
     for bwd in (False, True):
-        name, smem, why = plan(H, ndir, sms, bwd, reg)
+        name, smem, why = plan(H, ndir, sms, bwd)
         out.append(name if why is None else "refused (%s: %s)" % (name, why))
     return " / ".join(out)
 
 
-def trainable(H, ndir, sms, reg=True):
-    return all(plan(H, ndir, sms, bwd, reg)[2] is None for bwd in (False, True))
+def trainable(H, ndir, sms):
+    return all(plan(H, ndir, sms, bwd)[2] is None for bwd in (False, True))
 
 
-def first_untrainable(ndir, sms, reg=True):
+def first_untrainable(ndir, sms):
     """The smallest H (a multiple of 4) whose forward runs but whose backward is refused."""
     H = 4
-    while trainable(H, ndir, sms, reg) or plan(H, ndir, sms, False, reg)[2] is not None:
+    while trainable(H, ndir, sms) or plan(H, ndir, sms, False)[2] is not None:
         H += 4
         assert H <= 4096
     return H
@@ -146,7 +145,7 @@ def _cases():
         T = 23 if H < 256 else 7          # the float64 loop runs on the CPU: short where H is large
         for ndir in (1, 2):
             shapes = [(1, T, "full"), (17, T, "desc"), (33, T, "unsorted"), (16, 1, "T=1")]
-            if H in (12, 260, 528):
+            if H in (12, 260, 516, 528):
                 shapes.append((128, T, "unsorted"))
             for B, Tc, kind in shapes:
                 cases.append(("H%d-%s-B%d-T%d-%s" % (H, "bi" if ndir == 2 else "uni", B, Tc, kind), B, Tc, H, ndir, kind))

@@ -18,14 +18,17 @@ from oracle import nnmnkwii_port as nnp
 
 VC_HP = dict(stream_sizes=[177], has_dynamic_features=[True], adversarial_streams=[True],
              mask_nth_mgc_for_adv_loss=0, num_windows=3, discriminator_linguistic_condition=False)
+# The reference's windows take the substitution MLPG kernels, a delta window two frames wide the FIR kernels.
+FAMILY_WINDOWS = {"substitution": WINDOWS,
+                  "fir": [WINDOWS[0], (2, 2, np.array([-0.2, -0.1, 0.0, 0.1, 0.2])), WINDOWS[2]]}
 LOSS_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mge", "loss_mse", "loss_adv", "loss_g")
 GOLD_KEYS = ("loss_d", "loss_fake_d", "loss_real_d", "loss_mse", "loss_mge", "loss_adv", "loss_g",
              "real_correct", "fake_correct")
 
 
-def vc_hp(width=177):
+def vc_hp(width=177, windows=WINDOWS):
     from gantts_b200 import step as gstep
-    return gstep.HParams(windows=WINDOWS, stream_sizes=[width], has_dynamic_features=[True], adversarial_streams=[True],
+    return gstep.HParams(windows=windows, stream_sizes=[width], has_dynamic_features=[True], adversarial_streams=[True],
                          mask_nth_mgc_for_adv_loss=0, discriminator_linguistic_condition=False)
 
 
@@ -127,22 +130,22 @@ def test_fused_highway_vc_adversarial_train_mode_injected_masks(dev):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("mode", ["0", "3"])
-def test_fused_highway_cfg1_two_steps(dev, monkeypatch, mode):
+@pytest.mark.parametrize("family", ["substitution", "fir"])
+def test_fused_highway_cfg1_two_steps(dev, family):
     """BASELINE cfg1 through the fused step: In2OutHighwayNet(177, static 59, 3 x 512, dropout 0.5), B = 8 x T = 200,
-    w_d = 0, mse_w = mge_w = 1 (the fp32 MLPG adjoint path), two consecutive steps against the oracle, under both MLPG
-    kernel families (0: FIR kernels with the elementwise highway passes, 3: substitution kernels with the fused
-    combine).  The second step starts the oracle from the product's post-step weights and accumulators (see
-    test_cfg1_highway_step_full_size)."""
+    w_d = 0, mse_w = mge_w = 1 (the fp32 MLPG adjoint path), two consecutive steps against the oracle, on the windows of
+    each MLPG kernel family (the reference's windows: substitution kernels with the fused combine; a delta window two
+    frames wide: FIR kernels with the elementwise highway passes).  The second step starts the oracle from the product's
+    post-step weights and accumulators (see test_cfg1_highway_step_full_size)."""
     from gantts_b200 import fused
-    monkeypatch.setenv("GANTTS_B200_MLPG_SOLVE", mode)
+    windows = FAMILY_WINDOWS[family]
     B, T, p = 8, 200, 0.5
     mg, md = vc_models(3, p, dev, d_hidden=16)
     gen = gp.GeneratorOracle("highway", sd_numpy(mg), static_dim=59)
     mg.to(dev).train(), md.to(dev).train()
     d_before = [q.detach().clone() for q in md.parameters()]
-    fs = fused.FusedGanStep(mg, md, vc_hp(), B, T, w_d=0.0, mse_w=1.0, mge_w=1.0, seed=70)
-    R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, T))
+    fs = fused.FusedGanStep(mg, md, vc_hp(windows=windows), B, T, w_d=0.0, mse_w=1.0, mge_w=1.0, seed=70)
+    R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(windows, T))
     for it in range(2):
         lens = ragged_lengths(B, T, 20 + it)
         x, y = make_batch(B, T, 177, 177, lens, 30 + it)

@@ -794,41 +794,52 @@ def test_mlp_bwd_input_grad_only_and_weight_grads_only(dev):
         assert rel_err(npy(a), npy(b.grad)) < 2e-5
 
 
-@pytest.mark.parametrize("mode", ["0", "3"])
+# The shape picks the MLPG kernel family: the reference's windows (half bandwidth l + u = 2) take the banded-Cholesky
+# substitution kernels, a delta window two frames wide (l + u = 4) the 49-tap FIR kernels.
+WIDE_DELTA = (2, 2, np.array([-0.2, -0.1, 0.0, 0.1, 0.2]))
+FAMILY_WINDOWS = {"substitution": WINDOWS, "fir": [WINDOWS[0], WIDE_DELTA, WINDOWS[2]]}
+
+
+@pytest.mark.parametrize("family", ["substitution", "fir"])
 @pytest.mark.parametrize("B,Tn", [(3, 257), (2, 31), (1, 1000), (2, 5)])
-def test_mlpg_both_kernel_families_vs_dense_R(dev, monkeypatch, mode, B, Tn):
-    """multi_stream_mlpg forward and backward with the 49-tap FIR kernels (mode 0) and with the banded-Cholesky
-    substitution kernels (mode 3) against the dense R matmul of the reference path (oracle/nnmnkwii_port), TTS stream
-    layout (three dynamic streams + the static vuv column), lengths that do not divide the time chunks."""
-    import gantts_b200
-    monkeypatch.setenv("GANTTS_B200_MLPG_SOLVE", mode)
-    torch.manual_seed(int(mode) + Tn)
+def test_mlpg_both_kernel_families_vs_dense_R(dev, family, B, Tn):
+    """The MLPG forward and backward on the windows of each kernel family against the dense R matmul of the reference
+    path (oracle/nnmnkwii_port), TTS stream layout (three dynamic streams + the static vuv column), lengths that do not
+    divide the time chunks."""
+    from gantts_b200 import multistream, ops
+    wins = FAMILY_WINDOWS[family]
+    torch.manual_seed(Tn)
     x = torch.randn(B, Tn, 187)
     g = torch.randn(B, Tn, 63)
-    R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(WINDOWS, Tn))
+    R = torch.from_numpy(nnp.unit_variance_mlpg_matrix(wins, Tn))
     xr = x.clone().requires_grad_(True)
     yr = gp.multi_stream_mlpg(xr, R)
     yr.backward(g)
+    entries, ncols = multistream.mlpg_stream_entries([180, 3, 1, 3], [True, True, False, True], [True] * 4, len(wins))
     xd = x.to(dev).requires_grad_(True)
-    yd = gantts_b200.multistream.multi_stream_mlpg(xd, R.to(dev), [180, 3, 1, 3], [True, True, False, True])
+    yd = ops.mlpg(xd, [(l, u, tuple(float(v) for v in c)) for l, u, c in wins], entries, ncols)
     yd.backward(g.to(dev))
     assert rel_err(npy(yd), npy(yr)) < 5e-6
     assert rel_err(npy(xd.grad), npy(xr.grad)) < 5e-6
     assert torch.equal(yd[:, :, 61].cpu(), x[:, :, 183])          # static stream copied bit-exactly
 
 
-@pytest.mark.parametrize("mode", ["0", "3"])
+DENSE_DELTA = {"substitution": (1, 1, np.array([-0.4, 0.1, 0.5])),
+               "fir": (2, 2, np.array([-0.2, -0.1, 0.1, 0.1, 0.2]))}
+
+
+@pytest.mark.parametrize("family", ["substitution", "fir"])
 @pytest.mark.parametrize("case", ["two_windows", "dense_delta"])
-def test_mlpg_generic_window_patterns(dev, monkeypatch, mode, case):
+def test_mlpg_generic_window_patterns(dev, family, case):
     """Window sets that do NOT have the sparsity pattern the substitution kernels are specialised for (`STD3`): static +
     delta only, and three windows whose delta window has a non-zero centre tap -- the generic path of both kernel families,
     forward and backward, against the dense R matmul."""
     from gantts_b200 import ops
-    monkeypatch.setenv("GANTTS_B200_MLPG_SOLVE", mode)
+    base = FAMILY_WINDOWS[family]
     if case == "two_windows":
-        wins = WINDOWS[:2]
+        wins = base[:2]
     else:
-        wins = [WINDOWS[0], (1, 1, np.array([-0.4, 0.1, 0.5])), WINDOWS[2]]
+        wins = [base[0], DENSE_DELTA[family], base[2]]
     nw, sd, B, Tn = len(wins), 7, 3, 203
     torch.manual_seed(11)
     x = torch.randn(B, Tn, nw * sd + 2)                 # one dynamic stream of 7 static dims + a static stream of 2

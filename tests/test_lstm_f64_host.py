@@ -130,14 +130,13 @@ def test_hprev_gather():
 # ------------------------------------------------------------------------------------------- kernel choice
 def test_kernel_choice_at_132_sms():
     """The thresholds of the variant table in DESIGN.md (H100 SXM, 132 SMs)."""
-    v = lambda H, nd, reg=True: ref.variant(H, nd, 132, reg)
+    v = lambda H, nd: ref.variant(H, nd, 132)
     assert v(256, 2) == "lstm_fwd_reg_kernel<32> / lstm_bwd_reg_kernel<4>"
     assert v(260, 2) == "lstm_fwd_reg_kernel<64> / lstm_bwd_reg_kernel<8>"
     assert v(512, 2) == v(512, 1) == "lstm_fwd_reg_kernel<64> / lstm_bwd_reg_kernel<8>"
     assert v(516, 2) == v(528, 2) == v(580, 1) == "lstm_fwd_kernel<8> / lstm_bwd_kernel<8>"
     assert v(532, 2).startswith("lstm_fwd_kernel<16> / refused (lstm_bwd_kernel<16>: shared memory")
     assert v(584, 1).startswith("lstm_fwd_kernel<8> / refused (lstm_bwd_kernel<8>: shared memory")
-    assert v(4, 1, reg=False) == v(512, 2, reg=False) == "lstm_fwd_kernel<8> / lstm_bwd_kernel<8>"
     assert ref.plan(532, 2, 132, True)[1] == 290304                       # (32 (4H + 4) + 4352) * 4 B
     assert ref.first_untrainable(2, 132) == 532 and ref.first_untrainable(1, 132) == 584
     assert ref.pick_hs(1056, 1, 132) == (8, 132) and ref.pick_hs(1060, 1, 132) == (16, 67)
@@ -156,16 +155,16 @@ def test_gpu_case_matrix_reaches_every_kernel_at_132_sms():
     ids = [c[0] for c in CASES]
     assert len(set(ids)) == len(ids)
     reached = {ref.variant(H, nd, 132) for _, B, T, H, nd, lens in CASES}
-    reached_smem = {ref.variant(H, nd, 132, reg=False) for _, B, T, H, nd, lens in CASES}
     assert reached >= {"lstm_fwd_reg_kernel<32> / lstm_bwd_reg_kernel<4>",
                        "lstm_fwd_reg_kernel<64> / lstm_bwd_reg_kernel<8>",
                        "lstm_fwd_kernel<8> / lstm_bwd_kernel<8>"}
-    assert reached_smem == {"lstm_fwd_kernel<8> / lstm_bwd_kernel<8>"}
     # every matrix case trains at 132 SMs; HS = 16 (forward only) is test_hs16_forward_vs_float64_and_backward_refused's
     assert all(ref.trainable(H, nd, 132) for _, B, T, H, nd, lens in CASES)
     # the lower edge of KR = 64 (H % 8 == 4: half of the last CTA's slice empty) and the batch edges
     assert {(260, 1), (260, 2), (516, 1), (516, 2)} <= {(H, nd) for _, B, T, H, nd, lens in CASES}
     assert {1, 16, 17, 33, 128} <= {B for _, B, T, H, nd, lens in CASES}
+    # the shared-memory kernels at their largest batch, on a full and a partial last slice
+    assert {(516, 128), (528, 128)} <= {(H, B) for _, B, T, H, nd, lens in CASES}
     assert any(T == 1 for _, B, T, H, nd, lens in CASES)
     for _, B, T, H, nd, lens in CASES:
         assert len(lens) == B and all(1 <= n <= T for n in lens) and max(lens) == T

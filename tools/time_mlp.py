@@ -43,8 +43,8 @@ def run(M, dims, p, last_act, tag):
     print("   gemm-only [%s]:" % tag, flush=True); print("    fwd KK %.1f us (%d launches/iter); fwd+bwd KK %.1f us MN %.1f us" % (
         msf / n * 1e3, cf // n, ms2[0] / n * 1e3, ms2[1] / n * 1e3), flush=True)
     fl = 2.0 * M * sum(a * b for a, b in zip(dims[:-1], dims[1:]))
-    print("%-28s dbg=%s fwd %.1f us (%.0f TF alg)  bwd %.1f us (%.0f TF alg)" % (
-        tag, os.environ.get("GANTTS_B200_DBG", "0"), tf / n * 1e3, fl / (tf / n * 1e-3) / 1e12,
+    print("%-28s fwd %.1f us (%.0f TF alg)  bwd %.1f us (%.0f TF alg)" % (
+        tag, tf / n * 1e3, fl / (tf / n * 1e-3) / 1e12,
         tb / n * 1e3, 2 * fl / (tb / n * 1e-3) / 1e12), flush=True)
 
 run(32000, [425, 512, 512, 512, 187], 0.0, _lib.ACT_NONE, "G 425-512x3-187 p=0")
