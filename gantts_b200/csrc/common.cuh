@@ -45,6 +45,12 @@ void prof_end(cudaStream_t st);
 
 static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
+// The library's non-blocking side stream of the current device, on which the fused step runs branches that its critical
+// path does not wait for (core.cu).  stream_wait makes `waiter` wait for everything enqueued on `on` so far, through an
+// event recorded on `on`: the fork and the join of such a branch, and graph capture follows them like any event edge.
+int side_stream(cudaStream_t* out);
+int stream_wait(cudaStream_t waiter, cudaStream_t on);
+
 // Programmatic dependent launch for the tensor-core GEMMs and the small streaming kernels of the fused step:
 // a kernel launched through GANTTS_PDL_LAUNCH may become resident while its predecessor in the stream is still in its last
 // wave; pdl_entry() at the top of the kernel (a) lets ITS successor do the same and (b) blocks until every prerequisite

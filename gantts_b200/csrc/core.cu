@@ -1,6 +1,7 @@
 // Error reporting, version, device probe.
 #include <stdarg.h>
 
+#include <mutex>
 #include <vector>
 
 #include "common.cuh"
@@ -60,6 +61,52 @@ void prof_end(cudaStream_t st) {
   cudaEventRecord(g_open.e1, st);
   g_recs.push_back(g_open);
   g_open_valid = false;
+}
+
+// The side stream of each device (created on first use) and the one event that orders it against the caller's stream.
+// stream_wait records and waits under one lock, so no other thread can re-record the event between the two calls.
+struct SideStream {
+  cudaStream_t st = nullptr;
+  cudaEvent_t ev = nullptr;
+};
+static std::mutex g_side_mu;
+static SideStream g_side[64];
+
+static int side_locked(SideStream** out) {
+  int dev = 0;
+  GANTTS_CUDA(cudaGetDevice(&dev));
+  GANTTS_CHECK_ARG(dev >= 0 && dev < 64, "side stream: device ordinal %d out of range", dev);
+  SideStream& s = g_side[dev];
+  if (!s.ev) GANTTS_CUDA(cudaEventCreateWithFlags(&s.ev, cudaEventDisableTiming));
+  if (!s.st) {
+    // the device's highest priority: when a running GEMM's last wave frees SMs, the block scheduler dispatches the side
+    // branch's waiting blocks before those of the next GEMM the caller's stream launched early under PDL, so the two
+    // chains alternate and each fills the other's tail instead of the whole input-gradient chain running first
+    int least = 0, greatest = 0;
+    GANTTS_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+    GANTTS_CUDA(cudaStreamCreateWithPriority(&s.st, cudaStreamNonBlocking, greatest));
+  }
+  *out = &s;
+  return GANTTS_OK;
+}
+
+int side_stream(cudaStream_t* out) {
+  std::lock_guard<std::mutex> lk(g_side_mu);
+  SideStream* s;
+  int rc = side_locked(&s);
+  if (rc) return rc;
+  *out = s->st;
+  return GANTTS_OK;
+}
+
+int stream_wait(cudaStream_t waiter, cudaStream_t on) {
+  std::lock_guard<std::mutex> lk(g_side_mu);
+  SideStream* s;
+  int rc = side_locked(&s);
+  if (rc) return rc;
+  GANTTS_CUDA(cudaEventRecord(s->ev, on));
+  GANTTS_CUDA(cudaStreamWaitEvent(waiter, s->ev, 0));
+  return GANTTS_OK;
 }
 }  // namespace gantts
 

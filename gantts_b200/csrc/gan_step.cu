@@ -1027,6 +1027,11 @@ static int lstm_stack_bwd(const LstmStack& k, const int64_t* lengths, int B, int
   return GANTTS_OK;
 }
 
+// The MLP stacks' backward passes run their weight gradients on the side stream (mlp_bwd_impl), beside the input-gradient
+// chain; an SRU or LSTM generator's head and a recurrent discriminator's head stay on one stream (DESIGN.md section 5).
+static bool g_side_bwd(const gantts_gan_step_t* c) { return c->sru.num_layers == 0 && c->lstm.num_layers == 0; }
+static bool d_side_bwd(const gantts_gan_step_t* c) { return c->d_lstm.num_layers == 0; }
+
 // The workspace is laid out once for the configured (B, T), the capacity: a call of shape (b, t) uses the first
 // M = b * t rows of every per-row buffer, and the split-K partials are sized for every M up to the capacity.  So the flat
 // gradient buffers (gantts_gan_step_grad_buffer) and every buffer one call leaves for the next (phases 1|2 then 4) sit at
@@ -1050,7 +1055,8 @@ static void layout(const gantts_gan_step_t* c, char* base, StepLayout* L) {
   L->g_tape = a.take(L->g_tape_bytes);
   L->d_tape_bytes = gantts_mlp_tape_bytes(&c->d, 2 * M);
   L->d_tape = a.take(L->d_tape_bytes);
-  const size_t gb = mlp_workspace_bytes(&c->g, M, true), db = mlp_workspace_bytes(&c->d, 2 * M, true);
+  const size_t gb = mlp_workspace_bytes(&c->g, M, true, g_side_bwd(c));
+  const size_t db = mlp_workspace_bytes(&c->d, 2 * M, true, d_side_bwd(c));
   L->mlp_ws_bytes = gb > db ? gb : db;
   L->mlp_ws = a.take(L->mlp_ws_bytes);
   L->red = reinterpret_cast<RedWs*>(a.take(R_COUNT * sizeof(RedWs)));
@@ -1084,6 +1090,7 @@ struct Step {
   uint64_t seed;
   void* stream;
   cudaStream_t st;
+  cudaStream_t side;        // the library's side stream (nullptr when no pass of the configuration uses it)
   const HighwayArgs* hw() const { return c->highway.static_dim > 0 ? &hwa : nullptr; }
   bool d_rnn() const { return c->d_lstm.num_layers > 0; }
   // the discriminator's LSTM stack in forward `which` (1 stacked, 2 adversarial)
@@ -1158,9 +1165,14 @@ static int generator_bwd(Step& s) {
   const int d_out = s.d_out, nS = s.nS;
   const bool sru = c->sru.num_layers > 0, lstm = c->lstm.num_layers > 0;
   const bool mse_grad = c->mse_w != 0.f && !lstm;
+  const cudaStream_t side = g_side_bwd(c) ? s.side : nullptr;
   int rc;
+  // without a gradient the MSE pass writes its loss partials alone: it runs on the side stream, which the head's backward
+  // joins back before it returns
+  const cudaStream_t mse_st = side && !mse_grad ? side : s.st;
+  if (mse_st != s.st && (rc = stream_wait(mse_st, s.st))) return rc;
   if ((rc = launch_sse(s.y_hat, d_out, s.y, d_out, L.mask, M, d_out, L.scal + S_MSE_SCALE, mse_grad ? L.g_yhat : nullptr,
-                       d_out, &L.red[R_MSE], s.st)))
+                       d_out, &L.red[R_MSE], mse_st)))
     return rc;
   bool direct = false;
   if (!mse_grad) {
@@ -1179,7 +1191,7 @@ static int generator_bwd(Step& s) {
   float* gx = sru ? L.sru.dx : (lstm ? L.lstm.dh : nullptr);
   const int gx_rs = sru ? sru_ncols(c->sru) : (lstm ? lstm_ndir(c->lstm) * c->lstm.hidden : 0);
   if ((rc = mlp_bwd_impl(&s.g, direct ? nullptr : L.g_yhat, d_out, nullptr, 0, M, L.g_tape, L.g_tape_bytes, gx, gx_rs, 0,
-                         s.pg.gW, s.pg.gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, -1, direct)))
+                         s.pg.gW, s.pg.gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, -1, direct, side)))
     return rc;
   if (sru) return sru_stack_bwd(c, L, s.pg, s.x, s.B, s.T, s.seed, s.st);
   if (lstm) return lstm_stack_bwd(g_lstm(c, L, s.pg), s.lengths, s.B, s.T, s.seed, true, nullptr, s.st);
@@ -1279,7 +1291,8 @@ static int discriminator_bwd(Step& s, bool stacked, bool input_grad = true) {
                              input_grad ? &din : nullptr, s.st)))
       return rc;
   } else if ((rc = mlp_bwd_impl(&s.d, L.g_dout, 1, L.d_out, 1, skip + M, L.d_tape, L.d_tape_bytes, gx, s.adv_window ? s.nS : s.dD,
-                                skip, gW, gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, s.adv_window ? 1 : -1))) {
+                                skip, gW, gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, s.adv_window ? 1 : -1, false,
+                                stacked ? s.side : nullptr))) {
     return rc;
   }
   if (s.adv_window || !input_grad) return GANTTS_OK;
@@ -1369,6 +1382,8 @@ extern "C" int gantts_gan_step_shaped(const gantts_gan_step_t* c, int B, int T, 
   s.table = mlpg_table;
   s.stream = stream;
   s.st = as_stream(stream);
+  s.side = nullptr;
+  if ((g_side_bwd(c) || d_side_bwd(c)) && (rc = side_stream(&s.side))) return rc;
   layout(c, reinterpret_cast<char*>(al256(reinterpret_cast<uintptr_t>(workspace))), &s.L);
   const StepLayout& L = s.L;
   const int64_t M = s.M = (int64_t)B * T;

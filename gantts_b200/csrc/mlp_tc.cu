@@ -508,8 +508,15 @@ extern "C" size_t gantts_mlp_tape_bytes(const gantts_mlp_t* m, int64_t M) {
 }
 
 namespace gantts {
-// upto = false: the workspace of M rows; true: enough for every row count in [1, M]
-static size_t mlp_workspace_bytes(const gantts_mlp_t* m, int64_t M, bool upto) {
+// Gradient plane buffers of a backward.  With the weight gradients on a side stream (mlp_bwd_impl), dW_l still reads G_l
+// while the input-gradient chain writes the layers below it: every layer's gradient gets its own buffer.
+static int mlp_grad_bufs(const gantts_mlp_t* m, bool side) {
+  return side && m->num_layers > MLP_GRAD_BUFS ? m->num_layers : MLP_GRAD_BUFS;
+}
+
+// upto = false: the workspace of M rows; true: enough for every row count in [1, M].  side: for a backward that runs the
+// weight gradients on a side stream.
+static size_t mlp_workspace_bytes(const gantts_mlp_t* m, int64_t M, bool upto, bool side = false) {
   if (!m || m->num_layers < 1 || m->num_layers > GANTTS_MAX_LAYERS || M < 1) return 0;
   int maxd = 0;
   size_t part = 0;
@@ -517,8 +524,8 @@ static size_t mlp_workspace_bytes(const gantts_mlp_t* m, int64_t M, bool upto) {
   for (int l = 0; l < m->num_layers; ++l)       // one partial region per layer: reductions are deferred
     part += (upto ? mn_partial_bytes_upto(M, m->dims[l + 1], m->dims[l])
                   : mn_partial_bytes(M, m->dims[l + 1], m->dims[l], nullptr, nullptr)) + 256;
-  return (size_t)2 * MLP_GRAD_BUFS * plane_bytes(M, maxd) + part + (size_t)MLP_COLSUM_CHUNKS * maxd * sizeof(float) +
-         (size_t)GEMV_BLOCKS * (GEMV_MAX_K + 1) * sizeof(float) + 4096;
+  return (size_t)2 * mlp_grad_bufs(m, side) * plane_bytes(M, maxd) + part +
+         (size_t)MLP_COLSUM_CHUNKS * maxd * sizeof(float) + (size_t)GEMV_BLOCKS * (GEMV_MAX_K + 1) * sizeof(float) + 4096;
 }
 }  // namespace gantts
 
@@ -636,7 +643,7 @@ namespace gantts {
 static int mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t gy_rs, const float* y, int64_t y_rs, int64_t M,
                         const void* tape, size_t tape_bytes, float* gx, int64_t gx_rs, int64_t gx_row0,
                         float* const* gW, float* const* gb, int accumulate, void* workspace, size_t workspace_bytes,
-                        void* stream, int gx_accumulate = -1, bool gy_planes_ready = false);
+                        void* stream, int gx_accumulate = -1, bool gy_planes_ready = false, cudaStream_t side = nullptr);
 // Where mlp_bwd_impl expects the output-gradient planes when gy_planes_ready (linear output, not the GEMV tail): the
 // producer of gy (the MLPG backward in the fused step) can write them directly instead of an fp32 matrix.
 static int mlp_bwd_gy_planes(const gantts_mlp_t* m, int64_t M, void* workspace, size_t workspace_bytes, Planes* out);
@@ -665,9 +672,13 @@ extern "C" int gantts_mlp_bwd(const gantts_mlp_t* m, const float* gy, int64_t gy
 static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t gy_rs, const float* y, int64_t y_rs,
                                 int64_t M, const void* tape, size_t tape_bytes, float* gx, int64_t gx_rs,
                                 int64_t gx_row0, float* const* gW, float* const* gb, int accumulate, void* workspace,
-                                size_t workspace_bytes, void* stream, int gx_accumulate, bool gy_planes_ready) {
+                                size_t workspace_bytes, void* stream, int gx_accumulate, bool gy_planes_ready,
+                                cudaStream_t side) {
   // gx_accumulate: -1 = like the parameter gradients, 0 = store, 1 = add to what gx holds (gx may be a column window of
   // a wider matrix with row stride gx_rs: the fused step scatters the input gradient into g_static this way)
+  // side: the weight and bias gradients (their GEMMs, the GEMV tail's reduction, the split-K reduction) run on this
+  // stream, each after the launch on `stream` that wrote the gradient planes it reads, while the input-gradient chain
+  // stays on `stream`; the call joins the side stream back into `stream` before it returns.
   if (gx_accumulate < 0) gx_accumulate = accumulate;
   int rc = check_mlp(m, M);
   GANTTS_CHECK_ARG(gx_row0 >= 0 && gx_row0 < M, "mlp_bwd: bad gx_row0");
@@ -681,19 +692,23 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
     set_error("mlp_bwd: tape too small");
     return GANTTS_E_WORKSPACE;
   }
-  size_t need = gantts_mlp_workspace_bytes(m, M);
+  size_t need = mlp_workspace_bytes(m, M, false, side != nullptr);
   if (!workspace || workspace_bytes < need) {
     set_error("mlp_bwd: workspace too small (%zu < %zu)", workspace_bytes, need);
     return GANTTS_E_WORKSPACE;
   }
   cudaStream_t st = as_stream(stream);
+  // ws: the stream of the weight-gradient launches; fork(): it waits for what `stream` has issued so far
+  const cudaStream_t ws = side ? side : st;
+  auto fork = [&]() { return side ? stream_wait(side, st) : GANTTS_OK; };
   MlpTape t;
   carve_tape(m, M, reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(const_cast<void*>(tape)) + 255) / 256 * 256), &t);
   int maxd = 0;
   for (int l = 0; l <= L; ++l) maxd = m->dims[l] > maxd ? m->dims[l] : maxd;
   char* cur = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(workspace) + 255) / 256 * 256);
-  char* gbuf[MLP_GRAD_BUFS];
-  for (int i = 0; i < MLP_GRAD_BUFS; ++i) {
+  const int nbuf = mlp_grad_bufs(m, side != nullptr);
+  char* gbuf[GANTTS_MAX_LAYERS > MLP_GRAD_BUFS ? GANTTS_MAX_LAYERS : MLP_GRAD_BUFS];
+  for (int i = 0; i < nbuf; ++i) {
     gbuf[i] = cur;
     cur += 2 * plane_bytes(M, maxd);
   }
@@ -731,7 +746,8 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
     GANTTS_LAUNCH_CHECK("gemv_bwd_kernel");
     if (want) {
       // partial rows are [K1 weights | 1 bias]: one column-parallel reduction for both
-      GANTTS_PDL_LAUNCH((gemv_partial_reduce_kernel), (K1 + 1 + 31) / 32, 256, 0, st, gemv_part, GEMV_BLOCKS, K1,
+      if ((rc = fork())) return rc;
+      GANTTS_PDL_LAUNCH((gemv_partial_reduce_kernel), (K1 + 1 + 31) / 32, 256, 0, ws, gemv_part, GEMV_BLOCKS, K1,
                                                                     gW ? gW[L - 1] : nullptr,
                                                                     gb ? gb[L - 1] : nullptr, accumulate);
       GANTTS_LAUNCH_CHECK("gemv_partial_reduce_kernel");
@@ -748,17 +764,18 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
   }
   for (int l = l_start; l >= 0; --l) {
     float* gbl = (gb && gb[l]) ? gb[l] : nullptr;
+    if (((gW && gW[l]) || gbl) && (rc = fork())) return rc;
     if (gW && gW[l]) {
       // gW_l and (via the ones-MMA) gb_l from one launch; the split reductions of all layers are
       // summed by a single launch at the end
       float* partial = reinterpret_cast<float*>(partial_cur);
       partial_cur += mn_partial_bytes(M, m->dims[l + 1], m->dims[l], nullptr, nullptr) + 256;
-      if ((rc = launch_gemm_mn(G, t.H[l], gW[l], gbl, accumulate, partial, st, &rl))) return rc;
+      if ((rc = launch_gemm_mn(G, t.H[l], gW[l], gbl, accumulate, partial, ws, &rl))) return rc;
     } else if (gbl) {
-      if ((rc = colsum_planes(G, gbl, accumulate, colpart, st))) return rc;
+      if ((rc = colsum_planes(G, gbl, accumulate, colpart, ws))) return rc;
     }
     if (l > 0) {
-      char* c1 = gbuf[pp ^ 1];
+      char* c1 = gbuf[(pp + 1) % nbuf];
       Planes Gn = carve_planes(c1, M, m->dims[l]);
       EpiArgs e;
       e.epi = EPI_PLANES_BWD;
@@ -771,7 +788,7 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
       e.p = m->dropout_p;
       if ((rc = launch_gemm_kk(G, t.Wt[l], e, st))) return rc;
       G = Gn;
-      pp ^= 1;
+      pp = (pp + 1) % nbuf;
     } else if (gx) {
       EpiArgs e;
       e.epi = EPI_F32;
@@ -785,5 +802,6 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
       if ((rc = launch_gemm_kk(Gs, t.Wt[0], e, st))) return rc;
     }
   }
-  return flush_reduce(rl, accumulate, st);
+  if ((rc = flush_reduce(rl, accumulate, ws))) return rc;
+  return side ? stream_wait(st, side) : GANTTS_OK;
 }

@@ -3,7 +3,9 @@
  *
  * Every entry point takes plain device/host pointers and sizes; no torch types.  All work is
  * enqueued on the caller's `stream` (a cudaStream_t passed as void*), nothing synchronises
- * internally unless stated.  Return value: 0 on success, otherwise a GANTTS_E_* code; the message
+ * internally unless stated.  The fused GAN step also runs some branches on a side stream the library
+ * owns (one per device); it forks them from `stream` and joins them back into it through events before
+ * it returns, so everything it writes is ordered on `stream` like the rest.  Return value: 0 on success, otherwise a GANTTS_E_* code; the message
  * for the calling thread's last failure is available from gantts_last_error_string().  The library
  * owns no device memory: every buffer, including workspaces, is the caller's.
  *
