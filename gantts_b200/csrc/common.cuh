@@ -49,6 +49,9 @@ static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStre
 // path does not wait for (core.cu).  stream_wait makes `waiter` wait for everything enqueued on `on` so far, through an
 // event recorded on `on`: the fork and the join of such a branch, and graph capture follows them like any event edge.
 int side_stream(cudaStream_t* out);
+// The library's branch stream of the current device, at the device's lowest stream priority: phase 1 of the fused step
+// runs the real half of D's stacked pass on it, beside the generator's forward.
+int branch_stream(cudaStream_t* out);
 int stream_wait(cudaStream_t waiter, cudaStream_t on);
 
 // Programmatic dependent launch for the tensor-core GEMMs and the small streaming kernels of the fused step:

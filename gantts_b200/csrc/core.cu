@@ -63,10 +63,12 @@ void prof_end(cudaStream_t st) {
   g_open_valid = false;
 }
 
-// The side stream of each device (created on first use) and the one event that orders it against the caller's stream.
+// The side and branch streams of each device (created on first use) and the one event that orders them against the
+// caller's stream.
 // stream_wait records and waits under one lock, so no other thread can re-record the event between the two calls.
 struct SideStream {
   cudaStream_t st = nullptr;
+  cudaStream_t branch = nullptr;
   cudaEvent_t ev = nullptr;
 };
 static std::mutex g_side_mu;
@@ -86,6 +88,13 @@ static int side_locked(SideStream** out) {
     GANTTS_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
     GANTTS_CUDA(cudaStreamCreateWithPriority(&s.st, cudaStreamNonBlocking, greatest));
   }
+  if (!s.branch) {
+    // the device's lowest priority (a caller's default stream has it too): at the highest, the branch's GEMMs took the
+    // SMs the generator forward's GEMMs were waiting for and the cfg2 step got slower (DESIGN.md section 5)
+    int least = 0, greatest = 0;
+    GANTTS_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+    GANTTS_CUDA(cudaStreamCreateWithPriority(&s.branch, cudaStreamNonBlocking, least));
+  }
   *out = &s;
   return GANTTS_OK;
 }
@@ -96,6 +105,15 @@ int side_stream(cudaStream_t* out) {
   int rc = side_locked(&s);
   if (rc) return rc;
   *out = s->st;
+  return GANTTS_OK;
+}
+
+int branch_stream(cudaStream_t* out) {
+  std::lock_guard<std::mutex> lk(g_side_mu);
+  SideStream* s;
+  int rc = side_locked(&s);
+  if (rc) return rc;
+  *out = s->branch;
   return GANTTS_OK;
 }
 

@@ -1031,6 +1031,9 @@ static int lstm_stack_bwd(const LstmStack& k, const int64_t* lengths, int B, int
 // chain; an SRU or LSTM generator's head and a recurrent discriminator's head stay on one stream (DESIGN.md section 5).
 static bool g_side_bwd(const gantts_gan_step_t* c) { return c->sru.num_layers == 0 && c->lstm.num_layers == 0; }
 static bool d_side_bwd(const gantts_gan_step_t* c) { return c->d_lstm.num_layers == 0; }
+// Phase 1 runs the real half of the stacked discriminator pass on the branch stream, beside the generator's forward,
+// when both stacks run their weight gradients on the side stream (DESIGN.md section 5).
+static bool d_real_branch(const gantts_gan_step_t* c) { return g_side_bwd(c) && d_side_bwd(c); }
 
 // The workspace is laid out once for the configured (B, T), the capacity: a call of shape (b, t) uses the first
 // M = b * t rows of every per-row buffer, and the split-K partials are sized for every M up to the capacity.  So the flat
@@ -1091,6 +1094,7 @@ struct Step {
   void* stream;
   cudaStream_t st;
   cudaStream_t side;        // the library's side stream (nullptr when no pass of the configuration uses it)
+  cudaStream_t branch;      // the library's branch stream (nullptr unless phase 1 runs D's real half on it)
   const HighwayArgs* hw() const { return c->highway.static_dim > 0 ? &hwa : nullptr; }
   bool d_rnn() const { return c->d_lstm.num_layers > 0; }
   // the discriminator's LSTM stack in forward `which` (1 stacked, 2 adversarial)
@@ -1217,40 +1221,54 @@ static int discriminator_stack_fwd(Step& s, bool stacked, const float* x, const 
 // adversarial columns of y's static features (real_cols), fake = those of y_hat_static; otherwise the fake rows alone
 // (the adversarial forward, train.py:307).  Unconditioned, the columns go straight into the operand planes of D's tape;
 // conditioned (train.py:254-256), D's input cat((x, columns), -1) is assembled in fp32 d_in, and the adversarial forward
-// re-uses the fake half the stacked one assembled.
-static int discriminator_fwd(Step& s, bool stacked) {
+// re-uses the fake half the stacked one assembled.  half (stacked, with the weight planes already split by
+// mlp_split_weights): 0 = the real rows [0, M) alone, 1 = the fake rows [M, 2M) alone; -1 = the whole pass.
+static int discriminator_fwd(Step& s, bool stacked, int half = -1) {
   const StepLayout& L = s.L;
   const int64_t M = s.M, rows = stacked ? 2 * M : M;
+  const int64_t r0 = half == 1 ? M : 0, r1 = half == 0 ? M : rows;
   int rc;
   Planes tape_in;
   if ((rc = mlp_tape_input_planes(&s.d, rows, L.d_tape, L.d_tape_bytes, &tape_in))) return rc;
   // a recurrent D (LSTMRNN / GRURNN): its stack reads the input planes, hidden2out the stack's top h in the tape
   const Planes din = s.d_rnn() ? lstm_in_planes(s.d_lstm(stacked ? 1 : 2), 0, rows) : tape_in;
+  ColList none;
+  none.n = 0;
   if (!s.cond_w) {
-    if (stacked) {
+    if (stacked && half < 0) {
       GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(2 * M * s.nA, 1024), 256, 0, s.st, s.y, s.d_out, s.real_cols, M,
                         s.y_hat_static, s.nS, s.adv_cols, M, din.hi, din.lo, din.pitch);
       GANTTS_LAUNCH_CHECK("gather_planes_kernel(real|fake)");
-    } else {
-      ColList none;
-      none.n = 0;
-      GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(M * s.nA, 1024), 256, 0, s.st, s.y_hat_static, s.nS, s.adv_cols, M,
+    } else if (half == 0) {
+      GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(M * s.nA, 1024), 256, 0, s.st, s.y, s.d_out, s.real_cols, M,
                         nullptr, 0, none, 0, din.hi, din.lo, din.pitch);
-      GANTTS_LAUNCH_CHECK("gather_planes_kernel(adv)");
+      GANTTS_LAUNCH_CHECK("gather_planes_kernel(real)");
+    } else {
+      // the fake rows: the adversarial forward's batch, or the stacked one's second half
+      const Planes fk = plane_rows(din, r0, r0 + M);
+      GANTTS_PDL_LAUNCH((gather_planes_kernel), blocks_1d(M * s.nA, 1024), 256, 0, s.st, s.y_hat_static, s.nS, s.adv_cols, M,
+                        nullptr, 0, none, 0, fk.hi, fk.lo, fk.pitch);
+      GANTTS_LAUNCH_CHECK("gather_planes_kernel(fake)");
     }
     if (s.d_rnn() && (rc = discriminator_stack_fwd(s, stacked, nullptr, tape_in))) return rc;
+    if (half >= 0) return mlp_fwd_rows(&s.d, nullptr, 0, rows, r0, r1, L.d_out, 1, L.d_tape, L.d_tape_bytes, s.st);
     return mlp_fwd_impl(&s.d, nullptr, 0, rows, L.d_out, 1, L.d_tape, L.d_tape_bytes, s.stream, true);
   }
   const int dD = s.dD;
   if (stacked) {
-    gather_cols_list_kernel<<<blocks_1d(M * s.nA, 1024), 256, 0, s.st>>>(s.y, s.d_out, L.d_in + s.cond_w, dD, s.real_cols, M);
-    GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(real)");
-    gather_cols_list_kernel<<<blocks_1d(M * s.nA, 1024), 256, 0, s.st>>>(s.y_hat_static, s.nS, L.d_in + M * dD + s.cond_w,
-                                                                          dD, s.adv_cols, M);
-    GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(fake)");
-    for (int64_t half = 0; half < 2; ++half)
-      GANTTS_CUDA(cudaMemcpy2DAsync(L.d_in + half * M * dD, (size_t)dD * sizeof(float), s.x, (size_t)s.d_in * sizeof(float),
+    if (half != 1) {
+      gather_cols_list_kernel<<<blocks_1d(M * s.nA, 1024), 256, 0, s.st>>>(s.y, s.d_out, L.d_in + s.cond_w, dD, s.real_cols, M);
+      GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(real)");
+    }
+    if (half != 0) {
+      gather_cols_list_kernel<<<blocks_1d(M * s.nA, 1024), 256, 0, s.st>>>(s.y_hat_static, s.nS, L.d_in + M * dD + s.cond_w,
+                                                                            dD, s.adv_cols, M);
+      GANTTS_LAUNCH_CHECK("gather_cols_list_kernel(fake)");
+    }
+    for (int64_t h = r0 / M; h < r1 / M; ++h)
+      GANTTS_CUDA(cudaMemcpy2DAsync(L.d_in + h * M * dD, (size_t)dD * sizeof(float), s.x, (size_t)s.d_in * sizeof(float),
                                     (size_t)s.cond_w * sizeof(float), (size_t)M, cudaMemcpyDeviceToDevice, s.st));
+    if (half >= 0) return mlp_fwd_rows(&s.d, L.d_in, dD, rows, r0, r1, L.d_out, 1, L.d_tape, L.d_tape_bytes, s.st);
   }
   if (s.d_rnn()) {
     if ((rc = discriminator_stack_fwd(s, stacked, L.d_in + (stacked ? 0 : M * dD), tape_in))) return rc;
@@ -1264,8 +1282,9 @@ static int discriminator_fwd(Step& s, bool stacked) {
 // adversarial batch, input gradient only.  When the adversarial columns form one window of y_hat_static the last GEMM
 // adds its result straight into g_static (the scatter of the column gather's backward); otherwise it goes to g_din and a
 // scatter kernel follows.  input_grad = false (the D-only step, where nothing consumes dL/dy_hat_static): parameter
-// gradients alone.
-static int discriminator_bwd(Step& s, bool stacked, bool input_grad = true) {
+// gradients alone.  fake_chain (stacked): the real rows' input-gradient chain already ran (discriminator_real_half), the
+// chain covers the fake rows.
+static int discriminator_bwd(Step& s, bool stacked, bool input_grad = true, bool fake_chain = false) {
   const StepLayout& L = s.L;
   const int64_t M = s.M, skip = stacked ? M : 0;      // the real rows' input gradient is not needed
   float* const* gW = stacked ? s.pd.gW : nullptr;
@@ -1290,16 +1309,40 @@ static int discriminator_bwd(Step& s, bool stacked, bool input_grad = true) {
     if ((rc = lstm_stack_bwd(k, stacked ? L.d_lstm.lengths : s.lengths, stacked ? 2 * s.B : s.B, s.T, s.seed, stacked,
                              input_grad ? &din : nullptr, s.st)))
       return rc;
-  } else if ((rc = mlp_bwd_impl(&s.d, L.g_dout, 1, L.d_out, 1, skip + M, L.d_tape, L.d_tape_bytes, gx, s.adv_window ? s.nS : s.dD,
-                                skip, gW, gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, s.adv_window ? 1 : -1, false,
-                                stacked ? s.side : nullptr))) {
-    return rc;
+  } else {
+    // the weight gradients on the side stream read both halves' gradient planes: it waits for the real half's branch
+    if (fake_chain && (rc = stream_wait(s.side, s.branch))) return rc;
+    if ((rc = mlp_bwd_impl(&s.d, L.g_dout, 1, L.d_out, 1, skip + M, L.d_tape, L.d_tape_bytes, gx, s.adv_window ? s.nS : s.dD,
+                           skip, gW, gb, 0, L.mlp_ws, L.mlp_ws_bytes, s.stream, s.adv_window ? 1 : -1, false,
+                           stacked ? s.side : nullptr, fake_chain ? M : 0)))
+      return rc;
   }
   if (s.adv_window || !input_grad) return GANTTS_OK;
   scatter_cols_list_add_kernel<<<blocks_1d(M * s.nA, 1024), 256, 0, s.st>>>(L.g_din + skip * s.dD + s.cond_w, s.dD,
                                                                              L.g_static, s.nS, s.adv_cols, M);
   GANTTS_LAUNCH_CHECK("scatter_cols_list_add_kernel");
   return GANTTS_OK;
+}
+
+// The real half of phase 1's stacked discriminator pass, on the branch stream from the end of the prologue: the real
+// rows' input gathered into D's tape, their forward, their BCE terms and dL/dD, and their input-gradient chain.  None
+// of it reads what the generator writes, so it runs beside the generator's forward, the MGE pass and the fake half's
+// forward.  D's weight planes are split on the caller's stream first, for both halves.  The stacked backward
+// (discriminator_bwd with fake_chain) makes the side stream wait for the branch before D's weight gradients, which read
+// both halves' gradient planes, and its closing join brings both back into the caller's stream.
+static int discriminator_real_half(Step& s) {
+  const StepLayout& L = s.L;
+  int rc;
+  if ((rc = mlp_split_weights(&s.d, 2 * s.M, L.d_tape, L.d_tape_bytes, s.st))) return rc;
+  if ((rc = stream_wait(s.branch, s.st))) return rc;
+  Step b = s;            // the same step, enqueued on the branch stream
+  b.st = s.branch;
+  b.stream = s.branch;
+  if ((rc = discriminator_fwd(b, true, 0))) return rc;
+  if ((rc = launch_bce(L.d_out, L.mask, s.M, 1, 0, 0, L.scal + S_INV_T, L.g_dout, &L.red[R_REAL], nullptr, b.st)))
+    return rc;
+  return mlp_bwd_impl(&s.d, L.g_dout, 1, L.d_out, 1, 2 * s.M, L.d_tape, L.d_tape_bytes, nullptr, 0, 0, nullptr, nullptr,
+                      0, L.mlp_ws, L.mlp_ws_bytes, b.stream, -1, false, nullptr, 0, s.M);
 }
 
 }  // namespace gantts
@@ -1383,7 +1426,9 @@ extern "C" int gantts_gan_step_shaped(const gantts_gan_step_t* c, int B, int T, 
   s.stream = stream;
   s.st = as_stream(stream);
   s.side = nullptr;
+  s.branch = nullptr;
   if ((g_side_bwd(c) || d_side_bwd(c)) && (rc = side_stream(&s.side))) return rc;
+  if (d_real_branch(c) && (rc = branch_stream(&s.branch))) return rc;
   layout(c, reinterpret_cast<char*>(al256(reinterpret_cast<uintptr_t>(workspace))), &s.L);
   const StepLayout& L = s.L;
   const int64_t M = s.M = (int64_t)B * T;
@@ -1462,6 +1507,11 @@ extern "C" int gantts_gan_step_shaped(const gantts_gan_step_t* c, int B, int T, 
   if (phases & 1) {
     NvtxRange r1("gantts_gan_step/phase1: G fwd, MLPG, MGE, D fwd+bwd");
     if ((rc = step_prologue(s, inv_frames, d_only))) return rc;
+    const bool branch = s.has_d && d_real_branch(c);
+    if (branch) {
+      s.d.seed = gantts_gan_step_seed(seed, 1);
+      if ((rc = discriminator_real_half(s))) return rc;
+    }
     if ((rc = generator_fwd(s, true))) return rc;
     // MGE loss (train.py:291) and its gradient in one pass; the gradient INITIALISES g_static, the two discriminator
     // passes then accumulate their input gradients on top of it.  D-only: forward values of MGE and MSE alone (the
@@ -1475,11 +1525,20 @@ extern "C" int gantts_gan_step_shaped(const gantts_gan_step_t* c, int B, int T, 
     if (s.has_d) {
       // ---- update_discriminator (train.py:245-279)
       s.d.seed = gantts_gan_step_seed(seed, 1);
-      if ((rc = discriminator_fwd(s, true))) return rc;
-      // real and fake BCE terms, counts and dL/dD of both halves (train.py:262-270) in one launch
-      if ((rc = launch_bce(L.d_out, L.mask, M, 2, 0, 1, L.scal + S_INV_T, L.g_dout, &L.red[R_REAL], &L.red[R_FAKE], st)))
-        return rc;
-      if ((rc = discriminator_bwd(s, true, !d_only))) return rc;
+      if (branch) {
+        // the fake half; the real half runs on the branch stream (discriminator_real_half), with the same launches per
+        // half, so both halves' terms, partials and gradients are those of the whole pass, bit for bit
+        if ((rc = discriminator_fwd(s, true, 1))) return rc;
+        if ((rc = launch_bce(L.d_out + M, L.mask, M, 1, 1, 0, L.scal + S_INV_T, L.g_dout + M, &L.red[R_FAKE], nullptr,
+                             st)))
+          return rc;
+      } else {
+        if ((rc = discriminator_fwd(s, true))) return rc;
+        // real and fake BCE terms, counts and dL/dD of both halves (train.py:262-270) in one launch
+        if ((rc = launch_bce(L.d_out, L.mask, M, 2, 0, 1, L.scal + S_INV_T, L.g_dout, &L.red[R_REAL], &L.red[R_FAKE], st)))
+          return rc;
+      }
+      if ((rc = discriminator_bwd(s, true, !d_only, branch))) return rc;
     }
   }
   if (d_only) {

@@ -694,6 +694,14 @@ static Planes carve_planes(char*& cur, int64_t rows, int64_t cols) {
   return pl;
 }
 
+// rows [r0, r1) of a planes matrix, as a matrix of their own (rows stay 32-byte aligned: TMA takes them as a base)
+static Planes plane_rows(Planes pl, int64_t r0, int64_t r1) {
+  pl.hi += r0 * pl.pitch;
+  pl.lo += r0 * pl.pitch;
+  pl.rows = r1 - r0;
+  return pl;
+}
+
 static int launch_split(const float* src, int64_t rs, int64_t rows, int cols, const Planes& pl, int transpose,
                         cudaStream_t st) {
   int64_t total = rows * cols;

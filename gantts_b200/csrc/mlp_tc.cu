@@ -175,14 +175,16 @@ gemv_fwd_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __res
   }
 }
 
-// partial[block][0..K) = sum over the block's rows of gz[m] * H[m][:], partial[block][K] = sum gz.
+// partial[block][0..K) = sum over the block's rows of gz[m] * H[m][:], partial[block][K] = sum gz (want_gw), and the
+// previous layer's gradient planes (want_gz).  A block's rows depend on the grid and M alone, so the partials of a launch
+// over M rows do not depend on which launches write the gradient planes of those rows.
 __global__ void __launch_bounds__(GEMV_THREADS)
 gemv_bwd_kernel(const float* __restrict__ gy, int64_t gy_rs, const float* __restrict__ y, int64_t y_rs,
                 const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __restrict__ lo, int64_t pitch,
                 const uint32_t* __restrict__ code, int64_t code_pitch, const float* __restrict__ w,
                 __nv_bfloat16* __restrict__ ghi, __nv_bfloat16* __restrict__ glo, int64_t gpitch,
                 float* __restrict__ partial, int64_t M, int K, int sigmoid, float dpos, float dneg, float dzero,
-                int want_gw) {
+                int want_gw, int want_gz) {
   __shared__ float ws[GEMV_MAX_K];
   __shared__ float gws[GEMV_THREADS / 32][GEMV_MAX_K + 1];
   for (int i = threadIdx.x; i < K; i += GEMV_THREADS) ws[i] = w[i];
@@ -211,6 +213,7 @@ gemv_bwd_kernel(const float* __restrict__ gy, int64_t gy_rs, const float* __rest
         gws[wid][c] = fmaf(g, a0, gws[wid][c]);
         if (c + 1 < K) gws[wid][c + 1] = fmaf(g, a1, gws[wid][c + 1]);
       }
+      if (!want_gz) continue;
       // gZ_prev = (g * w) * act'(H), derivative class from the 2-bit code plane
       const uint32_t cw = code[r * code_pitch + (c >> 4)];
       const uint32_t c0 = (cw >> (2 * (c & 15))) & 3u, c1 = (cw >> (2 * ((c + 1) & 15))) & 3u;
@@ -318,7 +321,7 @@ gemv_bwd_vec_kernel(const float* __restrict__ gy, int64_t gy_rs, const float* __
                     const uint32_t* __restrict__ code, int64_t code_pitch, const float* __restrict__ w,
                     __nv_bfloat16* __restrict__ ghi, __nv_bfloat16* __restrict__ glo, int64_t gpitch,
                     float* __restrict__ partial, int64_t M, int K, int sigmoid, float dpos, float dneg, float dzero,
-                    int want_gw) {
+                    int want_gw, int want_gz) {
   pdl_entry();
   __shared__ float gws[GEMV_THREADS / 32][GEMV_MAX_K + 1];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -357,7 +360,7 @@ gemv_bwd_vec_kernel(const float* __restrict__ gy, int64_t gy_rs, const float* __
             h[u][ch] = ldg_stream16(hi + r * pitch + c);
             l[u][ch] = ldg_stream16(lo + r * pitch + c);
           }
-          cw[u][ch] = __ldg(code + r * code_pitch + (c >> 4)) >> (2 * (c & 15));
+          if (want_gz) cw[u][ch] = __ldg(code + r * code_pitch + (c >> 4)) >> (2 * (c & 15));
         }
       }
     }
@@ -376,6 +379,7 @@ gemv_bwd_vec_kernel(const float* __restrict__ gy, int64_t gy_rs, const float* __
 #pragma unroll
           for (int j = 0; j < 8; ++j) gw[ch][j] = fmaf(g[u], a[j], gw[ch][j]);
         }
+        if (!want_gz) continue;
         // gZ_prev = (g * w) * act'(H), derivative class from the 2-bit code plane
         uint32_t oh[4], ol[4];
 #pragma unroll
@@ -536,6 +540,93 @@ extern "C" size_t gantts_mlp_workspace_bytes(const gantts_mlp_t* m, int64_t M) {
 namespace gantts {
 static int mlp_fwd_impl(const gantts_mlp_t* m, const float* x, int64_t x_rs, int64_t M, float* y, int64_t y_rs, void* tape,
                         size_t tape_bytes, void* stream, bool input_ready);
+// The forward of an M-row batch in row windows, which may run on different streams (the fused step's real and fake
+// halves of the stacked discriminator batch): mlp_split_weights writes the tape's weight planes once, then
+// mlp_fwd_rows runs every layer over rows [r0, r1), from x's rows (split into the tape's input planes first) or, with
+// x = nullptr, from input planes the caller wrote.  Dropout is keyed by the batch row, so each row's output, tape
+// planes and derivative codes are those of one launch over all M rows, bit for bit.
+static int mlp_split_weights(const gantts_mlp_t* m, int64_t M, void* tape, size_t tape_bytes, cudaStream_t st);
+static int mlp_fwd_rows(const gantts_mlp_t* m, const float* x, int64_t x_rs, int64_t M, int64_t r0, int64_t r1, float* y,
+                        int64_t y_rs, void* tape, size_t tape_bytes, cudaStream_t st);
+
+// every weight matrix into its [N][K] and transposed [K][N] planes in the tape, one launch
+static int split_weights(const gantts_mlp_t* m, const MlpTape& t, cudaStream_t st) {
+  const int L = m->num_layers;
+  WeightSplitList wl;
+  wl.n = L;
+  wl.off[0] = 0;
+  for (int l = 0; l < L; ++l) {
+    wl.W[l] = m->W[l];
+    wl.N[l] = m->dims[l + 1];
+    wl.K[l] = m->dims[l];
+    wl.hi[l] = t.W[l].hi;
+    wl.lo[l] = t.W[l].lo;
+    wl.pitch[l] = t.W[l].pitch;
+    wl.thi[l] = t.Wt[l].hi;
+    wl.tlo[l] = t.Wt[l].lo;
+    wl.tpitch[l] = t.Wt[l].pitch;
+    wl.off[l + 1] = wl.off[l] + (int64_t)((m->dims[l + 1] + 31) / 32) * ((m->dims[l] + 31) / 32);
+  }
+  int nb = (int)wl.off[L];
+  if (nb > num_sms() * 8) nb = num_sms() * 8;
+  if (nb < 1) nb = 1;
+  GANTTS_PDL_LAUNCH((split_weights_kernel), nb, 256, 0, st, wl);
+  GANTTS_LAUNCH_CHECK("split_weights_kernel");
+  return GANTTS_OK;
+}
+
+// every layer over rows [r0, r1) of the tape's batch, y's row r the batch's row r
+static int fwd_layers(const gantts_mlp_t* m, const MlpTape& t, int64_t r0, int64_t r1, float* y, int64_t y_rs,
+                      cudaStream_t st) {
+  const int L = m->num_layers;
+  const int64_t M = r1 - r0;
+  y += r0 * y_rs;
+  int rc;
+  for (int l = 0; l < L; ++l) {
+    const Planes A = plane_rows(t.H[l], r0, r1);
+    EpiArgs e;
+    e.bias = m->b[l];
+    e.row0 = r0;
+    if (l < L - 1) {
+      const Planes O = plane_rows(t.H[l + 1], r0, r1);
+      e.epi = EPI_PLANES_FWD;
+      e.out_hi = O.hi;
+      e.out_lo = O.lo;
+      e.out_pitch = O.pitch;
+      e.code = t.code[l + 1] + r0 * t.code_pitch[l + 1];
+      e.code_pitch = t.code_pitch[l + 1];
+      e.act = GANTTS_ACT_LEAKY_DROPOUT;
+      e.slope = m->slope;
+      e.p = m->dropout_p;
+      e.seed = layer_seed(m->seed, l);
+    } else {
+      if (m->dims[L] == 1 && L >= 2 && m->dims[l] <= GEMV_MAX_K && (m->dims[l] & 1) == 0) {
+        // single-output last layer: GEMV + sigmoid, one warp per row
+        const int Kl = m->dims[l], sg = m->last_act == GANTTS_ACT_SIGMOID;
+        if (Kl % 8 == 0 && Kl <= 256)
+          GANTTS_PDL_LAUNCH((gemv_fwd_vec_kernel<1, 4>), 2 * GEMV_BLOCKS, GEMV_THREADS, 0, st, A.hi, A.lo, A.pitch, m->W[l],
+                                                                          m->b[l], y, y_rs, M, Kl, sg);
+        else if (Kl % 8 == 0 && Kl <= 512)
+          gemv_fwd_vec_kernel<2, 2><<<2 * GEMV_BLOCKS, GEMV_THREADS, 0, st>>>(A.hi, A.lo, A.pitch, m->W[l],
+                                                                          m->b[l], y, y_rs, M, Kl, sg);
+        else if (Kl % 8 == 0)
+          gemv_fwd_vec_kernel<4, 1><<<2 * GEMV_BLOCKS, GEMV_THREADS, 0, st>>>(A.hi, A.lo, A.pitch, m->W[l],
+                                                                          m->b[l], y, y_rs, M, Kl, sg);
+        else
+          gemv_fwd_kernel<<<GEMV_BLOCKS, GEMV_THREADS, 0, st>>>(A.hi, A.lo, A.pitch, m->W[l], m->b[l], y,
+                                                                y_rs, M, Kl, sg);
+        GANTTS_LAUNCH_CHECK("gemv_fwd_kernel");
+        continue;
+      }
+      e.epi = EPI_F32;
+      e.C = y;
+      e.ldc = y_rs;
+      e.act = m->last_act;
+    }
+    if ((rc = launch_gemm_kk(A, t.W[l], e, st))) return rc;
+  }
+  return GANTTS_OK;
+}
 
 static int mlp_tape_input_planes(const gantts_mlp_t* m, int64_t M, void* tape, size_t tape_bytes, Planes* out) {
   int rc = check_mlp(m, M);
@@ -570,80 +661,53 @@ static int gantts::mlp_fwd_impl(const gantts_mlp_t* m, const float* x, int64_t x
   cudaStream_t st = as_stream(stream);
   MlpTape t;
   carve_tape(m, M, reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(tape) + 255) / 256 * 256), &t);
-  const int L = m->num_layers;
   if (!input_ready && (rc = launch_split(x, x_rs, M, m->dims[0], t.H[0], 0, st))) return rc;
-  {
-    WeightSplitList wl;
-    wl.n = L;
-    wl.off[0] = 0;
-    for (int l = 0; l < L; ++l) {
-      wl.W[l] = m->W[l];
-      wl.N[l] = m->dims[l + 1];
-      wl.K[l] = m->dims[l];
-      wl.hi[l] = t.W[l].hi;
-      wl.lo[l] = t.W[l].lo;
-      wl.pitch[l] = t.W[l].pitch;
-      wl.thi[l] = t.Wt[l].hi;
-      wl.tlo[l] = t.Wt[l].lo;
-      wl.tpitch[l] = t.Wt[l].pitch;
-      wl.off[l + 1] = wl.off[l] + (int64_t)((m->dims[l + 1] + 31) / 32) * ((m->dims[l] + 31) / 32);
-    }
-    int nb = (int)wl.off[L];
-    if (nb > num_sms() * 8) nb = num_sms() * 8;
-    if (nb < 1) nb = 1;
-    GANTTS_PDL_LAUNCH((split_weights_kernel), nb, 256, 0, st, wl);
-    GANTTS_LAUNCH_CHECK("split_weights_kernel");
+  if ((rc = split_weights(m, t, st))) return rc;
+  return fwd_layers(m, t, 0, M, y, y_rs, st);
+}
+
+static int gantts::mlp_split_weights(const gantts_mlp_t* m, int64_t M, void* tape, size_t tape_bytes, cudaStream_t st) {
+  int rc = check_mlp(m, M);
+  if (rc) return rc;
+  if (!tape || tape_bytes < gantts_mlp_tape_bytes(m, M)) {
+    set_error("mlp_split_weights: tape too small");
+    return GANTTS_E_WORKSPACE;
   }
-  for (int l = 0; l < L; ++l) {
-    EpiArgs e;
-    e.bias = m->b[l];
-    if (l < L - 1) {
-      e.epi = EPI_PLANES_FWD;
-      e.out_hi = t.H[l + 1].hi;
-      e.out_lo = t.H[l + 1].lo;
-      e.out_pitch = t.H[l + 1].pitch;
-      e.code = t.code[l + 1];
-      e.code_pitch = t.code_pitch[l + 1];
-      e.act = GANTTS_ACT_LEAKY_DROPOUT;
-      e.slope = m->slope;
-      e.p = m->dropout_p;
-      e.seed = layer_seed(m->seed, l);
-    } else {
-      if (m->dims[L] == 1 && L >= 2 && m->dims[l] <= GEMV_MAX_K && (m->dims[l] & 1) == 0) {
-        // single-output last layer: GEMV + sigmoid, one warp per row
-        const int Kl = m->dims[l], sg = m->last_act == GANTTS_ACT_SIGMOID;
-        if (Kl % 8 == 0 && Kl <= 256)
-          GANTTS_PDL_LAUNCH((gemv_fwd_vec_kernel<1, 4>), 2 * GEMV_BLOCKS, GEMV_THREADS, 0, st, t.H[l].hi, t.H[l].lo, t.H[l].pitch, m->W[l],
-                                                                          m->b[l], y, y_rs, M, Kl, sg);
-        else if (Kl % 8 == 0 && Kl <= 512)
-          gemv_fwd_vec_kernel<2, 2><<<2 * GEMV_BLOCKS, GEMV_THREADS, 0, st>>>(t.H[l].hi, t.H[l].lo, t.H[l].pitch, m->W[l],
-                                                                          m->b[l], y, y_rs, M, Kl, sg);
-        else if (Kl % 8 == 0)
-          gemv_fwd_vec_kernel<4, 1><<<2 * GEMV_BLOCKS, GEMV_THREADS, 0, st>>>(t.H[l].hi, t.H[l].lo, t.H[l].pitch, m->W[l],
-                                                                          m->b[l], y, y_rs, M, Kl, sg);
-        else
-          gemv_fwd_kernel<<<GEMV_BLOCKS, GEMV_THREADS, 0, st>>>(t.H[l].hi, t.H[l].lo, t.H[l].pitch, m->W[l], m->b[l], y,
-                                                                y_rs, M, Kl, sg);
-        GANTTS_LAUNCH_CHECK("gemv_fwd_kernel");
-        continue;
-      }
-      e.epi = EPI_F32;
-      e.C = y;
-      e.ldc = y_rs;
-      e.act = m->last_act;
-    }
-    if ((rc = launch_gemm_kk(t.H[l], t.W[l], e, st))) return rc;
+  MlpTape t;
+  carve_tape(m, M, reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(tape) + 255) / 256 * 256), &t);
+  return split_weights(m, t, st);
+}
+
+static int gantts::mlp_fwd_rows(const gantts_mlp_t* m, const float* x, int64_t x_rs, int64_t M, int64_t r0, int64_t r1,
+                                float* y, int64_t y_rs, void* tape, size_t tape_bytes, cudaStream_t st) {
+  int rc = check_mlp(m, M);
+  if (rc) return rc;
+  GANTTS_CHECK_ARG(r0 >= 0 && r0 < r1 && r1 <= M, "mlp_fwd_rows: bad row window [%lld, %lld) of %lld rows",
+                   (long long)r0, (long long)r1, (long long)M);
+  GANTTS_CHECK_ARG((!x || x_rs >= m->dims[0]) && y && y_rs >= m->dims[m->num_layers], "mlp_fwd_rows: bad pointers/strides");
+  if (!tape || tape_bytes < gantts_mlp_tape_bytes(m, M)) {
+    set_error("mlp_fwd_rows: tape too small");
+    return GANTTS_E_WORKSPACE;
   }
-  return GANTTS_OK;
+  MlpTape t;
+  carve_tape(m, M, reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(tape) + 255) / 256 * 256), &t);
+  if (x && (rc = launch_split(x + r0 * x_rs, x_rs, r1 - r0, m->dims[0], plane_rows(t.H[0], r0, r1), 0, st))) return rc;
+  return fwd_layers(m, t, r0, r1, y, y_rs, st);
 }
 
 // gx_row0: the input gradient is only produced for rows [gx_row0, M) (the fused step stacks real | fake rows and
 // needs the gradient w.r.t. the fake half only: the real half's input is data).
+// chain_r0, chain_r1: the input-gradient chain -- the output gradient's planes, every layer's gradient planes, gx --
+// covers rows [chain_r0, chain_r1) of the batch (chain_r1 < 0: M), while the weight gradients cover all M rows.  A
+// windowed call reads the other rows' gradient planes as an earlier windowed call left them: the fused step runs the
+// real half's chain with no weight gradients on its branch stream, then the fake half's with the weight gradients.  Each
+// row's planes are those of one chain over all M rows, and so are the weight gradients, bit for bit.
 namespace gantts {
 static int mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t gy_rs, const float* y, int64_t y_rs, int64_t M,
                         const void* tape, size_t tape_bytes, float* gx, int64_t gx_rs, int64_t gx_row0,
                         float* const* gW, float* const* gb, int accumulate, void* workspace, size_t workspace_bytes,
-                        void* stream, int gx_accumulate = -1, bool gy_planes_ready = false, cudaStream_t side = nullptr);
+                        void* stream, int gx_accumulate = -1, bool gy_planes_ready = false, cudaStream_t side = nullptr,
+                        int64_t chain_r0 = 0, int64_t chain_r1 = -1);
 // Where mlp_bwd_impl expects the output-gradient planes when gy_planes_ready (linear output, not the GEMV tail): the
 // producer of gy (the MLPG backward in the fused step) can write them directly instead of an fp32 matrix.
 static int mlp_bwd_gy_planes(const gantts_mlp_t* m, int64_t M, void* workspace, size_t workspace_bytes, Planes* out);
@@ -673,7 +737,7 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
                                 int64_t M, const void* tape, size_t tape_bytes, float* gx, int64_t gx_rs,
                                 int64_t gx_row0, float* const* gW, float* const* gb, int accumulate, void* workspace,
                                 size_t workspace_bytes, void* stream, int gx_accumulate, bool gy_planes_ready,
-                                cudaStream_t side) {
+                                cudaStream_t side, int64_t chain_r0, int64_t chain_r1) {
   // gx_accumulate: -1 = like the parameter gradients, 0 = store, 1 = add to what gx holds (gx may be a column window of
   // a wider matrix with row stride gx_rs: the fused step scatters the input gradient into g_static this way)
   // side: the weight and bias gradients (their GEMMs, the GEMV tail's reduction, the split-K reduction) run on this
@@ -683,6 +747,11 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
   int rc = check_mlp(m, M);
   GANTTS_CHECK_ARG(gx_row0 >= 0 && gx_row0 < M, "mlp_bwd: bad gx_row0");
   if (rc) return rc;
+  if (chain_r1 < 0) chain_r1 = M;
+  GANTTS_CHECK_ARG(chain_r0 >= 0 && chain_r0 < chain_r1 && chain_r1 <= M, "mlp_bwd: bad chain rows [%lld, %lld)",
+                   (long long)chain_r0, (long long)chain_r1);
+  const bool windowed = chain_r0 > 0 || chain_r1 < M;
+  GANTTS_CHECK_ARG(!windowed || !gy_planes_ready, "mlp_bwd: a row window needs gy, not gy planes");
   const int L = m->num_layers;
   GANTTS_CHECK_ARG(gy_planes_ready || (gy && gy_rs >= m->dims[L]), "mlp_bwd: bad gy");
   GANTTS_CHECK_ARG(!gy_planes_ready || (m->last_act == GANTTS_ACT_NONE && m->dims[L] > 1),
@@ -692,7 +761,9 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
     set_error("mlp_bwd: tape too small");
     return GANTTS_E_WORKSPACE;
   }
-  size_t need = mlp_workspace_bytes(m, M, false, side != nullptr);
+  // windowed calls over the same batch keep a buffer per layer, so that their gradient planes meet at one address
+  const bool per_layer = side != nullptr || windowed;
+  size_t need = mlp_workspace_bytes(m, M, false, per_layer);
   if (!workspace || workspace_bytes < need) {
     set_error("mlp_bwd: workspace too small (%zu < %zu)", workspace_bytes, need);
     return GANTTS_E_WORKSPACE;
@@ -706,7 +777,7 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
   int maxd = 0;
   for (int l = 0; l <= L; ++l) maxd = m->dims[l] > maxd ? m->dims[l] : maxd;
   char* cur = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(workspace) + 255) / 256 * 256);
-  const int nbuf = mlp_grad_bufs(m, side != nullptr);
+  const int nbuf = mlp_grad_bufs(m, per_layer);
   char* gbuf[GANTTS_MAX_LAYERS > MLP_GRAD_BUFS ? GANTTS_MAX_LAYERS : MLP_GRAD_BUFS];
   for (int i = 0; i < nbuf; ++i) {
     gbuf[i] = cur;
@@ -730,23 +801,37 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
     G = carve_planes(cg, M, K1);
     const float ks = m->dropout_p > 0.f ? 1.f / (1.f - m->dropout_p) : 1.f;
     const int want = (gW && gW[L - 1]) || (gb && gb[L - 1]);
+    // rows [r0, r1): their gradient planes (gz) and / or the block partials of gW, gb over them (gw)
+    auto gemv_bwd = [&](int64_t r0, int64_t r1, int gw, int gz, cudaStream_t s) {
+      const Planes H = plane_rows(t.H[L - 1], r0, r1), Gw = plane_rows(G, r0, r1);
 #define GANTTS_GEMV_BWD_ARGS                                                                                     \
-  gy, gy_rs, y, y_rs, t.H[L - 1].hi, t.H[L - 1].lo, t.H[L - 1].pitch, t.code[L - 1], t.code_pitch[L - 1],       \
-      m->W[L - 1], G.hi, G.lo, G.pitch, gemv_part, M, K1, m->last_act == GANTTS_ACT_SIGMOID ? 1 : 0, ks,        \
-      m->slope * ks, m->dropout_p > 0.f ? 0.f : m->slope, want
-    if (K1 % 8 == 0 && K1 <= 256)
-      GANTTS_PDL_LAUNCH((gemv_bwd_vec_kernel<1, 4>), GEMV_BLOCKS, GEMV_THREADS, 0, st, GANTTS_GEMV_BWD_ARGS);
-    else if (K1 % 8 == 0 && K1 <= 512)
-      gemv_bwd_vec_kernel<2, 2><<<GEMV_BLOCKS, GEMV_THREADS, 0, st>>>(GANTTS_GEMV_BWD_ARGS);
-    else if (K1 % 8 == 0)
-      gemv_bwd_vec_kernel<4, 1><<<GEMV_BLOCKS, GEMV_THREADS, 0, st>>>(GANTTS_GEMV_BWD_ARGS);
-    else
-      gemv_bwd_kernel<<<GEMV_BLOCKS, GEMV_THREADS, 0, st>>>(GANTTS_GEMV_BWD_ARGS);
+  gy + r0 * gy_rs, gy_rs, y ? y + r0 * y_rs : nullptr, y_rs, H.hi, H.lo, H.pitch,                              \
+      t.code[L - 1] + r0 * t.code_pitch[L - 1], t.code_pitch[L - 1], m->W[L - 1], Gw.hi, Gw.lo, Gw.pitch,       \
+      gemv_part, r1 - r0, K1, m->last_act == GANTTS_ACT_SIGMOID ? 1 : 0, ks, m->slope * ks,                     \
+      m->dropout_p > 0.f ? 0.f : m->slope, gw, gz
+      if (K1 % 8 == 0 && K1 <= 256)
+        GANTTS_PDL_LAUNCH((gemv_bwd_vec_kernel<1, 4>), GEMV_BLOCKS, GEMV_THREADS, 0, s, GANTTS_GEMV_BWD_ARGS);
+      else if (K1 % 8 == 0 && K1 <= 512)
+        gemv_bwd_vec_kernel<2, 2><<<GEMV_BLOCKS, GEMV_THREADS, 0, s>>>(GANTTS_GEMV_BWD_ARGS);
+      else if (K1 % 8 == 0)
+        gemv_bwd_vec_kernel<4, 1><<<GEMV_BLOCKS, GEMV_THREADS, 0, s>>>(GANTTS_GEMV_BWD_ARGS);
+      else
+        gemv_bwd_kernel<<<GEMV_BLOCKS, GEMV_THREADS, 0, s>>>(GANTTS_GEMV_BWD_ARGS);
 #undef GANTTS_GEMV_BWD_ARGS
-    GANTTS_LAUNCH_CHECK("gemv_bwd_kernel");
+      GANTTS_LAUNCH_CHECK("gemv_bwd_kernel");
+      return GANTTS_OK;
+    };
+    // a window's chain writes its rows' planes; the partials of gW, gb come from one launch over all M rows, on the
+    // weight-gradient stream, with the same row-to-block mapping as the single launch of an unwindowed call
+    if (!windowed) {
+      if ((rc = gemv_bwd(0, M, want, 1, st))) return rc;
+    } else if ((rc = gemv_bwd(chain_r0, chain_r1, 0, 1, st))) {
+      return rc;
+    }
     if (want) {
       // partial rows are [K1 weights | 1 bias]: one column-parallel reduction for both
       if ((rc = fork())) return rc;
+      if (windowed && (rc = gemv_bwd(0, M, 1, 0, ws))) return rc;
       GANTTS_PDL_LAUNCH((gemv_partial_reduce_kernel), (K1 + 1 + 31) / 32, 256, 0, ws, gemv_part, GEMV_BLOCKS, K1,
                                                                     gW ? gW[L - 1] : nullptr,
                                                                     gb ? gb[L - 1] : nullptr, accumulate);
@@ -754,11 +839,13 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
     }
     l_start = L - 2;
   } else if (!gy_planes_ready) {
-    int64_t total = M * m->dims[L];
+    const int64_t rows = chain_r1 - chain_r0, total = rows * m->dims[L];
     int nb = (int)((total + 1023) / 1024);
     if (nb > num_sms() * 8) nb = num_sms() * 8;
     if (nb < 1) nb = 1;
-    grad_out_to_planes_kernel<<<nb, 256, 0, st>>>(gy, gy_rs, y, y_rs, M, m->dims[L], G.hi, G.lo, G.pitch,
+    const Planes Gw = plane_rows(G, chain_r0, chain_r1);
+    grad_out_to_planes_kernel<<<nb, 256, 0, st>>>(gy + chain_r0 * gy_rs, gy_rs, y ? y + chain_r0 * y_rs : nullptr, y_rs,
+                                                  rows, m->dims[L], Gw.hi, Gw.lo, Gw.pitch,
                                                   m->last_act == GANTTS_ACT_SIGMOID ? 1 : 0);
     GANTTS_LAUNCH_CHECK("grad_out_to_planes_kernel");
   }
@@ -777,29 +864,27 @@ static int gantts::mlp_bwd_impl(const gantts_mlp_t* m, const float* gy, int64_t 
     if (l > 0) {
       char* c1 = gbuf[(pp + 1) % nbuf];
       Planes Gn = carve_planes(c1, M, m->dims[l]);
+      const Planes O = plane_rows(Gn, chain_r0, chain_r1);
       EpiArgs e;
       e.epi = EPI_PLANES_BWD;
-      e.out_hi = Gn.hi;
-      e.out_lo = Gn.lo;
-      e.out_pitch = Gn.pitch;
-      e.code = t.code[l];
+      e.out_hi = O.hi;
+      e.out_lo = O.lo;
+      e.out_pitch = O.pitch;
+      e.code = t.code[l] + chain_r0 * t.code_pitch[l];
       e.code_pitch = t.code_pitch[l];
       e.slope = m->slope;
       e.p = m->dropout_p;
-      if ((rc = launch_gemm_kk(G, t.Wt[l], e, st))) return rc;
+      if ((rc = launch_gemm_kk(plane_rows(G, chain_r0, chain_r1), t.Wt[l], e, st))) return rc;
       G = Gn;
       pp = (pp + 1) % nbuf;
-    } else if (gx) {
+    } else if (gx && (gx_row0 > chain_r0 ? gx_row0 : chain_r0) < chain_r1) {
+      const int64_t g0 = gx_row0 > chain_r0 ? gx_row0 : chain_r0;
       EpiArgs e;
       e.epi = EPI_F32;
-      e.C = gx + gx_row0 * gx_rs;
+      e.C = gx + g0 * gx_rs;
       e.ldc = gx_rs;
       e.accumulate = gx_accumulate;
-      Planes Gs = G;
-      Gs.hi += gx_row0 * G.pitch;
-      Gs.lo += gx_row0 * G.pitch;
-      Gs.rows = G.rows - gx_row0;
-      if ((rc = launch_gemm_kk(Gs, t.Wt[0], e, st))) return rc;
+      if ((rc = launch_gemm_kk(plane_rows(G, g0, chain_r1), t.Wt[0], e, st))) return rc;
     }
   }
   if ((rc = flush_reduce(rl, accumulate, ws))) return rc;
