@@ -139,6 +139,7 @@ FRAMES_BAD_DURATION, FRAMES_TOO_LONG = 1, 2     # GANTTS_FRAMES_*: gantts_state_
 MAX_FRAMES = 1 << 24        # per state duration and per row
 CORPUS_BAD_ROW = 1          # GANTTS_CORPUS_BAD_ROW: gantts_corpus_gather's status bit
 WORLD_BAD_F0, WORLD_SHORT = 1, 2    # GANTTS_WORLD_*: gantts_world_time_base's status bits
+ANALYSIS_BAD_INPUT, ANALYSIS_SHORT, ANALYSIS_FFT = 1, 2, 4      # GANTTS_ANALYSIS_*: the analysis chain's status bits
 GANTTS_E_BADARG = 1
 
 _lib = None
@@ -173,6 +174,7 @@ SIGNATURES = {
     "gantts_mlpg_ragged": (_i, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, ctypes.POINTER(StreamsT),
                                 ctypes.POINTER(WindowsT), _vp, _i, _i, _vp, _sz, _vp]),
     "gantts_mcep_operator": (_i, [ctypes.c_double, _i, _i, _i, _vp]),
+    "gantts_sp2mc_operator": (_i, [ctypes.c_double, _i, _i, _vp]),
     "gantts_mcep_postfilter": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, ctypes.c_double, _vp, _i, _i, _i, _i, _vp]),
     "gantts_mcep_to_sp": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _i, _i, _i, _i, _vp]),
     "gantts_modspec": (_i, [_vp, _i64, _i64, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
@@ -191,6 +193,15 @@ SIGNATURES = {
     "gantts_world_synthesize_workspace_bytes": (_sz, [_i, _i, _i64]),
     "gantts_world_synthesize": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i, _i64, _vp, _i, _i,
                                      _i, ctypes.c_double, _i, _i, _vp, _vp, _sz, _vp]),
+    "gantts_world_dio_frames": (_i64, [_i64, _i, ctypes.c_double]),
+    "gantts_world_dio_workspace_bytes": (_sz, [_i, _i, _i, ctypes.c_double]),
+    "gantts_world_dio": (_i, [_vp, _i64, _vp, _i, _i, _i, ctypes.c_double, _vp, _vp, _vp, _sz, _vp]),
+    "gantts_world_stonemask": (_i, [_vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, ctypes.c_double, _vp, _vp, _vp]),
+    "gantts_world_cheaptrick_draws": (_i64, [_i, _i, _i]),
+    "gantts_world_cheaptrick": (_i, [_vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, ctypes.c_double, _i, _vp, _i64, _vp,
+                                     _vp, _vp, _vp]),
+    "gantts_sp2mc": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "gantts_modspec_smoothing": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "gantts_distortions_workspace_bytes": (_sz, []),
     "gantts_distortions": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp,
                                 ctypes.POINTER(DistortionColsT), _vp, _vp, _sz, _vp]),

@@ -167,6 +167,24 @@ static int mcep_launch(const McepParams& p, int B, void* stream) {
   return GANTTS_OK;
 }
 
+// C[i * cols + m]: coefficient i (0..m2) of freqt(e_m, m2, a) for m < cols, SPTK's recursion run on each unit vector
+// (coefficients above m are 0 and leave g at 0, so the recursion starts at m).  Shared by every kind of operator.
+static std::vector<double> freqt_columns(double a, int cols, int m2) {
+  const double bb = 1.0 - a * a;
+  std::vector<double> C((size_t)(m2 + 1) * cols, 0.0), g(m2 + 1), d(m2 + 1);
+  for (int m = 0; m < cols; ++m) {
+    std::fill(g.begin(), g.end(), 0.0);
+    for (int i = m; i >= 0; --i) {
+      d = g;
+      g[0] = (i == m ? 1.0 : 0.0) + a * d[0];
+      if (m2 >= 1) g[1] = bb * d[0] + a * d[1];
+      for (int j = 2; j <= m2; ++j) g[j] = d[j - 1] + a * (d[j] - g[j - 1]);
+    }
+    for (int i = 0; i <= m2; ++i) C[(size_t)i * cols + m] = g[i];
+  }
+  return C;
+}
+
 }  // namespace gantts
 
 using namespace gantts;
@@ -180,24 +198,14 @@ extern "C" int gantts_mcep_operator(double alpha, int order, int fftlen, int kin
                    "mcep_operator: kind %d must be GANTTS_MCEP_R0 (0) or GANTTS_MCEP_SP (1)", kind);
   GANTTS_CHECK_ARG(out != nullptr, "mcep_operator: null output");
   const int M1 = order + 1, n = fftlen, half = n / 2, K = half + 1;
+  std::vector<double> cs(n);
+  for (int j = 0; j < n; ++j) cs[j] = cos(2.0 * M_PI * (double)j / (double)n);
   const int m2 = kind == GANTTS_MCEP_SP ? half : half - 1;   // freqt order: n/2 (mc2sp), n/2 - 1 (merlin_post_filter)
-  // C[i][m]: coefficient i of freqt(e_m, m2, -alpha), the SPTK recursion run on each unit vector
-  const double a = -alpha, bb = 1.0 - a * a;
-  std::vector<double> C((size_t)(m2 + 1) * M1, 0.0), g(m2 + 1), d(m2 + 1);
-  for (int m = 0; m < M1; ++m) {
-    std::fill(g.begin(), g.end(), 0.0);
-    for (int i = m; i >= 0; --i) {                        // coefficients above m are 0 and leave g at 0
-      d = g;
-      g[0] = (i == m ? 1.0 : 0.0) + a * d[0];
-      if (m2 >= 1) g[1] = bb * d[0] + a * d[1];
-      for (int j = 2; j <= m2; ++j) g[j] = d[j - 1] + a * (d[j] - g[j - 1]);
-    }
-    for (int i = 0; i <= m2; ++i) C[(size_t)i * M1 + m] = g[i];
-  }
+  // C[i][m]: coefficient i of freqt(e_m, m2, -alpha)
+  const std::vector<double> C = freqt_columns(-alpha, M1, m2);
   // log power at bin k: 2 (c0 + sum_{0 < i < n/2} c_i cos(2 pi i k / n) [+ c_{n/2} (-1)^k / 2 for mc2sp's symmetric
   // cepstrum, whose Nyquist term is counted once])
-  std::vector<double> cs(n), row(M1);
-  for (int j = 0; j < n; ++j) cs[j] = cos(2.0 * M_PI * (double)j / (double)n);
+  std::vector<double> row(M1);
   for (int k = 0; k < K; ++k) {
     for (int m = 0; m < M1; ++m) row[m] = C[m];
     for (int i = 1; i < half; ++i) {
@@ -238,4 +246,27 @@ extern "C" int gantts_mcep_to_sp(const float* mc, int64_t mc_bstride, int64_t mc
   p.op = op_s; p.lengths = lengths_dev; p.coef = 1.0;
   p.T = T; p.M1 = M + 1; p.K = K;
   return mcep_launch<false>(p, B, stream);
+}
+
+extern "C" int gantts_sp2mc_operator(double alpha, int order, int fftlen, double* out) {
+  GANTTS_CHECK_ARG(fabs(alpha) < 1.0, "sp2mc_operator: alpha = %g must satisfy |alpha| < 1", alpha);
+  GANTTS_CHECK_ARG(order >= 0 && order + 1 <= MCEP_MAX_COLS, "sp2mc_operator: order M = %d: M + 1 must be in [1, %d]",
+                   order, MCEP_MAX_COLS);
+  GANTTS_CHECK_ARG(mcep_fftlen_ok(fftlen), "sp2mc_operator: fftlen = %d must be a power of two in [64, 4096]", fftlen);
+  GANTTS_CHECK_ARG(out != nullptr, "sp2mc_operator: null output");
+  const int M1 = order + 1, n = fftlen, half = n / 2, K = half + 1;
+  std::vector<double> cs(n);
+  for (int j = 0; j < n; ++j) cs[j] = cos(2.0 * M_PI * (double)j / (double)n);
+  // c = irfft(log sp) with c0 halved: c_j = h_j / n (L_0 + L_N (-1)^j + 2 sum_{0<k<N} L_k cos(2 pi j k / n)), h_0 = 1/2;
+  // mc = freqt(c, M, alpha), C[m][j] = freqt(e_j, M, alpha)[m]
+  const std::vector<double> C = freqt_columns(alpha, n, order);
+  for (int k = 0; k < K; ++k) {
+    const double wk = (k == 0 || k == half) ? 1.0 : 2.0;
+    for (int m = 0; m < M1; ++m) {
+      double acc = 0.0;
+      for (int j = 0; j < n; ++j) acc += C[(size_t)m * n + j] * (j == 0 ? 0.5 : 1.0) * cs[((int64_t)j * k) & (n - 1)];
+      out[(size_t)k * M1 + m] = acc * wk / (double)n;
+    }
+  }
+  return GANTTS_OK;
 }

@@ -418,9 +418,11 @@ __device__ void min_phase(double* u, double2* z, const double2* w, double2* X, i
   __syncthreads();
 }
 
-// out[(j + N) mod n] = r[j], r[j] = sum_k X[k] e^{2 pi i j k / n} over the Hermitian X given on 0..N (the imaginary parts
-// of X[0] and X[N] are ignored, as a real inverse FFT does): the unnormalised inverse real FFT, then fftshift.
-__device__ void irfft_shift(const double2* X, double2* z, const double2* w, double* out, int n, int N, int logN) {
+// out[(j + rot) mod n] = r[j], r[j] = sum_k X[k] e^{2 pi i j k / n} over the Hermitian X given on 0..N (the imaginary
+// parts of X[0] and X[N] are ignored, as a real inverse FFT does): the unnormalised inverse real FFT, then rotated by rot
+// (N: fftshift).  out may alias X.
+__device__ void irfft_shift(const double2* X, double2* z, const double2* w, double* out, int n, int N, int logN,
+                            int rot) {
   for (int k = threadIdx.x; k < N; k += blockDim.x) {
     const double2 a = k == 0 ? make_double2(X[0].x, 0.0) : X[k];
     const double2 c = k == 0 ? make_double2(X[N].x, 0.0) : X[N - k];
@@ -434,8 +436,8 @@ __device__ void irfft_shift(const double2* X, double2* z, const double2* w, doub
   fft_radix2_stages(z, w, N);
   for (int m = threadIdx.x; m < N; m += blockDim.x) {
     const double2 v = z[m];
-    out[(2 * m + N) & (n - 1)] = v.x;
-    out[(2 * m + 1 + N) & (n - 1)] = -v.y;
+    out[(2 * m + rot) & (n - 1)] = v.x;
+    out[(2 * m + 1 + rot) & (n - 1)] = -v.y;
   }
   __syncthreads();
 }
@@ -512,7 +514,7 @@ __global__ void __launch_bounds__(WD_THREADS) world_response_kernel(const SynthP
       X[k] = make_double2(re * c + im * s, im * c - re * s);
     }
     __syncthreads();
-    irfft_shift(X, z, w, per, n, N, logN);
+    irfft_shift(X, z, w, per, n, N, logN, N);
     double part = 0.0;
     for (int j = N + threadIdx.x; j < n; j += blockDim.x) part += per[j];
     const double dc = block_sum_f64(part, red);
@@ -545,7 +547,7 @@ __global__ void __launch_bounds__(WD_THREADS) world_response_kernel(const SynthP
     X[k] = make_double2(m.x * ns.x - m.y * ns.y, m.x * ns.y + m.y * ns.x);
   }
   __syncthreads();
-  irfft_shift(X, z, w, u, n, N, logN);
+  irfft_shift(X, z, w, u, n, N, logN, N);
   const double sq = sqrt((double)Ni);
   double* r = p.resp + (int64_t)blockIdx.x * n;
   for (int j = threadIdx.x; j < n; j += blockDim.x) r[j] = (per[j] * sq + u[j]) / n;

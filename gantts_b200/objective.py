@@ -10,12 +10,16 @@ options:
     --batch-size=<N>            Utterances per batch (default: hp.batch_size).
     --no-mge                    tts_acoustic: the generator was trained without MGE.
     --ms-fftlen=<n>             FFT length of the modulation spectrum [default: 4096].
-    --fs=<fs>                   Sampling frequency, only for the modulation frequencies ms_freq [default: 16000].
+    --fs=<fs>                   Sampling frequency of ms_freq and of the --wav-dir wavs [default: 16000].
+    --wav-dir=<dir>             Also analyse <dir>/<name>.wav of every utterance with WORLD, as the notebooks do, and
+                                compare against those features too (label natural_wav).
     -h, --help                  Show this help message and exit
 
 "Natural" features are the prepared targets of <outputs_dir> (Y, not normalised): the static mc columns for vc, the
-static mgc columns for tts_acoustic.  The reference notebooks re-analyse the target wavs with WORLD instead, which this
-command does not do.  tts_acoustic generates from the prepared inputs, so with natural durations.
+static mgc columns for tts_acoustic.  The reference notebooks re-analyse the target wavs with WORLD instead; --wav-dir
+adds those features beside the prepared ones (gantts_b200.analysis: DIO, StoneMask, CheapTrick, sp2mc, and for
+tts_acoustic the modulation-spectrum smoothing), for vc from the target speaker's wavs.  tts_acoustic generates from the
+prepared inputs, so with natural durations.
 """
 # The measures of the reference notebooks (notebooks/Test VC.ipynb, Test RNN VC.ipynb, Test TTS.ipynb): vis_gv's
 # np.var(mgc, axis=0) per utterance and mean_modspec's mean over utterances of np.log(P.modspec(mgc, n=4096)), for the
@@ -29,6 +33,7 @@ from os.path import abspath, basename, dirname, join, splitext
 import numpy as np
 import torch
 
+from . import analysis
 from . import generate
 from . import models
 from . import multistream
@@ -89,8 +94,9 @@ def natural_columns(hp):
     return slice(cols[0], cols[-1] + 1)
 
 
-def check_labels(labels, checkpoints):
-    """The labels as given, or each checkpoint's parent directory name; ValueError naming the rule otherwise."""
+def check_labels(labels, checkpoints, wavs=False):
+    """The labels as given, or each checkpoint's parent directory name; ValueError naming the rule otherwise.  wavs:
+    "natural_wav" is taken too."""
     if labels is None:
         labels = [basename(dirname(abspath(c))) for c in checkpoints]
         hint = " (the default labels are the checkpoints' directory names; pass --labels)"
@@ -101,10 +107,11 @@ def check_labels(labels, checkpoints):
                          % (len(labels), len(checkpoints)))
     if any(not lab for lab in labels):
         raise ValueError("--labels: a label must not be empty")
-    seen = ["natural"]
+    seen = ["natural"] + (["natural_wav"] if wavs else [])
+    note = "\"natural\" is the prepared targets' label" + (", \"natural_wav\" the analysed wavs'" if wavs else "")
     for lab in labels:
         if lab in seen:
-            raise ValueError("label %r is used twice (\"natural\" is the prepared targets' label)%s" % (lab, hint))
+            raise ValueError("label %r is used twice (%s)%s" % (lab, note, hint))
         seen.append(lab)
     return labels
 
@@ -128,6 +135,43 @@ def check_frames(files, X, Y):
         if len(x) != len(y):
             raise ValueError("%s: %d input frames but %d target frames; X and Y must be time-aligned (train.load_data)"
                              % (basename(f), len(x), len(y)))
+
+
+def read_wavs(wav_dir, files, fs):
+    """The samples of <wav_dir>/<name>.wav for every utterance file, as the notebooks read them (scipy.io.wavfile,
+    cast to float64 later); ValueError naming the wav when one is missing, is not at fs or is not mono."""
+    from scipy.io import wavfile
+    waves = []
+    for f in files:
+        path = join(wav_dir, splitext(basename(f))[0] + ".wav")
+        if not os.path.isfile(path):
+            raise ValueError("%s is missing (--wav-dir holds one <name>.wav per utterance)" % path)
+        rate, data = wavfile.read(path)
+        if rate != fs:
+            raise ValueError("%s is at %d Hz, but --fs=%d" % (path, rate, fs))
+        if data.ndim != 1:
+            raise ValueError("%s has %d channels; the analysis takes mono wavs" % (path, data.shape[1]))
+        waves.append(data)
+    return waves
+
+
+def wav_stats(hp, waves, fs, batch_size, n, device):
+    """FeatureStats.result() of the natural features analysed from the wavs (analysis.analyse), with gv in input order,
+    and each utterance's DIO frame count.  The batches are generate.plan_batches' over the sample counts, so the means
+    have the same bits for any batch size."""
+    kind = "vc" if hp.name == "vc" else "tts_acoustic"
+    fp = getattr(hp, "frame_period", FRAME_PERIOD)
+    stats = FeatureStats(analysis.feature_width(kind, int(hp.order)), n, device)
+    frames = np.zeros(len(waves), np.int64)
+    plan = generate.plan_batches([len(w) for w in waves], batch_size)
+    for idx in plan:
+        mc, host, lengths = analysis.analyse([waves[i] for i in idx], fs, fp, int(hp.order), kind, device)
+        stats.add(mc.float(), lengths)
+        frames[idx] = host
+    gv, gv_mean, ms_mean = stats.result()
+    gv_in = np.empty_like(gv)
+    gv_in[np.array([i for idx in plan for i in idx])] = gv
+    return (gv_in, gv_mean, ms_mean), frames
 
 
 def pad_batch(arrays, device):
@@ -174,13 +218,13 @@ def split_arrays(labels, files, Y, ms_freq, results):
             "ms_mean": np.stack([r[2] for r in results])}
 
 
-def summary(labels, gv_mean, ms_mean):
-    """[(label, mean over columns of log10(gv_mean / natural's), RMS over bins and columns of ms_mean - natural's)]
-    for every label after the first (natural)."""
+def summary(labels, gv_mean, ms_mean, ref=0):
+    """[(label, mean over columns of log10(gv_mean / the reference's), RMS over bins and columns of ms_mean - the
+    reference's)] for every label after the reference labels[ref] (natural, or natural_wav at 1)."""
     rows = []
-    for i in range(1, len(labels)):
-        rows.append((labels[i], float(np.mean(np.log10(gv_mean[i] / gv_mean[0]))),
-                     float(np.sqrt(np.mean((ms_mean[i] - ms_mean[0]) ** 2)))))
+    for i in range(ref + 1, len(labels)):
+        rows.append((labels[i], float(np.mean(np.log10(gv_mean[i] / gv_mean[ref]))),
+                     float(np.sqrt(np.mean((ms_mean[i] - ms_mean[ref]) ** 2)))))
     return rows
 
 
@@ -215,13 +259,21 @@ def main(argv=None, hp=None):
         if fs <= 0:
             raise ValueError("--fs must be > 0 (got %d)" % fs)
         ms_freq = modulation_frequencies(n, fs, getattr(hp, "frame_period", FRAME_PERIOD))
-        labels = ["natural"] + check_labels(args["--labels"], checkpoints)
+        wav_dir = args["--wav-dir"]
+        labels = (["natural"] + (["natural_wav"] if wav_dir else [])
+                  + check_labels(args["--labels"], checkpoints, wavs=bool(wav_dir)))
         inputs_dir, outputs_dir, dst_dir = args["<inputs_dir>"], args["<outputs_dir>"], args["<dst_dir>"]
         splits = []
         for sub, xf, yf in paired_files(inputs_dir, outputs_dir):
             X, Y = [np.load(f) for f in xf], [np.load(f) for f in yf]
             check_frames(xf, X, Y)
-            splits.append((sub, xf, X, Y))
+            splits.append((sub, xf, X, Y, read_wavs(wav_dir, xf, fs) if wav_dir else None))
+        if wav_dir:
+            kind = "vc" if hp.name == "vc" else "tts_acoustic"
+            cols = natural_columns(hp)
+            if analysis.feature_width(kind, int(hp.order)) != cols.stop - cols.start:
+                raise ValueError("hp.order = %d gives %d analysed columns, but the prepared targets have %d"
+                                 % (hp.order, analysis.feature_width(kind, int(hp.order)), cols.stop - cols.start))
     except ValueError as e:
         raise SystemExit("gantts_b200.objective: %s" % e)
     if not torch.cuda.is_available():
@@ -237,14 +289,21 @@ def main(argv=None, hp=None):
         generators.append(generate.ParameterGenerator(model_g.to(device), hp, stats, mge_training))
 
     os.makedirs(dst_dir, exist_ok=True)
-    for sub, xf, X, Y in splits:
-        arrays = split_arrays(labels, xf, Y, ms_freq, split_stats(hp, generators, X, Y, batch_size, n, device))
+    for sub, xf, X, Y, waves in splits:
+        results = split_stats(hp, generators, X, Y, batch_size, n, device)
+        if waves is not None:
+            wav_result, wav_frames = wav_stats(hp, waves, fs, batch_size, n, device)
+            results.insert(1, wav_result)
+        arrays = split_arrays(labels, xf, Y, ms_freq, results)
+        if waves is not None:
+            arrays["wav_lengths"] = wav_frames
         path = join(dst_dir, sub + ".npz")
         np.savez(path, **arrays)
         print(path)
-        for label, gv_ratio, ms_rms in summary(labels, arrays["gv_mean"], arrays["ms_mean"]):
-            print("%s %s: mean log10 GV ratio to natural %+.4f, RMS log MS difference to natural %.4f"
-                  % (sub, label, gv_ratio, ms_rms))
+        for ref in ((0, 1) if waves is not None else (0,)):
+            for label, gv_ratio, ms_rms in summary(labels, arrays["gv_mean"], arrays["ms_mean"], ref):
+                print("%s %s: mean log10 GV ratio to %s %+.4f, RMS log MS difference to %s %.4f"
+                      % (sub, label, labels[ref], gv_ratio, labels[ref], ms_rms))
     return 0
 
 

@@ -575,6 +575,153 @@ def world_synthesize(f0, sp, ap, lengths, fs, frame_period, pulses=None, noise=N
     return y, y_lengths
 
 
+# ------------------------------------------------------------- WORLD analysis, sp2mc and modulation-spectrum smoothing
+def world_dio_frames(samples, fs, frame_period):
+    """WORLD's GetSamplesForDIO: the frames pyworld.dio makes of `samples` samples."""
+    return int(_lib.load().gantts_world_dio_frames(int(samples), int(fs), float(frame_period)))
+
+
+def _waves(x, lengths, what):
+    if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float64 and x.dim() == 2):
+        raise RuntimeError("gantts_b200: %s needs x (B, S) float64 CUDA" % what)
+    if not (torch.is_tensor(lengths) and lengths.is_cuda and lengths.dtype == torch.int64 and lengths.dim() == 1
+            and lengths.numel() == x.shape[0]):
+        raise RuntimeError("gantts_b200: %s needs int64 CUDA lengths (B,)" % what)
+    return (x if x.stride(1) == 1 else x.contiguous()), lengths.contiguous()
+
+
+def _frames_f0(f0, info, B, what):
+    if not (torch.is_tensor(f0) and f0.is_cuda and f0.dtype == torch.float64 and f0.dim() == 2 and f0.shape[0] == B):
+        raise RuntimeError("gantts_b200: %s needs f0 (B, T) float64 CUDA" % what)
+    if not (torch.is_tensor(info) and info.is_cuda and info.dtype == torch.int64 and tuple(info.shape) == (B + 1,)):
+        raise RuntimeError("gantts_b200: %s needs world_dio's info, int64 CUDA (B + 1,)" % what)
+    return f0.contiguous()
+
+
+def world_dio(x, lengths, fs, frame_period):
+    """pyworld.dio(x[b, :lengths[b]], fs, frame_period=frame_period) of every row b (gantts_world_dio): x (B, S) float64
+    CUDA.  Returns (f0 (B, T) float64 CUDA, T = world_dio_frames(S), 0 beyond each row's frames; info int64 CUDA (B + 1,):
+    each row's frame count, then the status word that world_stonemask and world_cheaptrick add to).  No host sync: read
+    info with world_analysis_check.  Frame j is at j frame_period / 1000 s."""
+    x, lengths = _waves(x, lengths, "world_dio")
+    lib = _lib.load()
+    B, S = x.shape
+    T = world_dio_frames(S, fs, frame_period)
+    nbytes = lib.gantts_world_dio_workspace_bytes(B, S, int(fs), float(frame_period))
+    if nbytes == 0:
+        raise RuntimeError("gantts_b200: world_dio: B = %d, S = %d, fs = %d, frame_period = %g out of range"
+                           % (B, S, fs, frame_period))
+    ws = workspace(nbytes, x.device, "world_dio")
+    f0 = torch.empty(B, T, dtype=torch.float64, device=x.device)
+    info = torch.empty(B + 1, dtype=torch.int64, device=x.device)
+    _lib.check(lib.gantts_world_dio(x.data_ptr(), x.stride(0), lengths.data_ptr(), B, S, int(fs), float(frame_period),
+                                    f0.data_ptr(), info.data_ptr(), ws.data_ptr(), nbytes, _stream()))
+    return f0, info
+
+
+def world_stonemask(x, lengths, f0, info, fs, frame_period):
+    """pyworld.stonemask(x[b, :lengths[b]], f0[b], timeaxis, fs) of every row over its info[b] frames
+    (gantts_world_stonemask): f0 and info world_dio's.  Returns (B, T) float64 CUDA.  No host sync."""
+    x, lengths = _waves(x, lengths, "world_stonemask")
+    B, S = x.shape
+    f0 = _frames_f0(f0, info, B, "world_stonemask")
+    out = torch.empty_like(f0)
+    _lib.check(_lib.load().gantts_world_stonemask(x.data_ptr(), x.stride(0), lengths.data_ptr(), f0.data_ptr(),
+                                                  info.data_ptr(), B, S, f0.shape[1], int(fs), float(frame_period),
+                                                  out.data_ptr(), info[B:].data_ptr(), _stream()))
+    return out
+
+
+def world_cheaptrick(x, lengths, f0, info, fs, frame_period, fftlen):
+    """pyworld.cheaptrick(x[b, :lengths[b]], f0[b], timeaxis, fs) with q1 -0.15, f0_floor 71 and fft_size fftlen
+    (generate.cheaptrick_fft_size(fs) is pyworld's) of every row over its info[b] frames (gantts_world_randn,
+    gantts_world_cheaptrick).  Returns (B, T, fftlen/2 + 1) float64 CUDA, 0 beyond each row's frames.  No host sync."""
+    x, lengths = _waves(x, lengths, "world_cheaptrick")
+    B, S = x.shape
+    f0 = _frames_f0(f0, info, B, "world_cheaptrick")
+    T = f0.shape[1]
+    lib = _lib.load()
+    count = int(lib.gantts_world_cheaptrick_draws(T, int(fs), int(fftlen)))
+    if count < 1:
+        raise RuntimeError("gantts_b200: world_cheaptrick: fftlen = %d must be a power of two in [64, 4096]" % fftlen)
+    noise = world_randn(count, x.device)
+    offsets = torch.empty(B, T, dtype=torch.int64, device=x.device)
+    sp = torch.empty(B, T, int(fftlen) // 2 + 1, dtype=torch.float64, device=x.device)
+    _lib.check(lib.gantts_world_cheaptrick(x.data_ptr(), x.stride(0), lengths.data_ptr(), f0.data_ptr(),
+                                           info.data_ptr(), B, S, T, int(fs), float(frame_period), int(fftlen),
+                                           noise.data_ptr(), count, offsets.data_ptr(), sp.data_ptr(),
+                                           info[B:].data_ptr(), _stream()))
+    return sp
+
+
+def world_analysis_check(info):
+    """The one host synchronisation of the analysis chain: copies world_dio's info (frame counts and the status word that
+    every analysis kernel adds to) and returns the frame counts as a host int64 array.  Raises RuntimeError naming the
+    rule when a status bit is set."""
+    host = info.cpu().numpy()
+    B = len(host) - 1
+    status = int(host[B])
+    if status & _lib.ANALYSIS_BAD_INPUT:
+        raise RuntimeError("gantts_b200: WORLD analysis: a sample within a row's length, or an f0, is not finite, or an "
+                           "f0 is beyond what CheapTrick's fft size can analyse")
+    if status & _lib.ANALYSIS_SHORT:
+        raise RuntimeError("gantts_b200: WORLD analysis: a row is too short for DIO (%d frames; FixF0Contour needs "
+                           "more frames than its window)" % int(host[:B].min()))
+    if status & _lib.ANALYSIS_FFT:
+        raise RuntimeError("gantts_b200: WORLD analysis: a StoneMask window needs an FFT over 4096 points")
+    return host[:B].copy()
+
+
+def sp2mc(sp, lengths, order, alpha):
+    """pysptk.sp2mc(sp[b, t], order, alpha) for t < lengths[b] (gantts_sp2mc): sp (B, T, K) float64 CUDA.  Returns
+    (B, T, order + 1) float64 CUDA, 0 beyond each length.  The operator is cached per (alpha, order, fftlen, device).
+    No host sync."""
+    if not (torch.is_tensor(sp) and sp.is_cuda and sp.dtype == torch.float64 and sp.dim() == 3):
+        raise RuntimeError("gantts_b200: sp2mc needs sp (B, T, K) float64 CUDA")
+    if not (torch.is_tensor(lengths) and lengths.is_cuda and lengths.dtype == torch.int64):
+        raise RuntimeError("gantts_b200: sp2mc needs int64 CUDA lengths")
+    sp = sp.contiguous()
+    B, T, K = sp.shape
+    key = (float(alpha), int(order), 2 * (K - 1), "sp2mc", sp.device.index)
+    op = _mcep_op_cache.get(key)
+    if op is None:
+        op = torch.from_numpy(sp2mc_operator_host(alpha, order, 2 * (K - 1))).to(sp.device)
+        _mcep_op_cache[key] = op
+    mc = torch.empty(B, T, int(order) + 1, dtype=torch.float64, device=sp.device)
+    _lib.check(_lib.load().gantts_sp2mc(sp.data_ptr(), op.data_ptr(), lengths.contiguous().data_ptr(), B, T, int(order),
+                                        K, mc.data_ptr(), _stream()))
+    return mc
+
+
+def sp2mc_operator_host(alpha, order, fftlen):
+    """The (fftlen/2 + 1, order + 1) float64 matrix of gantts_sp2mc_operator: column m maps a frame's log power to
+    pysptk.sp2mc's coefficient m.  Host computation."""
+    op = np.zeros((int(fftlen) // 2 + 1, int(order) + 1), dtype=np.float64)
+    _lib.check(_lib.load().gantts_sp2mc_operator(float(alpha), int(order), int(fftlen), op.ctypes.data))
+    return op
+
+
+def smoothing_bin(n, modfs, cutoff=50.0):
+    """The first modulation-frequency bin modspec_smoothing removes: int(n * cutoff / modfs)."""
+    return int(n * (float(cutoff) / float(modfs)))
+
+
+def modspec_smoothing(x, lengths, modfs, n=4096, cutoff=50.0):
+    """nnmnkwii.preprocessing.modspec_smoothing(x[b, :lengths[b]], modfs, n=n, cutoff=cutoff) of every row b
+    (gantts_modspec_smoothing): x (B, T, D) float64 CUDA with T <= n.  Returns (B, T, D) float64 CUDA, 0 beyond each
+    length.  No host sync."""
+    if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.float64 and x.dim() == 3):
+        raise RuntimeError("gantts_b200: modspec_smoothing needs x (B, T, D) float64 CUDA")
+    if not (torch.is_tensor(lengths) and lengths.is_cuda and lengths.dtype == torch.int64):
+        raise RuntimeError("gantts_b200: modspec_smoothing needs int64 CUDA lengths")
+    x = x.contiguous()
+    B, T, D = x.shape
+    out = torch.empty_like(x)
+    _lib.check(_lib.load().gantts_modspec_smoothing(x.data_ptr(), lengths.contiguous().data_ptr(), B, T, D, int(n),
+                                                    smoothing_bin(n, modfs, cutoff), out.data_ptr(), _stream()))
+    return out
+
+
 # ------------------------------------------------------------- mini-batches from a corpus on the device
 def corpus_gather(X, Y, offsets, lengths, t, x_out=None, y_out=None, status=None):
     """One padded mini-batch from a packed corpus on the device (gantts_corpus_gather): X (N, Dx), Y (N, Dy) contiguous

@@ -593,10 +593,15 @@ int gantts_mlpg_ragged(const float* in, int64_t in_bstride, int64_t in_tstride, 
  *                   mc2sp(mc)[k] = exp(row_k . mc).
  * gantts_mcep_operator builds either matrix on the host in double by running SPTK's freqt recursion on unit vectors; it
  * writes out[k * (M+1) + m].  Rules: |alpha| < 1, 1 <= M+1 <= 128, fftlen a power of two in [64, 4096], kind 0 or 1,
- * out non-null.  No device work. */
+ * out non-null.  No device work.
+ * gantts_sp2mc_operator is the other way (pysptk.sp2mc(sp, order, alpha), Test VC.ipynb / Test RNN VC.ipynb
+ * compute_static_features, Test TTS.ipynb compute_mgc_from_waveform): the K x (M+1) matrix, built by the same freqt
+ * recursion, of freqt(., M, alpha) of the inverse real FFT of the log power with c0 halved, so that
+ * sp2mc(sp)[m] = sum_k out[k * (M+1) + m] log sp[k].  Same rules but kind, no device work. */
 #define GANTTS_MCEP_R0 0
 #define GANTTS_MCEP_SP 1
 int gantts_mcep_operator(double alpha, int order, int fftlen, int kind, double* out);
+int gantts_sp2mc_operator(double alpha, int order, int fftlen, double* out);
 /* Merlin's post filter on every valid frame of a padded batch: mc float32 [B][T][M+1] (element strides mc_bstride,
  * mc_tstride; unit column stride), op_r the GANTTS_MCEP_R0 matrix on the device at fftlen = 2 (K - 1) (the reference's
  * defaults are fftlen 1024, minimum-phase order 511).  Writes w*mc with c0 shifted by log(r0(mc) / r0(w*mc)) / 2,
@@ -735,6 +740,58 @@ int gantts_world_synthesize(const float* sp, int64_t sp_bstride, int64_t sp_tstr
                             const double* pulse_shift, const uint8_t* pulse_vuv, const int64_t* info_dev, int cap,
                             int64_t total_pulses, const double* noise, int B, int T, int fs, double frame_period,
                             int fftlen, int y_max, double* y, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Analysis of natural waveforms: WORLD's DIO, StoneMask and CheapTrick with pyworld's defaults, pysptk.sp2mc and
+ * nnmnkwii.preprocessing.modspec_smoothing (replace, per utterance, the notebooks' compute_static_features in Test VC.ipynb
+ * and Test RNN VC.ipynb, and compute_mgc_from_waveform in Test TTS.ipynb: pyworld.dio(x, fs, frame_period=hp.frame_period),
+ * pyworld.stonemask(x, f0, timeaxis, fs), pyworld.cheaptrick(x, f0, timeaxis, fs), pysptk.sp2mc(sp, order, alpha) and,
+ * for TTS, P.modspec_smoothing(mc, modfs, cutoff=50)), in fp64.  x is fp64 [B][S] (row stride x_bstride >= S); row b is
+ * processed over its own L = lengths_dev[b] samples (int64[B], clamped to [0, S]) and its results depend only on that row:
+ * the same bits at any batch position, padded length or padding contents.  Frame j of a row is at j frame_period / 1000 s.
+ * gantts_world_dio_frames: WORLD's GetSamplesForDIO, int(1000 samples / fs / frame_period) + 1.
+ * gantts_world_dio: f0 fp64 [B][T], T = gantts_world_dio_frames(S), pyworld.dio with f0_floor 71, f0_ceil 800,
+ *   channels_in_octave 2, speed 1, allowed_range 0.1; 0 beyond a row's frames.  info_dev int64 [B + 1]: each row's frame
+ *   count, then the status word, zeroed here: GANTTS_ANALYSIS_BAD_INPUT when a sample within a row's length is not
+ *   finite, GANTTS_ANALYSIS_SHORT when a row has no more frames than FixF0Contour's window (WORLD leaves its f0 unset;
+ *   7 frames at 5 ms), whose f0 is then written as 0.  The mean removed is a fixed-order sum, and both filters are direct
+ *   FIR sums.  Workspace: gantts_world_dio_workspace_bytes(B, S, fs, frame_period).
+ * gantts_world_stonemask: out fp64 [B][T] = pyworld.stonemask of f0 [B][T] (DIO's) over the frames_dev[b] frames of each
+ *   row (DIO's info_dev).  An f0 whose window needs an FFT over 4096 points sets GANTTS_ANALYSIS_FFT in status_dev (DIO's
+ *   info_dev + B) and is written as 0; a non-finite one sets GANTTS_ANALYSIS_BAD_INPUT.
+ * gantts_world_cheaptrick: sp fp64 [B][T][fftlen/2 + 1] = pyworld.cheaptrick(x, f0, timeaxis, fs, q1=-0.15,
+ *   f0_floor=71, fft_size=fftlen).  noise: gantts_world_randn's draws, at least gantts_world_cheaptrick_draws(T, fs,
+ *   fftlen) of them (WORLD reseeds randn per utterance, so every row reads the same stream); offsets int64 [B][T] is
+ *   scratch for each frame's first draw.  An f0 that is not finite, or above what fftlen can analyse (2 + f0 fftlen / fs
+ *   beyond fftlen / 2), sets GANTTS_ANALYSIS_BAD_INPUT and its frame is written as 0.
+ * gantts_sp2mc: mc fp64 [B][T][M+1] = sp2mc(sp[b][t], M, alpha) through op, gantts_sp2mc_operator's matrix on the device,
+ *   for t < frames_dev[b], 0 beyond; sp fp64 [B][T][K] contiguous.
+ * gantts_modspec_smoothing: out fp64 [B][T][D] = modspec_smoothing of x fp64 [B][T][D] (contiguous) over each row's
+ *   lengths_dev[b] frames, 0 beyond: every column's n-point real FFT along time, bins cutoff_bin .. n/2 set to 0 (the
+ *   notebooks' cut-off bin is int(n cutoff / modfs)), the inverse real FFT, its first L frames.  Defined for L <= n only,
+ *   so T <= n is a rule.
+ * Rules, checked before any device work (the error string names the one that failed): non-null pointers,
+ * 1 <= B <= 65535, 1 <= S <= 2^28, 4000 <= fs <= 96000, 1 <= frame_period <= 100 ms, 1 <= T <= 2^24, fftlen and n powers
+ * of two in [64, 4096], 1 <= M+1 <= 128, 2 (K - 1) a power of two in [64, 4096], 1 <= D <= 65535, cutoff_bin >= 0. */
+#define GANTTS_ANALYSIS_BAD_INPUT 1
+#define GANTTS_ANALYSIS_SHORT 2
+#define GANTTS_ANALYSIS_FFT 4
+int64_t gantts_world_dio_frames(int64_t samples, int fs, double frame_period);
+size_t gantts_world_dio_workspace_bytes(int B, int S, int fs, double frame_period);
+int gantts_world_dio(const double* x, int64_t x_bstride, const int64_t* lengths_dev, int B, int S, int fs,
+                     double frame_period, double* f0, int64_t* info_dev, void* workspace, size_t workspace_bytes,
+                     void* stream);
+int gantts_world_stonemask(const double* x, int64_t x_bstride, const int64_t* lengths_dev, const double* f0,
+                           const int64_t* frames_dev, int B, int S, int T, int fs, double frame_period, double* out,
+                           int64_t* status_dev, void* stream);
+int64_t gantts_world_cheaptrick_draws(int T, int fs, int fftlen);
+int gantts_world_cheaptrick(const double* x, int64_t x_bstride, const int64_t* lengths_dev, const double* f0,
+                            const int64_t* frames_dev, int B, int S, int T, int fs, double frame_period, int fftlen,
+                            const double* noise, int64_t noise_count, int64_t* offsets, double* sp, int64_t* status_dev,
+                            void* stream);
+int gantts_sp2mc(const double* sp, const double* op, const int64_t* frames_dev, int B, int T, int M, int K, double* mc,
+                 void* stream);
+int gantts_modspec_smoothing(const double* x, const int64_t* lengths_dev, int B, int T, int D, int n, int cutoff_bin,
+                             double* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Objective distortions of the training loop (reference train.py:399-432 compute_distortions, :383-396
