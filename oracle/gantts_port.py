@@ -380,9 +380,10 @@ def gan_step_mlp(state, x, y, lengths, R, hp, w_d=1.0, mse_w=0.0, mge_w=1.0, adv
                     d_opt=d_opt, g_opt=g_opt)
 
 
-def _pair(sd, k, named):
-    """(``k``.weight, ``k``.bias) of a reference state_dict as leaf tensors (requires_grad), recorded in ``named``."""
-    pair = tuple(torch.as_tensor(np.asarray(sd[k + s])).clone().float().requires_grad_(True)
+def _pair(sd, k, named, dtype=torch.float32):
+    """(``k``.weight, ``k``.bias) of a reference state_dict as ``dtype`` leaf tensors (requires_grad), recorded in
+    ``named``."""
+    pair = tuple(torch.as_tensor(np.asarray(sd[k + s])).clone().to(dtype).requires_grad_(True)
                  for s in (".weight", ".bias"))
     named[k + ".weight"], named[k + ".bias"] = pair
     return pair
@@ -392,18 +393,20 @@ def _count(sd, pre):
     return len([k for k in sd if k.startswith(pre) and k.endswith(".weight")])
 
 
-def _linear_layers(sd, pre, named):
+def _linear_layers(sd, pre, named, dtype=torch.float32):
     """[(W, b), ...] of the ``pre``.i layers then last_linear of a reference state_dict, recorded in ``named``."""
-    return [_pair(sd, k, named) for k in ["%s.%d" % (pre, i) for i in range(_count(sd, pre + "."))] + ["last_linear"]]
+    return [_pair(sd, k, named, dtype)
+            for k in ["%s.%d" % (pre, i) for i in range(_count(sd, pre + "."))] + ["last_linear"]]
 
 
-def _lstm_layers(sd, prefix, num_layers, hidden, bidirectional, named):
-    """One single-layer torch nn.LSTM per layer of the nn.LSTM stored under ``prefix`` in a reference state_dict (see
-    ``lstm_stack``); their parameters are recorded in ``named`` under the stack's names, in its parameters() order."""
+def _lstm_layers(sd, prefix, num_layers, hidden, bidirectional, named, dtype=torch.float32):
+    """One single-layer ``dtype`` torch nn.LSTM per layer of the nn.LSTM stored under ``prefix`` in a reference
+    state_dict (see ``lstm_stack``); their parameters are recorded in ``named`` under the stack's names, in its
+    parameters() order."""
     layers = []
     for k in range(num_layers):
         n_in = np.asarray(sd["%s.weight_ih_l%d" % (prefix, k)]).shape[1]
-        lstm = torch.nn.LSTM(n_in, hidden, 1, batch_first=True, bidirectional=bidirectional)
+        lstm = torch.nn.LSTM(n_in, hidden, 1, batch_first=True, bidirectional=bidirectional).to(dtype)
         with torch.no_grad():
             for s in ("", "_reverse")[:2 if bidirectional else 1]:
                 for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"):
@@ -426,24 +429,27 @@ class GeneratorOracle(object):
     ``forward``'s ``masks`` injects the product's dropout decisions: the hidden-layer multipliers of "mlp" /
     "highway" (see ``mlp_forward``), the inter-layer multipliers of "rnn_highway" / "lstm" (see ``lstm_stack``)
     and [(mask_x, mask_h or None)] per layer of "sru" (see ``sru_layer_forward``).  ``dropout_p`` / ``training``
-    apply to "mlp" / "highway" without masks; the recurrent kinds drop out nothing of their own."""
+    apply to "mlp" / "highway" without masks; the recurrent kinds drop out nothing of their own.
+
+    ``dtype`` is that of every parameter (float32 as the reference trains; float64 gives a reference for the product's
+    fp32 gradients, fed float64 inputs and a float64 R)."""
 
     def __init__(self, kind, sd, static_dim=None, num_hidden=None, hidden_dim=None, bidirectional=False,
-                 rnn_attr="lstm", activation_type=2):
+                 rnn_attr="lstm", activation_type=2, dtype=torch.float32):
         self.kind, self.static_dim = kind, static_dim
         self.bidirectional, self.activation_type = bidirectional, activation_type
         self.named = {}
         if kind in ("highway", "rnn_highway"):
-            self.gate = _pair(sd, "T", self.named)
+            self.gate = _pair(sd, "T", self.named, dtype)
         if kind in ("mlp", "highway"):
-            self.layers = _linear_layers(sd, "layers" if kind == "mlp" else "H", self.named)
+            self.layers = _linear_layers(sd, "layers" if kind == "mlp" else "H", self.named, dtype)
         else:
             if kind == "sru":
                 n = _count(sd, "gru.rnn_lst.")
-                self.layers = [_pair(sd, "gru.rnn_lst.%d" % i, self.named) for i in range(n)]
+                self.layers = [_pair(sd, "gru.rnn_lst.%d" % i, self.named, dtype) for i in range(n)]
             else:
-                self.layers = _lstm_layers(sd, rnn_attr, num_hidden, hidden_dim, bidirectional, self.named)
-            self.h2o = _pair(sd, "hidden2out", self.named)
+                self.layers = _lstm_layers(sd, rnn_attr, num_hidden, hidden_dim, bidirectional, self.named, dtype)
+            self.h2o = _pair(sd, "hidden2out", self.named, dtype)
         self.sums = [torch.zeros_like(p) for p in self.params()]
 
     def params(self):
@@ -467,9 +473,9 @@ class GeneratorOracle(object):
         return apply_generator(out, x, R, hp, self.include_parameter_generation())
 
 
-def discriminator_layers(sd):
-    """[(W, b), ...] (requires_grad) of a reference ``MLP`` state_dict (``layers.i``, ``last_linear``)."""
-    return _linear_layers(sd, "layers", {})
+def discriminator_layers(sd, dtype=torch.float32):
+    """[(W, b), ...] (``dtype``, requires_grad) of a reference ``MLP`` state_dict (``layers.i``, ``last_linear``)."""
+    return _linear_layers(sd, "layers", {}, dtype)
 
 
 class DiscriminatorOracle(object):
@@ -477,19 +483,19 @@ class DiscriminatorOracle(object):
     give its kind and whose tensors give its shape: ``MLP`` (``layers.i.*``, ``last_linear.*``; models.py:121-141) or
     ``LSTMRNN`` / ``GRURNN`` (an nn.LSTM under ``lstm.`` or ``gru.``, then ``hidden2out.*``; models.py:170-213), with
     last_sigmoid=True as train.py:774 builds it.  ``named`` / ``params()`` follow the state_dict.  A recurrent one
-    runs ``lstm_stack`` and drops out nothing but the injected masks."""
+    runs ``lstm_stack`` and drops out nothing but the injected masks.  ``dtype`` as for ``GeneratorOracle``."""
 
-    def __init__(self, sd):
+    def __init__(self, sd, dtype=torch.float32):
         self.named = {}
         if "last_linear.weight" in sd:
-            self.mlp = _linear_layers(sd, "layers", self.named)
+            self.mlp = _linear_layers(sd, "layers", self.named, dtype)
             return
         self.mlp = None
         pre = "lstm" if "lstm.weight_ih_l0" in sd else "gru"
         n = len([k for k in sd if k.startswith(pre + ".weight_ih_l") and not k.endswith("_reverse")])
         hidden = np.asarray(sd[pre + ".weight_hh_l0"]).shape[1]
-        self.layers = _lstm_layers(sd, pre, n, hidden, pre + ".weight_ih_l0_reverse" in sd, self.named)
-        self.h2o = _pair(sd, "hidden2out", self.named)
+        self.layers = _lstm_layers(sd, pre, n, hidden, pre + ".weight_ih_l0_reverse" in sd, self.named, dtype)
+        self.h2o = _pair(sd, "hidden2out", self.named, dtype)
 
     @classmethod
     def of_layers(cls, layers):

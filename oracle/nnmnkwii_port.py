@@ -51,11 +51,11 @@ def normal_matrix(windows, T):
     return P
 
 
-def unit_variance_mlpg_matrix(windows, T):
-    """Dense ``R = (W^T W)^-1 W^T`` as float32 ``(T, num_windows*T)``.
+def unit_variance_mlpg_matrix(windows, T, dtype=np.float32):
+    """Dense ``R = (W^T W)^-1 W^T`` as ``dtype`` (float32 by default) ``(T, num_windows*T)``.
 
     nnmnkwii computes the inverse through a banded Cholesky factorisation (bandmat); the
-    result is the same matrix up to float64 round-off, then cast to float32.
+    result is the same matrix up to float64 round-off, then cast to ``dtype``.
     """
     T = int(T)
     mats = window_matrices(windows, T)
@@ -64,7 +64,7 @@ def unit_variance_mlpg_matrix(windows, T):
         P += W.T @ W
     Wfull = np.vstack(mats)                       # (nw*T, T), window-major rows
     R = np.linalg.solve(P, Wfull.T)               # (T, nw*T)
-    return np.ascontiguousarray(R.astype(np.float32))
+    return np.ascontiguousarray(R.astype(dtype))
 
 
 def _to_window_major(means, num_windows):

@@ -150,25 +150,52 @@ def make_models(kind, seed, cond, d_layers=2, d_hidden=12, bidir=True, p_d=0.5, 
     return mg, md, ohp, d_in
 
 
-def generator_oracle(mg):
+def generator_oracle(mg, dtype=torch.float32):
     """gp.GeneratorOracle of the product's generator mg (MLP, In2OutHighwayNet, In2OutRNNHighwayNet or SRURNN)."""
     sd, name = sd_numpy(mg), type(mg).__name__
     if name == "MLP":
-        return gp.GeneratorOracle("mlp", sd)
+        return gp.GeneratorOracle("mlp", sd, dtype=dtype)
     if name == "In2OutHighwayNet":
-        return gp.GeneratorOracle("highway", sd, static_dim=mg.static_dim)
+        return gp.GeneratorOracle("highway", sd, static_dim=mg.static_dim, dtype=dtype)
     if name == "SRURNN":
         cell = mg.gru.rnn_lst[0]
-        return gp.GeneratorOracle("sru", sd, bidirectional=cell.bidirectional, activation_type=cell.activation_type)
+        return gp.GeneratorOracle("sru", sd, bidirectional=cell.bidirectional, activation_type=cell.activation_type,
+                                  dtype=dtype)
     lm = mg.lstm
     return gp.GeneratorOracle("rnn_highway", sd, static_dim=mg.static_dim, num_hidden=lm.num_layers,
-                              hidden_dim=lm.hidden_size, bidirectional=lm.bidirectional)
+                              hidden_dim=lm.hidden_size, bidirectional=lm.bidirectional, dtype=dtype)
 
 
 def fused(mg, md, hp, B, T, optimizer="Adagrad", **kw):
     from gantts_b200 import fused as F
     return F.FusedGanStep(mg, md, step_hp(hp), B, T, weight_decay=0.0, optimizer=optimizer,
                           optimizer_params=ADAM if optimizer == "Adam" else None, **kw)
+
+
+def split_step(fs, x, y, lengths, update_g=True, phases=(1, 6), between=None, frames=None):
+    """FusedGanStep.step's training call as one native call per entry of `phases` (GANTTS_STEP_D = 1, _G = 2, _FINISH =
+    4; the default is the discriminator phase, then the generator and finishing phases), with between(phase) called after
+    each of them but the last, where a data-parallel caller all-reduces the gradient buffers.  frames: the normaliser a
+    caller passes (the GLOBAL count of valid frames); None lets the step count the mask."""
+    from gantts_b200 import _lib
+    b, t = int(x.shape[0]), int(x.shape[1])
+    fs._set_shape(b, t)
+    fs._shape = (b, t, fs._mlpg_table(t).data_ptr())
+    fs.cfg.adv_w = 1.0
+    fs._bind_params(fs.cfg)
+    seed = (fs._seed + fs._step) & ((1 << 61) - 1)
+    fs.last_seed = seed
+    fs._step += 1
+    fs._set_optimizers(fs.opt_g.steps + 1, fs.opt_d.steps + 1)
+    d_only = 0 if update_g else _lib.STEP_D_ONLY
+    inv = 0.0 if frames is None else 1.0 / float(frames)
+    for i, ph in enumerate(phases):
+        fs._call(ph | d_only, x, y, lengths, inv, seed)
+        if between is not None and i + 1 < len(phases):
+            between(ph)
+    fs.opt_d.steps += 1
+    if update_g:
+        fs.opt_g.steps += 1
 
 
 # ---- the dropout masks of the product's last training step, regenerated from its seeds

@@ -10,10 +10,10 @@ import pytest
 import torch
 
 from conftest import TTS_HP, WINDOWS, rel_err
-from fused_step_helpers import build, dev, fused, make_batch, npy, ragged_lengths, tts_ohp  # noqa: F401
+from fused_step_helpers import build, dev, fused, make_batch, npy, ragged_lengths, split_step, tts_ohp  # noqa: F401
 from oracle import gantts_port as gp
 from oracle import nnmnkwii_port as nnp
-from test_gpu_step_streams import assert_same, record, split_step
+from test_gpu_step_streams import assert_same, record
 
 B, T = 3, 337
 # (b, t, update_g): the capacity, less than one GEMM tile, a D-only step, the capacity again

@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from conftest import TTS_HP
-from fused_step_helpers import build, dev, fused, make_batch, ragged_lengths  # noqa: F401
+from fused_step_helpers import build, dev, fused, make_batch, ragged_lengths, split_step  # noqa: F401
 
 SHAPES = ["cfg2", "small"]
 
@@ -49,25 +49,6 @@ def assert_same(a, b, what):
     assert len(a) == len(b)
     for i, (u, v) in enumerate(zip(a, b)):
         assert torch.equal(u, v), (what, i)
-
-
-def split_step(fs, x, y, lengths, update_g=True):
-    """FusedGanStep.step's training call as two native calls: GANTTS_STEP_D, then GANTTS_STEP_G | GANTTS_STEP_FINISH."""
-    from gantts_b200 import _lib
-    b, t = int(x.shape[0]), int(x.shape[1])
-    fs._set_shape(b, t)
-    fs._shape = (b, t, fs._mlpg_table(t).data_ptr())
-    fs.cfg.adv_w = 1.0
-    fs._bind_params(fs.cfg)
-    seed = (fs._seed + fs._step) & ((1 << 61) - 1)
-    fs._step += 1
-    fs._set_optimizers(fs.opt_g.steps + 1, fs.opt_d.steps + 1)
-    d_only = 0 if update_g else _lib.STEP_D_ONLY
-    fs._call(1 | d_only, x, y, lengths, 0.0, seed)
-    fs._call(6 | d_only, x, y, lengths, 0.0, seed)
-    fs.opt_d.steps += 1
-    if update_g:
-        fs.opt_g.steps += 1
 
 
 @pytest.mark.gpu
