@@ -202,6 +202,9 @@ SIGNATURES = {
                                      _vp, _vp, _vp]),
     "gantts_sp2mc": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "gantts_modspec_smoothing": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "gantts_vc_inputs": (_i, [_vp, _i64, _i64, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gantts_mc2b": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i, _i, _i, ctypes.c_double, _vp, _vp]),
+    "gantts_mlsa_filter": (_i, [_vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, ctypes.c_double, _i, _vp, _vp]),
     "gantts_distortions_workspace_bytes": (_sz, []),
     "gantts_distortions": (_i, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i, _i, _i, _vp, _vp,
                                 ctypes.POINTER(DistortionColsT), _vp, _vp, _sz, _vp]),

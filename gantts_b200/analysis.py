@@ -45,9 +45,14 @@ def analyse(waves, fs, frame_period, order, kind, device):
     (B, T, D) float64 CUDA, 0 beyond each row's frames, D = order for vc and order + 1 for tts_acoustic; frame counts as
     a host int64 array; the same counts as int64 CUDA).  The read of the frame counts and the status word after the last
     kernel is the one host synchronisation; RuntimeError names the rule a row broke."""
+    x, lengths = pad_waves([np.asarray(w).astype(np.float64) for w in waves], device)
+    return analyse_batch(x, lengths, fs, frame_period, order, kind)
+
+
+def analyse_batch(x, lengths, fs, frame_period, order, kind):
+    """analyse on a padded device batch: x (B, S) float64 CUDA samples, lengths int64 CUDA (B,)."""
     if kind not in KINDS:
         raise ValueError("kind must be one of %s (got %r)" % (", ".join(KINDS), kind))
-    x, lengths = pad_waves([np.asarray(w).astype(np.float64) for w in waves], device)
     T = ops.world_dio_frames(x.shape[1], fs, frame_period)
     if kind == "tts_acoustic" and T > SMOOTHING_N:
         raise ValueError("modspec_smoothing is defined for at most %d frames; the longest utterance has %d"

@@ -137,17 +137,23 @@ def check_frames(files, X, Y):
                              % (basename(f), len(x), len(y)))
 
 
-def read_wavs(wav_dir, files, fs):
+def read_wavs(wav_dir, files, fs=None):
     """The samples of <wav_dir>/<name>.wav for every utterance file, as the notebooks read them (scipy.io.wavfile,
-    cast to float64 later); ValueError naming the wav when one is missing, is not at fs or is not mono."""
+    cast to float64 later); ValueError naming the wav when one is missing, is not at fs (None: at the first wav's rate)
+    or is not mono."""
     from scipy.io import wavfile
-    waves = []
+    waves, first = [], None
     for f in files:
         path = join(wav_dir, splitext(basename(f))[0] + ".wav")
         if not os.path.isfile(path):
             raise ValueError("%s is missing (--wav-dir holds one <name>.wav per utterance)" % path)
         rate, data = wavfile.read(path)
-        if rate != fs:
+        if fs is None and first is None:
+            first = (path, rate)
+        if first is not None and rate != first[1]:
+            raise ValueError("%s is at %d Hz, but %s is at %d Hz: the wavs must share one rate"
+                             % (path, rate, first[0], first[1]))
+        if fs is not None and rate != fs:
             raise ValueError("%s is at %d Hz, but --fs=%d" % (path, rate, fs))
         if data.ndim != 1:
             raise ValueError("%s has %d channels; the analysis takes mono wavs" % (path, data.shape[1]))

@@ -722,6 +722,82 @@ def modspec_smoothing(x, lengths, modfs, n=4096, cutoff=50.0):
     return out
 
 
+# ------------------------------------------------------------- voice conversion with the difference MLSA filter
+def _int64_lengths(lengths, B, what):
+    if not (torch.is_tensor(lengths) and lengths.is_cuda and lengths.dtype == torch.int64 and lengths.dim() == 1
+            and lengths.numel() == B):
+        raise RuntimeError("gantts_b200: %s needs int64 CUDA lengths (B,)" % what)
+    return lengths.contiguous()
+
+
+def vc_inputs(mc, lengths, windows, mean, std):
+    """The generator's inputs of test_vc_from_path (gantts_vc_inputs) for every frame t < lengths[b] of row b:
+    P.delta_features(mc[b, :L], windows).astype(np.float32) and P.scale of it by mean, std (float64, as
+    generate.normalize_input scales).  mc (B, T, D) float64 CUDA, any batch and time strides (a column slice is read in
+    place); windows: any window set ops.windows_key accepts.  Returns (xin (B, T, len(windows) D) float32, the static block
+    (B, T, D) float32, the first window's D columns), 0 beyond each length.  No host sync."""
+    if not (torch.is_tensor(mc) and mc.is_cuda and mc.dtype == torch.float64 and mc.dim() == 3):
+        raise RuntimeError("gantts_b200: vc_inputs needs mc (B, T, D) float64 CUDA")
+    if mc.stride(2) != 1:
+        mc = mc.contiguous()
+    B, T, D = mc.shape
+    lengths = _int64_lengths(lengths, B, "vc_inputs")
+    windows = windows_key(windows)
+    W = len(windows) * D
+    col = lambda v: torch.as_tensor(v, dtype=torch.float64, device=mc.device).reshape(-1).contiguous()
+    mean, std = col(mean), col(std)
+    if mean.numel() != W or std.numel() != W:
+        raise RuntimeError("gantts_b200: vc_inputs: mean and std need %d values (got %d, %d)"
+                           % (W, mean.numel(), std.numel()))
+    n = len(windows)
+    l = (ctypes.c_int * n)(*[w[0] for w in windows])
+    u = (ctypes.c_int * n)(*[w[1] for w in windows])
+    taps = [c for w in windows for c in w[2]]
+    coef = (ctypes.c_double * max(len(taps), 1))(*taps)
+    xin = torch.empty(B, T, W, dtype=torch.float32, device=mc.device)
+    stat = torch.empty(B, T, D, dtype=torch.float32, device=mc.device)
+    _lib.check(_lib.load().gantts_vc_inputs(mc.data_ptr(), mc.stride(0), mc.stride(1), lengths.data_ptr(), B, T, D, n,
+                                            l, u, coef, mean.data_ptr(), std.data_ptr(), xin.data_ptr(),
+                                            stat.data_ptr(), _stream()))
+    return xin, stat
+
+
+def mc2b(pred, src, lengths, alpha):
+    """pysptk.mc2b([0, pred - src], alpha) of every frame t < lengths[b] of row b (gantts_mc2b), the difference
+    filter's coefficients of test_vc_from_path: pred, src (B, T, M) CUDA float32 (the converted and the source statics).
+    Returns (B, T, M + 1) float64, 0 beyond each length.  No host sync."""
+    require_cuda(pred, src)
+    if pred.dim() != 3 or tuple(src.shape) != tuple(pred.shape):
+        raise RuntimeError("gantts_b200: mc2b needs pred and src of one shape (B, T, M)")
+    pred = pred if pred.stride(2) == 1 else pred.contiguous()
+    src = src if src.stride(2) == 1 else src.contiguous()
+    B, T, M = pred.shape
+    lengths = _int64_lengths(lengths, B, "mc2b")
+    b = torch.empty(B, T, M + 1, dtype=torch.float64, device=pred.device)
+    _lib.check(_lib.load().gantts_mc2b(pred.data_ptr(), pred.stride(0), pred.stride(1), src.data_ptr(), src.stride(0),
+                                       src.stride(1), lengths.data_ptr(), B, T, M, float(alpha), b.data_ptr(),
+                                       _stream()))
+    return b
+
+
+def mlsa_filter(x, lengths, b, frames, alpha, hop):
+    """Synthesizer(MLSADF(order=M, alpha=alpha), hopsize=hop).synthesis(x[r, :lengths[r]], b[r, :frames[r]]) of every
+    row r (gantts_mlsa_filter): x (B, S) float64 CUDA samples, b (B, T, M + 1) float64 CUDA (mc2b's), lengths and frames
+    int64 CUDA (B,).  SPTK's mlsadf at Pade order 5 without the gain exp(b[0]); M <= 63.  Returns (B, S) float64, 0 at and
+    beyond min(lengths[r], frames[r] hop).  No host sync."""
+    x, lengths = _waves(x, lengths, "mlsa_filter")
+    B, S = x.shape
+    if not (torch.is_tensor(b) and b.is_cuda and b.dtype == torch.float64 and b.dim() == 3 and b.shape[0] == B):
+        raise RuntimeError("gantts_b200: mlsa_filter needs b (B, T, M + 1) float64 CUDA")
+    b = b.contiguous()
+    frames = _int64_lengths(frames, B, "mlsa_filter")
+    y = torch.empty(B, S, dtype=torch.float64, device=x.device)
+    _lib.check(_lib.load().gantts_mlsa_filter(x.data_ptr(), x.stride(0), lengths.data_ptr(), b.data_ptr(),
+                                              frames.data_ptr(), B, S, b.shape[1], b.shape[2] - 1, float(alpha),
+                                              int(hop), y.data_ptr(), _stream()))
+    return y
+
+
 # ------------------------------------------------------------- mini-batches from a corpus on the device
 def corpus_gather(X, Y, offsets, lengths, t, x_out=None, y_out=None, status=None):
     """One padded mini-batch from a packed corpus on the device (gantts_corpus_gather): X (N, Dx), Y (N, Dy) contiguous

@@ -793,6 +793,36 @@ int gantts_sp2mc(const double* sp, const double* op, const int64_t* frames_dev, 
 int gantts_modspec_smoothing(const double* x, const int64_t* lengths_dev, int B, int T, int D, int n, int cutoff_bin,
                              double* out, void* stream);
 
+/* Voice conversion with the difference MLSA filter (reference evaluation_vc.py:40-110, test_vc_from_path with
+ * diffvc=True), over each row's own frames or samples; every row gives the same bits at any batch position, padded length
+ * or padding contents.
+ * gantts_vc_inputs (evaluation_vc.py:61-71): for t < lengths_dev[b], stat float32 [B][T][D] = float32(window 0 of mc) and
+ *   xin float32 [B][T][n_windows D] = float32((float32(delta_features(mc)) - mean) / std), mean and std fp64 device vectors
+ *   of n_windows D.  mc is fp64 with strides (mc_bstride, mc_tstride) and unit column stride.  Window k spans l[k] frames
+ *   back and u[k] ahead; coef holds the l[k] + u[k] + 1 taps of each window in turn (host memory).  Each window runs over
+ *   the row's own frames, 0 outside them (nnmnkwii's correlate, mode "same"), summing tap products in tap order in fp64.
+ *   Both outputs are 0 beyond each row's length.
+ * gantts_mc2b (:95-98): b fp64 [B][T][M+1] = pysptk.mc2b([0, pred - src], alpha) for t < lengths_dev[b], 0 beyond: the
+ *   difference in fp64, then b[M] = mc[M], b[m] = mc[m] - alpha b[m+1], rounded as written.  pred and src float32
+ *   [..][..][M] with the given strides and unit column stride.
+ * gantts_mlsa_filter (:99-101): y fp64 [B][S] = Synthesizer(MLSADF(order=M, alpha=alpha), hopsize=hop).synthesis(x, b) of
+ *   each row's lengths_dev[b] samples of x (fp64, row stride x_bstride) with the frames_dev[b] frames of b (fp64
+ *   [B][T][M+1], gantts_mc2b's): SPTK's mlsadf at Pade order 5, without the gain exp(b[0]).  Hop t covers samples
+ *   [t hop, min((t+1) hop, L)); its coefficients start at frame max(t-1, 0) and after each sample add
+ *   (b[t] - b[max(t-1, 0)]) / (the hop's sample count).  Samples at or beyond min(L, frames hop) are 0.
+ * Rules, checked before any device work: non-null pointers, 1 <= B <= 65535 (mlsa_filter: 4 x 65535), 1 <= T <= 2^24,
+ * 1 <= D <= 65535, 1 to 4 windows of at most 5 taps, 1 <= M <= 65535 (mlsa_filter: M <= 63), |alpha| < 1,
+ * 1 <= S <= 2^28, hop >= 1. */
+int gantts_vc_inputs(const double* mc, int64_t mc_bstride, int64_t mc_tstride, const int64_t* lengths_dev, int B, int T,
+                     int D, int n_windows, const int* l, const int* u, const double* coef, const double* mean,
+                     const double* std, float* xin, float* stat, void* stream);
+int gantts_mc2b(const float* pred, int64_t pred_bstride, int64_t pred_tstride, const float* src, int64_t src_bstride,
+                int64_t src_tstride, const int64_t* lengths_dev, int B, int T, int M, double alpha, double* b,
+                void* stream);
+int gantts_mlsa_filter(const double* x, int64_t x_bstride, const int64_t* lengths_dev, const double* b,
+                       const int64_t* frames_dev, int B, int S, int T, int M, double alpha, int hop, double* y,
+                       void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Objective distortions of the training loop (reference train.py:399-432 compute_distortions, :383-396
  * split_streams, :358-380 inv_scale; nnmnkwii.metrics.{melcd, lf0_mean_squared_error, vuv_error,
